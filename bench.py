@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""bench.py -- Whisper large-v2 realtime multiple on B200 (BASELINE.json metric).
+"""bench.py -- Whisper large-v2 realtime multiple on H100 (BASELINE.json metric).
 
     python bench.py --gpus 1 --steps K --warmup W                  # our arm (CUDA engine through the C ABI)
     python bench.py --impl reference --gpus 1 --steps K --warmup W # reference arm: CTranslate2 on the host cores when it
-                                                                   # is installed on the box, else the oracle port
+                                                                   # is installed, else the oracle port
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
+    python bench.py ... --dump-outputs DIR   # also write what the last timed steps computed as DIR/<name>.npy
 
 Headline workload (configs[1] of BASELINE.json): whisper-large-v2, beam 5, one 3.84 s synthetic 16 kHz utterance per step,
 padded to a 30 s window exactly as WIS does (main.py:613).  Weights are seeded synthetic (no checkpoints in the image),
@@ -70,33 +71,12 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
-
-
-def ncu_dram_traffic_per_launch(*names):
-    """dram__bytes_read + dram__bytes_write per launch from a committed ncu --set full capture under profiles/
-    (the first of `names` that exists), averaged over the captured launches; None if no summary is there."""
-    import csv
-
-    for summary in names:
-        p = os.path.join(ROOT, "profiles", summary)
-        if not os.path.exists(p):
-            continue
-        rows = list(csv.reader(open(p)))
-        hdr, units = rows[0], rows[1]
-        try:
-            ir, iw = hdr.index("dram__bytes_read.sum"), hdr.index("dram__bytes_write.sum")
-        except ValueError:
-            continue
-        scale = {"Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0, "Gbyte": 1e9}
-        tot = [float(r[ir]) * scale.get(units[ir], 1e6) + float(r[iw]) * scale.get(units[iw], 1e6) for r in rows[2:]]
-        if tot:
-            return int(sum(tot) / len(tot)), summary
-    return None, None
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense FP16 / BF16 -- not measured here
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet"
 
 
 def encoder_gemm_flops(dims, windows=1):
-    """Algorithmic FLOPs of the tcgen05 GEMM launches per window (SURVEY.md section 8d): conv2 + 4 GEMMs per encoder
+    """Algorithmic FLOPs of the wgmma GEMM launches per window (SURVEY.md section 8d): conv2 + 4 GEMMs per encoder
     layer + the cross-K/V projection, 1500 valid rows each."""
     d, L = dims.d_model, dims.n_enc_layers
     conv2 = 2 * 1500 * (3 * d) * d
@@ -305,7 +285,16 @@ def cpu_port_small(size, beam, pcm, n_threads):
     return {"kind": "port", "cores": n_threads, "seconds": round(dt, 3), "logmel_seconds": round(t_mel, 4),
             "value": round(len(pcm) / 16000.0 / dt, 3), "unit": "x realtime", "tokens": res[0].sequences_ids[0][:8],
             "sample": "1 request, fp32 torch oracle port incl. the numpy restatement of wis.audio.log_mel_spectrogram "
-                      "(/root/reference is not on the GPU box; published anchor: base / beam 1 / 3.84 s = 245 ms on 16 cores, README.md:100)"}
+                      "(published anchor of the reference server: base / beam 1 / 3.84 s = 245 ms on 16 cores, its README.md:100)"}
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """Write each array as out_dir/<name>.npy: token ids as float64 (exact), everything else as float32."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = a.astype(np.float64 if np.issubdtype(a.dtype, np.integer) else np.float32)
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def run_ours(args):
@@ -348,10 +337,13 @@ def run_ours(args):
     off, ns = np.zeros(1, np.int64), np.array([AUDIO_SAMPLES], np.int32)
     extra = [dims.eot]
 
+    last = {}  # what the most recent step of each timed region handed back to its caller (--dump-outputs)
+
     def step_device():
         handle.logmel(pcm_dev.data_ptr(), off, ns, to_host=False, keep=True, pcm_on_device=True, pcm_dtype=_lib.PCM_F32, B=1)
         t_l = handle.timing()["logmel_ms"]
-        ids, _ = handle.generate(None, prompts, BEAM, 1.0, 1.0, MAX_LENGTH, extra, B=1)
+        ids, scores = handle.generate(None, prompts, BEAM, 1.0, 1.0, MAX_LENGTH, extra, B=1)
+        last["tokens"], last["scores"] = ids, scores
         t = handle.timing()
         return ids, t_l + t["generate_ms"], t
 
@@ -363,6 +355,7 @@ def run_ours(args):
         mel = audio.log_mel_spectrogram(pcm_pin).numpy()[None]  # H2D pcm, D2H mel (what WIS does, main.py:613-616)
         res = model.generate(models.StorageView.from_array(mel), [PROMPT], beam_size=BEAM, max_length=MAX_LENGTH,
                              suppress_tokens=[-1, dims.eot])  # H2D mel, D2H ids
+        last["e2e_mel"], last["e2e_tokens"] = mel, res[0].sequences_ids[0]
         return res[0].sequences_ids[0]
 
     def barrier():
@@ -393,6 +386,7 @@ def run_ours(args):
             stage[k] = stage.get(k, 0.0) + t[k]
     barrier()
     wall_dev = time.perf_counter() - w0
+    dumped = {"tokens": last["tokens"], "scores": last["scores"]}
     # ---- timed region 2: end to end through the reference-facing surface
     barrier()
     w0 = time.perf_counter()
@@ -401,6 +395,9 @@ def run_ours(args):
     barrier()
     wall_e2e = time.perf_counter() - w0
     clocks = sampler.stop()
+    dumped.update(e2e_mel=last["e2e_mel"], e2e_tokens=last["e2e_tokens"])
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dumped)
 
     # ---- kernel-level profile pass (not timed): per-family CUDA-event sums
     handle.set_option("profile", 1)
@@ -427,14 +424,13 @@ def run_ours(args):
     pk, pk_src = peaks()
     flops, n_gemm = encoder_gemm_flops(dims)
     gemm_tf = flops / (prof["gemm_ms"] * 1e-3) / 1e12 if prof.get("gemm_ms") else None
-    peak_tf = pk.get("bf16_tflops_sustained", pk["bf16_tflops"])
+    peak_key = "bf16_tflops_sustained" if "bf16_tflops_sustained" in pk else "bf16_tflops"
+    peak_tf = pk[peak_key]
     ms_per_step = dev_ms / args.steps
     value = world * AUDIO_SECONDS / (ms_per_step * 1e-3)
     e2e_value = world * AUDIO_SECONDS * args.steps / wall_e2e
     dec_bytes = decoder_pass_bytes(dims, 1)
     steps_per = int(t["decode_steps"])  # decoder passes per utterance (prompt prefix in one pass + N_OUT search steps)
-    dec_traffic, dec_traffic_src = ncu_dram_traffic_per_launch("r02_dec_pass_mma_kernel_full.csv", "r02_dec_pass_kernel_full.csv", "r01_dec_pass_kernel_full.csv")
-    gemm_traffic, gemm_traffic_src = ncu_dram_traffic_per_launch("r02_gemm_tc_full.csv", "r01_gemm_tc_full.csv")
     out = {
         "metric": "Whisper large-v2 realtime multiple (audio s / s), beam 5, 3.84 s utterance",
         "value": round(value, 2), "unit": "x realtime", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
@@ -444,7 +440,7 @@ def run_ours(args):
                                "(BASELINE.json configs[1])",
                    "model": MODEL, "beam": BEAM, "prompt_len": 4, "generated_tokens": N_OUT, "decoder_passes": steps_per,
                    "weights": f"seeded synthetic (seed {SEED}, peaked output distribution), fp16 weights / fp32 accumulate",
-                   "l2": "no explicit flush: each step streams 3.1 GB of weights (>> 126 MB L2)",
+                   "l2": "no explicit flush: each step streams 3.1 GB of weights (>> 50 MB L2)",
                    "timer": "CUDA events on the library's launching stream (wisb_get_timing), max over ranks",
                    "parallelism": f"dp{world} (independent utterances, weights broadcast once over NCCL)"},
         "p50_latency_ms": round(ms_per_step, 3),
@@ -459,8 +455,6 @@ def run_ours(args):
         "roofline": {"bound": "hbm", "kernel": "dec_pass_mma_kernel<5> (persistent decoder pass on the warp-level tensor path, one launch per generated token)",
                      "achieved": round(dec_bytes * steps_per / (stage["decode_ms"] / args.steps * 1e-3) / 1e9, 1),
                      "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": None,
-                     "traffic": dec_traffic,
-                     "traffic_note": f"dram bytes per launch from the ncu --set full capture in profiles/{dec_traffic_src}",
                      "peak_source": pk_src + " hbm_gbs",
                      "algorithmic_bytes_per_launch": dec_bytes,
                      "algorithmic_bytes_formula": "2 (14 L d^2 + V d) + 4 L 1500 d  (fp16 weights + one utterance's cross K/V)",
@@ -468,12 +462,10 @@ def run_ours(args):
                      "avg_launch_ms": round(stage["decode_ms"] / args.steps / steps_per, 4),
                      "timing_note": "CUDA events around the decode stage on the launching stream / passes; the stage also holds "
                                     "the small search kernels of every pass (about 2 % of it)"},
-        "encoder_roofline": {"bound": "tensor", "kernel": "gemm_tc_kernel (tcgen05, encoder + cross-K/V GEMMs)",
+        "encoder_roofline": {"bound": "tensor", "kernel": "gemm_tc_kernel (wgmma, encoder + cross-K/V GEMMs)",
                              "achieved": round(gemm_tf, 1) if gemm_tf else None, "peak": peak_tf, "unit": "TFLOP/s",
                              "frac": round(gemm_tf / peak_tf, 4) if gemm_tf else None,
-                             "traffic": gemm_traffic,
-                             "traffic_note": f"bytes per launch, mean of the ncu --set full capture in profiles/{gemm_traffic_src}",
-                             "peak_source": pk_src + " bf16_tflops_sustained (kernel timed inside a long step)",
+                             "peak_source": f"{pk_src} {peak_key} (kernel timed inside a long step)",
                              "algorithmic_flops_per_step": flops, "launches_per_step": n_gemm,
                              "avg_launch_ms": round(prof["gemm_ms"] / n_gemm, 4) if prof.get("gemm_ms") else None,
                              "encoder_share": {k: round(prof[k], 3) for k in ("gemm_ms", "attn_ms", "ln_ms", "conv1_ms")}},
@@ -643,7 +635,7 @@ def probe_ctranslate2():
         sys.path.insert(0, ref)
     try:
         import ctranslate2  # noqa: F401
-    except Exception as e:  # ModuleNotFoundError in this image
+    except Exception as e:  # ModuleNotFoundError when it is not installed
         return None, f"import ctranslate2 failed ({type(e).__name__})"
     import ctranslate2
 
@@ -672,15 +664,13 @@ def run_reference_ct2(args, ct2, model_dir):
         return model.generate(ct2.StorageView.from_array(np.ascontiguousarray(mel)), [PROMPT], beam_size=BEAM,
                               max_length=MAX_LENGTH, suppress_tokens=[-1, 50257], return_scores=False)
 
-    for _ in range(max(1, args.warmup)):
+    for _ in range(args.warmup):
         step()
     t0 = time.perf_counter()
-    done = 0
-    while done < args.steps and (done == 0 or time.perf_counter() - t0 < 150.0):
-        step()
-        done += 1
-    dt = (time.perf_counter() - t0) / done
-    return dt, done, {"kind": "ct2", "cores": cores,
+    for _ in range(args.steps):
+        res = step()
+    dt = (time.perf_counter() - t0) / args.steps
+    return dt, res[0].sequences_ids[0], {"kind": "ct2", "cores": cores,
                       "sample": f"CTranslate2 {getattr(ct2, '__version__', '?')} int8 on the host cores, inter_threads = intra_threads = {half} "
                                 f"(main.py:297-301, 349-355), real weights from {model_dir}, each step = 1 utterance"}
 
@@ -691,7 +681,7 @@ def run_reference(args):
         return
     ct2, where = probe_ctranslate2()
     if ct2 is not None:
-        dt, done, base = run_reference_ct2(args, ct2, where)
+        dt, tokens, base = run_reference_ct2(args, ct2, where)
         probe_note = f"ctranslate2 found, model {where}"
     else:
         probe_note = where
@@ -713,25 +703,20 @@ def run_reference(args):
             mel = om.log_mel_spectrogram(om.pad_or_trim(pcm))[None]
             return oracle.generate(mel, [PROMPT], beam_size=BEAM, max_length=MAX_LENGTH, suppress_tokens=(-1, dims.eot))
 
-        # warm-up is bounded too (a step is ~10-20 s of host work): at least one step, then stop after ~30 s
-        t_w = time.perf_counter()
-        warmed = 0
-        while warmed < args.warmup and (warmed == 0 or time.perf_counter() - t_w < 30.0):
+        # a step is ~10-30 s of host work: choose --steps / --warmup accordingly
+        for _ in range(args.warmup):
             step()
-            warmed += 1
-        args.warmup = warmed
-        # bounded: stop after K steps or ~150 s of host work, whichever comes first (slow hosts: a single step)
         t0 = time.perf_counter()
-        done = 0
-        while done < args.steps and (done == 0 or time.perf_counter() - t0 < 150.0):
-            step()
-            done += 1
-        dt = (time.perf_counter() - t0) / done
+        for _ in range(args.steps):
+            res = step()
+        dt = (time.perf_counter() - t0) / args.steps
+        tokens = res[0].sequences_ids[0]
         base = {"kind": "port", "cores": cores,
                 "sample": f"each step = 1 utterance of the same workload on the host cores (fp32 torch oracle port, {cores} threads); "
-                          "the reference's own engine, ctranslate2==4.1.0, is an un-vendored pip dependency that is absent from "
-                          "this image and cannot be installed offline"}
-    args.steps = done
+                          "the reference's own engine, ctranslate2==4.1.0, is an un-vendored pip dependency that was not found "
+                          "(see reference_probe)"}
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"tokens": [tokens]})
     v = round(AUDIO_SECONDS / dt, 4)
     print(json.dumps({
         "impl": "reference", "metric": "Whisper large-v2 realtime multiple (audio s / s), beam 5, 3.84 s utterance",
@@ -755,8 +740,14 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="headline config only (skip configs0 / 2 / 3 / 4)")
     ap.add_argument("--opt", action="append", default=[], help="engine option key=value (diagnostics), e.g. --opt mega_barrier=1")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step of each timed region returned as DIR/<name>.npy "
+                         "(tokens and scores of the device-resident path, log-mel features and tokens of the host-buffer path; "
+                         "with --impl reference, the tokens of the reference arm)")
     ap.add_argument("--cpu-baseline-only", action="store_true", help=argparse.SUPPRESS)
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if args.cpu_baseline_only:
         from willow_inference_server_b200 import weights as W
 
@@ -764,9 +755,6 @@ def main():
         print(json.dumps(cpu_baseline(dims, W.synth_engine_tensors(dims, **SYNTH_KW), steps=1)))
         return
     if args.impl == "reference":
-        if args.steps > 3:
-            args.steps = 3  # bounded: each step is ~10-30 s of host work
-        args.warmup = min(args.warmup, 1)
         run_reference(args)
     else:
         run_ours(args)

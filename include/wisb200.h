@@ -1,9 +1,9 @@
-/* libwisb200 -- C ABI of the B200-native Whisper hot path that replaces, inside toverainc/willow-inference-server,
- *   (1) wis.audio.log_mel_spectrogram / pad_or_trim        (/root/reference/wis/audio.py:28-51, :72-103)
- *   (2) ctranslate2.models.Whisper(...)                     (/root/reference/main.py:341-355 and the four copies :363-443)
- *   (3) ctranslate2.StorageView.from_array(features)        (/root/reference/main.py:638, :685)
- *   (4) Whisper.generate(features, prompts, beam_size=...)  (/root/reference/main.py:687-692, positional form :535-537)
- *   (5) Whisper.detect_language(features)                   (/root/reference/main.py:638-640)
+/* libwisb200 -- C ABI of the H100-native Whisper hot path that replaces, inside toverainc/willow-inference-server,
+ *   (1) wis.audio.log_mel_spectrogram / pad_or_trim        (wis/audio.py:28-51, :72-103)
+ *   (2) ctranslate2.models.Whisper(...)                     (main.py:341-355 and the four copies :363-443)
+ *   (3) ctranslate2.StorageView.from_array(features)        (main.py:638, :685)
+ *   (4) Whisper.generate(features, prompts, beam_size=...)  (main.py:687-692, positional form :535-537)
+ *   (5) Whisper.detect_language(features)                   (main.py:638-640)
  *
  * Plain C: pointers and sizes only, no C++/torch types.  Every host buffer is owned by the caller and only borrowed for
  * the duration of the call; the handle owns device weights, workspaces, KV caches, streams and CUDA graphs.
@@ -64,7 +64,7 @@ int wisb_generate(wisb_handle* h, const float* mel, int B, const int32_t* prompt
 
 /* Same call with a per-utterance `max_length` (int32 [B], may be NULL = `max_length` for all): lets a cross-request
  * batcher put requests with different length limits into ONE shared decoder pass (CTranslate2's generate takes a single
- * max_length per call, /root/reference/main.py:687-692; the per-utterance form is what its semantics become when
+ * max_length per call, main.py:687-692; the per-utterance form is what its semantics become when
  * several such calls are coalesced).  out_stride >= the largest per-utterance limit of new tokens. */
 int wisb_generate_ex(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
                      float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
@@ -88,9 +88,9 @@ int wisb_get_timing(wisb_handle* h, float* out16);
 int wisb_set_option(wisb_handle* h, const char* key, int value);
 
 /* ---- diagnostics used by tests/ (run the product kernels on caller data) ---- */
-/* C[M,N] (float32) = A[M,K] . W[N,K]^T with fp16 inputs given as raw uint16; impl 0 = tcgen05 kernel, 1 = SIMT check */
+/* C[M,N] (float32) = A[M,K] . W[N,K]^T with fp16 inputs given as raw uint16; impl 0 = wgmma kernel, 1 = SIMT check */
 int wisb_debug_gemm(wisb_handle* h, const uint16_t* a, const uint16_t* w, float* c, int M, int N, int K, int impl, int bn);
-/* the tcgen05 skinny-GEMV building block of the decoder pass on caller data: out[R,N] (float32) = x[R,K] (float32, rounded
+/* the wgmma skinny-GEMV building block of the decoder pass on caller data: out[R,N] (float32) = x[R,K] (float32, rounded
  * to fp16 inside) . W[N,K]^T (fp16 as raw uint16) + bias (may be NULL); R <= 8, K % 64 == 0, K <= 5120.  avg_us (may be
  * NULL) receives the average kernel time over `iters` back-to-back launches. */
 int wisb_debug_gemv_tc(wisb_handle* h, const float* x, const uint16_t* w, const float* bias, float* out, int R, int N, int K,
@@ -103,7 +103,7 @@ int wisb_debug_encode(wisb_handle* h, const float* mel, int B, float* enc_out, i
 int wisb_debug_forced_logits(wisb_handle* h, const float* mel, const int32_t* tokens, int n_tokens, float* logits_out);
 
 /* ---- (6) FLAC ingest (host code, no handle, no GPU): replaces the decode half of `librosa.load(audio_file, sr=16000)`
- * (/root/reference/main.py:579) for the FLAC files WIS is tested with (client/{3sec,10sec,30sec}.flac).
+ * (main.py:579) for the FLAC files WIS is tested with (client/{3sec,10sec,30sec}.flac).
  * wisb_flac_info: stream parameters, number of inter-channel frames and the PCM MD5 from STREAMINFO (any pointer may be NULL).
  * wisb_flac_decode: interleaved int32 samples [n_frames, channels]; every frame's CRC-8 / CRC-16 is checked.
  * Both return 0 or a non-zero code with the reason in wisb_flac_last_error() (thread-local). */

@@ -3,14 +3,14 @@
 TEST INFRASTRUCTURE ONLY -- see ``oracle/__init__.py``.
 
 Follows, step for step:
-  * constants                 /root/reference/wis/audio.py:17-25
-  * ``pad_or_trim``           /root/reference/wis/audio.py:28-51 (numpy branch :43-49)
-  * ``mel_filters``           /root/reference/wis/audio.py:54-69 -- the asset
+  * constants                 wis/audio.py:17-25
+  * ``pad_or_trim``           wis/audio.py:28-51 (numpy branch :43-49)
+  * ``mel_filters``           wis/audio.py:54-69 -- the asset
     ``wis/assets/mel_filters.npz`` is ``librosa.filters.mel(sr=16000, n_fft=400,
     n_mels=80)`` (docstring :59-63); ``slaney_mel_filterbank`` below recomputes
     that published algorithm and reproduces the asset BIT-EXACTLY
     (sha256 of the raw f32 = 85818f15...b405498, checked in tests).
-  * ``log_mel_spectrogram``   /root/reference/wis/audio.py:72-103
+  * ``log_mel_spectrogram``   wis/audio.py:72-103
       - periodic Hann(400)                       :93
       - torch.stft(n_fft=400, hop=160, center=True -> reflect pad 200,
         onesided) -> [201, 3001]                 :94

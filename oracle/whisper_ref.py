@@ -3,11 +3,11 @@
 TEST INFRASTRUCTURE ONLY -- see ``oracle/__init__.py``.
 
 What it restates (reference call sites; the arithmetic itself lives in the
-un-vendored dependency ctranslate2==4.1.0, /root/reference/requirements.txt:22):
+un-vendored dependency ctranslate2==4.1.0, requirements.txt:22):
   * ``Whisper.generate(features, prompts, beam_size=, return_scores=False)``
-        /root/reference/main.py:687-692 (positional form :535-537)
-  * ``Whisper.detect_language(features)``          /root/reference/main.py:638-640
-  * result use ``results[i].sequences_ids[0]``     /root/reference/main.py:707,713
+        main.py:687-692 (positional form :535-537)
+  * ``Whisper.detect_language(features)``          main.py:638-640
+  * result use ``results[i].sequences_ids[0]``     main.py:707,713
 
 Model arithmetic follows the Whisper architecture as implemented in
 [HF] transformers/models/whisper/modeling_whisper.py (conv stem :567-568,:619-620;
@@ -33,7 +33,7 @@ SURVEY.md section 8a rows A11-A14:
     hypotheses exist (length_penalty != 0 disables the early exit) or at the last
     step, best normalised score wins (num_hypotheses=1).
 **PARITY UNPINNED for the decoding rules**: no CTranslate2 binary, source or
-golden transcript exists under /root/reference or in this image.
+golden transcript ships with the reference server.
 """
 from __future__ import annotations
 

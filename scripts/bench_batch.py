@@ -76,7 +76,7 @@ def main():
             t = h.timing()
             prof[name] = {k: round(t[k], 2) for k in ("gemm_ms", "attn_ms", "ln_ms", "conv1_ms", "decode_ms", "encoder_ms", "decode_steps")}
         prof["decode_only"] = {k: round(prof["full"][k] - prof["short"][k], 2) for k in prof["full"]}
-        prof["legend"] = "decode_only: gemm_ms = tcgen05 GEMMs, attn_ms = cross-attention, ln_ms = LayerNorm/residual/embed, conv1_ms = self-attention"
+        prof["legend"] = "decode_only: gemm_ms = wgmma GEMMs, attn_ms = cross-attention, ln_ms = LayerNorm/residual/embed, conv1_ms = self-attention"
         out["profile"] = prof
         h.set_option("profile", 0)
     print(json.dumps(out))

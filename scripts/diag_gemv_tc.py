@@ -1,4 +1,4 @@
-"""Cost of the tcgen05 skinny GEMV at the large-v2 decoder shapes (stand-alone launches, weights from HBM every time)."""
+"""Cost of the wgmma skinny GEMV at the large-v2 decoder shapes (stand-alone launches, weights from HBM every time)."""
 import os
 import sys
 

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """GPU diagnostics: numerical error of the CUDA path vs the oracle on the small synthetic models (used to set the
-test tolerances) -- run under gpurun."""
+test tolerances) -- needs a GPU."""
 import os
 import sys
 

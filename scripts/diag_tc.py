@@ -1,4 +1,4 @@
-"""Diagnostics for the tcgen05 cross-attention of the batched pass: teacher-forced logits with 1..8 positions per pass,
+"""Diagnostics for the wgmma cross-attention of the batched pass: teacher-forced logits with 1..8 positions per pass,
 tensor-core kernel vs SIMT kernel vs the fp32 oracle, error per position."""
 import os
 import sys

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Generate tests/golden/logmel_*.npz and host_logic.json by RUNNING THE REFERENCE.
 
-Run in the build container only (needs /root/reference):
-    python scripts/gen_golden_logmel.py
+Needs a checkout of the reference server (its directory as the first argument):
+    python scripts/gen_golden_logmel.py <path to willow-inference-server>
 
 Imports the reference's own ``wis.audio`` (wis/audio.py:28-159) and records its
 outputs on seeded inputs.  The inputs are not stored: tests regenerate them from
@@ -16,7 +16,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, sys.argv[1])
 
 from wis import audio as ref_audio  # noqa: E402  (the reference itself)
 

@@ -1,10 +1,8 @@
 #!/usr/bin/env python
-"""Run N steps of the bench workload (large-v2, beam 5, one 3.84 s utterance) with nothing else around them, for ncu:
+"""Run N steps of the bench workload (large-v2, beam 5, one 3.84 s utterance) with nothing else around them, for a
+profiler, e.g. Nsight Compute:
 
-  ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches.csv \
-      python scripts/profile_step.py --steps 1
-  ncu --set full --clock-control none --import-source on -k regex:gemm_tc_kernel -s 40 -c 4 -o gpurun_out/gemm \
-      python scripts/profile_step.py --steps 1 --model large-v2
+  ncu --metrics gpu__time_duration.sum --csv --log-file launches.csv python scripts/profile_step.py --steps 1
 """
 import argparse
 import os

@@ -1,45 +1,33 @@
-"""Drop-in test through the reference's OWN orchestration code (SURVEY.md section 7 step 2, section 8b).
+"""Drop-in test against the reference's OWN orchestration code (SURVEY.md section 7 step 2, section 8b).
 
-`do_whisper`, `do_translate` and `chunkit` are taken UNMODIFIED from the reference's main.py (main.py:91-94, 514-547,
-554-770) -- extracted with `ast` at test time, nothing is copied into this repository -- and executed with
-  ctranslate2            := willow_inference_server_b200              (the two-line integration diff of INTEGRATION.md)
-  log_mel_spectrogram .. := willow_inference_server_b200.audio
-and stubs for what stays outside the hot path (librosa, the HF tokenizer / processor, settings, the logger).
+`do_whisper`, `do_translate` and `chunkit` of the reference server's main.py (main.py:91-94, 514-547, 554-770) were run
+unmodified over this package (`ctranslate2 := willow_inference_server_b200`, `wis.audio` := the log-mel oracle) with a
+recording engine in place of the model; scripts/gen_golden_dropin.py stores every call they made on the engine in
+tests/golden/dropin_calls.json -- method, positional vs keyword form, prompt ids, beam size, the windows of each call --
+together with what do_whisper / do_translate returned for the canned engine results below.
 
-main.py itself cannot be imported (aiortc, av, librosa, ctranslate2 ... are absent), which is why the functions are cut out.
-The reference source is found at /root/reference/main.py (build container) or baseline/_ref/wis_reference/main.py (staged
-there, git-ignored, by scripts/stage_reference.py so that it travels to the GPU box); without either the tests skip.
-
-  * CPU test: a recording engine with the signature of models.Whisper.generate / detect_language behind the real
-    StorageView and the log-mel oracle: every call do_whisper makes binds to the shim's API.
-  * GPU test: the real engine; the token ids do_whisper returns equal a direct wisb_generate on the same features.
+  * CPU test: every recorded call binds to the signature of models.Whisper.generate / detect_language, and the record
+    shows the reference behaviour the shim has to serve (one window at beam 5; detect_language first, 75 s -> 6 windows
+    in 3 calls of 2 at the long-mode beam 3; the positional do_translate form).
+  * GPU test: the recorded calls are replayed, exactly as the reference makes them, on the real engine; the token ids
+    equal a direct wisb_generate on the same features.
 """
-import ast
-import datetime
 import inspect
-import logging
-import math
+import json
 import os
-import re
-import types
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CANDIDATES = ["/root/reference/main.py", os.path.join(ROOT, "baseline", "_ref", "wis_reference", "main.py")]
-MAIN_PY = next((p for p in CANDIDATES if os.path.isfile(p)), None)
-needs_reference = pytest.mark.skipif(MAIN_PY is None, reason="reference main.py is not available on this box")
-
 PROMPT = [50258, 50259, 50359, 50363]
 
 
-def _extract(names):
-    src = open(MAIN_PY).read()
-    tree = ast.parse(src)
-    picked = [n for n in tree.body if isinstance(n, ast.FunctionDef) and n.name in names]
-    assert {n.name for n in picked} == set(names)
-    return ast.Module(body=picked, type_ignores=[])
+def dims_table():
+    from willow_inference_server_b200 import weights as W
+
+    d = W.WhisperDims()
+    return {"sot": d.sot, "eot": d.eot, "transcribe": d.transcribe, "translate": d.translate, "no_timestamps": d.no_timestamps,
+            "lang_first": d.lang_first, "n_vocab": d.n_vocab}
 
 
 class FakeTokenizer:
@@ -66,129 +54,107 @@ class FakeProcessor:
         return " ".join(str(int(t)) for t in tokens)
 
 
-def _namespace(engine_pkg, audio_mod, model, dims, pcm, concurrent_gpu_chunks=2):
-    """Globals do_whisper / do_translate read in main.py (main.py:186-232 copies them from settings)."""
-    librosa = types.SimpleNamespace(load=lambda f, sr=16000, mono=True: (pcm, sr),
-                                    get_duration=lambda y, sr: len(y) / float(sr))
-    ns = {
-        "datetime": datetime, "math": math, "re": re, "np": np, "librosa": librosa, "ctranslate2": engine_pkg,
-        "logger": logging.getLogger("dropin"), "settings": types.SimpleNamespace(language="en"),
-        "models": types.SimpleNamespace(whisper_model_large=model, whisper_model_medium=model, whisper_model_small=model,
-                                        whisper_model_base=model, whisper_model_tiny=model, whisper_processor=FakeProcessor(dims)),
-        "chunk_iter": audio_mod.chunk_iter, "pad_or_trim": audio_mod.pad_or_trim,
-        "log_mel_spectrogram": audio_mod.log_mel_spectrogram, "find_longest_common_sequence": audio_mod.find_longest_common_sequence,
-        "beam_size": 1, "long_beam_size": 3, "long_beam_size_threshold": 12000, "support_chunking": True,
-        "concurrent_gpu_chunks": concurrent_gpu_chunks,
-    }
-    code = compile(_extract({"chunkit", "do_translate", "do_whisper"}), MAIN_PY, "exec")
-    exec(code, ns)
-    return ns
+def canned_generate(n):
+    """What the recording engine answered to a generate call of n windows."""
+    from willow_inference_server_b200 import models
+
+    return [models.WhisperGenerationResult([[100 + i, 200 + i, 50257]]) for i in range(n)]
 
 
-def _synth(n, seed):
-    from oracle import logmel as om
+def canned_language():
+    return [[("<|de|>", 0.9), ("<|en|>", 0.1)]]
 
-    return om.synth_utterance(n, seed)
+
+def _record():
+    with open(os.path.join(os.path.dirname(__file__), "golden", "dropin_calls.json")) as f:
+        return json.load(f)
+
+
+def _decode(v, windows):
+    """A recorded argument -> the value the reference passed (feature windows rebuilt from `windows`)."""
+    from willow_inference_server_b200 import models
+
+    if isinstance(v, dict) and set(v) == {"features"}:
+        return models.StorageView.from_array(np.ascontiguousarray(np.stack([windows[i] for i in v["features"]])))
+    return v
+
+
+def _bind(method, call, windows):
+    from willow_inference_server_b200 import models
+
+    args = [_decode(a, windows) for a in call["args"]]
+    kwargs = {k: _decode(v, windows) for k, v in call["kwargs"].items()}
+    bound = inspect.signature(getattr(models.Whisper, method)).bind(None, *args, **kwargs)
+    bound.apply_defaults()
+    return args, kwargs, bound.arguments
 
 
 # ------------------------------------------------------------------------------------------------------------------ CPU
-class RecordingWhisper:
-    """Binds every call to the signature of the real shim methods and returns canned results."""
-
-    def __init__(self):
-        self.calls = []
-
-    def generate(self, *a, **kw):
-        from willow_inference_server_b200 import models
-
-        bound = inspect.signature(models.Whisper.generate).bind(self, *a, **kw)
-        feats, prompts = bound.arguments["features"], bound.arguments["prompts"]
-        assert isinstance(feats, models.StorageView) and feats.shape[1:] == [80, 3000]
-        assert len(prompts) == feats.shape[0] and all(len(p) == 4 for p in prompts)
-        self.calls.append(("generate", feats.shape[0], list(prompts[0]), bound.arguments.get("beam_size", 5)))
-        return [models.WhisperGenerationResult([[100 + i, 200 + i, 50257]]) for i in range(feats.shape[0])]
-
-    def detect_language(self, *a, **kw):
-        from willow_inference_server_b200 import models
-
-        bound = inspect.signature(models.Whisper.detect_language).bind(self, *a, **kw)
-        assert bound.arguments["features"].shape == [1, 80, 3000]
-        self.calls.append(("detect_language",))
-        return [[("<|de|>", 0.9), ("<|en|>", 0.1)]]
-
-
-class OracleAudio:
-    """wis.audio surface on the CPU: the log-mel oracle with the `.numpy()` the reference calls on the result."""
-
-    def __init__(self):
-        from oracle import logmel as om
-        from willow_inference_server_b200 import audio
-
-        self.chunk_iter, self.find_longest_common_sequence = audio.chunk_iter, audio.find_longest_common_sequence
-        self.pad_or_trim = om.pad_or_trim
-        self.log_mel_spectrogram = lambda x: types.SimpleNamespace(numpy=lambda: om.log_mel_spectrogram(x))
-
-
-@needs_reference
 def test_reference_do_whisper_drives_the_shim_api_on_cpu():
-    import willow_inference_server_b200 as pkg
-    from willow_inference_server_b200 import weights as W
-
-    d = W.WhisperDims()
-    dims = {"sot": d.sot, "eot": d.eot, "transcribe": d.transcribe, "translate": d.translate, "no_timestamps": d.no_timestamps,
-            "lang_first": d.lang_first, "n_vocab": d.n_vocab}
-    eng = RecordingWhisper()
-    ns = _namespace(pkg, OracleAudio(), eng, dims, _synth(61440, 1))
-    lang, text, ms, translation, speedup, dur = ns["do_whisper"]("x.flac", "large", 5, "transcribe", False, "en")
-    assert (lang, text, translation, dur) == ("en", "100 200 50257", None, 3840)
-    assert eng.calls == [("generate", 1, PROMPT, 5)]
+    rec = _record()
+    d = dims_table()
+    zeros = [np.zeros((80, 3000), np.float32)] * 8
+    calls = rec["short"]["calls"] + rec["long"]["calls"] + rec["long"]["translate"]["calls"]
+    for call in calls:  # every call the reference makes binds to the shim's signature, with what the shim accepts
+        _, _, a = _bind(call["method"], call, zeros)
+        assert a["features"].shape[1:] == [80, 3000]
+        if call["method"] == "generate":
+            assert len(a["prompts"]) == a["features"].shape[0] and all(len(p) == 4 for p in a["prompts"])
+    # one short utterance: one window, beam 5, the English transcribe prompt
+    short = rec["short"]
+    assert short["windows"] == 1
+    assert short["result"] == {"lang": "en", "text": "100 200 50257", "translation": None, "duration_ms": 3840}
+    assert [(c["method"], _bind(c["method"], c, zeros)[2]["prompts"], _bind(c["method"], c, zeros)[2]["beam_size"]) for c in short["calls"]] == \
+        [("generate", [PROMPT], 5)]
     # language detection + the long-audio path: 75 s -> 6 windows, two per engine call, beam 3 (long mode), LCS merge
-    eng.calls.clear()
-    ns = _namespace(pkg, OracleAudio(), eng, dims, _synth(75 * 16000, 2))
-    lang, text, *_ = ns["do_whisper"]("x.flac", "medium", 5, "transcribe", True, None)
-    assert lang == "de"
-    assert eng.calls[0] == ("detect_language",)
-    assert [c[1] for c in eng.calls[1:]] == [2, 2, 2] and all(c[3] == 3 for c in eng.calls[1:])
-    assert eng.calls[1][2] == [d.sot, d.lang_first + 2, d.transcribe, d.no_timestamps]  # <|de|>
+    long = rec["long"]
+    assert long["windows"] == 6 and long["result"]["lang"] == "de"
+    assert long["calls"][0]["method"] == "detect_language" and long["calls"][0]["args"] == [{"features": [0]}]
+    gen = [_bind("generate", c, zeros)[2] for c in long["calls"][1:]]
+    assert [c["method"] for c in long["calls"][1:]] == ["generate"] * 3
+    assert [g["features"].shape[0] for g in gen] == [2, 2, 2] and all(g["beam_size"] == 3 for g in gen)
+    assert [w for c in long["calls"][1:] for w in c["args"][0]["features"]] == list(range(6))
+    assert gen[0]["prompts"][0] == [d["sot"], d["lang_first"] + 2, d["transcribe"], d["no_timestamps"]]  # <|de|>
     # do_translate: positional generate(features, prompts, beam_size=...) with the <|translate|> prompt (main.py:535-537)
-    eng.calls.clear()
-    out = ns["do_translate"](eng, pkg.StorageView.from_array(np.zeros((1, 80, 3000), np.float32)), 1, "<|de|>", 4)
-    assert eng.calls == [("generate", 1, [d.sot, d.lang_first + 2, d.translate, d.no_timestamps], 4)] and out == "100 200 50257"
+    tr = long["translate"]
+    (c,) = tr["calls"]
+    assert c["method"] == "generate" and len(c["args"]) == 2
+    g = _bind("generate", c, zeros)[2]
+    assert g["prompts"] == [[d["sot"], d["lang_first"] + 2, d["translate"], d["no_timestamps"]]] and g["beam_size"] == 4
+    assert tr["result"] == "100 200 50257"
     # the latent reference bug is still the reference's: translate=True trips over len(int) (main.py:729, SURVEY section 2)
-    with pytest.raises(TypeError):
-        ns["do_whisper"]("x.flac", "large", 5, "transcribe", False, "en", True)
+    assert rec["translate_flag"]["raises"] == "TypeError"
 
 
 # ------------------------------------------------------------------------------------------------------------------ GPU
-@needs_reference
 @pytest.mark.gpu
 def test_reference_do_whisper_over_the_real_engine():
-    import willow_inference_server_b200 as pkg
+    from oracle import logmel as om
     from tests.gpu_common import model_pair
     from willow_inference_server_b200 import audio, models
 
+    rec = _record()
     dims, oracle, h = model_pair()
     model = models.Whisper(None, device="cuda", _handles=[h])
-    d = model.dims
-    # ---- one short utterance: the tokens do_whisper decodes are the tokens of a direct engine call on the same features
-    pcm = _synth(61440, 7)
-    ns = _namespace(pkg, audio, model, d, pcm)
-    lang, text, ms, translation, speedup, dur = ns["do_whisper"]("x.flac", "large", 5, "transcribe", False, "en")
-    mel = audio.log_mel_spectrogram(audio.pad_or_trim(pcm)).numpy()[None]
-    want, _ = h.generate(mel, [PROMPT], beam_size=5)
-    assert text == " ".join(str(t) for t in want[0]) and lang == "en" and dur == 3840 and translation is None
-    # ---- 75 s: chunked, long-mode beam 3, two windows per call, stitched by the LCS merge; detect_language first
-    pcm = _synth(75 * 16000, 8)
-    ns = _namespace(pkg, audio, model, d, pcm)
-    lang, text, *_ = ns["do_whisper"]("x.flac", "base", 5, "transcribe", True, None)
-    mels, strides = audio.log_mel_chunks(pcm)
-    top = model.detect_language(models.StorageView.from_array(mels[:1]))[0][0][0]
-    assert lang == top.strip("<|>")
-    prompt = ns["models"].whisper_processor.tokenizer.convert_tokens_to_ids(["<|startoftranscript|>", top, "<|transcribe|>", "<|notimestamps|>"])
-    seqs, _ = h.generate(mels, [prompt] * mels.shape[0], beam_size=3)
-    merged = audio.find_longest_common_sequence(list(zip(seqs, strides)), ns["models"].whisper_processor.tokenizer)
-    assert text == " ".join(str(int(t)) for t in merged)
-    # ---- do_translate on the features do_whisper left in `gpu_features`
-    out = ns["do_translate"](model, models.StorageView.from_array(mel), 1, "<|en|>", 5)
-    tr, _ = h.generate(mel, [[PROMPT[0], PROMPT[1], d["translate"], PROMPT[3]]], beam_size=5)
-    assert out == " ".join(str(t) for t in tr[0])
+    pcm_short = om.synth_utterance(rec["short"]["n_samples"], 7)
+    pcm_long = om.synth_utterance(rec["long"]["n_samples"], 8)
+    short_windows = audio.log_mel_spectrogram(audio.pad_or_trim(pcm_short)).numpy()[None]
+    long_windows, _ = audio.log_mel_chunks(pcm_long)
+    assert long_windows.shape[0] == rec["long"]["windows"]
+    replays = [(rec["short"]["calls"], short_windows), (rec["long"]["calls"], long_windows),
+               (rec["long"]["translate"]["calls"], long_windows)]
+    n_gen = 0
+    for calls, windows in replays:
+        for call in calls:
+            args, kwargs, a = _bind(call["method"], call, windows)
+            mel = a["features"].array
+            got = getattr(model, call["method"])(*args, **kwargs)  # exactly the form the reference uses
+            if call["method"] == "generate":
+                want, _ = h.generate(mel, a["prompts"], beam_size=a["beam_size"])
+                assert [r.sequences_ids[0] for r in got] == want
+                assert all(len(w) > 0 for w in want)
+                n_gen += 1
+            else:
+                _, probs = h.detect_language(mel)
+                assert [[p for _, p in row] for row in got] == [[float(x) for x in row] for row in probs]
+    assert n_gen == 5

@@ -1,5 +1,5 @@
 """GPU tests of the batched decoder pass (one pass over the decoder weights for every row of a batch of utterances;
-csrc/decoder_batch.cu) -- the path /root/reference/main.py:676-693 takes when it feeds several windows per generate call,
+csrc/decoder_batch.cu) -- the path main.py:676-693 takes when it feeds several windows per generate call,
 and what BASELINE.json configs[2] / configs[3] (batch 64 / 512) measure.
 
   * teacher-forced logits of the batched pass vs the fp32 oracle (tolerance LOGIT_TOL)
@@ -87,7 +87,7 @@ def test_per_utterance_max_length_in_one_pass(pair):
 
 
 def test_cross_attention_tensor_core_vs_simt(pair):
-    # the tcgen05 cross-attention of the batched pass against the SIMT cluster kernel (two implementations of the same sum)
+    # the wgmma cross-attention of the batched pass against the SIMT cluster kernel (two implementations of the same sum)
     dims, oracle, h = pair
     mel = mel_inputs(4)[:1]
     toks = PROMPT + [100, 2000, 30000, 41000, 12]

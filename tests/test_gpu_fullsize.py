@@ -134,7 +134,7 @@ def test_large_v2_numeric_parity_against_the_oracle():
     want = oracle.forced_logits(enc[0], toks).numpy()
     got = h.debug_forced_logits(mel[:1], toks)           # persistent SIMT pass (fp32 activations)
     h.set_option("decoder_batch", 2)
-    got_b = h.debug_forced_logits(mel[:1], toks)         # batched pass (fp16 GEMM operands, tcgen05)
+    got_b = h.debug_forced_logits(mel[:1], toks)         # batched pass (fp16 GEMM operands, wgmma)
     h.set_option("decoder_batch", 1)
     err, err_b = float(np.abs(got - want).max()), float(np.abs(got_b - want).max())
     print(f"large-v2: encoder max abs err {enc_err:.4f}; logits err {err:.4f} (SIMT pass) {err_b:.4f} (batched pass); "
@@ -153,7 +153,7 @@ def test_large_v2_numeric_parity_against_the_oracle():
         assert out[i].sequences_ids[0] == base[i].sequences_ids[0], i
         assert 5 <= len(out[i].sequences_ids[0]) < 40
         assert abs(out[i].scores[0] - base[i].scores[0]) < 5e-2
-    # the same two utterances as rows of one batched pass (10 rows: tcgen05 GEMM chain + tcgen05 cross-attention)
+    # the same two utterances as rows of one batched pass (10 rows: wgmma GEMM chain + wgmma cross-attention)
     outb = m.generate(models.StorageView.from_array(mel), [PROMPT] * 2, beam_size=5)
     for i in robust:
         assert outb[i].sequences_ids[0] == base[i].sequences_ids[0], i

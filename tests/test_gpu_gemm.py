@@ -1,4 +1,4 @@
-"""GPU parity: tcgen05 GEMM (csrc/gemm_tc.cu) vs an fp32 numpy product of the same fp16 operands, and vs the SIMT
+"""GPU parity: wgmma GEMM (csrc/gemm_tc.cu) vs an fp32 numpy product of the same fp16 operands, and vs the SIMT
 cross-check kernel.  fp32 accumulation of exactly representable products: tolerance covers summation order only."""
 import numpy as np
 import pytest
@@ -69,7 +69,7 @@ def test_gemm_rejects_bad_shapes(h):
 
 @pytest.mark.parametrize("R,N,K", [(5, 3840, 1280), (8, 1280, 5120), (1, 1280, 1280), (5, 5120, 1280), (3, 10240, 256), (5, 384, 384)])
 def test_gemv_tc_matches_fp32_reference(h, R, N, K):
-    # the tcgen05 skinny GEMV (weight rows on the MMA's M, activation rows on its N): x is rounded to fp16 inside, so the
+    # the wgmma skinny GEMV (weight rows on the MMA's M, activation rows on its N): x is rounded to fp16 inside, so the
     # reference multiplies the fp16-rounded x by the fp16 weights in fp32
     rng = np.random.default_rng(R * 1000 + N + K)
     x = rng.standard_normal((R, K)).astype(np.float32) * 3.0

@@ -93,7 +93,7 @@ def test_graphs_and_eager_agree(pair):
 
 def test_persistent_pass_kernel_vs_per_op_chain(pair):
     # three implementations of the same decoder arithmetic for <= 8 rows: the persistent pass with its GEMV phases on
-    # tcgen05 (default; fp16 B operand), the persistent SIMT pass (fp32 activations) and the per-op kernel chain
+    # wgmma (default; fp16 B operand), the persistent SIMT pass (fp32 activations) and the per-op kernel chain
     dims, oracle, h = pair
     mel = mel_inputs(4)[:2]
     toks = PROMPT + [100, 2000, 30000, 41000, 12]

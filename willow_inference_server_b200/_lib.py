@@ -209,7 +209,7 @@ class Handle:
         return c
 
     def debug_gemv_tc(self, x: np.ndarray, w16: np.ndarray, bias=None, iters: int = 0):
-        """tcgen05 skinny GEMV on caller data -> (out float32 [R, N], average kernel time in us over `iters` launches)."""
+        """wgmma skinny GEMV on caller data -> (out float32 [R, N], average kernel time in us over `iters` launches)."""
         x = np.ascontiguousarray(x, np.float32)
         w16 = np.ascontiguousarray(w16, np.float16)
         R, K = x.shape

@@ -1,9 +1,9 @@
-"""Drop-in for ``wis/audio.py`` (the names ``main.py:52-57`` imports), running on the B200.
+"""Drop-in for ``wis/audio.py`` (the names ``main.py:52-57`` imports), running on the H100.
 
     from willow_inference_server_b200.audio import (
         log_mel_spectrogram, pad_or_trim, chunk_iter, find_longest_common_sequence)
 
-* ``log_mel_spectrogram`` replaces /root/reference/wis/audio.py:72-103: same argument (float32 numpy PCM), returns an
+* ``log_mel_spectrogram`` replaces wis/audio.py:72-103: same argument (float32 numpy PCM), returns an
   object with ``.numpy()`` -> float32 [80, n_frames] exactly as the call sites use it (main.py:608,614).  The STFT /
   mel / log pipeline runs in the CUDA kernel csrc/logmel.cu; there is no CPU path.
 * ``pad_or_trim`` (wis/audio.py:28-51) is kept for API compatibility; the kernel fuses padding/trimming, so calling
@@ -213,7 +213,7 @@ def find_longest_common_sequence(sequences, tokenizer):
 
 def decode_flac(src, verify: bool = True, return_bps: bool = False):
     """FLAC file path / bytes -> (pcm, sample_rate[, bits_per_sample]).  pcm: int16 (<= 16 bits per sample) or int32, shape [n] for mono,
-    [n, channels] otherwise.  The decode half of ``librosa.load`` (/root/reference/main.py:579) for the FLAC inputs WIS
+    [n, channels] otherwise.  The decode half of ``librosa.load`` (main.py:579) for the FLAC inputs WIS
     is tested with; with ``verify`` the decoded PCM is checked against the MD5 the encoder stored in STREAMINFO (an
     all-zero signature means "not set" and is skipped).  Host code in libwisb200 (csrc/flac.cu); no GPU involved."""
     import hashlib

@@ -1,13 +1,13 @@
 """Cross-request dynamic batcher in front of ``models.Whisper`` (SURVEY.md section 8(f) row 2).
 
 The reference serialises requests: ``do_whisper`` is called synchronously on the asyncio event-loop thread of a
-single-worker gunicorn (/root/reference/main.py:1174-1215, 1243-1348; entrypoint.sh:19-21), two windows per engine call
-(``concurrent_gpu_chunks``, main.py:91-94, 676-693).  The B200 engine decodes every window of a call in ONE shared
+single-worker gunicorn (main.py:1174-1215, 1243-1348; entrypoint.sh:19-21), two windows per engine call
+(``concurrent_gpu_chunks``, main.py:91-94, 676-693).  The engine decodes every window of a call in ONE shared
 decoder pass per generated token (rows = windows x beams up to the engine's row capacity, 320 by default = 64 windows at
 beam 5; csrc/decoder_batch.cu): the 1.6 GB of decoder weights stream once per pass whatever the number of rows, finished
 windows leave the pass, and requests with different ``max_length`` ride the same pass (per-window limits).  So
-concurrent ``/api/asr`` and ``/api/willow`` requests should be coalesced -- measured on a B200 (large-v2, beam 5): 64
-mixed-length windows in one call decode about 8x faster than one after the other (bench.py ``configs2``).
+concurrent ``/api/asr`` and ``/api/willow`` requests should be coalesced (bench.py ``configs2`` measures 64 mixed-length
+large-v2 windows at beam 5 in one call against one after the other).
 This module is the piece a WIS maintainer puts between the endpoints and the engine:
 
     batcher = TranscribeBatcher(whisper_model, max_batch=64, max_wait_ms=2)

@@ -1,4 +1,4 @@
-"""Build libwisb200.so in-tree with nvcc for sm_100a (the only target: no multi-arch, no fallback)."""
+"""Build libwisb200.so in-tree with nvcc for sm_90a (H100, the only target: no multi-arch, no fallback)."""
 from __future__ import annotations
 
 import os
@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libwisb200.so")
 SOURCES = ["engine.cu", "gemm_tc.cu", "logmel.cu", "encoder.cu", "decoder.cu", "decoder_mega.cu", "decoder_batch.cu", "gemv_tc.cu", "search.cu", "flac.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC,-O3,-Wall,-Wno-unused-function", "--expt-relaxed-constexpr",
 ]
 
@@ -52,7 +52,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError(f"nvcc failed on {src}:\n{out}")
         if verbose and out:
             print(out)
-    link = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    link = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}")

@@ -38,7 +38,7 @@ struct Error : std::runtime_error {
   } while (0)
 
 // Function attributes (dynamic shared memory size ...) belong to a device's context: a process that drives several GPUs
-// (ctranslate2-style device_index=[0..N-1] replicas, /root/reference/main.py:295,346) must set them once PER DEVICE.
+// (ctranslate2-style device_index=[0..N-1] replicas, main.py:295,346) must set them once PER DEVICE.
 // `done` is a per-call-site bit mask of devices already configured (a benign race sets an attribute twice).
 template <typename F>
 inline void once_per_device(std::atomic<unsigned long long>& done, F&& f) {

@@ -1,5 +1,5 @@
 // Decoder step kernels for a handful of rows (utterances x beams <= 16): the HBM-bandwidth-bound part of
-// ctranslate2.models.Whisper.generate (/root/reference/main.py:687-692; SURVEY.md section 8a row A10).
+// ctranslate2.models.Whisper.generate (main.py:687-692; SURVEY.md section 8a row A10).
 // Architecture per [HF] modeling_whisper.py:417-508 (decoder layer), :650-700 (embeddings), :966-971 (tied projection).
 //
 // Activations stay fp32 end to end here (weights fp16 -> fp32 on the fly, fp32 FMA): with <= 16 rows the step is bound by

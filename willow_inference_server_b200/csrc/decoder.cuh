@@ -1,5 +1,5 @@
 // Decoder-side kernel interface (decoder.cu / search.cu).  Token loop of ctranslate2.models.Whisper.generate
-// (/root/reference/main.py:687-692; SURVEY.md section 8a rows A10-A14).
+// (main.py:687-692; SURVEY.md section 8a rows A10-A14).
 #pragma once
 #include "common.cuh"
 #include "kernels.h"
@@ -130,8 +130,8 @@ struct BatchArgs {
   const int* flip = nullptr;
   const int* done = nullptr;      // [n_utt] or null (prefill)
   const GemmPlan* vocab = nullptr;
-  // tcgen05 cross-attention: one tensor map over the whole cross-K/V buffer viewed as [rows][64] fp16
-  int cross_tc = 1, num_sms = 148;
+  // wgmma cross-attention: one tensor map over the whole cross-K/V buffer viewed as [rows][64] fp16
+  int cross_tc = 1, num_sms = 132;
   const CUtensorMap* ckv_map = nullptr;
   const __half* ckv_base = nullptr;
   // optional per-kernel-family timing hook (engine option "profile", eager launches only):
@@ -208,7 +208,7 @@ void mega_ln_fold(const __half* w, const float* g, const float* b, const float* 
                   cudaStream_t stream);
 void dec_pass_run(const MegaArgs& a, int num_sms, cudaStream_t stream);
 
-// tcgen05 skinny GEMV (gemv_tc.cu), diagnostics entry: returns the average kernel time in microseconds
+// wgmma skinny GEMV (gemv_tc.cu), diagnostics entry: returns the average kernel time in microseconds
 float gemv_tc_debug_run(const float* x, const __half* w, const float* bias, float* out, int R, int N, int K, int num_sms,
                         int iters, cudaStream_t stream);
 

@@ -1,11 +1,11 @@
 // Batched decoder pass: ONE pass over the decoder weights serves every row (utterance x beam) of a batch of utterances.
 //
 // Reference semantics: the decoder step of ctranslate2.models.Whisper.generate for a batch of feature windows
-// (/root/reference/main.py:676-693 feeds several windows per call; SURVEY.md section 8a row A10, section 7 step 5:
+// (main.py:676-693 of the reference server feeds several windows per call; SURVEY.md section 8a row A10, section 7 step 5:
 // "decoder with M = B x beam rows").  Architecture per [HF] modeling_whisper.py:417-508.
 //
 // Up to 8 rows the persistent SIMT pass (decoder_mega.cu) is the latency path.  Beyond that the pass is a chain of
-//   * tcgen05 GEMMs (gemm_tc.cu): rows are the M dimension (padded to 128-row tiles), the weight matrix streams through
+//   * wgmma GEMMs (gemm_tc.cu): rows are the M dimension (padded to 128-row tiles), the weight matrix streams through
 //     the TMA ring exactly once per pass whatever the number of rows; narrow tiles (BN = 64) and split-K keep >= ~100 CTAs
 //     streaming even when the weight matrix has only d_model output columns;
 //   * the small kernels below: embedding + LayerNorm, split-K reduction + bias + residual + LayerNorm (one kernel),
@@ -346,33 +346,34 @@ bd_cross_attn_kernel(const float* __restrict__ q, const __half* __restrict__ kma
 }
 
 // =====================================================================================================================
-// cross-attention on tcgen05 (the default for the batched pass): persistent CTAs walk (utterance, head) items; the item's
+// cross-attention on wgmma (the default for the batched pass): persistent CTAs walk (utterance, head) items; the item's
 // K and V (2 x 1500 x 64 fp16 = 384 KB) stream ONCE through a TMA ring for all rows of the utterance.
-//   S^T = K Q^T : per 128-key tile, tcgen05.mma M=128 (keys) x N=16 (query rows, zero padded) x K=64, fp32 in TMEM
-//                 (12 tiles x 16 columns) -- keys sit on the TMEM lanes, so all 128 softmax threads have work even with
-//                 5 query rows (with queries on the lanes only 5 threads would)
-//   softmax     : thread = key; the scores of all 12 tiles of its key stay in registers (12 x rows values), one exact
-//                 row maximum / row sum over the 1500 keys (shuffles + 4-way shared memory), P^T -> fp16, swizzled smem
-//   O^T = V^T P : tcgen05.mma M=64 (head dim; A = the V tile as loaded, MN-major) x N=16 x K=128 per tile, accumulated
-//                 over the 12 tiles in TMEM; rows are scaled by 1/rowsum on the way out
-// Warp roles: 0 = TMA producer, 1 = MMA issuer, 2..5 = softmax / epilogue.  Finished utterances are skipped.
+//   S^T = K Q^T : per 128-key tile, two wgmma.m64n8k16 x 4 (keys on M, the <= 8 query rows of the utterance on N), so
+//                 all 128 threads of the warpgroup have softmax work even with 5 query rows; the scores of all 12 tiles
+//                 stay in registers (96 per thread)
+//   softmax     : one exact row maximum / row sum over the 1500 keys (shuffles + 4-way shared memory), P^T -> fp16,
+//                 swizzled shared memory
+//   O^T = V^T P : wgmma.m64n8k16 (A = the V tile as loaded, MN-major; head dim on M) x 8 per tile, accumulated over the
+//                 12 tiles in registers; rows are scaled by 1/rowsum on the way out
+// Warps 0..3 = the consumer warpgroup, warp 4 = TMA producer (ring order per item: 12 K tiles, then 12 V tiles, so the
+// V tiles stream while the softmax runs).  Finished utterances are skipped.
 // =====================================================================================================================
-constexpr int XT_THREADS = 192;
+constexpr int XT_CONS = 128;
+constexpr int XT_THREADS = XT_CONS + 32;
 constexpr int XT_TILE = 128 * HEAD_DIM * 2;        // 16 KB: 128 keys of K or of V
 constexpr int XT_STAGES = 8;
 constexpr int XT_NT = T_ENC_PAD / 128;             // 12 key tiles per item
-constexpr int XT_NQ = 16;                          // query rows padded to the MMA N
-constexpr int XT_P_TILE = XT_NQ * 128 * 2;         // 4 KB: P^T [16 rows][128 keys] = two swizzled 64-key halves
-constexpr int XT_Q_BYTES = XT_NQ * HEAD_DIM * 2;   // 2 KB
+constexpr int XT_NQ = 8;                           // query rows padded to the MMA N
+static_assert(MAX_BEAM <= XT_NQ, "cross-attention: one MMA column per row of an utterance");
+constexpr int XT_P_TILE = XT_NQ * 128 * 2;         // 2 KB: P^T [8 rows][128 keys] = two swizzled 64-key halves
+constexpr int XT_Q_BYTES = XT_NQ * HEAD_DIM * 2;   // 1 KB
 constexpr int XT_OFF_P = XT_STAGES * XT_TILE;
 constexpr int XT_OFF_Q = XT_OFF_P + XT_NT * XT_P_TILE;
-constexpr int XT_OFF_BAR = XT_OFF_Q + 2 * XT_Q_BYTES;
+constexpr int XT_OFF_BAR = XT_OFF_Q + 1024;
 constexpr int XT_MAX_UTT = 512;                    // utterances of one pass (row capacity <= 1024, >= 2 ... rows each, or greedy)
-constexpr int XT_SMEM = XT_OFF_BAR + 2048 + 1024;  // + barriers / scratch / live list (1748 B) + alignment slack
-constexpr int XT_D2_COL = XT_NT * XT_NQ;           // 192: O^T accumulator columns
+constexpr int XT_SMEM = XT_OFF_BAR + 2048 + 1024;  // + barriers / scratch / live list (1412 B) + alignment slack
 constexpr float XT_LOG2E = 1.4426950408889634f;
 
-template <int NB>
 __global__ void __launch_bounds__(XT_THREADS, 1)
 bd_cross_attn_tc_kernel(const __grid_constant__ CUtensorMap map_kv, const float* __restrict__ q, long long row_k0,
                         long long row_v0, const int* __restrict__ done, __half* __restrict__ ctx, int n_utt,
@@ -386,46 +387,28 @@ bd_cross_attn_tc_kernel(const __grid_constant__ CUtensorMap map_kv, const float*
   const uint32_t bar0 = smem_u32(bars);
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (XT_STAGES + s); };
-  const uint32_t q_full0 = bar0 + 8u * (2 * XT_STAGES);  // [2]
-  const uint32_t s_full = q_full0 + 16, d1_empty = q_full0 + 24, p_full = q_full0 + 32, d2_empty = q_full0 + 40,
-                 o_full = q_full0 + 48;
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(bars + 2 * XT_STAGES + 8);
-  float* s_red = reinterpret_cast<float*>(bars + 2 * XT_STAGES + 10);  // [2][4][8] row max / row sum partials
+  float* s_red = reinterpret_cast<float*>(bars + 2 * XT_STAGES);  // [2][4 warps][8 rows]: row max, row sum partials
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   pdl_launch_dependents();
   if (threadIdx.x == 0) {
     for (int s = 0; s < XT_STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), XT_CONS / 32);  // one arrival per consumer warp
     }
-    mbar_init(q_full0, 4);
-    mbar_init(q_full0 + 8, 4);
-    mbar_init(s_full, 1);
-    mbar_init(d1_empty, 4);
-    mbar_init(p_full, 4);
-    mbar_init(d2_empty, 4);
-    mbar_init(o_full, 1);
     fence_mbar_init();
     tma_prefetch_desc(&map_kv);
   }
   // P^T and Q^T rows beyond the live query rows are zero for the whole kernel
-  for (int i = threadIdx.x; i < (XT_NT * XT_P_TILE + 2 * XT_Q_BYTES) / 16; i += XT_THREADS)
+  for (int i = threadIdx.x; i < (XT_NT * XT_P_TILE + XT_Q_BYTES) / 16; i += XT_THREADS)
     *reinterpret_cast<uint4*>(smem + XT_OFF_P + i * 16) = make_uint4(0u, 0u, 0u, 0u);
-  if (warp == 1) {
-    tmem_alloc<256>(smem_u32(const_cast<uint32_t*>(tmem_slot)));
-    tmem_relinquish();
-  }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();  // q and the `done` flags come from the previous kernels of the chain
 
   // live utterances, compacted: item k of this CTA is (s_live[idx / H], idx % H) with idx = blockIdx.x + k * gridDim.x, so the
   // CTAs stay balanced whichever utterances have finished
-  unsigned short* s_live = reinterpret_cast<unsigned short*>(s_red + 128);
+  unsigned short* s_live = reinterpret_cast<unsigned short*>(s_red + 64);
   int* s_nlive = reinterpret_cast<int*>(s_live + XT_MAX_UTT);
   if (threadIdx.x == 0) {
     int n = 0;
@@ -441,9 +424,7 @@ bd_cross_attn_tc_kernel(const __grid_constant__ CUtensorMap map_kv, const float*
     return static_cast<int>(s_live[idx / H]) * H + idx % H;
   };
 
-  // Unit order through the ring: K(0); then per item i: K(i+1), V(i).  The keys of the NEXT item stream (and their S^T MMAs
-  // run) while the softmax of item i is busy, so the TMA stream never waits for the softmax.
-  if (warp == 0) {
+  if (warp == XT_CONS / 32) {
     // ------------------------------------------------------------ TMA producer
     if (lane == 0) {
       unsigned unit = 0;
@@ -455,175 +436,142 @@ bd_cross_attn_tc_kernel(const __grid_constant__ CUtensorMap map_kv, const float*
           tma_load_2d(base + st * XT_TILE, &map_kv, full_bar(st), 0, static_cast<int>(row0 + j * 128));
         }
       };
-      if (n_my > 0) load12(row_k0 + static_cast<long long>(item_of(0)) * T_ENC_PAD);
       for (int k = 0; k < n_my; ++k) {
-        if (k + 1 < n_my) load12(row_k0 + static_cast<long long>(item_of(k + 1)) * T_ENC_PAD);
+        load12(row_k0 + static_cast<long long>(item_of(k)) * T_ENC_PAD);
         load12(row_v0 + static_cast<long long>(item_of(k)) * T_ENC_PAD);
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_f16(128, XT_NQ, false, false);
-      constexpr uint32_t idesc_o = make_idesc_f16(64, XT_NQ, true, false);  // A = V tile, MN-major (head dim contiguous)
-      unsigned unit = 0;
-      auto mma_scores = [&](int it) {  // S^T of item `it` -> D1
-        mbar_wait(q_full0 + 8u * (it & 1), (it >> 1) & 1u);
-        if (it > 0) mbar_wait(d1_empty, (it - 1) & 1u);
-        tc_fence_after();
-        const uint32_t qb = sQ + (it & 1) * XT_Q_BYTES;
-        for (int j = 0; j < XT_NT; ++j, ++unit) {
-          const int st = unit % XT_STAGES;
-          mbar_wait(full_bar(st), (unit / XT_STAGES) & 1u);
-          tc_fence_after();
-          const uint64_t da = make_desc_sw128(base + st * XT_TILE, 1024);
-          const uint64_t db = make_desc_sw128(qb, 1024);
+    return;
+  }
+  // ------------------------------------------------------------ consumer warpgroup
+  // accumulator fragment: M rows 16 warp + lane / 4 (+ 8), N columns (query rows) cq + {0, 1}
+  const int cq = 2 * (lane & 3);
+  auto cons_sync = [] { asm volatile("bar.sync 1, 128;" ::: "memory"); };
+  unsigned unit = 0;
+  auto take = [&]() {  // wait for the next ring unit -> its shared memory address
+    const int st = unit % XT_STAGES;
+    mbar_wait(full_bar(st), (unit / XT_STAGES) & 1u);
+    return base + st * XT_TILE;
+  };
+  auto give_back = [&]() {  // this warp's MMAs on the current unit have completed
+    if (lane == 0) mbar_arrive(empty_bar(unit % XT_STAGES));
+    ++unit;
+  };
+  for (int it = 0; it < n_my; ++it) {
+    const int item = item_of(it);
+    const int u = item / H, h = item - u * H;
+    // Q rows of the item -> fp16, pre-scaled by head_dim^-0.5 (exact), K-major 128-byte-swizzled rows
+    if (threadIdx.x < rows_per_utt * 8) {
+      const int r = threadIdx.x >> 3, c = threadIdx.x & 7;
+      const float* qr = q + static_cast<long long>(u * rows_per_utt + r) * d + h * HEAD_DIM + c * 8;
+      const float4 a0 = *reinterpret_cast<const float4*>(qr), a1 = *reinterpret_cast<const float4*>(qr + 4);
+      __half2 h0 = __floats2half2_rn(a0.x * 0.125f, a0.y * 0.125f), h1 = __floats2half2_rn(a0.z * 0.125f, a0.w * 0.125f);
+      __half2 h2 = __floats2half2_rn(a1.x * 0.125f, a1.y * 0.125f), h3 = __floats2half2_rn(a1.z * 0.125f, a1.w * 0.125f);
+      uint4 v4;
+      v4.x = *reinterpret_cast<uint32_t*>(&h0); v4.y = *reinterpret_cast<uint32_t*>(&h1);
+      v4.z = *reinterpret_cast<uint32_t*>(&h2); v4.w = *reinterpret_cast<uint32_t*>(&h3);
+      *reinterpret_cast<uint4*>(smem + XT_OFF_Q + r * 128 + ((c ^ (r & 7)) << 4)) = v4;
+    }
+    fence_proxy_async_smem();
+    cons_sync();
+    // S^T: sc[j][half][i]: key 128 j + 64 half + 16 warp + lane / 4 + 8 (i >> 1), query row cq + (i & 1)
+    float sc[XT_NT][2][4];
+    const uint64_t dq = make_desc_sw128(sQ, 1024);
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_f16_ss(tmem_base + static_cast<uint32_t>(j * XT_NQ), da + 2u * k, db + 2u * k, idesc_s, k != 0 ? 1u : 0u);
-          umma_commit(empty_bar(st));
-        }
-        umma_commit(s_full);
-      };
-      if (n_my > 0) mma_scores(0);
-      for (int it = 0; it < n_my; ++it) {
-        if (it + 1 < n_my) mma_scores(it + 1);
-        mbar_wait(p_full, it & 1u);
-        if (it > 0) mbar_wait(d2_empty, (it - 1) & 1u);
-        tc_fence_after();
-        for (int j = 0; j < XT_NT; ++j, ++unit) {
-          const int st = unit % XT_STAGES;
-          mbar_wait(full_bar(st), (unit / XT_STAGES) & 1u);
-          tc_fence_after();
+    for (int j = 0; j < XT_NT; ++j) {
+      const uint32_t tile = take();
+      wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const uint64_t dv = make_desc_sw128(base + st * XT_TILE + k * 2048, 1024);
-            const uint64_t dp = make_desc_sw128(sP + j * XT_P_TILE + (k >> 2) * 2048, 1024) + 2u * (k & 3);
-            umma_f16_ss(tmem_base + XT_D2_COL, dv, dp, idesc_o, (j | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(empty_bar(st));
+      for (int hf = 0; hf < 2; ++hf) {
+        const uint64_t dk = make_desc_sw128(tile + hf * (XT_TILE / 2), 1024);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_ss<XT_NQ, 0, 0>(sc[j][hf], dk + 2u * k, dq + 2u * k, k != 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_reg_fence(sc[j][0]);
+      wgmma_reg_fence(sc[j][1]);
+      give_back();
+    }
+    // keys >= 1500 are padding rows of the window
+    const int key_lo = warp * 16 + (lane >> 2);
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+        if ((XT_NT - 1) * 128 + hf * 64 + key_lo + 8 * (i >> 1) >= T_ENC) sc[XT_NT - 1][hf][i] = -INFINITY;
+    // exact row maximum over all keys (lanes with the same lane % 4 hold the same query rows)
+    float* red = s_red;
+    float mx[2];
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      float m = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < XT_NT; ++j)
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) m = fmaxf(m, fmaxf(sc[j][hf][e], sc[j][hf][2 + e]));
+      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
+      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
+      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
+      if (lane < 4) red[warp * 8 + cq + e] = m;
+    }
+    cons_sync();
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+      mx[e] = fmaxf(fmaxf(red[cq + e], red[8 + cq + e]), fmaxf(red[16 + cq + e], red[24 + cq + e])) * XT_LOG2E;
+    // probabilities -> P^T tiles (fp16), row sums
+    float sum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < XT_NT; ++j) {
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int e = i & 1, r = cq + e, kk = key_lo + 8 * (i >> 1);
+          const __half ph = __float2half_rn(exp2f(fmaf(sc[j][hf][i], XT_LOG2E, -mx[e])));
+          sum[e] += __half2float(ph);  // the sum of what the tensor core will actually multiply
+          if (r < rows_per_utt)
+            *reinterpret_cast<__half*>(smem + XT_OFF_P + j * XT_P_TILE + hf * 1024 + r * 128 + (((kk >> 3) ^ (r & 7)) << 4) +
+                                       (kk & 7) * 2) = ph;
         }
-        umma_commit(o_full);
       }
     }
-  } else {
-    // ------------------------------------------------------------ softmax / epilogue: 128 threads = 128 keys of a tile
-    const int qd = warp & 3;                       // TMEM lane quarter this warp may access
-    const int key = qd * 32 + lane;                // key inside a tile == TMEM lane
-    const int st_tid = (warp - 2) * 32 + lane;     // 0..127
-    const uint32_t lane_off = static_cast<uint32_t>(qd * 32) << 16;
-    auto soft_sync = [] { asm volatile("bar.sync 1, 128;" ::: "memory"); };
-    auto write_q = [&](int item, int buf) {
-      // Q rows of the item -> fp16, pre-scaled by head_dim^-0.5 (exact), K-major 128-byte-swizzled rows
-      const int u = item / H, h = item - u * H;
-      if (st_tid < rows_per_utt * 8) {
-        const int r = st_tid >> 3, c = st_tid & 7;
-        const float* qr = q + static_cast<long long>(u * rows_per_utt + r) * d + h * HEAD_DIM + c * 8;
-        const float4 a0 = *reinterpret_cast<const float4*>(qr), a1 = *reinterpret_cast<const float4*>(qr + 4);
-        __half2 h0 = __floats2half2_rn(a0.x * 0.125f, a0.y * 0.125f), h1 = __floats2half2_rn(a0.z * 0.125f, a0.w * 0.125f);
-        __half2 h2 = __floats2half2_rn(a1.x * 0.125f, a1.y * 0.125f), h3 = __floats2half2_rn(a1.z * 0.125f, a1.w * 0.125f);
-        uint4 v4;
-        v4.x = *reinterpret_cast<uint32_t*>(&h0); v4.y = *reinterpret_cast<uint32_t*>(&h1);
-        v4.z = *reinterpret_cast<uint32_t*>(&h2); v4.w = *reinterpret_cast<uint32_t*>(&h3);
-        *reinterpret_cast<uint4*>(smem + XT_OFF_Q + buf * XT_Q_BYTES + r * 128 + ((c ^ (r & 7)) << 4)) = v4;
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      float t = sum[e];
+      t += __shfl_xor_sync(0xffffffffu, t, 4);
+      t += __shfl_xor_sync(0xffffffffu, t, 8);
+      t += __shfl_xor_sync(0xffffffffu, t, 16);
+      if (lane < 4) red[32 + warp * 8 + cq + e] = t;
+    }
+    fence_proxy_async_smem();
+    cons_sync();
+    // O^T [64 dims x 8 rows]
+    float o[4];
+#pragma unroll 1
+    for (int j = 0; j < XT_NT; ++j) {
+      const uint32_t tile = take();
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const uint64_t dv = make_desc_sw128(tile + k * 2048, 1024);
+        const uint64_t dp = make_desc_sw128(sP + j * XT_P_TILE + (k >> 2) * 1024, 1024) + 2u * (k & 3);
+        wgmma_ss<XT_NQ, 1, 0>(o, dv, dp, (j | k) != 0 ? 1u : 0u);
       }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(q_full0 + 8u * buf);
-    };
-    if (n_my > 0) write_q(item_of(0), 0);
-    for (int it = 0; it < n_my; ++it) {
-      const int item = item_of(it);
-      // Q of the next item (its S^T MMAs are issued while this item's softmax runs); that buffer's last reader, MMA1 of
-      // item it - 1, completed before s_full(it - 1)
-      if (it + 1 < n_my) write_q(item_of(it + 1), (it + 1) & 1);
-      mbar_wait(s_full, it & 1u);
-      tc_fence_after();
-      float sc[XT_NT][NB];
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_reg_fence(o);
+      give_back();
+    }
 #pragma unroll
-      for (int j = 0; j < XT_NT; ++j) {
-        uint32_t v[8];
-        tmem_ld_32x32b_x8(tmem_base + lane_off + static_cast<uint32_t>(j * XT_NQ), v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int r = 0; r < NB; ++r) sc[j][r] = __uint_as_float(v[r]);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(d1_empty);
-      // keys >= 1500 are padding rows of the window
-#pragma unroll
-      for (int r = 0; r < NB; ++r)
-        if ((XT_NT - 1) * 128 + key >= T_ENC) sc[XT_NT - 1][r] = -INFINITY;
-      // exact row maximum over all keys
-      float mx[NB];
-#pragma unroll
-      for (int r = 0; r < NB; ++r) {
-        float m = sc[0][r];
-#pragma unroll
-        for (int j = 1; j < XT_NT; ++j) m = fmaxf(m, sc[j][r]);
-        mx[r] = warp_max(m);
-      }
-      float* red = s_red + (it & 1) * 64;
-      if (lane == 0) {
-#pragma unroll
-        for (int r = 0; r < NB; ++r) red[(warp - 2) * 8 + r] = mx[r];
-      }
-      soft_sync();
-#pragma unroll
-      for (int r = 0; r < NB; ++r) mx[r] = fmaxf(fmaxf(red[r], red[8 + r]), fmaxf(red[16 + r], red[24 + r])) * XT_LOG2E;
-      // probabilities -> P^T tiles (fp16), row sums
-      float sum[NB];
-#pragma unroll
-      for (int r = 0; r < NB; ++r) sum[r] = 0.f;
-      const int half = key >> 6, kk = key & 63;
-      const uint32_t p_off = XT_OFF_P + half * 2048 + (kk & 7) * 2;
-#pragma unroll
-      for (int j = 0; j < XT_NT; ++j) {
-#pragma unroll
-        for (int r = 0; r < NB; ++r) {
-          const float pr = exp2f(fmaf(sc[j][r], XT_LOG2E, -mx[r]));
-          const __half ph = __float2half_rn(pr);
-          sum[r] += __half2float(ph);  // the sum of what the tensor core will actually multiply
-          if (r < rows_per_utt)
-            *reinterpret_cast<__half*>(smem + p_off + j * XT_P_TILE + r * 128 + (((kk >> 3) ^ (r & 7)) << 4)) = ph;
-        }
-      }
-#pragma unroll
-      for (int r = 0; r < NB; ++r) sum[r] = warp_sum(sum[r]);
-      if (lane == 0) {
-#pragma unroll
-        for (int r = 0; r < NB; ++r) red[32 + (warp - 2) * 8 + r] = sum[r];
-      }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-      soft_sync();
-      // epilogue: O^T [64 dims x rows]; with M = 64 the accumulator occupies lanes 0..15 of every 32-lane quarter
-      mbar_wait(o_full, it & 1u);
-      tc_fence_after();
-      uint32_t ov[8];
-      tmem_ld_32x32b_x8(tmem_base + lane_off + XT_D2_COL, ov);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(d2_empty);
-      if (lane < 16) {
-        const int u = item / H, h = item - u * H;
-        const int e = qd * 16 + lane;
-#pragma unroll
-        for (int r = 0; r < NB; ++r) {
-          if (r < rows_per_utt) {
-            const float l = (red[32 + r] + red[40 + r]) + (red[48 + r] + red[56 + r]);
-            ctx[static_cast<long long>(u * rows_per_utt + r) * d + h * HEAD_DIM + e] = __float2half_rn(__uint_as_float(ov[r]) / l);
-          }
-        }
+    for (int i = 0; i < 4; ++i) {
+      const int r = cq + (i & 1), e = key_lo + 8 * (i >> 1);
+      if (r < rows_per_utt) {
+        const float l = (red[32 + r] + red[40 + r]) + (red[48 + r] + red[56 + r]);
+        ctx[static_cast<long long>(u * rows_per_utt + r) * d + h * HEAD_DIM + e] = __float2half_rn(o[i] / l);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<256>(tmem_base);
 }
 
 template <typename Kern, typename... Args>
@@ -643,24 +591,21 @@ void bd_launch(Kern kern, dim3 grid, dim3 block, size_t smem, cudaStream_t strea
 
 int bd_ca_smem(int nb) { return 2 * BD_CA_KEYS * HEAD_DIM * 2 + BD_CA_GROUPS * nb * HEAD_DIM * 4; }
 
-template <int NB>
 void cross_tc_launch(const BatchArgs& a, const BatchLayer& ly, cudaStream_t s) {
   WISB_REQUIRE(a.n_utt <= XT_MAX_UTT, "cross-attention: more than 512 utterances in one pass");
   static std::atomic<unsigned long long> once{0};
   once_per_device(once, [] {
-    WISB_CUDA(cudaFuncSetAttribute(bd_cross_attn_tc_kernel<NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, XT_SMEM));
+    WISB_CUDA(cudaFuncSetAttribute(bd_cross_attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XT_SMEM));
   });
   const int items = a.n_utt * a.H;
   const long long row_k0 = (ly.ck - a.ckv_base) / HEAD_DIM, row_v0 = (ly.cv - a.ckv_base) / HEAD_DIM;
-  bd_launch(bd_cross_attn_tc_kernel<NB>, dim3(items < a.num_sms ? items : a.num_sms), dim3(XT_THREADS), XT_SMEM, s, a.pdl != 0,
+  bd_launch(bd_cross_attn_tc_kernel, dim3(items < a.num_sms ? items : a.num_sms), dim3(XT_THREADS), XT_SMEM, s, a.pdl != 0,
             *a.ckv_map, a.q, row_k0, row_v0, a.done, a.ctx, a.n_utt, a.rows_per_utt, a.d, a.H);
 }
 
 void cross_attn_launch(const BatchArgs& a, const BatchLayer& ly, cudaStream_t s) {
   if (a.cross_tc) {
-    if (a.rows_per_utt <= 1) cross_tc_launch<1>(a, ly, s);
-    else if (a.rows_per_utt <= 5) cross_tc_launch<5>(a, ly, s);
-    else cross_tc_launch<MAX_BEAM>(a, ly, s);
+    cross_tc_launch(a, ly, s);
     return;
   }
   static std::atomic<unsigned long long> once{0};

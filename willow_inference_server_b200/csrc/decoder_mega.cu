@@ -3,8 +3,7 @@
 // final LN + vocabulary projection) for <= 8 rows, instead of ~260 dependent kernel launches.
 //
 // Why: at <= 8 rows the pass is bound by streaming 1.8 GB of fp16 decoder weights (SURVEY.md section 8d), but a chain
-// of per-op kernels exposes launch + HBM latency ~260 times per pass (measured: 2.1 ms / pass = 7 % of the HBM
-// roofline even with PDL).  Here
+// of per-op kernels exposes launch + HBM latency ~260 times per pass, even with PDL.  Here
 //   * one CTA per SM, every CTA owns a fixed column slice of every weight matrix;
 //   * a dedicated producer thread per CTA walks the (static) list of weight chunks of ALL phases and streams them into a
 //     2-stage shared-memory ring with cp.async.bulk (TMA, L2 evict-first) + mbarrier complete_tx -- it never waits for
@@ -17,7 +16,7 @@
 // rows in registers and streams the CTA's <= 12 columns through them (weights from the ring), then a transposing warp
 // reduction + one shared-memory hop produce the outputs.
 //
-// Reference semantics: decoder step of ctranslate2.models.Whisper.generate (/root/reference/main.py:687-692);
+// Reference semantics: decoder step of ctranslate2.models.Whisper.generate (main.py:687-692);
 // architecture [HF] modeling_whisper.py:417-508, :650-700, :966-971.
 #include <cooperative_groups.h>
 
@@ -101,8 +100,7 @@ __device__ __forceinline__ int row_token(const MegaArgs& A, int r) {
 // fp16 activation exchange of the warp-MMA pass: element (row r, feature k) of a [K/64 k-blocks][R rows][64] buffer stored in
 // B-FRAGMENT order: inside a k-block, lane slot (g = r, t = (k / 2) % 4) holds the 8 words that lane of mma.m16n8k16 feeds
 // to the 4 k-steps ({b0, b1} x 4), as two 16-byte planes -- exactly the B-operand image a consumer CTA wants in shared memory.
-// Its reload is ONE bulk copy (scripts/ubench_reload: 0.7 us against 1.4 us for the ld.global reload of the same 25.6 KB)
-// and a lane fetches a whole k-block's fragments with two 16-byte loads.
+// Its reload is ONE bulk copy instead of a per-thread ld.global reload of the same bytes, and a lane fetches a whole k-block's fragments with two 16-byte loads.
 __device__ __forceinline__ long long act16_off(int R, int r, int k) {
   // k-block: [plane p = k-steps {0,1} | {2,3}][lane slot r * 4 + t][4 words]: a warp's 16-byte fragment load touches 512
   // consecutive bytes (32-byte strides gave 2-way bank conflicts)
@@ -159,8 +157,8 @@ __device__ __noinline__ void produce_gemv(Ring& rg, const MegaGemv& g, int gp) {
       const int st = rg.unit % MG_NSTAGE;
       mbar_wait(rg.empty(st), ((rg.unit / MG_NSTAGE) & 1u) ^ 1u);
       // one TMA request per unit: rows g0..g0+nc of a K-chunk are contiguous (multi-chunk matrices are stored
-      // chunk-major [chunk][N][kc] by the engine at load time).  Many small copies (one per 2.5 KB row) were bound by
-      // the per-request rate of the copy engine (~0.6 us each, 590 GB/s aggregate).
+      // chunk-major [chunk][N][kc] by the engine at load time): many small copies (one per 2.5 KB row) would be bound by
+      // the per-request rate of the copy engine.
       mbar_arrive_expect_tx(rg.full(st), static_cast<uint32_t>(nc * kc * 2));
       bulk_load_1d_hint(rg.data0 + st * MG_STAGE_BYTES, g.w + (static_cast<long long>(ch) * g.N + g0) * kc,
                         static_cast<uint32_t>(nc * kc * 2), rg.full(st), pol);
@@ -171,7 +169,7 @@ __device__ __noinline__ void produce_gemv(Ring& rg, const MegaGemv& g, int gp) {
 
 // cross-attention: task = (utterance, head, key split): the 1500 keys of a head are split over S CTAs (one K unit and
 // one V unit of <= 288 keys each through the ring); the last split to finish merges the partials (split-K fix-up).
-// (One CTA per head without a split was measured 3x slower: the online-softmax walk over 1500 keys is compute-bound.)
+// (Splitting the keys spreads the online-softmax walk over 1500 keys, which is compute-bound, over several CTAs.)
 struct CrossGeom {
   int S, KS, n_tasks;
 };
@@ -194,14 +192,17 @@ __device__ __forceinline__ void produce_cross_impl(Ring& rg, const MegaArgs& A, 
   for (int task = blockIdx.x; task < cg.n_tasks; task += gridDim.x) {
     const int split = task % cg.S, uh = task / cg.S;
     const int t0 = split * cg.KS;
-    const int nk = min(cg.KS, T_ENC_PAD - t0);  // buffer has 1536 rows; keys >= 1500 are skipped by the consumer
+    // buffer has 1536 rows; keys >= 1500 are skipped by the consumer.  Rounding KS up can leave the last splits without
+    // any rows (132 CTAs over 12 heads: 11 splits of 160 keys): their stages complete on the arrival alone
+    const int nk = max(0, min(cg.KS, T_ENC_PAD - t0));
     const long long off = (static_cast<long long>(uh) * T_ENC_PAD + t0) * HEAD_DIM;
     for (int kv = 0; kv < 2; ++kv) {
       const int st = rg.unit % NS;
       mbar_wait(rg.empty(st), ((rg.unit / NS) & 1u) ^ 1u);
       mbar_arrive_expect_tx(rg.full(st), static_cast<uint32_t>(nk * HEAD_DIM * 2));
-      bulk_load_1d_hint(rg.data0 + st * MG_STAGE_BYTES, (kv == 0 ? ly.ck : ly.cv) + off,
-                        static_cast<uint32_t>(nk * HEAD_DIM * 2), rg.full(st), pol);
+      if (nk > 0)
+        bulk_load_1d_hint(rg.data0 + st * MG_STAGE_BYTES, (kv == 0 ? ly.ck : ly.cv) + off,
+                          static_cast<uint32_t>(nk * HEAD_DIM * 2), rg.full(st), pol);
       ++rg.unit;
     }
   }
@@ -216,8 +217,8 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
 }
 
 // fine-grained event trace of thread 0 of ONE CTA over one layer (debug): (event id, SM clock) pairs collected in shared
-// memory -- a clock read and two shared stores per event, ~20 cycles, against ~130 ns for a globaltimer read plus global
-// stores -- and copied to trace[1024..] when the kernel ends.  s_tr[0] = events so far, < 0 while the window is closed.
+// memory -- a clock read and two shared stores per event, far cheaper than a globaltimer read plus global stores -- and
+// copied to trace[1024..] when the kernel ends.  s_tr[0] = events so far, < 0 while the window is closed.
 __device__ __forceinline__ void trace_ev(const MegaArgs& A, int ctid, int* s_tr, int id) {
   if (A.trace != nullptr && ctid == 0) {
     const int i = s_tr[0];
@@ -259,8 +260,7 @@ __device__ __forceinline__ void grid_barrier(const MegaArgs& A, unsigned& epoch,
   cons_sync();
   ++epoch;
   if (A.barrier_mode == 1) {
-    // one release-add per CTA on a shared counter, thread 0 spins on it (scripts/ubench_sync: 1.23 us vs 1.54 us for the
-    // flag barrier on 148 CTAs); the counter equals epoch * gridDim.x whenever all CTAs have passed barrier `epoch`
+    // one release-add per CTA on a shared counter, thread 0 spins on it (barrier_mode 0: the flag barrier); the counter equals epoch * gridDim.x whenever all CTAs have passed barrier `epoch`
     if (ctid == 0) {
       unsigned* counter = A.epoch_base + 8;
       asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
@@ -590,8 +590,7 @@ __device__ __noinline__ void consume_self_attn(const MegaArgs& A, const MegaLaye
 // 28 groups of 8 lanes walk the split's keys with an online softmax for all beams at once (K/V are read once for every
 // beam); groups are merged by shuffles (4 per warp) and shared memory into one partial (acc[64], m, l) per beam; the
 // last split of a head to arrive (atomic counter) merges the S partials into ctx.
-// kOneArrive: the ring's empty barriers count ONE arrival per stage (tensor-core pass: tcgen05.commit releases the weight
-// stages) instead of one per consumer warp
+// kOneArrive: the ring's empty barriers count ONE arrival per stage instead of one per consumer warp
 // second half of a cross-attention task: the warps' partials (s_part: [warp][beam][64 acc, m, l]) are merged into the CTA's
 // partial for its key split, published, and split 0 of the head merges the S partials into the attention output
 template <int NB, bool kOneArrive, bool kMma>
@@ -955,12 +954,11 @@ __global__ void __launch_bounds__(MG_THREADS, 1) dec_pass_kernel(const MegaArgs 
 // Warp-MMA variant of the pass: the six GEMV phases of a layer and the vocabulary projection run on the warp-level tensor
 // path (mma.sync.m16n8k16, fp16 x fp16 -> fp32): the CTA's weight rows are the MMA's M (16-row tiles), the <= 8 activation
 // rows its N, K is split over the 7 consumer warps and their partial tiles are summed through shared memory.
-// Why not tcgen05 here (it is what the encoder, the batched pass and the cross-attention of the batched pass use): at
-// N = 8 a tcgen05.mma of 64 x 8 x 16 is issue-latency bound at ~50 cycles (scripts/diag_gemv_tc.py: 8.2 us for ANY of the
-// layer shapes, 16.8 us at K = 5120), so a K = 1280 phase costs 2 us and fc2 8 us -- slower than the fp32 FMA loop it was
-// meant to replace (the tcgen05 pass measured 43.1 ms per 16 passes against 29.6 ms).  The warp MMA has no such floor:
-// 18 (k-block, m-tile) items of 4 HMMAs each per warp cover the QKV phase.  What disappears against the SIMT pass: the
-// fp32 FMA loop over the weight stage (1.05 us per 12 columns) and the transposing shuffle reductions.  What stays: the
+// Why not wgmma here (it is what the encoder, the batched pass and the cross-attention of the batched pass use): at N = 8
+// a warpgroup MMA is one 64 x 8 x 16 instruction for four warps, and this pass splits K over 7 consumer warps that each
+// work on their own 16-row tiles; the warp MMA fits that split directly (scripts/diag_gemv_tc.py times the wgmma GEMV
+// at the same shapes for comparison).  18 (k-block, m-tile) items of 4 HMMAs each per warp cover the QKV phase.  What disappears against the SIMT pass: the
+// fp32 FMA loop over the weight stage and the transposing shuffle reductions.  What stays: the
 // producer thread and its static weight schedule (2-D TMA boxes, 128-byte swizzle, straight from the row-major W -- the
 // swizzle is what makes ldmatrix conflict-free), the grid barrier between phases, the attention phases, LayerNorm folded
 // into the epilogue, residual columns owned by the CTA.  Columns are dealt to the CTAs in whole octets (8-row swizzle
@@ -994,11 +992,10 @@ constexpr int MM_GROUP_ROWS = 64;       // weight rows per accumulation group (4
 constexpr int MM_PART_LD = 68;          // partial tiles [warp][8 rows][68]: conflict-free fragment stores
 
 // columns of a GEMV phase owned by this CTA: N / grid each, the first N % grid CTAs one more (row granularity: with whole
-// octets the twelve CTAs that owned 16 of the 1280 columns streamed twice the bytes of the others and closed every d-wide
-// phase ~0.8 us late, scripts/mega_arrivals.py); ring units of a group of `rows` weight rows: as many 64-wide k-blocks as
+// octets some CTAs would own twice the columns of the others and close every d-wide phase late); ring units of a group of `rows` weight rows: as many 64-wide k-blocks as
 // fit a stage, evenly sized.  Computed once per kernel for the five
 // GEMV shapes (qkv, d x d, fc1, fc2, vocabulary): at one warp per scheduler every instruction on a phase's critical path
-// costs ~2.5 ns, the integer divisions of this would be 0.4 us per phase.
+// counts, and these integer divisions would otherwise sit on it in every phase.
 struct MmaGeom {
   int lo, hi, rows_pad, n_full, tail;
   int units_full, kbu_full, units_tail, kbu_tail, pad[7];
@@ -1075,7 +1072,7 @@ template <int NMT>
 __device__ __forceinline__ void mma_unit(float (&acc)[4][4], uint32_t a_kb, uint32_t a_step, uint32_t b_kb, uint32_t b_step,
                                          int n_it, const uint32_t (&sw)[4], uint32_t b_plane) {
   // two k-blocks per trip into two accumulator sets: the second block's loads are in flight under the first block's
-  // HMMA chain (one warp per scheduler: a trip's latency chain is LDS -> ldmatrix -> 4 dependent HMMAs, ~135 ns measured)
+  // HMMA chain (one warp per scheduler: a trip's latency chain is LDS -> ldmatrix -> 4 dependent HMMAs)
   float acc2[NMT][4];
 #pragma unroll
   for (int m = 0; m < NMT; ++m)
@@ -1480,7 +1477,7 @@ __device__ __forceinline__ void consume_gemv_mma(Ring& rg, const MegaArgs& A, co
 }
 
 // ------------------------------------------------------------------ warp-MMA pass: cross-query GEMV fused into the cross-attention
-// A grid-wide phase costs ~3.3 us of fixed latency (release fence, counter, poll, reload) whatever it computes, so the
+// A grid-wide phase has a fixed latency (release fence, counter, poll, reload) whatever it computes, so the
 // LayerNorm + cross-query projection no longer has one: every key-split CTA of head h computes the head's 64 query columns
 // itself (all R rows: 64 x 1280 weights = 164 KB per CTA through the ring, the same bytes for the 7 splits of a head, so HBM
 // still reads W once and the L2 serves the rest), then walks its keys as before.  Weight image: mega_mma_image with one
@@ -1504,13 +1501,15 @@ __device__ __forceinline__ void produce_cross_fused(Ring& rg, const MegaArgs& A,
       ++rg.unit;
     }
     const int t0 = split * cg.KS;
-    const int nk = min(cg.KS, T_ENC_PAD - t0);
+    const int nk = max(0, min(cg.KS, T_ENC_PAD - t0));  // (splits past the last row: see produce_cross_impl)
     const long long off = (static_cast<long long>(uh) * T_ENC_PAD + t0) * HEAD_DIM;
     for (int kv = 0; kv < 2; ++kv) {
       const int st = rg.unit % NS;
       mbar_wait(rg.empty(st), ((rg.unit / NS) & 1u) ^ 1u);
       mbar_arrive_expect_tx(rg.full(st), static_cast<uint32_t>(nk * HEAD_DIM * 2));
-      bulk_load_1d_hint(rg.data0 + st * MG_STAGE_BYTES, (kv == 0 ? ly.ck : ly.cv) + off, static_cast<uint32_t>(nk * HEAD_DIM * 2), rg.full(st), pol);
+      if (nk > 0)
+        bulk_load_1d_hint(rg.data0 + st * MG_STAGE_BYTES, (kv == 0 ? ly.ck : ly.cv) + off, static_cast<uint32_t>(nk * HEAD_DIM * 2),
+                          rg.full(st), pol);
       ++rg.unit;
     }
   }
@@ -1889,8 +1888,8 @@ __global__ void chunk_major_kernel(const __half* __restrict__ src, __half* __res
 // W [N][K] row-major -> the warp-MMA image: CTA b of a `G`-CTA pass owns the rows [lo_b, lo_b + rows_b) (N / G each, the first
 // N % G CTAs one more); inside, groups of 64 rows, each stored [k-block][rows][64] with the 16-byte chunks of a row
 // XOR-swizzled by (row & 7).  One ring unit = a contiguous run of k-blocks = ONE bulk copy, and the bytes land in
-// shared memory exactly as ldmatrix wants them (a TMA tensor-map load per k-block was measured slower: the weights of
-// a phase were not there when its barrier opened).
+// shared memory exactly as ldmatrix wants them (one contiguous copy per unit instead of a TMA tensor-map load per
+// k-block, so that a phase's weights are in place when its barrier opens).
 __global__ void mma_image_kernel(const __half* __restrict__ src, __half* __restrict__ dst, int N, int K, int G) {
   const int base = N / G, rem = N - base * G;
   const int big = rem * (base + 1);

@@ -1,7 +1,7 @@
 // Whisper encoder pieces that are not plain GEMMs: conv1 stem, LayerNorm, non-causal self-attention.
 //
 // Replaces (reference side) the encoder half of ctranslate2.models.Whisper.generate
-// (/root/reference/main.py:687-692; SURVEY.md section 2b rows K2, K4, K6).  Architecture per
+// (main.py:687-692 of the reference server; SURVEY.md section 2b rows K2, K4, K6).  Architecture per
 // [HF] modeling_whisper.py:567-568,619-625 (conv stem), :361-415 (encoder layer).
 #include <mutex>
 
@@ -128,227 +128,166 @@ layernorm_f32_to_f16_kernel(const float* __restrict__ x, const float* __restrict
 }
 
 // =====================================================================================================================
-// Encoder self-attention on tcgen05: one CTA per (128-query tile, head, window), 2 CTAs per SM.
-//   S = Q K^T          : tcgen05.mma M=128 N=128 K=64 (4 instr), fp32 in TMEM cols [0,128)
-//   softmax            : 128 threads, one query row each, tcgen05.ld from TMEM, exp2, P (fp16) -> swizzled smem
-//   O_j = P V_j        : tcgen05.mma M=128 N=64 K=128 (8 instr), TMEM cols [128,192); rescaled/accumulated in registers
-// Keys >= 1500 (padding rows of the 1536-row window layout) are masked.
+// Encoder self-attention on wgmma: one CTA = one warpgroup per (64-query tile, head, window), 3 CTAs per SM.
+//   S = Q K^T          : wgmma.m64n128k16 (4 instr per 128-key block), fp32 in registers
+//   softmax            : online (running max / sum per query row) on the accumulator fragment, exp2; the probabilities
+//                        become the fp16 A operand in registers without a trip through shared memory
+//   O += P V_j         : wgmma.m64n64k16 with A from registers (8 instr per block), O rescaled in registers
+// Thread 0 also feeds the 2-stage K/V ring with TMA.  Keys >= 1500 (padding rows of the 1536-row window) are masked.
 // V operand: kVMN = true  -> V tile as loaded [kv][dh] (MN-major B descriptor)
 //            kVMN = false -> pre-transposed Vt [dh][kv] written by the QKV GEMM epilogue (K-major B descriptor)
 // =====================================================================================================================
-constexpr int AT_THREADS = 192;
-constexpr int AT_BM = 128, AT_BN = 128;
+constexpr int AT_THREADS = 128;
+constexpr int AT_BM = 64, AT_BN = 128;
 constexpr int AT_NB = T_ENC_PAD / AT_BN;  // 12 key blocks
-constexpr int AT_TILE = 128 * 64 * 2;     // 16 KB
-constexpr int AT_SMEM = AT_TILE /*Q*/ + 2 * AT_TILE /*K*/ + 2 * AT_TILE /*V*/ + 2 * AT_TILE /*P*/ + 128;
+constexpr int AT_TILE = 128 * 64 * 2;     // 16 KB: 128 keys of K or of V
+constexpr int AT_Q_BYTES = AT_BM * 64 * 2;
+constexpr int AT_SMEM = AT_Q_BYTES + 4 * AT_TILE /*K, V x 2 stages*/ + 64 /*barriers*/ + 1024 /*alignment slack*/;
+
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
+  __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
 
 template <bool kVMN>
-__global__ void __launch_bounds__(AT_THREADS, 2)
+__global__ void __launch_bounds__(AT_THREADS, 3)
 enc_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                 const __grid_constant__ CUtensorMap map_v, __half* __restrict__ ctx, int d, int H) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const uint32_t base = smem_u32(smem);
-  if ((base & 1023u) != 0) __trap();
+  extern __shared__ uint8_t at_raw[];
+  const uint32_t raw_addr = smem_u32(at_raw);
+  const uint32_t base = (raw_addr + 1023u) & ~1023u;
   const uint32_t sQ = base;
-  const uint32_t sK = base + AT_TILE;
-  const uint32_t sV = base + 3 * AT_TILE;
-  const uint32_t sP = base + 5 * AT_TILE;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 7 * AT_TILE);
-  const uint32_t bar0 = smem_u32(bars);
+  const uint32_t sK = base + AT_Q_BYTES;
+  const uint32_t sV = sK + 2 * AT_TILE;
+  const uint32_t bar0 = sV + 2 * AT_TILE;
   const uint32_t q_full = bar0;
   auto kv_full = [&](int s) { return bar0 + 8u * (1 + s); };
-  auto kv_empty = [&](int s) { return bar0 + 8u * (3 + s); };
-  const uint32_t s_full = bar0 + 8u * 5, s_empty = bar0 + 8u * 6, p_full = bar0 + 8u * 7, o_full = bar0 + 8u * 8;
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(bars + 9);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int row0 = b * T_ENC_PAD + qt * AT_BM;
 
-  if (threadIdx.x == 0) {
+  if (tid == 0) {
     mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(kv_full(s), 1);
-      mbar_init(kv_empty(s), 1);
-    }
-    mbar_init(s_full, 1);
-    mbar_init(s_empty, 4);
-    mbar_init(p_full, 4);
-    mbar_init(o_full, 1);
+    mbar_init(kv_full(0), 1);
+    mbar_init(kv_full(1), 1);
     fence_mbar_init();
     tma_prefetch_desc(&map_q);
     tma_prefetch_desc(&map_k);
     tma_prefetch_desc(&map_v);
   }
-  if (warp == 1) {
-    tmem_alloc<256>(smem_u32(const_cast<uint32_t*>(tmem_slot)));
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_s = tmem_base, tmem_o = tmem_base + 128;
   pdl_launch_dependents();
-  pdl_wait();  // barriers, TMEM and descriptors were set up under the QKV GEMM's tail; its output is visible from here on
+  pdl_wait();  // barriers and descriptors were set up under the QKV GEMM's tail; its output is visible from here on
 
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_arrive_expect_tx(q_full, AT_TILE);
-      tma_load_2d(sQ, &map_q, q_full, h * HEAD_DIM, row0);
-      for (int j = 0; j < AT_NB; ++j) {
-        const int st = j & 1;
-        const uint32_t ph = (j >> 1) & 1u;
-        mbar_wait(kv_empty(st), ph ^ 1u);
-        mbar_arrive_expect_tx(kv_full(st), 2 * AT_TILE);
-        tma_load_2d(sK + st * AT_TILE, &map_k, kv_full(st), d + h * HEAD_DIM, b * T_ENC_PAD + j * AT_BN);
-        if (kVMN) {
-          tma_load_2d(sV + st * AT_TILE, &map_v, kv_full(st), 2 * d + h * HEAD_DIM, b * T_ENC_PAD + j * AT_BN);
-        } else {
-          // Vt viewed as [B*H*64 rows, 1536 cols]; two 64x64 halves of the key block
-          tma_load_2d(sV + st * AT_TILE, &map_v, kv_full(st), j * AT_BN, (b * H + h) * HEAD_DIM);
-          tma_load_2d(sV + st * AT_TILE + AT_TILE / 2, &map_v, kv_full(st), j * AT_BN + 64, (b * H + h) * HEAD_DIM);
-        }
-      }
+  auto load_kv = [&](int j) {
+    const int st = j & 1;
+    mbar_arrive_expect_tx(kv_full(st), 2 * AT_TILE);
+    tma_load_2d(sK + st * AT_TILE, &map_k, kv_full(st), d + h * HEAD_DIM, b * T_ENC_PAD + j * AT_BN);
+    if (kVMN) {
+      tma_load_2d(sV + st * AT_TILE, &map_v, kv_full(st), 2 * d + h * HEAD_DIM, b * T_ENC_PAD + j * AT_BN);
+    } else {
+      // Vt viewed as [B*H*64 rows, 1536 cols]; two 64x64 halves of the key block
+      tma_load_2d(sV + st * AT_TILE, &map_v, kv_full(st), j * AT_BN, (b * H + h) * HEAD_DIM);
+      tma_load_2d(sV + st * AT_TILE + AT_TILE / 2, &map_v, kv_full(st), j * AT_BN + 64, (b * H + h) * HEAD_DIM);
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_f16(AT_BM, AT_BN, false, false);
-      constexpr uint32_t idesc_o = make_idesc_f16(AT_BM, HEAD_DIM, false, kVMN);
-      mbar_wait(q_full, 0);
-      for (int j = 0; j < AT_NB; ++j) {
-        const int st = j & 1;
-        mbar_wait(kv_full(st), (j >> 1) & 1u);
-        if (j > 0) mbar_wait(s_empty, (j - 1) & 1u);
-        tc_fence_after();
-        const uint64_t dq = make_desc_sw128(sQ, 1024);
-        const uint64_t dk = make_desc_sw128(sK + st * AT_TILE, 1024);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma_f16_ss(tmem_s, dq + 2u * k, dk + 2u * k, idesc_s, k != 0 ? 1u : 0u);
-        umma_commit(s_full);
-        mbar_wait(p_full, j & 1u);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const uint64_t dp = make_desc_sw128(sP + (k >> 2) * AT_TILE, 1024) + 2u * (k & 3);
-          uint64_t dv;
-          if (kVMN)
-            dv = make_desc_sw128(sV + st * AT_TILE + k * 2048, 1024);
-          else
-            dv = make_desc_sw128(sV + st * AT_TILE + (k >> 2) * (AT_TILE / 2), 1024) + 2u * (k & 3);
-          umma_f16_ss(tmem_o, dp, dv, idesc_o, k != 0 ? 1u : 0u);
-        }
-        umma_commit(o_full);
-        umma_commit(kv_empty(st));
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    const int r = q * 32 + lane;  // query row inside the tile == TMEM lane
-    const uint32_t lane_off = static_cast<uint32_t>(q * 32) << 16;
-    const float c = 0.125f * 1.4426950408889634f;  // dh^-0.5 * log2(e)
-    float m_run = -INFINITY, l_run = 0.f;
-    float acc[HEAD_DIM];
-#pragma unroll
-    for (int i = 0; i < HEAD_DIM; ++i) acc[i] = 0.f;
-    uint8_t* sp_gen = smem + 5 * AT_TILE;
-    for (int j = 0; j < AT_NB; ++j) {
-      mbar_wait(s_full, j & 1u);
-      tc_fence_after();
-      const int kv0 = j * AT_BN;
-      const bool tail = (kv0 + AT_BN > T_ENC);
-      float mx = -INFINITY;
-#pragma unroll 1
-      for (int ch = 0; ch < 4; ++ch) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_s + lane_off + ch * 32, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          float s = __uint_as_float(v[i]);
-          if (tail && kv0 + ch * 32 + i >= T_ENC) s = -INFINITY;
-          mx = fmaxf(mx, s);
-        }
-      }
-      const float m_new = fmaxf(m_run, mx);
-      const float alpha = exp2f((m_run - m_new) * c);
-      if (j > 0) {
-        mbar_wait(o_full, (j - 1) & 1u);
-        tc_fence_after();
-#pragma unroll
-        for (int ch = 0; ch < 2; ++ch) {
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(tmem_o + lane_off + ch * 32, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) acc[ch * 32 + i] = (acc[ch * 32 + i] + __uint_as_float(v[i])) * alpha;
-        }
-      }
-      float rowsum = 0.f;
-      const float mc = m_new * c;
-#pragma unroll 1
-      for (int ch = 0; ch < 4; ++ch) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_s + lane_off + ch * 32, v);
-        tmem_ld_wait();
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          float p0 = exp2f(fmaf(__uint_as_float(v[2 * i]), c, -mc));
-          float p1 = exp2f(fmaf(__uint_as_float(v[2 * i + 1]), c, -mc));
-          if (tail) {
-            if (kv0 + ch * 32 + 2 * i >= T_ENC) p0 = 0.f;
-            if (kv0 + ch * 32 + 2 * i + 1 >= T_ENC) p1 = 0.f;
-          }
-          rowsum += p0 + p1;
-          __half2 hh = __floats2half2_rn(p0, p1);
-          pk[i] = *reinterpret_cast<uint32_t*>(&hh);
-        }
-        // P is the K-major A operand [128 rows, 128 keys] as two 64-key halves of 128-byte swizzled rows
-        uint8_t* half_base = sp_gen + (ch >> 1) * AT_TILE + r * 128;
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const int chunk = (ch & 1) * 4 + g;  // 16-byte chunk index inside the 128-byte row
-          uint4 u = make_uint4(pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]);
-          *reinterpret_cast<uint4*>(half_base + ((chunk ^ (r & 7)) << 4)) = u;
-        }
-      }
-      l_run = l_run * alpha + rowsum;
-      m_run = m_new;
-      tc_fence_before();
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(s_empty);
-        mbar_arrive(p_full);
-      }
-    }
-    mbar_wait(o_full, (AT_NB - 1) & 1u);
-    tc_fence_after();
-    const float inv = 1.0f / l_run;
-    __half* o = ctx + static_cast<long long>(row0 + r) * d + h * HEAD_DIM;
-#pragma unroll
-    for (int ch = 0; ch < 2; ++ch) {
-      uint32_t v[32];
-      tmem_ld_32x32b_x32(tmem_o + lane_off + ch * 32, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        uint32_t w4[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int e = g * 8 + 2 * i;
-          __half2 hh = __floats2half2_rn((acc[ch * 32 + e] + __uint_as_float(v[e])) * inv,
-                                         (acc[ch * 32 + e + 1] + __uint_as_float(v[e + 1])) * inv);
-          w4[i] = *reinterpret_cast<uint32_t*>(&hh);
-        }
-        *reinterpret_cast<uint4*>(o + ch * 32 + g * 8) = make_uint4(w4[0], w4[1], w4[2], w4[3]);
-      }
-    }
+  };
+  if (tid == 0) {
+    mbar_arrive_expect_tx(q_full, AT_Q_BYTES);
+    tma_load_2d(sQ, &map_q, q_full, h * HEAD_DIM, row0);
+    load_kv(0);
+    load_kv(1);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<256>(tmem_base);
+
+  // this thread's accumulator rows: r0 = 16 warp + lane / 4 and r0 + 8; columns 8 j + 2 (lane % 4) + {0, 1}
+  const int cq = 2 * (lane & 3);
+  const float c = 0.125f * 1.4426950408889634f;  // dh^-0.5 * log2(e)
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  float o[HEAD_DIM / 2];
+#pragma unroll
+  for (int i = 0; i < HEAD_DIM / 2; ++i) o[i] = 0.f;
+  const uint64_t dq = make_desc_sw128(sQ, 1024);
+  mbar_wait(q_full, 0);
+#pragma unroll 1
+  for (int j = 0; j < AT_NB; ++j) {
+    const int st = j & 1;
+    mbar_wait(kv_full(st), (j >> 1) & 1u);
+    float s[AT_BN / 2];
+    const uint64_t dk = make_desc_sw128(sK + st * AT_TILE, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_ss<AT_BN, 0, 0>(s, dq + 2u * k, dk + 2u * k, k != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_reg_fence(s);
+    const int kv0 = j * AT_BN;
+    if (kv0 + AT_BN > T_ENC) {
+#pragma unroll
+      for (int i = 0; i < AT_BN / 2; ++i)
+        if (kv0 + (i >> 2) * 8 + cq + (i & 1) >= T_ENC) s[i] = -INFINITY;
+    }
+    float alpha[2], mc[2];
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int nb = 0; nb < AT_BN / 8; ++nb) mx = fmaxf(mx, fmaxf(s[4 * nb + 2 * hr], s[4 * nb + 2 * hr + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[hr], mx);
+      alpha[hr] = exp2f((m_run[hr] - m_new) * c);
+      mc[hr] = m_new * c;
+      m_run[hr] = m_new;
+    }
+    uint32_t pa[AT_BN / 16][4];
+    float rs[2] = {0.f, 0.f};
+#pragma unroll
+    for (int kk = 0; kk < AT_BN / 16; ++kk) {
+      float p[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        p[i] = exp2f(fmaf(s[8 * kk + i], c, -mc[(i >> 1) & 1]));
+        rs[(i >> 1) & 1] += p[i];
+      }
+      pa[kk][0] = pack_half2(p[0], p[1]);
+      pa[kk][1] = pack_half2(p[2], p[3]);
+      pa[kk][2] = pack_half2(p[4], p[5]);
+      pa[kk][3] = pack_half2(p[6], p[7]);
+    }
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) l_run[hr] = l_run[hr] * alpha[hr] + rs[hr];
+#pragma unroll
+    for (int i = 0; i < HEAD_DIM / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < AT_BN / 16; ++kk) {
+      uint64_t dv;
+      if (kVMN)
+        dv = make_desc_sw128(sV + st * AT_TILE + kk * 2048, 1024);
+      else
+        dv = make_desc_sw128(sV + st * AT_TILE + (kk >> 2) * (AT_TILE / 2), 1024) + 2u * (kk & 3);
+      wgmma_rs<HEAD_DIM, kVMN ? 1 : 0>(o, pa[kk], dv, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_reg_fence(o);
+    __syncthreads();  // every thread's MMAs have read stage st: refill it
+    if (tid == 0 && j + 2 < AT_NB) load_kv(j + 2);
+  }
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    l_run[hr] += __shfl_xor_sync(0xffffffffu, l_run[hr], 1);
+    l_run[hr] += __shfl_xor_sync(0xffffffffu, l_run[hr], 2);
+  }
+  const float inv[2] = {1.0f / l_run[0], 1.0f / l_run[1]};
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int r = warp * 16 + (lane >> 2) + 8 * hr;
+    __half* out = ctx + static_cast<long long>(row0 + r) * d + h * HEAD_DIM + cq;
+#pragma unroll
+    for (int nb = 0; nb < HEAD_DIM / 8; ++nb)
+      *reinterpret_cast<uint32_t*>(out + nb * 8) = pack_half2(o[4 * nb + 2 * hr] * inv[hr], o[4 * nb + 2 * hr + 1] * inv[hr]);
+  }
 }
 
 // SIMT cross-check (diagnostics / tests only): one thread per query row, online softmax in fp32
@@ -415,7 +354,7 @@ void enc_attn_plan(AttnPlan& p, const __half* qkv, const __half* vt, __half* ctx
   p.ctx = ctx;
   p.v_mn_major = v_mn_major;
   const long long rows = static_cast<long long>(B) * T_ENC_PAD;
-  make_tmap_f16_2d(&p.map_q, qkv, 3LL * d, rows, 3LL * d, 64, 128);
+  make_tmap_f16_2d(&p.map_q, qkv, 3LL * d, rows, 3LL * d, 64, AT_BM);
   make_tmap_f16_2d(&p.map_k, qkv, 3LL * d, rows, 3LL * d, 64, 128);
   if (v_mn_major)
     make_tmap_f16_2d(&p.map_v, qkv, 3LL * d, rows, 3LL * d, 64, 128);

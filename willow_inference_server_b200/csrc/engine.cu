@@ -96,7 +96,7 @@ using namespace wisb;
 
 struct wisb_handle {
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   std::mutex mu;
   cudaStream_t stream = nullptr;
   Dims dims{};
@@ -351,7 +351,7 @@ void finish_create(wisb_handle* h) {
   const bool has_model = h->blob != nullptr;
   cudaDeviceProp prop;
   WISB_CUDA(cudaGetDeviceProperties(&prop, h->device));
-  WISB_REQUIRE(prop.major == 10, "libwisb200 is built for sm_100a (Blackwell B200) only");
+  WISB_REQUIRE(prop.major == 9 && prop.minor == 0, "libwisb200 is built for sm_90a (Hopper H100) only");
   h->num_sms = prop.multiProcessorCount;
   WISB_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
   for (auto& e : h->ev) WISB_CUDA(cudaEventCreate(&e));
@@ -488,7 +488,7 @@ void ensure_encoder(wisb_handle* h, int B) {
     h->hbuf.ensure(M * 4 * d, true);
     h->enc_out.ensure(M * d, true);
     h->ckv.ensure(static_cast<size_t>(dm.n_dec_layers) * 2 * M * d, true);
-    // the whole cross-K/V buffer as rows of one head's 64 values (for the tcgen05 cross-attention of the batched pass)
+    // the whole cross-K/V buffer as rows of one head's 64 values (for the wgmma cross-attention of the batched pass)
     make_tmap_f16_2d(&h->ckv_map, h->ckv.p, HEAD_DIM, static_cast<long long>(h->ckv.n / HEAD_DIM), HEAD_DIM, HEAD_DIM, 128);
     h->enc_cap = B;
   }
@@ -1457,7 +1457,7 @@ int wisb_set_option(wisb_handle* h, const char* key, int value) {
       WISB_REQUIRE(!value || h->mega_img.p != nullptr, "mega_mma needs d_model <= 1280 and a multiple of 64");
       h->mega_tc = value ? 1 : 0;
     }
-    else if (k == "cross_tc") {  // 1: tcgen05 cross-attention in the batched pass, 0: the SIMT cluster kernel (cross-check)
+    else if (k == "cross_tc") {  // 1: wgmma cross-attention in the batched pass, 0: the SIMT cluster kernel (cross-check)
       h->cross_tc = value ? 1 : 0;
       drop_graphs(h);
     }

@@ -1,5 +1,5 @@
 // FLAC stream decoder (host code, no device work): the ingest format of the reference's fixtures and of /api/asr
-// uploads.  The reference decodes with librosa/soundfile (/root/reference/main.py:579 `librosa.load(audio_file,
+// uploads.  The reference decodes with librosa/soundfile (main.py:579 `librosa.load(audio_file,
 // sr=16000)`; fixtures client/{3sec,10sec,30sec}.flac); SURVEY.md section 8(f) row 3a asks for a decoder verified by the
 // PCM MD5 every FLAC file carries in STREAMINFO.  Written from the FLAC format specification (frame / subframe /
 // residual layout, CRC-8 0x07 on the frame header, CRC-16 0x8005 on the frame); integer exact.

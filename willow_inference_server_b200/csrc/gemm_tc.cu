@@ -1,15 +1,17 @@
-// tcgen05 GEMM for sm_100a:  D[M,N] = A[M,K] . W[N,K]^T   (fp16 x fp16 -> fp32 in TMEM) with fused epilogues.
+// wgmma GEMM for sm_90a:  D[M,N] = A[M,K] . W[N,K]^T   (fp16 x fp16 -> fp32 in registers) with fused epilogues.
 //
 // Replaces (reference side): every dense layer CTranslate2 runs through cuBLAS `gemmEx` for
-// ctranslate2.models.Whisper.generate (/root/reference/main.py:687-692; SURVEY.md section 2b rows K3,K5,K7-K9,K11).
+// ctranslate2.models.Whisper.generate (main.py:687-692 of the reference server; SURVEY.md section 2b rows K3,K5,K7-K9,K11).
 //
-// Structure (one persistent CTA per SM, 192 threads):
-//   warp 0      TMA producer   : cp.async.bulk.tensor 128x64 (A) and BNx64 (W) fp16 tiles, 128B swizzle, STAGES-deep ring
-//   warp 1      MMA issuer     : one lane issues tcgen05.mma.cta_group::1.kind::f16 (M=128, N=BN, K=16) x4 per stage,
-//                                tcgen05.commit frees the smem stage / publishes the accumulator
-//   warps 2..5  epilogue       : tcgen05.ld 32x32b from the double-buffered TMEM accumulator, bias / GELU / residual /
-//                                scatter epilogues, vectorised global stores
-// The accumulator is double buffered in TMEM (2 x BN columns) so the epilogue of tile i overlaps the main loop of i+1.
+// Structure (one persistent CTA per SM, 384 threads = 3 warpgroups):
+//   warps 0..7  two consumer warpgroups: warpgroup g issues wgmma.m64nBNk16 (x4 per stage) for rows [64 g, 64 g + 64) of
+//               the 128-row tile, accumulates in registers, then runs the bias / GELU / residual / scatter epilogues
+//               (each warp stages its accumulator through shared memory, 16 rows x 64 columns at a time, so that each
+//               of its 32 threads writes one row's 32 consecutive columns with vector stores)
+//   warps 8..11 producer warpgroup, one thread of which issues cp.async.bulk.tensor 128x64 (A) and BNx64 (W) fp16 tiles,
+//               128B swizzle, into a STAGES-deep ring; it gives most of its registers to the consumers (setmaxnreg), which
+//               hold up to 128 fp32 accumulators per thread at BN = 256
+// The ring keeps streaming the next tiles' operands while the consumers run an epilogue.
 #include <mutex>
 
 #include "kernels.h"
@@ -22,14 +24,19 @@ namespace {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int A_STAGE_BYTES = BM * BK * 2;
-constexpr int GEMM_THREADS = 192;
+constexpr int GEMM_CONSUMERS = 256;                 // two warpgroups
+constexpr int GEMM_THREADS = GEMM_CONSUMERS + 128;  // + producer warpgroup
+// a warp's epilogue staging slice: 16 rows x two 32-column halves, fp32; row stride 66 and half offset 33 put the 32
+// lanes' reads (lane = row + 16 half) in 32 different banks
+constexpr int EPI_LD = 66, EPI_HALF = 33;
+constexpr int EPI_BYTES = (GEMM_CONSUMERS / 32) * 16 * EPI_LD * 4;
 
 template <int BN>
 struct GemmCfg {
   static constexpr int STAGES = (BN == 256) ? 4 : (BN == 160 ? 5 : (BN == 128 ? 6 : 8));
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
-  static constexpr int TMEM_COLS = (2 * BN <= 128) ? 128 : ((2 * BN <= 256) ? 256 : 512);  // power of two >= two accumulator buffers
-  static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + EPI_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(SMEM_BYTES <= 232448, "gemm: shared memory per block");
 };
 
 __device__ __forceinline__ void store_f16x32(__half* dst, const float (&f)[32]) {
@@ -50,21 +57,21 @@ __device__ __forceinline__ void store_f16x32(__half* dst, const float (&f)[32]) 
 }
 
 // One thread owns one output row and 32 consecutive columns [col0, col0+32).
-__device__ __forceinline__ void epilogue_chunk(const GemmEpi& e, int row, int col0, const uint32_t (&v)[32], int split) {
+__device__ __forceinline__ void epilogue_chunk(const GemmEpi& e, int row, int col0, const float (&v)[32], int split) {
   float f[32];
   if (e.bias != nullptr) {
     const float4* b4 = reinterpret_cast<const float4*>(e.bias + col0);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       float4 b = __ldg(b4 + i);
-      f[4 * i + 0] = __uint_as_float(v[4 * i + 0]) + b.x;
-      f[4 * i + 1] = __uint_as_float(v[4 * i + 1]) + b.y;
-      f[4 * i + 2] = __uint_as_float(v[4 * i + 2]) + b.z;
-      f[4 * i + 3] = __uint_as_float(v[4 * i + 3]) + b.w;
+      f[4 * i + 0] = v[4 * i + 0] + b.x;
+      f[4 * i + 1] = v[4 * i + 1] + b.y;
+      f[4 * i + 2] = v[4 * i + 2] + b.z;
+      f[4 * i + 3] = v[4 * i + 3] + b.w;
     }
   } else {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
+    for (int i = 0; i < 32; ++i) f[i] = v[i];
   }
   switch (e.mode) {
     case EPI_F16_GELU:
@@ -116,8 +123,8 @@ __device__ __forceinline__ void epilogue_chunk(const GemmEpi& e, int row, int co
       long long idx = ((((static_cast<long long>(layer) * 2 + kv) * e.batch + e.batch_off + b) * e.n_heads + head) * T_ENC_PAD + t) * 64;
       if (e.kv_swizzle) {
         // persistent warp-MMA decoder pass: the 16-byte chunks of a key's 128-byte row are XOR-swizzled by the key index, so
-        // that the bulk-copied rows are ldmatrix-conflict-free in shared memory (unswizzled: 8-way conflicts, ~190 cycles
-        // per ldmatrix.x4 measured).  The batched pass reads the linear layout through a TMA swizzle instead.
+        // that the bulk-copied rows are ldmatrix-conflict-free in shared memory (unswizzled: 8-way bank conflicts per
+        // ldmatrix.x4).  The batched pass reads the linear layout through a TMA swizzle instead.
         uint4* row = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out) + idx);
         const int c0 = e0 >> 3;
 #pragma unroll
@@ -179,8 +186,8 @@ __device__ __forceinline__ void epilogue_chunk(const GemmEpi& e, int row, int co
 }
 
 // kMC: launched as clusters of 2 CTAs that own vertically adjacent M tiles of the same N tile; each CTA fetches half of
-// the W tile and TMA-multicasts it to both, which cuts the L2->SM operand traffic per MMA from (128+BN) to (128+BN/2) rows
-// (the 1-CTA kernel is L2-feed limited at ~50 % of the tensor peak, DESIGN.md section 7).  MMAs stay cta_group::1.
+// the W tile and TMA-multicasts it to both, which cuts the L2->SM operand traffic per MMA from (128+BN) to (128+BN/2) rows.
+// A stage is free again once the consumers of BOTH CTAs have read it (the peer multicasts into it too).
 template <int BN, bool kMC>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, int M, int N, int K,
@@ -193,13 +200,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   uint8_t* smem = smem_raw + (base - raw_addr);
   const uint32_t smem_a0 = base;
   const uint32_t smem_b0 = base + STAGES * A_STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * (A_STAGE_BYTES + Cfg::B_STAGE_BYTES));
+  float* epi_stage = reinterpret_cast<float*>(smem + STAGES * (A_STAGE_BYTES + Cfg::B_STAGE_BYTES));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * (A_STAGE_BYTES + Cfg::B_STAGE_BYTES) + EPI_BYTES);
   const uint32_t bar0 = smem_u32(bars);
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int s) { return bar0 + 8u * (2 * STAGES + s); };
-  auto tempty_bar = [&](int s) { return bar0 + 8u * (2 * STAGES + 2 + s); };
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(bars + 2 * STAGES + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -216,28 +221,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), kMC ? 2 : 1);  // kMC: the stage is free once BOTH CTAs' MMAs have consumed it
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), 4);
+      mbar_init(empty_bar(s), (GEMM_CONSUMERS / 128) * (kMC ? 2 : 1));  // one arrival per consumer warpgroup (and CTA)
     }
     fence_mbar_init();
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
   }
-  if (warp == 1) {
-    tmem_alloc<Cfg::TMEM_COLS>(smem_u32(const_cast<uint32_t*>(tmem_slot)));
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  if (kMC) cluster_sync_all();  // peer barriers are initialised before any multicast copy / remote commit can arrive
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (kMC) cluster_sync_all();  // peer barriers are initialised before any multicast copy / remote arrival can reach them
   pdl_wait();  // everything above overlapped the previous kernel's tail; its results are visible from here on
   // rows actually present (device-side count, e.g. the rows of the utterances still decoding): whole M tiles beyond it
-  // are skipped by all three roles alike
+  // are skipped by both roles alike
   int m_tiles = M / BM;
   if (epi.m_dyn != nullptr) {
     const int mt = (*epi.m_dyn + BM - 1) / BM;
@@ -250,9 +244,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   auto unit_m0 = [&](int unit) { return (((unit / k_splits) % m_units) * (kMC ? 2 : 1) + static_cast<int>(crank)) * BM; };
   auto unit_n0 = [&](int unit) { return ((unit / k_splits) / m_units) * BN; };
 
-  if (warp == 0) {
+  if (warp >= GEMM_CONSUMERS / 32) {
     // ------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == GEMM_CONSUMERS / 32 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = first_unit; tile < total_tiles; tile += unit_stride) {
@@ -283,71 +278,90 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(BM, BN, false, false);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = first_unit; tile < total_tiles; tile += unit_stride, ++it) {
-        const int as = it & 1;
-        const uint32_t aphase = (it >> 1) & 1u;
-        mbar_wait(tempty_bar(as), aphase ^ 1u);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(as * BN);
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint64_t da = make_desc_sw128(smem_a0 + stage * A_STAGE_BYTES, 1024);
-          const uint64_t db = make_desc_sw128(smem_b0 + stage * Cfg::B_STAGE_BYTES, 1024);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            // advance 16 fp16 = 32 bytes inside the 128-byte swizzle row: +2 in the (addr >> 4) field
-            umma_f16_ss(tmem_d, da + 2u * k, db + 2u * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          // frees this smem stage once the MMAs above have read it (kMC: in both CTAs, the peer multicasts into it too)
-          if (kMC) umma_commit_mcast(empty_bar(stage), 0x3); else umma_commit(empty_bar(stage));
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        umma_commit(tfull_bar(as));  // accumulator complete -> epilogue
-      }
-    }
   } else {
-    // ------------------------------------------------------------ epilogue (warps 2..5)
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    int it = 0;
-    for (int tile = first_unit; tile < total_tiles; tile += unit_stride, ++it) {
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1u;
+    // ------------------------------------------------------------ consumers: MMA + epilogue
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;                          // rows [64 wg, 64 wg + 64) of the tile
+    const bool signaller = (threadIdx.x & 127) == 0;   // one arrival per warpgroup on the empty barriers
+    auto release = [&](int s) {
+      if (signaller) {
+        if (kMC) {
+          mbar_arrive_cluster(empty_bar(s), 0);
+          mbar_arrive_cluster(empty_bar(s), 1);
+        } else {
+          mbar_arrive(empty_bar(s));
+        }
+      }
+    };
+    float* stg = epi_stage + warp * 16 * EPI_LD;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = first_unit; tile < total_tiles; tile += unit_stride) {
       const int m0 = unit_m0(tile);
       const int n0 = unit_n0(tile);
       const int split = unit_split(tile);
-      mbar_wait(tfull_bar(as), aphase);
-      tc_fence_after();
-      const int row = m0 + q * 32 + lane;
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(as * BN);
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        const int col0 = n0 + c * 32;
-        if (col0 >= epi.n_valid) break;  // warp-uniform
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(taddr + static_cast<uint32_t>(c * 32), v);
-        tmem_ld_wait();
-        if (row < epi.m_valid) epilogue_chunk(epi, row, col0, v, split);
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < k_blocks; ++kb) {
+        mbar_wait(full_bar(stage), phase);
+        const uint64_t da = make_desc_sw128(smem_a0 + stage * A_STAGE_BYTES + wg * (A_STAGE_BYTES / 2), 1024);
+        const uint64_t db = make_desc_sw128(smem_b0 + stage * Cfg::B_STAGE_BYTES, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          // advance 16 fp16 = 32 bytes inside the 128-byte swizzle row: +2 in the (addr >> 4) field
+          wgmma_ss<BN, 0, 0>(acc, da + 2u * k, db + 2u * k, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous stage's MMAs are done: hand its buffers back to the producer
+        if (prev >= 0) release(prev);
+        prev = stage;
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1u;
+        }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(as));
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc);
+      if (prev >= 0) release(prev);
+      // epilogue: pairs of 32-column slices of the warp's 16 rows through shared memory; lane (r + 16 h) then owns
+      // row r's 32 columns of slice 2 p + h, so every lane writes one row chunk per pair
+      const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane & 15);
+      const int hl = lane >> 4;
+      const int r0 = lane >> 2, c0 = (lane & 3) * 2;
+#pragma unroll
+      for (int p = 0; p < (BN / 32 + 1) / 2; ++p) {
+        if (n0 + 64 * p >= epi.n_valid) break;  // warp-uniform
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int c = 2 * p + h;
+          if (c < BN / 32) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const int nb = 4 * c + j;
+              stg[r0 * EPI_LD + h * EPI_HALF + j * 8 + c0] = acc[4 * nb + 0];
+              stg[r0 * EPI_LD + h * EPI_HALF + j * 8 + c0 + 1] = acc[4 * nb + 1];
+              stg[(r0 + 8) * EPI_LD + h * EPI_HALF + j * 8 + c0] = acc[4 * nb + 2];
+              stg[(r0 + 8) * EPI_LD + h * EPI_HALF + j * 8 + c0 + 1] = acc[4 * nb + 3];
+            }
+          }
+        }
+        __syncwarp();
+        const int col0 = n0 + (2 * p + hl) * 32;
+        if (2 * p + hl < BN / 32 && col0 < epi.n_valid && row < epi.m_valid) {
+          float v[32];
+#pragma unroll
+          for (int i = 0; i < 32; ++i) v[i] = stg[(lane & 15) * EPI_LD + hl * EPI_HALF + i];
+          epilogue_chunk(epi, row, col0, v, split);
+        }
+        __syncwarp();
+      }
     }
   }
-  tc_fence_before();
   __syncthreads();
-  if (kMC) cluster_sync_all();  // the peer may still be multicasting into / committing onto this CTA's shared memory
-  if (warp == 1) tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+  if (kMC) cluster_sync_all();  // the peer may still be multicasting into / arriving on this CTA's shared memory
 }
 
 // ------------------------------------------------------------------ SIMT cross-check

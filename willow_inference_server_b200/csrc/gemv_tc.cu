@@ -1,16 +1,15 @@
-// Skinny GEMV on tcgen05 for <= 8 activation rows: out[R, N] = x[R, K] . W[N, K]^T (+ bias), W fp16 streamed once.
+// Skinny GEMV on wgmma for <= 8 activation rows: out[R, N] = x[R, K] . W[N, K]^T (+ bias), W fp16 streamed once.
 //
-// This is the building block of the tensor-core variant of the persistent decoder pass (decoder_mega.cu), kept as a
-// stand-alone kernel behind wisb_debug_gemv_tc so that its arithmetic and its cost can be checked in isolation.
+// A diagnostic kernel behind wisb_debug_gemv_tc, so that the arithmetic and the cost of a tensor-core GEMV at decoder
+// sizes can be checked in isolation (the persistent decoder pass, decoder_mega.cu, uses the warp-level mma.sync instead).
 //
 // Swap-AB: the CTA's weight rows are the MMA's M dimension, the activation rows its N dimension:
-//   A = W tile   [<= 64 weight rows x 64 k]  K-major, 128-byte swizzle, straight from a 2-D TMA box (64 x rows_box)
-//   B = x (fp16) [8 rows x 64 k]             K-major, 128-byte swizzle, written once per phase by the consumer threads
-//   D            [64 lanes x 8 columns]      fp32 in TMEM (M = 64: rows 16 j .. 16 j + 15 on lanes 32 j .. 32 j + 15)
-// tcgen05.mma M = 64, N = 8, K = 16: the reduction over K happens in the tensor core, so the SIMT pass's FMA loop and its
-// transposing shuffle reductions disappear; a CTA owns ceil(N / gridDim.x) weight rows exactly as the SIMT pass does.
-// The MMA always reads 64 rows = 8 swizzle atoms; a CTA that owns fewer rows lets it read whatever follows in shared
-// memory (those output rows are never looked at), so no padding is ever streamed from HBM.
+//   A = W tile   [64 weight rows x 64 k]  K-major, 128-byte swizzle, straight from a 2-D TMA box (64 x rows_box)
+//   B = x (fp16) [8 rows x 64 k]          K-major, 128-byte swizzle, written once by the consumer warpgroup
+//   D            [64 x 8]                 fp32 in the warpgroup's registers
+// wgmma.m64n8k16: the reduction over K happens in the tensor core; a CTA owns ceil(N / gridDim.x) weight rows in groups
+// of 64.  The MMA always reads 64 rows = 8 swizzle atoms; a CTA that owns fewer rows lets it read whatever follows in
+// shared memory (those output rows are never looked at), so no padding is ever streamed from HBM.
 #include "decoder.cuh"
 #include "ptx.cuh"
 
@@ -18,7 +17,7 @@ namespace wisb {
 
 namespace {
 
-constexpr int GT_CONS = 224;               // 7 consumer warps
+constexpr int GT_CONS = 128;               // one consumer warpgroup
 constexpr int GT_THREADS = GT_CONS + 32;   // + producer warp (lane 0 only)
 constexpr int GT_STAGE = 36864;
 constexpr int GT_NSTAGE = 2;
@@ -42,8 +41,6 @@ gemv_tc_kernel(const __grid_constant__ CUtensorMap map_w, const float* __restric
   const uint32_t bar0 = smem_u32(bars);
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (GT_NSTAGE + s); };
-  const uint32_t d_full = bar0 + 8u * (2 * GT_NSTAGE);
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(bars + 2 * GT_NSTAGE + 2);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   if (tid == 0) {
@@ -51,22 +48,13 @@ gemv_tc_kernel(const __grid_constant__ CUtensorMap map_w, const float* __restric
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 1);
     }
-    mbar_init(d_full, 1);
     fence_mbar_init();
     tma_prefetch_desc(&map_w);
   }
   for (int i = tid; i < GT_B_BYTES / 16; i += GT_THREADS) *reinterpret_cast<uint4*>(smem + GT_OFF_B + i * 16) = make_uint4(0u, 0u, 0u, 0u);
-  if (warp == 0) {
-    tmem_alloc<64>(smem_u32(const_cast<uint32_t*>(tmem_slot)));
-    tmem_relinquish();
-  }
-  fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // column slice of this CTA, in groups of 64 weight rows (one accumulator of 8 TMEM columns per group)
+  // row slice of this CTA, in groups of 64 weight rows (one 64 x 8 accumulator per group)
   const int per = (N + gridDim.x - 1) / gridDim.x;
   int lo = blockIdx.x * per, hi = min(N, lo + per);
   if (lo > hi) lo = hi;
@@ -91,7 +79,7 @@ gemv_tc_kernel(const __grid_constant__ CUtensorMap map_w, const float* __restric
       }
     }
   } else if (tid < GT_CONS) {
-    // ------------------------------------------------------------ consumers
+    // ------------------------------------------------------------ consumer warpgroup
     // B operand: x -> fp16, [k-block][8 rows][128 B] with the 16-byte chunks XOR-swizzled by the row (rows >= R stay zero)
     for (int v = tid; v < K / 8; v += GT_CONS) {
       const int kb = v >> 3, c = v & 7;
@@ -111,51 +99,40 @@ gemv_tc_kernel(const __grid_constant__ CUtensorMap map_w, const float* __restric
     }
     fence_proxy_async_smem();
     gt_cons_sync();
-    if (tid == 0) {
-      // one thread issues every MMA of the phase: 4 per k-block (K = 16 each)
-      constexpr uint32_t idesc = make_idesc_f16(64, 8, false, false);
-      unsigned unit = 0;
-      tc_fence_after();
-      for (int g = 0; g < n_groups; ++g) {
-        for (int u = 0; u < units_per_group; ++u, ++unit) {
-          const int kb0 = u * kbu, nkb = min(kbu, kblocks - kb0);
-          const int st = unit % GT_NSTAGE;
-          mbar_wait(full_bar(st), (unit / GT_NSTAGE) & 1u);
-          tc_fence_after();
-          for (int i = 0; i < nkb; ++i) {
-            const uint64_t da = make_desc_sw128(base + st * GT_STAGE + i * rows_box * 128, 1024);
-            const uint64_t db = make_desc_sw128(sB + (kb0 + i) * 1024, 1024);
+    unsigned unit = 0;
+    for (int g = 0; g < n_groups; ++g) {
+      float acc[4] = {0.f, 0.f, 0.f, 0.f};
+      for (int u = 0; u < units_per_group; ++u, ++unit) {
+        const int kb0 = u * kbu, nkb = min(kbu, kblocks - kb0);
+        const int st = unit % GT_NSTAGE;
+        mbar_wait(full_bar(st), (unit / GT_NSTAGE) & 1u);
+        wgmma_fence();
+        for (int i = 0; i < nkb; ++i) {
+          const uint64_t da = make_desc_sw128(base + st * GT_STAGE + i * rows_box * 128, 1024);
+          const uint64_t db = make_desc_sw128(sB + (kb0 + i) * 1024, 1024);
 #pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_f16_ss(tmem_base + static_cast<uint32_t>(g * 8), da + 2u * k, db + 2u * k, idesc, ((kb0 + i) | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(empty_bar(st));
+          for (int k = 0; k < 4; ++k) wgmma_ss<8, 0, 0>(acc, da + 2u * k, db + 2u * k, 1u);
         }
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (tid == 0) mbar_arrive(empty_bar(st));
       }
-      umma_commit(d_full);
-    }
-    __syncwarp();
-    mbar_wait(d_full, 0);
-    tc_fence_after();
-    if (warp < 4) {
-      const uint32_t lane_off = static_cast<uint32_t>(warp * 32) << 16;
-      for (int g = 0; g < n_groups; ++g) {
-        uint32_t v[8];
-        tmem_ld_32x32b_x8(tmem_base + lane_off + static_cast<uint32_t>(g * 8), v);
-        tmem_ld_wait();
-        const int n = lo + g * 64 + warp * 16 + lane;
-        if (lane < 16 && n < hi) {
+      wgmma_reg_fence(acc);
+      // acc[0..1]: weight row 16 warp + lane / 4, x rows 2 (lane % 4) + {0,1}; acc[2..3]: weight row + 8
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int n = lo + g * 64 + warp * 16 + (lane >> 2) + 8 * h;
+        if (n < hi) {
           const float b = bias != nullptr ? __ldg(bias + n) : 0.f;
 #pragma unroll
-          for (int r = 0; r < NR; ++r)
-            if (r < R) out[static_cast<long long>(r) * N + n] = __uint_as_float(v[r]) + b;
+          for (int e = 0; e < 2; ++e) {
+            const int r = 2 * (lane & 3) + e;
+            if (r < R && r < NR) out[static_cast<long long>(r) * N + n] = acc[2 * h + e] + b;
+          }
         }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc<64>(tmem_base);
 }
 
 }  // namespace

@@ -4,8 +4,8 @@
 
 namespace wisb {
 
-// ------------------------------------------------------------------ tcgen05 GEMM  (gemm_tc.cu)
-// D[M,N] = A[M,K] . W[N,K]^T, fp16 operands (both K-major), fp32 accumulation in TMEM, fused epilogues.
+// ------------------------------------------------------------------ wgmma GEMM  (gemm_tc.cu)
+// D[M,N] = A[M,K] . W[N,K]^T, fp16 operands (both K-major), fp32 accumulation in registers, fused epilogues.
 enum EpiMode : int {
   EPI_F16 = 0,        // out16[row, col] = acc + bias
   EPI_F16_GELU = 1,   // out16 = gelu(acc + bias)

@@ -1,6 +1,6 @@
-// Batched log-mel front end for sm_100a.
+// Batched log-mel front end for sm_90a.
 //
-// Replaces /root/reference/wis/audio.py:28-51 (pad_or_trim) and :72-103 (log_mel_spectrogram):
+// Replaces wis/audio.py:28-51 (pad_or_trim) and :72-103 (log_mel_spectrogram):
 //   hann(400) periodic, STFT n_fft=400 hop=160 center/reflect, |.|^2 of the first 3000 frames, 80x201 Slaney mel
 //   filterbank, log10(clamp 1e-10), max(x, utterance_max - 8), (x + 4) / 4.
 // Differences in HOW (not what): zero-padding / trimming to 480000 samples and the optional s16 -> f32 conversion are

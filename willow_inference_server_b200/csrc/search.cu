@@ -2,7 +2,7 @@
 // beam / greedy bookkeeping, all without a host round trip (the host only polls DecState::all_done).
 //
 // Semantics restated from CTranslate2 4.1.0 as listed in SURVEY.md section 8a rows A11-A13 (the reference call is
-// /root/reference/main.py:687-692 with the library defaults patience=1, length_penalty=1, suppress_blank=True,
+// main.py:687-692 with the library defaults patience=1, length_penalty=1, suppress_blank=True,
 // suppress_tokens=[-1], num_hypotheses=1):
 //   * processors: `suppress_ids` -> -inf every step; {blank, eot} -> -inf at the first generated step
 //   * scores: log_softmax(logits) + cumulative beam score, divided by (step+1)^length_penalty
@@ -77,7 +77,7 @@ constexpr int TK_PER = 8;  // 256 * 8 = 2048 >= ceil(51865 / 32) = 1621
 __global__ void __launch_bounds__(TK_THREADS) topk_partial_kernel(const SearchArgs a) {
   // Within one row the ranking by processed logit equals the ranking by score, so the per-chunk stage needs no
   // log-sum-exp: it emits the chunk's top-n_cand logits plus (max, sum exp) partials; the merge stage turns them into
-  // the row's lse and into scores.  (This replaced a separate two-pass lse kernel: 55 us -> 0.)
+  // the row's lse and into scores, with no separate two-pass lse kernel.
   __shared__ unsigned long long s_red[32];
   __shared__ float s_f[32];
   if (a.st->all_done) return;  // a step enqueued ahead of the host's poll

@@ -1,7 +1,7 @@
 """Checkpoint readers: Hugging Face Whisper directories and CTranslate2 model directories -> ``model.wisb``.
 
 SURVEY.md section 8(f) row 3b.  The reference loads CTranslate2 directories ``models/tovera-wis-whisper-<size>/``
-(/root/reference/main.py:341-443; fetched by /root/reference/utils.sh:99-108, 265-269); those hold ``model.bin`` +
+(main.py:341-443; fetched by utils.sh:99-108, 265-269); those hold ``model.bin`` +
 ``config.json`` (suppress_ids, suppress_ids_begin, lang_ids) produced by ``ct2-transformers-converter`` from the HF
 checkpoints.  Neither a checkpoint nor the ``ctranslate2`` package exists in the build image, so:
 

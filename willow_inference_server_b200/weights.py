@@ -1,8 +1,8 @@
 """Flat weight blob shared by the CUDA engine (csrc/weights.cu) and the CPU oracle.
 
 The reference loads CTranslate2 model directories ``models/tovera-wis-whisper-<size>/``
-(/root/reference/main.py:342,364,386,408,430) -- none exist in this image and
-ctranslate2 is absent, so the engine defines its own container: one file, one
+(main.py:342,364,386,408,430); the project vendors neither those directories nor
+ctranslate2, so the engine defines its own container: one file, one
 ``cudaMemcpy`` (or one NCCL broadcast) to place it in HBM.
 
 Layout (little endian):
@@ -11,7 +11,7 @@ Layout (little endian):
     data                       : every tensor 256-byte aligned (TMA needs >= 16 B)
 
 dtypes: 0 = float16, 1 = float32, 2 = int32.  GEMM weights are float16 [N, K]
-row-major (K contiguous = "K-major" for tcgen05 / TMA); biases, LayerNorm
+row-major (K contiguous = "K-major" for wgmma / TMA); biases, LayerNorm
 parameters and positional tables are float32.
 
 Canonical (HF-named) state dict -> engine tensors is done by ``pack_state_dict``;
@@ -196,7 +196,7 @@ def pack_state_dict(sd: dict, dims: WhisperDims) -> dict:
 
 
 # ---------------------------------------------------------------------------
-# seeded synthetic weights (there are no real checkpoints in this image)
+# seeded synthetic weights (the project ships no real checkpoints)
 # ---------------------------------------------------------------------------
 def synth_state_dict(dims: WhisperDims, seed: int = 0, logit_std: float = 4.0, qk_gain: float = 2.5,
                      resid_std: float = 8.0, eot_ramp: tuple | None = None, script: tuple | None = None) -> dict:
