@@ -88,8 +88,22 @@ int wisb_get_timing(wisb_handle* h, float* out16);
 int wisb_set_option(wisb_handle* h, const char* key, int value);
 
 /* ---- diagnostics used by tests/ (run the product kernels on caller data) ---- */
-/* C[M,N] (float32) = A[M,K] . W[N,K]^T with fp16 inputs given as raw uint16; impl 0 = wgmma kernel, 1 = SIMT check */
-int wisb_debug_gemm(wisb_handle* h, const uint16_t* a, const uint16_t* w, float* c, int M, int N, int K, int impl, int bn);
+/* One GEMM A[M,K] . W[N,K]^T (fp16 as raw uint16) through any production epilogue, on caller data.
+ * prm[17] int32: M, N, K, impl (0 = wgmma kernel, 1 = SIMT check into float32 out [M,N]), bn (0 = encoder planner's
+ * choice, 64/128/160/256, negative = that width without 2-CTA multicast), planner (0 = encoder planner, 1 = decoder
+ * planner, 2 = decoder planner with split-K: float32 partial slabs of M*N), mode (EpiMode of csrc/kernels.h), a_wrap
+ * (> 0: A is given as its physical [M+1, a_wrap] rows, the overlapping-row view of conv2), k_splits (> 1: float32 slabs
+ * of M*ldo), m_valid, n_valid (0 = M, N), ldo (0 = N), d_model, n_heads, batch, kv_swizzle, t_cap.
+ * bias [N] and pos [1500, ldo] may be NULL; row_slot / row_pos [M] are the cache slot / position of each row (DEC_QKV).
+ * out / aux / aux2 are uploaded before the launch and downloaded after it, so that untouched elements keep what the
+ * caller put there; every address the epilogue can form is checked against their byte sizes first.
+ * plan_out (may be NULL) receives the launched plan: BN, multicast (0/1), K splits, grid. */
+int wisb_debug_gemm(wisb_handle* h, const int32_t* prm, int n_prm, const uint16_t* a, const uint16_t* w, const float* bias,
+                    const float* pos, const int32_t* row_slot, const int32_t* row_pos, void* out, size_t out_bytes, void* aux,
+                    size_t aux_bytes, void* aux2, size_t aux2_bytes, int32_t* plan_out);
+/* encoder self-attention on caller data: qkv [B*1536, 3d] fp16 -> ctx [B*1536, d] fp16, d = 64 H; impl 0 = wgmma with
+ * MN-major V, 1 = wgmma with the transposed Vt layout (built from the same qkv), 2 = SIMT check */
+int wisb_debug_enc_attn(wisb_handle* h, const uint16_t* qkv16, int B, int d, int H, int impl, uint16_t* ctx16_out);
 /* the wgmma skinny-GEMV building block of the decoder pass on caller data: out[R,N] (float32) = x[R,K] (float32, rounded
  * to fp16 inside) . W[N,K]^T (fp16 as raw uint16) + bias (may be NULL); R <= 8, K % 64 == 0, K <= 5120.  avg_us (may be
  * NULL) receives the average kernel time over `iters` back-to-back launches. */

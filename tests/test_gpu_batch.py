@@ -2,7 +2,9 @@
 csrc/decoder_batch.cu) -- the path main.py:676-693 takes when it feeds several windows per generate call,
 and what BASELINE.json configs[2] / configs[3] (batch 64 / 512) measure.
 
-  * teacher-forced logits of the batched pass vs the fp32 oracle (tolerance LOGIT_TOL)
+  * teacher-forced logits of the batched pass vs the fp32 oracle (tolerance LOGIT_TOL), also with 2..8 positions as
+    rows of one pass, for both cross-attention kernels
+  * 16 utterances greedy with a 2- and a 4-token prompt: both cross-attention kernels equal the oracle on robust cases
   * B = 16, beam 5, mixed durations: every transcript identical to the B = 1 result (persistent SIMT pass) AND to the
     oracle on every robust case (tests/gpu_common.robust_cases)
   * per-utterance length limits in one shared pass == separate calls
@@ -111,6 +113,46 @@ def test_cross_attention_tensor_core_vs_simt(pair):
     assert len(robust) >= 4
     for i in robust:
         assert ids_tc[i] == res[i].sequences_ids[0] == ids_simt[i], i
+
+
+@pytest.mark.parametrize("cross_tc", [1, 0])
+def test_multi_row_teacher_forcing_matches_oracle(pair, cross_tc):
+    # 1..8 consecutive positions as rows of one pass (the way a prompt prefix is prefilled): every position's logits,
+    # with the wgmma and with the SIMT cross-attention
+    dims, oracle, h = pair
+    mel = mel_inputs(4)[:1]
+    toks = PROMPT + [100, 2000, 30000, 41000, 12, 50000, 7, 999]
+    want = oracle.forced_logits(oracle.encode(mel)[0], toks).numpy()
+    h.set_option("decoder_batch", 2)
+    h.set_option("cross_tc", cross_tc)
+    try:
+        for chunk in (1, 2, 3, 5, 8):
+            h.set_option("debug_chunk", chunk)
+            err = np.abs(h.debug_forced_logits(mel, toks) - want).max(axis=1)
+            assert err.shape == (len(toks),)
+            assert np.all(err <= LOGIT_TOL), (chunk, err)
+    finally:
+        h.set_option("debug_chunk", 1)
+        h.set_option("cross_tc", 1)
+        h.set_option("decoder_batch", 1)
+
+
+@pytest.mark.parametrize("prompt", [[50258, 50363], PROMPT])
+def test_greedy16_both_cross_attention_kernels_match_oracle(pair, prompt):
+    # 16 utterances, greedy: with a 2-token prompt the prefix pass has one row per utterance too
+    dims, oracle, h = pair
+    mel = mel_inputs(16)
+    prompts = [prompt] * 16
+    res, robust = robust_cases(oracle, mel, prompts, 1, n_probe=2, max_length=24)
+    assert len(robust) >= 10, f"only {len(robust)} of 16 oracle transcripts are robust decisions"
+    for tc in (1, 0):
+        h.set_option("cross_tc", tc)
+        try:
+            ids, _ = h.generate(mel, np.asarray(prompts, np.int32), beam_size=1, max_length=24)
+        finally:
+            h.set_option("cross_tc", 1)
+        for i in robust:
+            assert ids[i] == res[i].sequences_ids[0], (tc, i)
 
 
 def test_row_capacity_groups(pair):

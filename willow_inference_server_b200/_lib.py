@@ -17,6 +17,8 @@ DIM_NAMES = [
     "blank", "lang_first", "n_langs",
 ]
 PCM_F32, PCM_S16 = 0, 1
+# GEMM epilogues (EpiMode in csrc/kernels.h)
+EPI_F16, EPI_F16_GELU, EPI_RESID_F32, EPI_CONV2, EPI_CROSSKV, EPI_F32, EPI_QKV_VT, EPI_DEC_QKV = range(8)
 
 _lib = None
 
@@ -37,7 +39,10 @@ _SIGS = {
     "wisb_detect_language": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_get_timing": (C.c_int, [C.c_void_p, C.c_void_p]),
     "wisb_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
-    "wisb_debug_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "wisb_debug_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
+                                  C.c_void_p]),
+    "wisb_debug_enc_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "wisb_debug_gemv_tc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                       C.c_void_p]),
     "wisb_debug_read_trace": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
@@ -199,14 +204,58 @@ class Handle:
         return ids, probs
 
     # ------------------------------------------------------------------ diagnostics (tests)
-    def debug_gemm(self, a16: np.ndarray, w16: np.ndarray, impl: int = 0, bn: int = 0) -> np.ndarray:
+    def debug_gemm(self, a16: np.ndarray, w16: np.ndarray, impl: int = 0, bn: int = 0, *, mode: int = EPI_F32,
+                   planner: int = 0, bias=None, pos=None, out=None, aux=None, aux2=None, row_slot=None, row_pos=None,
+                   a_wrap: int = 0, k_splits: int = 1, m_valid: int = 0, n_valid: int = 0, ldo: int = 0, d_model: int = 0,
+                   n_heads: int = 0, batch: int = 0, kv_swizzle: int = 0, t_cap: int = 0, return_plan: bool = False):
+        """One GEMM A . W^T through epilogue `mode` (EPI_*) -> `out` (or (out, plan) with return_plan).  out / aux / aux2
+        are C-contiguous arrays updated in place: elements the epilogue does not write keep their values.  Without `out`
+        (plain EPI_F32) a zero float32 [M, N] array is returned.  With a_wrap, a16 holds the physical [M + 1, a_wrap] rows.
+        plan = {"bn", "mcast", "k_splits", "grid"} as launched."""
         a16 = np.ascontiguousarray(a16, np.float16)
         w16 = np.ascontiguousarray(w16, np.float16)
-        M, K = a16.shape
-        N = w16.shape[0]
-        c = np.zeros((M, N), np.float32)
-        check(lib().wisb_debug_gemm(self._h, ptr(a16), ptr(w16), ptr(c), M, N, K, impl, bn))
-        return c
+        N, K = w16.shape
+        M = a16.shape[0] - (1 if a_wrap else 0)
+        if a16.shape[1] != (a_wrap if a_wrap else K):
+            raise ValueError("A and W disagree on K")
+        if out is None:
+            if mode != EPI_F32 or k_splits != 1 or planner == 2:
+                raise ValueError("this epilogue needs an explicit out buffer")
+            out = np.zeros((M, N), np.float32)
+        for buf in (out, aux, aux2):
+            if buf is not None and not buf.flags["C_CONTIGUOUS"]:
+                raise ValueError("out / aux / aux2 must be C-contiguous")
+        bias = None if bias is None else np.ascontiguousarray(bias, np.float32)
+        pos = None if pos is None else np.ascontiguousarray(pos, np.float32)
+        if bias is not None and bias.size != N:
+            raise ValueError("bias must have N elements")
+        if pos is not None and pos.size != 1500 * (ldo or N):
+            raise ValueError("pos must be [1500, ldo]")
+        slot = None if row_slot is None else np.ascontiguousarray(row_slot, np.int32)
+        rpos = None if row_pos is None else np.ascontiguousarray(row_pos, np.int32)
+        if (slot is not None and slot.size != M) or (rpos is not None and rpos.size != M):
+            raise ValueError("row_slot / row_pos must have M entries")
+        prm = np.asarray([M, N, K, impl, bn, planner, mode, a_wrap, k_splits, m_valid, n_valid, ldo, d_model, n_heads, batch,
+                          kv_swizzle, t_cap], np.int32)
+        plan = np.zeros(4, np.int32)
+        nbytes = lambda b: 0 if b is None else b.nbytes  # noqa: E731
+        check(lib().wisb_debug_gemm(self._h, ptr(prm), prm.size, ptr(a16), ptr(w16), ptr(bias), ptr(pos), ptr(slot), ptr(rpos),
+                                    ptr(out), out.nbytes, ptr(aux), nbytes(aux), ptr(aux2), nbytes(aux2), ptr(plan)))
+        if return_plan:
+            return out, dict(zip(("bn", "mcast", "k_splits", "grid"), (int(v) for v in plan)))
+        return out
+
+    def debug_enc_attn(self, qkv16: np.ndarray, n_heads: int, impl: int = 0) -> np.ndarray:
+        """Encoder self-attention on qkv fp16 [B, 1536, 3d] -> ctx fp16 [B, 1536, d]; impl 0 = wgmma (MN-major V),
+        1 = wgmma (transposed Vt), 2 = SIMT check."""
+        qkv16 = np.ascontiguousarray(qkv16, np.float16)
+        B, T, three_d = qkv16.shape
+        if T != 1536 or three_d % 3:
+            raise ValueError("qkv must be [B, 1536, 3 d_model]")
+        d = three_d // 3
+        ctx = np.zeros((B, 1536, d), np.float16)
+        check(lib().wisb_debug_enc_attn(self._h, ptr(qkv16), B, d, n_heads, impl, ptr(ctx)))
+        return ctx
 
     def debug_gemv_tc(self, x: np.ndarray, w16: np.ndarray, bias=None, iters: int = 0):
         """wgmma skinny GEMV on caller data -> (out float32 [R, N], average kernel time in us over `iters` launches)."""

@@ -1676,29 +1676,151 @@ int wisb_detect_language(wisb_handle* h, const float* mel, int B, int32_t* lang_
 }
 
 // --------------------------------------------------------------------------------------------------------------------- diagnostics
-int wisb_debug_gemm(wisb_handle* h, const uint16_t* a, const uint16_t* w, float* c, int M, int N, int K, int impl, int bn) {
+int wisb_debug_gemm(wisb_handle* h, const int32_t* prm, int n_prm, const uint16_t* a, const uint16_t* w, const float* bias,
+                    const float* pos, const int32_t* row_slot, const int32_t* row_pos, void* out, size_t out_bytes, void* aux,
+                    size_t aux_bytes, void* aux2, size_t aux2_bytes, int32_t* plan_out) {
   return guarded(h, [&] {
-    WISB_REQUIRE(a && w && c, "NULL pointer");
+    WISB_REQUIRE(prm != nullptr && n_prm == 17 && a && w && out, "debug_gemm: bad arguments");
+    const int M = prm[0], N = prm[1], K = prm[2], impl = prm[3], bn = prm[4], planner = prm[5], a_wrap = prm[7],
+              k_splits = prm[8];
+    GemmEpi e;
+    e.mode = prm[6];
+    e.m_valid = prm[9] > 0 ? prm[9] : M;
+    e.n_valid = prm[10] > 0 ? prm[10] : N;
+    e.ldo = prm[11] > 0 ? prm[11] : N;
+    e.d_model = prm[12];
+    e.n_heads = prm[13];
+    e.batch = prm[14];
+    e.kv_swizzle = prm[15];
+    e.t_cap = prm[16];
+    WISB_REQUIRE(M > 0 && N > 0 && K > 0 && a_wrap >= 0 && k_splits >= 1 && impl >= 0 && impl <= 1 && planner >= 0 && planner <= 2,
+                 "debug_gemm: bad scalar parameters");
+    WISB_REQUIRE(e.mode >= EPI_F16 && e.mode <= EPI_DEC_QKV, "debug_gemm: unknown epilogue");
+    WISB_REQUIRE(e.m_valid <= M && e.n_valid <= N && e.n_valid % 32 == 0 && e.ldo >= e.n_valid, "debug_gemm: bad m_valid / n_valid / ldo");
+    WISB_REQUIRE(planner == 0 || (a_wrap == 0 && k_splits == 1 && bn == 0), "debug_gemm: the decoder planner picks BN and the split itself");
+    WISB_REQUIRE(impl == 0 || (e.mode == EPI_F32 && planner == 0 && a_wrap == 0 && k_splits == 1), "debug_gemm: the SIMT check computes plain F32 only");
     cudaStream_t s = h->stream;
+    const long long lda = a_wrap > 0 ? a_wrap : K;
+    const size_t a_elems = static_cast<size_t>(a_wrap > 0 ? M + 1 : M) * lda;
     DevBuf<__half> da, dw;
-    DevBuf<float> dc;
-    da.ensure(static_cast<size_t>(M) * K);
+    DevBuf<float> dbias, dpos;
+    DevBuf<int> dslot, dpos_row;
+    DevBuf<uint8_t> dout, daux, daux2;
+    da.ensure(a_elems);
     dw.ensure(static_cast<size_t>(N) * K);
-    dc.ensure(static_cast<size_t>(M) * N, true);
-    WISB_CUDA(cudaMemcpyAsync(da.p, a, sizeof(__half) * M * K, cudaMemcpyHostToDevice, s));
+    WISB_CUDA(cudaMemcpyAsync(da.p, a, sizeof(__half) * a_elems, cudaMemcpyHostToDevice, s));
     WISB_CUDA(cudaMemcpyAsync(dw.p, w, sizeof(__half) * N * K, cudaMemcpyHostToDevice, s));
+    if (bias) {
+      dbias.ensure(N);
+      WISB_CUDA(cudaMemcpyAsync(dbias.p, bias, sizeof(float) * N, cudaMemcpyHostToDevice, s));
+      e.bias = dbias.p;
+    }
+    auto upload = [&](DevBuf<uint8_t>& d, const void* src, size_t bytes) -> void* {
+      if (src == nullptr || bytes == 0) return nullptr;
+      d.ensure(bytes);
+      WISB_CUDA(cudaMemcpyAsync(d.p, src, bytes, cudaMemcpyHostToDevice, s));
+      return d.p;
+    };
+    e.out = upload(dout, out, out_bytes);
+    e.aux = upload(daux, aux, aux_bytes);
+    e.aux2 = upload(daux2, aux2, aux2_bytes);
+
+    GemmPlan p;
     if (impl == 1) {
-      gemm_ref_run(da.p, K, dw.p, dc.p, M, N, K, s);
+      WISB_REQUIRE(out_bytes >= sizeof(float) * M * N, "debug_gemm: out is too small");
+      gemm_ref_run(da.p, K, dw.p, static_cast<float*>(e.out), M, N, K, s);
     } else {
-      GemmPlan p;
-      GemmEpi e;
-      e.mode = EPI_F32;
-      e.out = dc.p;
-      e.ldo = N;
-      gemm_plan(p, da.p, K, dw.p, M, N, K, e, h->num_sms, bn);
+      // every address the epilogue can form is checked against the caller's buffers before the launch
+      const size_t mv = static_cast<size_t>(e.m_valid), d = static_cast<size_t>(e.d_model), H = static_cast<size_t>(e.n_heads);
+      const bool win = e.mode == EPI_CONV2 || e.mode == EPI_CROSSKV || e.mode == EPI_QKV_VT;
+      if (e.mode == EPI_CROSSKV || e.mode == EPI_QKV_VT || e.mode == EPI_DEC_QKV)
+        WISB_REQUIRE(d > 0 && d % 64 == 0 && (e.mode == EPI_DEC_QKV || H * HEAD_DIM == d), "debug_gemm: d_model / n_heads");
+      if (win && e.mode != EPI_CONV2) WISB_REQUIRE(e.batch >= 1 && static_cast<long long>(e.batch) * T_ENC_PAD >= M, "debug_gemm: batch");
+      size_t es = 2, need_out = 0, need_aux = 0, need_aux2 = 0;
+      switch (e.mode) {
+        case EPI_RESID_F32: case EPI_CONV2: case EPI_F32: case EPI_DEC_QKV: es = 4; break;
+        default: break;
+      }
+      need_out = mv * e.ldo * es;
+      if (e.mode == EPI_CONV2) {
+        WISB_REQUIRE(pos != nullptr, "debug_gemm: CONV2 needs pos");
+        dpos.ensure(static_cast<size_t>(T_ENC) * e.ldo);
+        WISB_CUDA(cudaMemcpyAsync(dpos.p, pos, sizeof(float) * T_ENC * e.ldo, cudaMemcpyHostToDevice, s));
+        e.pos = dpos.p;
+      } else if (e.mode == EPI_CROSSKV) {
+        WISB_REQUIRE(N % (2 * d) == 0, "debug_gemm: CROSSKV needs N = layers x 2 d_model");
+        need_out = static_cast<size_t>(N) * e.batch * T_ENC_PAD * es;
+      } else if (e.mode == EPI_QKV_VT) {
+        WISB_REQUIRE(N == static_cast<int>(3 * d), "debug_gemm: QKV_VT needs N = 3 d_model");
+        need_aux = static_cast<size_t>(e.batch) * d * T_ENC_PAD * 2;
+      } else if (e.mode == EPI_DEC_QKV) {
+        WISB_REQUIRE(N == static_cast<int>(3 * d) && row_slot && row_pos && e.t_cap > 0, "debug_gemm: DEC_QKV needs N = 3 d_model and rows");
+        size_t top = 0;
+        for (size_t r = 0; r < mv; ++r) {
+          WISB_REQUIRE(row_slot[r] >= 0 && row_pos[r] >= 0 && row_pos[r] < e.t_cap, "debug_gemm: row slot / position out of range");
+          const size_t end = (static_cast<size_t>(row_slot[r]) * e.t_cap + row_pos[r] + 1) * d * 2;
+          if (end > top) top = end;
+        }
+        need_aux = need_aux2 = top;
+        dslot.ensure(M);
+        dpos_row.ensure(M);
+        WISB_CUDA(cudaMemcpyAsync(dslot.p, row_slot, sizeof(int) * M, cudaMemcpyHostToDevice, s));
+        WISB_CUDA(cudaMemcpyAsync(dpos_row.p, row_pos, sizeof(int) * M, cudaMemcpyHostToDevice, s));
+        e.row_slot = dslot.p;
+        e.row_pos = dpos_row.p;
+      }
+      if (planner == 0) {
+        if (e.mode == EPI_F32) e.split_stride = static_cast<long long>(M) * e.ldo;
+        gemm_plan(p, da.p, lda, dw.p, M, N, K, e, h->num_sms, bn, a_wrap, k_splits);
+      } else {
+        plan_dec_gemm(h, p, da.p, lda, dw.p, M, N, K, e, planner == 2);
+      }
+      if (p.epi.mode == EPI_F32) need_out = ((p.k_splits - 1) * static_cast<size_t>(p.epi.split_stride) + mv * e.ldo) * 4;
+      WISB_REQUIRE(out_bytes >= need_out && aux_bytes >= need_aux && aux2_bytes >= need_aux2 &&
+                       (need_aux == 0 || e.aux != nullptr) && (need_aux2 == 0 || e.aux2 != nullptr),
+                   "debug_gemm: an output buffer is too small for the epilogue");
       gemm_run(p, s);
     }
-    WISB_CUDA(cudaMemcpyAsync(c, dc.p, sizeof(float) * M * N, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(out, e.out, out_bytes, cudaMemcpyDeviceToHost, s));
+    if (e.aux) WISB_CUDA(cudaMemcpyAsync(aux, e.aux, aux_bytes, cudaMemcpyDeviceToHost, s));
+    if (e.aux2) WISB_CUDA(cudaMemcpyAsync(aux2, e.aux2, aux2_bytes, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+    if (plan_out) {
+      plan_out[0] = impl == 1 ? 0 : p.BN;
+      plan_out[1] = impl == 1 ? 0 : p.mcast;
+      plan_out[2] = impl == 1 ? 1 : p.k_splits;
+      plan_out[3] = impl == 1 ? 0 : p.grid;
+    }
+  });
+}
+
+int wisb_debug_enc_attn(wisb_handle* h, const uint16_t* qkv16, int B, int d, int H, int impl, uint16_t* ctx16_out) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(qkv16 && ctx16_out && B >= 1 && H >= 1 && d == H * HEAD_DIM && impl >= 0 && impl <= 2, "debug_enc_attn: bad arguments");
+    cudaStream_t s = h->stream;
+    const size_t rows = static_cast<size_t>(B) * T_ENC_PAD;
+    DevBuf<__half> dq, dvt, dctx;
+    dq.ensure(rows * 3 * d);
+    dctx.ensure(rows * d, true);
+    WISB_CUDA(cudaMemcpyAsync(dq.p, qkv16, sizeof(__half) * rows * 3 * d, cudaMemcpyHostToDevice, s));
+    if (impl == 2) {
+      enc_attn_ref_run(dq.p, dctx.p, B, d, H, s);
+    } else {
+      if (impl == 1) {  // the layout EPI_QKV_VT writes: vt[((b H + head) 64 + e) 1536 + t] = V[b 1536 + t][head 64 + e]
+        std::vector<uint16_t> vt(rows * d);
+        for (size_t r = 0; r < rows; ++r) {
+          const size_t b = r / T_ENC_PAD, t = r % T_ENC_PAD;
+          for (int c = 0; c < d; ++c) vt[((b * H + c / HEAD_DIM) * HEAD_DIM + c % HEAD_DIM) * T_ENC_PAD + t] = qkv16[r * 3 * d + 2 * d + c];
+        }
+        dvt.ensure(rows * d);
+        WISB_CUDA(cudaMemcpyAsync(dvt.p, vt.data(), sizeof(__half) * rows * d, cudaMemcpyHostToDevice, s));
+        WISB_CUDA(cudaStreamSynchronize(s));  // (vt is a host temporary)
+      }
+      AttnPlan ap;
+      enc_attn_plan(ap, dq.p, dvt.p, dctx.p, B, d, H, impl == 0);
+      enc_attn_run(ap, s);
+    }
+    WISB_CUDA(cudaMemcpyAsync(ctx16_out, dctx.p, sizeof(__half) * rows * d, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaStreamSynchronize(s));
   });
 }
