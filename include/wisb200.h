@@ -53,7 +53,8 @@ int wisb_logmel(wisb_handle* h, const void* pcm, int pcm_dtype, int pcm_on_devic
                 const int32_t* n_samples, int B, float* mel_out, int keep_on_device);
 
 /* (3)+(4) features [B,80,3000] float32 host (or NULL: use the features kept by wisb_logmel) -> token ids.
- * prompts: int32 [B, prompt_len] (WIS passes the same 4-token prompt for every window, main.py:689).
+ * prompts: int32 [B, prompt_len] (WIS passes the same 4-token prompt for every window, main.py:689).  This entry always
+ * decodes without timestamp rules; wisb_generate_ts switches them on.
  * beam_size 1 = greedy.  patience / length_penalty / max_length: CTranslate2 defaults 1, 1, 448.
  * extra_suppress: ids suppressed in addition to the model's suppress_ids (CT2 `suppress_tokens=[-1, ...]`), may be NULL.
  * out_ids: int32 [B, out_stride] (out_stride >= min(max_length/2, max_length-prompt_len)); out_len: int32 [B];
@@ -70,6 +71,17 @@ int wisb_generate_ex(wisb_handle* h, const float* mel, int B, const int32_t* pro
                      float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
                      const int32_t* extra_suppress, int n_extra, int32_t* out_ids, int out_stride, int32_t* out_len,
                      float* out_score);
+
+/* Same call with Whisper's timestamp rules switched on (timestamps = 1) or off (0: exactly wisb_generate_ex).
+ * Timestamp mode is what CTranslate2 does for a prompt WITHOUT <|notimestamps|> (the 3-token sot, language, task
+ * prompt): the returned ids then contain timestamp tokens (ids > no_timestamps), which come in pairs except directly
+ * before <|endoftext|> and never decrease; the first generated token is a timestamp <= no_timestamps + 1 +
+ * max_initial_timestamp_index (CTranslate2 default 50, i.e. 1.00 s).  In timestamp mode the prompt must contain neither
+ * <|notimestamps|> nor timestamp tokens.  max_initial_timestamp_index >= 0 in both modes. */
+int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
+                     float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
+                     const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
+                     int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score);
 
 /* (5) per utterance: language token ids sorted by probability (descending) and the probabilities.
  * lang_ids_out int32 [B, n_langs], probs_out float32 [B, n_langs]. */
@@ -101,6 +113,16 @@ int wisb_set_option(wisb_handle* h, const char* key, int value);
 int wisb_debug_gemm(wisb_handle* h, const int32_t* prm, int n_prm, const uint16_t* a, const uint16_t* w, const float* bias,
                     const float* pos, const int32_t* row_slot, const int32_t* row_pos, void* out, size_t out_bytes, void* aux,
                     size_t aux_bytes, void* aux2, size_t aux2_bytes, int32_t* plan_out);
+/* ONE production token-search step (wisb_generate's processors, top-k and beam bookkeeping) on caller data.
+ * prm[8] int32: n_utt, beam, gen (index of the token being generated), V, eot, no_timestamps, timestamps (0/1),
+ * max_initial_timestamp_index.  logits float32 [n_utt*beam, V]; hist int32 [n_utt*beam, gen] each row's generated
+ * tokens (may be NULL at gen 0); mask uint8 [V] (bit 0: suppressed every step, bit 1: suppressed at gen 0); cum float32
+ * [n_utt*beam] cumulative beam scores (NULL = 0); done int32 [n_utt] finished utterances (NULL = none).  Length penalty 1.
+ * Outputs: cand_idx int32 [n_utt, 16] (beam * V + token, -1 = none) and cand_score float32 [n_utt, 16], the first
+ * 2*beam entries used; row_lse float32 [n_utt*beam], the log-softmax normaliser of each fully processed row. */
+int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, const float* logits, const int32_t* hist,
+                           const uint8_t* mask, const float* cum, const int32_t* done, int32_t* cand_idx, float* cand_score,
+                           float* row_lse);
 /* encoder self-attention on caller data: qkv [B*1536, 3d] fp16 -> ctx [B*1536, d] fp16, d = 64 H; impl 0 = wgmma with
  * MN-major V, 1 = wgmma with the transposed Vt layout (built from the same qkv), 2 = SIMT check */
 int wisb_debug_enc_attn(wisb_handle* h, const uint16_t* qkv16, int B, int d, int H, int impl, uint16_t* ctx16_out);

@@ -36,12 +36,17 @@ _SIGS = {
                                 C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_generate_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
                                    C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "wisb_generate_ts": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
+                                   C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                   C.c_void_p, C.c_void_p]),
     "wisb_detect_language": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_get_timing": (C.c_int, [C.c_void_p, C.c_void_p]),
     "wisb_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
     "wisb_debug_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
                                   C.c_void_p]),
+    "wisb_debug_search_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_enc_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "wisb_debug_gemv_tc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                       C.c_void_p]),
@@ -168,7 +173,9 @@ class Handle:
         return out
 
     def generate(self, mel, prompts, beam_size=5, patience=1.0, length_penalty=1.0, max_length=448, extra_suppress=(),
-                 B=None):
+                 B=None, timestamps=False, max_initial_timestamp_index=50):
+        """-> (token ids per utterance, length-normalised scores).  timestamps=True applies Whisper's timestamp rules
+        (wisb_generate_ts); the prompt must then contain neither <|notimestamps|> nor timestamp tokens."""
         prompts = np.ascontiguousarray(prompts, np.int32)
         if prompts.ndim != 2:
             raise ValueError("prompts must be [B, prompt_len]")
@@ -189,9 +196,16 @@ class Handle:
         lens = np.zeros(B, np.int32)
         scores = np.zeros(B, np.float32)
         extra = np.ascontiguousarray(list(extra_suppress), np.int32)
-        check(lib().wisb_generate_ex(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], int(beam_size), float(patience),
-                                     float(length_penalty), int(max_length), ptr(per_utt), ptr(extra) if extra.size else None,
-                                     extra.size, ptr(ids), stride, ptr(lens), ptr(scores)))
+        if timestamps or max_initial_timestamp_index != 50:
+            check(lib().wisb_generate_ts(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], int(beam_size),
+                                         float(patience), float(length_penalty), int(max_length), ptr(per_utt),
+                                         ptr(extra) if extra.size else None, extra.size, 1 if timestamps else 0,
+                                         int(max_initial_timestamp_index), ptr(ids), stride, ptr(lens), ptr(scores)))
+        else:
+            check(lib().wisb_generate_ex(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], int(beam_size),
+                                         float(patience), float(length_penalty), int(max_length), ptr(per_utt),
+                                         ptr(extra) if extra.size else None, extra.size, ptr(ids), stride, ptr(lens),
+                                         ptr(scores)))
         return [ids[b, : lens[b]].tolist() for b in range(B)], scores.tolist()
 
     def detect_language(self, mel, B=None):
@@ -244,6 +258,31 @@ class Handle:
         if return_plan:
             return out, dict(zip(("bn", "mcast", "k_splits", "grid"), (int(v) for v in plan)))
         return out
+
+    def debug_search_step(self, logits, hist, mask, *, beam: int, gen: int, eot: int, no_timestamps: int,
+                          timestamps: bool, max_initial_timestamp_index: int = 50, cum=None, done=None):
+        """One production search step on caller data.  logits float32 [n_utt*beam, V]; hist int [n_utt*beam, gen];
+        mask uint8 [V] (bit 0 every step, bit 1 at gen 0).  -> (cand_idx int32 [n_utt, 2*beam] = beam*V + token,
+        cand_score float32 [n_utt, 2*beam], row_lse float32 [n_utt*beam])."""
+        logits = np.ascontiguousarray(logits, np.float32)
+        R, V = logits.shape
+        if R % beam:
+            raise ValueError("logits rows must be n_utt * beam")
+        n_utt = R // beam
+        hist = np.ascontiguousarray(np.asarray(hist, np.int32).reshape(R, gen))
+        mask = np.ascontiguousarray(mask, np.uint8)
+        if mask.shape != (V,):
+            raise ValueError("mask must have V entries")
+        cum = None if cum is None else np.ascontiguousarray(cum, np.float32).reshape(R)
+        done = None if done is None else np.ascontiguousarray(done, np.int32).reshape(n_utt)
+        prm = np.asarray([n_utt, beam, gen, V, eot, no_timestamps, 1 if timestamps else 0, max_initial_timestamp_index],
+                         np.int32)
+        ci = np.zeros((n_utt, 16), np.int32)
+        cs = np.zeros((n_utt, 16), np.float32)
+        lse = np.zeros(R, np.float32)
+        check(lib().wisb_debug_search_step(self._h, ptr(prm), prm.size, ptr(logits), ptr(hist) if gen else None, ptr(mask),
+                                           ptr(cum), ptr(done), ptr(ci), ptr(cs), ptr(lse)))
+        return ci[:, : 2 * beam], cs[:, : 2 * beam], lse
 
     def debug_enc_attn(self, qkv16: np.ndarray, n_heads: int, impl: int = 0) -> np.ndarray:
         """Encoder self-attention on qkv fp16 [B, 1536, 3d] -> ctx fp16 [B, 1536, d]; impl 0 = wgmma (MN-major V),

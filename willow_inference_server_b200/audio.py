@@ -164,7 +164,11 @@ def transcribe_long(model, audio, prompt, tokenizer, *, beam_size: int = 5, batc
     utterance, decode all windows as batch rows (the reference goes two at a time, ``concurrent_gpu_chunks``), stitch
     the token lists with ``find_longest_common_sequence``.  ``model`` is a ``models.Whisper`` (or anything with its
     ``generate``); with ``batcher`` (a ``TranscribeBatcher``) the windows join other requests' batches.
-    Returns the merged token ids (numpy int array), ready for ``whisper_processor.decode``."""
+    Returns the merged token ids (numpy int array), ready for ``whisper_processor.decode``.
+
+    A timestamp prompt (one without <|notimestamps|>) works for audio of one window only: the overlap merge matches
+    plain text tokens and is not defined on timestamps, which restart at 0.00 in every window, so longer audio with a
+    timestamp prompt raises ``ValueError``."""
     from .models import StorageView
 
     pcm = np.asarray(audio)
@@ -176,6 +180,11 @@ def transcribe_long(model, audio, prompt, tokenizer, *, beam_size: int = 5, batc
         mel, strides = log_mel_chunks(audio)
     if not strides:
         return np.zeros(0, np.int64)
+    if mel.shape[0] > 1:
+        no_ts = _no_timestamps_id(model, tokenizer)
+        if no_ts is not None and no_ts not in list(prompt):
+            raise ValueError("timestamp decoding of audio longer than one 30-s window is not supported: the window merge "
+                             "is not defined on timestamp tokens (keep <|notimestamps|> in the prompt)")
     seqs = []
     for s in range(0, mel.shape[0], max_windows_per_call):
         part = mel[s : s + max_windows_per_call]
@@ -189,6 +198,14 @@ def transcribe_long(model, audio, prompt, tokenizer, *, beam_size: int = 5, batc
         special = set(tokenizer.all_special_ids)
         return np.array([t for t in seqs[0] if t not in special])
     return find_longest_common_sequence([(ids, st) for ids, st in zip(seqs, strides)], tokenizer)
+
+
+def _no_timestamps_id(model, tokenizer):
+    dims = getattr(model, "dims", None)
+    if isinstance(dims, dict) and "no_timestamps" in dims:
+        return int(dims["no_timestamps"])
+    convert = getattr(tokenizer, "convert_tokens_to_ids", None)
+    return int(convert("<|notimestamps|>")) if convert is not None else None
 
 
 def find_longest_common_sequence(sequences, tokenizer):

@@ -68,12 +68,15 @@ struct SearchArgs {
   int n_utt = 0, beam = 0, n_cand = 0;
   int max_new = 0, max_hyp = 0, eot = 0, t_max = 0, prompt_len = 0;
   float length_penalty = 1.f;
-  // workspaces / state (device)
+  // timestamp mode (the prompt has no <|notimestamps|>): ids in [ts_begin, n_vocab) are timestamps,
+  // ts_begin = no_ts + 1; ts_max_init = ts_begin + max_initial_timestamp_index, the last one allowed at the first step
+  int ts = 0, ts_begin = 0, no_ts = 0, ts_max_init = 0;
+  // workspaces / state (device); NCH = TOPK_CHUNKS chunks per row, TOPK_CHUNKS + 1 in timestamp mode
   float* row_lse = nullptr;       // [R]
-  float* part_max = nullptr;      // [R][TOPK_CHUNKS] chunk max of the processed logits
-  float* part_sum = nullptr;      // [R][TOPK_CHUNKS] chunk sum exp(logit - chunk max)
+  float* part_max = nullptr;      // [R][NCH] chunk max of the processed logits
+  float* part_sum = nullptr;      // [R][NCH] chunk sum exp(logit - chunk max)
   float* cum = nullptr;           // [R] cumulative log-prob of the alive beams
-  unsigned long long* part = nullptr;  // [R][TOPK_CHUNKS][MAX_CAND] packed (score, ~index)
+  unsigned long long* part = nullptr;  // [R][NCH][MAX_CAND] packed (score, ~index)
   float* cand_score = nullptr;    // [n_utt][MAX_CAND]
   int* cand_idx = nullptr;        // [n_utt][MAX_CAND]   beam * V + token
   int* tokens = nullptr;          // [R] token fed next step

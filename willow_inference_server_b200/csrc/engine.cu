@@ -79,6 +79,7 @@ struct DecLayerW {
 
 struct GraphKey {
   int n_utt, beam, prompt_len, max_new, max_hyp, u0, b_total, batched;
+  int ts, ts_max_init;  // timestamp mode: the step graph bakes SearchArgs in, so a mode never reuses another's graph
   float lp;
   bool operator<(const GraphKey& o) const {
     return memcmp(this, &o, sizeof(GraphKey)) < 0;
@@ -329,8 +330,9 @@ void ensure_search(wisb_handle* h, int rows) {
   drop_graphs(h);  // captured graphs hold the old pointers
   const size_t R = static_cast<size_t>(rows);
   h->row_lse.ensure(R); h->cum.ensure(R);
-  h->part_max.ensure(R * TOPK_CHUNKS); h->part_sum.ensure(R * TOPK_CHUNKS);
-  h->part.ensure(R * TOPK_CHUNKS * MAX_CAND);
+  // (TOPK_CHUNKS + 1 chunks per row: timestamp mode adds one for the timestamp ids)
+  h->part_max.ensure(R * (TOPK_CHUNKS + 1)); h->part_sum.ensure(R * (TOPK_CHUNKS + 1));
+  h->part.ensure(R * (TOPK_CHUNKS + 1) * MAX_CAND);
   h->cand_score.ensure(R * MAX_CAND); h->cand_idx.ensure(R * MAX_CAND);
   h->tokens.ensure(R);
   h->seq0.ensure(R * T_MAX, true); h->seq1.ensure(R * T_MAX, true);
@@ -658,6 +660,8 @@ struct DecodeCfg {
   int u0, n_utt, B_total, beam, prompt_len, max_new, max_hyp;
   float lp;
   int per_utt_max_new = 0;  // h->max_new_u holds a per-utterance cap (<= max_new)
+  int ts = 0;               // timestamp rules on (the prompt has no <|notimestamps|>)
+  int ts_max_init = 0;      // max_initial_timestamp_index
 };
 
 SearchArgs make_search_args(wisb_handle* h, const DecodeCfg& c) {
@@ -698,6 +702,12 @@ SearchArgs make_search_args(wisb_handle* h, const DecodeCfg& c) {
   a.row_pos = h->row_pos.p;
   a.row_slot = h->row_slot.p;
   a.max_new_u = c.per_utt_max_new ? h->max_new_u.p : nullptr;
+  if (c.ts) {
+    a.ts = 1;
+    a.no_ts = dm.no_timestamps;
+    a.ts_begin = dm.no_timestamps + 1;
+    a.ts_max_init = std::min(a.ts_begin + c.ts_max_init, dm.n_vocab - 1);
+  }
   return a;
 }
 
@@ -905,6 +915,7 @@ DecGraphs& get_graphs(wisb_handle* h, const DecodeCfg& c) {
   key.n_utt = c.n_utt; key.beam = c.beam; key.prompt_len = c.prompt_len; key.max_new = c.max_new;
   key.max_hyp = c.max_hyp; key.lp = c.lp;
   key.u0 = c.u0; key.b_total = c.B_total;  // they move the cross-K/V base pointers baked into the graph
+  key.ts = c.ts; key.ts_max_init = c.ts ? c.ts_max_init : 0;
   auto it = h->graphs.find(key);
   if (it != h->graphs.end()) return it->second;
   if (h->graphs.size() > 64) {  // bound the cache
@@ -1233,6 +1244,7 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
       key.n_utt = c.n_utt; key.beam = c.beam; key.prompt_len = c.prompt_len; key.max_new = c.max_new;
       key.max_hyp = c.max_hyp; key.lp = c.lp; key.u0 = c.u0; key.b_total = c.B_total;
       key.batched = 1 + c.per_utt_max_new;
+      key.ts = c.ts; key.ts_max_init = c.ts ? c.ts_max_init : 0;
       auto it = h->graphs.find(key);
       if (it == h->graphs.end()) {
         if (h->graphs.size() > 64) drop_graphs(h);
@@ -1512,10 +1524,10 @@ int wisb_logmel(wisb_handle* h, const void* pcm, int pcm_dtype, int pcm_on_devic
   });
 }
 
-int wisb_generate_ex(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
+int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
                      float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                     const int32_t* extra_suppress, int n_extra, int32_t* out_ids, int out_stride, int32_t* out_len,
-                     float* out_score) {
+                     const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
+                     int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score) {
   return guarded(h, [&] {
     const Dims& dm = h->dims;
     WISB_REQUIRE(h->blob != nullptr, "handle has no model (created by wisb_create_frontend)");
@@ -1528,6 +1540,15 @@ int wisb_generate_ex(wisb_handle* h, const float* mel, int B, const int32_t* pro
     WISB_REQUIRE(n_extra >= 0 && (n_extra == 0 || extra_suppress != nullptr), "bad extra_suppress");
     for (long long i = 0; i < static_cast<long long>(B) * prompt_len; ++i)
       WISB_REQUIRE(prompts[i] >= 0 && prompts[i] < dm.n_vocab, "prompt token outside the vocabulary");
+    WISB_REQUIRE(timestamps == 0 || timestamps == 1, "timestamps must be 0 or 1");
+    WISB_REQUIRE(max_initial_timestamp_index >= 0, "max_initial_timestamp_index must be >= 0");
+    if (timestamps) {
+      WISB_REQUIRE(dm.no_timestamps > dm.eot && dm.no_timestamps + 1 < dm.n_vocab, "this vocabulary has no timestamp tokens");
+      for (long long i = 0; i < static_cast<long long>(B) * prompt_len; ++i) {
+        WISB_REQUIRE(prompts[i] != dm.no_timestamps, "timestamp decoding: the prompt must not contain <|notimestamps|>");
+        WISB_REQUIRE(prompts[i] <= dm.no_timestamps, "timestamp decoding: the prompt must not contain timestamp tokens");
+      }
+    }
     auto new_tokens = [&](int ml) {  // CTranslate2: at most max_length / 2 new tokens, max_length in total
       int v = ml / 2 < ml - prompt_len ? ml / 2 : ml - prompt_len;
       return v < 0 ? 0 : v;
@@ -1561,6 +1582,8 @@ int wisb_generate_ex(wisb_handle* h, const float* mel, int B, const int32_t* pro
     c.max_hyp = static_cast<int>(beam_size * patience + 0.5f);
     if (c.max_hyp < 1) c.max_hyp = 1;
     c.lp = length_penalty;
+    c.ts = timestamps;
+    c.ts_max_init = max_initial_timestamp_index;
     // Utterances are encoded and decoded in groups that share every decoder pass: the group's rows (utterances x beams)
     // are the M dimension of the batched pass, so the decoder weights stream once per generated token for the whole
     // group.  The group size only bounds the workspaces (cross K/V: 252 MB per large-v2 utterance).
@@ -1616,6 +1639,14 @@ int wisb_generate_ex(wisb_handle* h, const float* mel, int B, const int32_t* pro
     h->timing[7] = static_cast<float>(h->launches);
     h->prof_collect();
   });
+}
+
+int wisb_generate_ex(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
+                     float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
+                     const int32_t* extra_suppress, int n_extra, int32_t* out_ids, int out_stride, int32_t* out_len,
+                     float* out_score) {
+  return wisb_generate_ts(h, mel, B, prompts, prompt_len, beam_size, patience, length_penalty, max_length,
+                          max_length_per_utt, extra_suppress, n_extra, 0, 0, out_ids, out_stride, out_len, out_score);
 }
 
 int wisb_generate(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
@@ -1791,6 +1822,104 @@ int wisb_debug_gemm(wisb_handle* h, const int32_t* prm, int n_prm, const uint16_
       plan_out[2] = impl == 1 ? 1 : p.k_splits;
       plan_out[3] = impl == 1 ? 0 : p.grid;
     }
+  });
+}
+
+int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, const float* logits, const int32_t* hist,
+                           const uint8_t* mask, const float* cum, const int32_t* done, int32_t* cand_idx, float* cand_score,
+                           float* row_lse) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(prm != nullptr && n_prm == 8 && logits && mask && cand_idx && cand_score && row_lse, "debug_search_step: bad arguments");
+    const int n_utt = prm[0], beam = prm[1], gen = prm[2], V = prm[3], eot = prm[4], no_ts = prm[5], ts = prm[6], max_init = prm[7];
+    WISB_REQUIRE(n_utt >= 1 && n_utt <= 64 && beam >= 1 && beam <= MAX_BEAM && gen >= 0 && gen + 2 <= T_MAX && V >= 2 &&
+                     eot >= 0 && eot < V && (ts == 0 || ts == 1) && max_init >= 0 && (gen == 0 || hist != nullptr),
+                 "debug_search_step: bad scalar parameters");
+    WISB_REQUIRE(!ts || (no_ts > eot && no_ts + 1 < V), "debug_search_step: bad timestamp geometry");
+    cudaStream_t s = h->stream;
+    const int R = n_utt * beam, max_new = gen + 2;
+    DevBuf<float> d_logits, d_lse, d_pmax, d_psum, d_cum, d_cs, d_best;
+    DevBuf<unsigned long long> d_part;
+    DevBuf<uint8_t> d_mask;
+    DevBuf<int> d_ci, d_tok, d_seq, d_ind, d_flip, d_done, d_nhyp, d_blen, d_btok;
+    DevBuf<DecState> d_st;
+    d_logits.ensure(static_cast<size_t>(R) * V);
+    d_mask.ensure(V);
+    d_lse.ensure(R);
+    d_pmax.ensure(static_cast<size_t>(R) * (TOPK_CHUNKS + 1));
+    d_psum.ensure(static_cast<size_t>(R) * (TOPK_CHUNKS + 1));
+    d_part.ensure(static_cast<size_t>(R) * (TOPK_CHUNKS + 1) * MAX_CAND);
+    d_cum.ensure(R, true);
+    d_cs.ensure(static_cast<size_t>(n_utt) * MAX_CAND);
+    d_ci.ensure(static_cast<size_t>(n_utt) * MAX_CAND);
+    d_tok.ensure(R);
+    d_seq.ensure(2ull * R * max_new, true);
+    d_ind.ensure(2ull * R, true);
+    d_flip.ensure(1, true);
+    d_done.ensure(n_utt, true);
+    d_nhyp.ensure(n_utt, true);
+    d_best.ensure(n_utt);
+    d_blen.ensure(n_utt, true);
+    d_btok.ensure(static_cast<size_t>(n_utt) * max_new, true);
+    d_st.ensure(1);
+    WISB_CUDA(cudaMemcpyAsync(d_logits.p, logits, sizeof(float) * R * V, cudaMemcpyHostToDevice, s));
+    WISB_CUDA(cudaMemcpyAsync(d_mask.p, mask, V, cudaMemcpyHostToDevice, s));
+    if (cum) WISB_CUDA(cudaMemcpyAsync(d_cum.p, cum, sizeof(float) * R, cudaMemcpyHostToDevice, s));
+    if (done) WISB_CUDA(cudaMemcpyAsync(d_done.p, done, sizeof(int) * n_utt, cudaMemcpyHostToDevice, s));
+    std::vector<int> seq(static_cast<size_t>(R) * max_new, 0);
+    for (int r = 0; r < R; ++r)
+      for (int t = 0; t < gen; ++t) seq[static_cast<size_t>(r) * max_new + t] = hist[static_cast<size_t>(r) * gen + t];
+    WISB_CUDA(cudaMemcpyAsync(d_seq.p, seq.data(), sizeof(int) * seq.size(), cudaMemcpyHostToDevice, s));
+    std::vector<float> best(n_utt, -INFINITY);
+    WISB_CUDA(cudaMemcpyAsync(d_best.p, best.data(), sizeof(float) * n_utt, cudaMemcpyHostToDevice, s));
+    int n_done = 0;
+    for (int u = 0; u < n_utt && done; ++u) n_done += done[u] != 0;
+    WISB_REQUIRE(n_done < n_utt, "debug_search_step: every utterance is finished");
+    DecState st{0, gen, n_done, 0, 0};
+    WISB_CUDA(cudaMemcpyAsync(d_st.p, &st, sizeof(st), cudaMemcpyHostToDevice, s));
+    SearchArgs a;
+    a.logits = d_logits.p;
+    a.ldl = V;
+    a.n_vocab = V;
+    a.mask = d_mask.p;
+    a.n_utt = n_utt;
+    a.beam = beam;
+    a.n_cand = 2 * beam;
+    a.max_new = max_new;
+    a.max_hyp = beam;
+    a.eot = eot;
+    a.t_max = 1;
+    a.prompt_len = 1;
+    a.length_penalty = 1.f;
+    if (ts) {
+      a.ts = 1;
+      a.no_ts = no_ts;
+      a.ts_begin = no_ts + 1;
+      a.ts_max_init = std::min(a.ts_begin + max_init, V - 1);
+    }
+    a.row_lse = d_lse.p;
+    a.part_max = d_pmax.p;
+    a.part_sum = d_psum.p;
+    a.cum = d_cum.p;
+    a.part = d_part.p;
+    a.cand_score = d_cs.p;
+    a.cand_idx = d_ci.p;
+    a.tokens = d_tok.p;
+    a.seq[0] = d_seq.p;
+    a.seq[1] = d_seq.p + static_cast<size_t>(R) * max_new;
+    a.indir[0] = d_ind.p;
+    a.indir[1] = d_ind.p + R;
+    a.flip = d_flip.p;
+    a.done = d_done.p;
+    a.n_hyp = d_nhyp.p;
+    a.best_score = d_best.p;
+    a.best_len = d_blen.p;
+    a.best_tokens = d_btok.p;
+    a.st = d_st.p;
+    search_step_run(a, s);  // the production step: processors, top-k partials, merge and the beam bookkeeping
+    WISB_CUDA(cudaMemcpyAsync(cand_idx, d_ci.p, sizeof(int) * n_utt * MAX_CAND, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(cand_score, d_cs.p, sizeof(float) * n_utt * MAX_CAND, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(row_lse, d_lse.p, sizeof(float) * R, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
   });
 }
 

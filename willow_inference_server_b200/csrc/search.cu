@@ -11,6 +11,11 @@
 //     next non-eot candidates; an utterance is finished once round(beam*patience) hypotheses exist or at the last step
 //   * result: best normalised score, first one on ties; eot itself is not part of the output
 //   * beam_size == 1 is the same procedure with 2 candidates, i.e. greedy arg-max decoding
+// Timestamp mode (SearchArgs::ts, prompt without <|notimestamps|>) adds Whisper's timestamp rules after those processors
+// (openai/whisper, transformers' WhisperTimeStampLogitsProcessor): <|notimestamps|> off; at the first step text off and
+// timestamps above ts_max_init off; after a timestamp pair timestamps off, after a lone timestamp text (< eot) off;
+// timestamps below the last one off (at or below it unless it opened a pair); and text off in a row whose timestamp
+// log-sum-exp exceeds its best text logit.  The vocabulary is then split as 32 text chunks + one timestamp chunk.
 #include "decoder.cuh"
 
 namespace wisb {
@@ -33,6 +38,43 @@ __device__ __forceinline__ float masked_logit(const SearchArgs& a, const float* 
   const unsigned char m = a.mask[v];
   if ((m & 1) || (first_step && (m & 2))) return -INFINITY;
   return row[v];
+}
+
+// Per-row state of the timestamp rules, from the row's own generated tokens seq[*flip][r][0, gen).
+struct TsRule {
+  int lo, hi;          // timestamps outside [lo, hi] are off (rules 2 and 4)
+  int text_off;        // gen == 0: every id < ts_begin is off (rule 2)
+  int below_eot_off;   // last token a timestamp, the one before it not: ids < eot are off (rule 3b)
+  int ts_off;          // last two tokens timestamps (or gen == 1 after one): timestamps are off (rule 3a)
+};
+
+// warp-cooperative: every lane returns the same state
+__device__ __forceinline__ TsRule ts_rule_state(const SearchArgs& a, int r, int gen) {
+  const int lane = threadIdx.x & 31;
+  const int* hist = a.seq[*a.flip] + static_cast<long long>(r) * a.max_new;
+  int last = -1;  // index of the last timestamp of the history
+  for (int t = lane; t < gen; t += 32)
+    if (hist[t] >= a.ts_begin) last = t;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) last = max(last, __shfl_xor_sync(0xffffffffu, last, o));
+  const bool last_ts = gen >= 1 && hist[gen - 1] >= a.ts_begin;
+  const bool pen_ts = gen < 2 || hist[gen - 2] >= a.ts_begin;
+  TsRule s;
+  s.text_off = gen == 0;
+  s.below_eot_off = last_ts && !pen_ts;
+  s.ts_off = last_ts && pen_ts;
+  s.lo = last >= 0 ? hist[last] + (s.below_eot_off ? 0 : 1) : a.ts_begin;
+  s.hi = gen == 0 ? a.ts_max_init : a.n_vocab - 1;
+  return s;
+}
+
+__device__ __forceinline__ float ts_masked_logit(const SearchArgs& a, const TsRule& s, const float* row, int v, bool first_step) {
+  if (v < a.ts_begin) {
+    if (s.text_off || v == a.no_ts || (s.below_eot_off && v < a.eot)) return -INFINITY;
+  } else if (s.ts_off || v < s.lo || v > s.hi) {
+    return -INFINITY;
+  }
+  return masked_logit(a, row, v, first_step);
 }
 
 // block-wide selection of the `n_cand` largest keys among each thread's private keys[0..cnt)
@@ -70,24 +112,47 @@ __device__ void block_select(unsigned long long (&keys)[PER], int n_cand, unsign
   }
 }
 
-// grid (TOPK_CHUNKS, R): partial top-n_cand of one chunk of one row
+// grid (NCH, R): partial top-n_cand of one chunk of one row.  NCH = TOPK_CHUNKS: the vocabulary in 32 chunks.
+// NCH = TOPK_CHUNKS + 1 (timestamp mode): chunks 0..31 split the text ids [0, ts_begin), chunk 32 holds the timestamps.
 constexpr int TK_THREADS = 256;
-constexpr int TK_PER = 8;  // 256 * 8 = 2048 >= ceil(51865 / 32) = 1621
+constexpr int TK_PER = 8;  // 256 * 8 = 2048 >= ceil(51865 / 32) = 1621 and >= the 1501 timestamps
 
+template <int NCH>
 __global__ void __launch_bounds__(TK_THREADS) topk_partial_kernel(const SearchArgs a) {
   // Within one row the ranking by processed logit equals the ranking by score, so the per-chunk stage needs no
   // log-sum-exp: it emits the chunk's top-n_cand logits plus (max, sum exp) partials; the merge stage turns them into
   // the row's lse and into scores, with no separate two-pass lse kernel.
+  constexpr bool TS = NCH > TOPK_CHUNKS;
   __shared__ unsigned long long s_red[32];
   __shared__ float s_f[32];
+  __shared__ TsRule s_rule;
   if (a.st->all_done) return;  // a step enqueued ahead of the host's poll
   const int chunk = blockIdx.x, r = blockIdx.y;
   const bool first = a.st->gen_step == 0;
   const float* row = a.logits + static_cast<long long>(r) * a.ldl;
-  const int per_chunk = (a.n_vocab + TOPK_CHUNKS - 1) / TOPK_CHUNKS;
-  const int v0 = chunk * per_chunk;
-  const int v1 = min(a.n_vocab, v0 + per_chunk);
+  int v0, v1;
+  if (!TS) {
+    const int per_chunk = (a.n_vocab + TOPK_CHUNKS - 1) / TOPK_CHUNKS;
+    v0 = chunk * per_chunk;
+    v1 = min(a.n_vocab, v0 + per_chunk);
+  } else if (chunk < TOPK_CHUNKS) {
+    const int per_chunk = (a.ts_begin + TOPK_CHUNKS - 1) / TOPK_CHUNKS;
+    v0 = chunk * per_chunk;
+    v1 = min(a.ts_begin, v0 + per_chunk);
+  } else {
+    v0 = a.ts_begin;
+    v1 = a.n_vocab;
+  }
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  TsRule rule;
+  if (TS) {
+    if (warp == 0) {
+      const TsRule t = ts_rule_state(a, r, a.st->gen_step);
+      if (lane == 0) s_rule = t;
+    }
+    __syncthreads();
+    rule = s_rule;
+  }
   unsigned long long keys[TK_PER];
   float lg[TK_PER];
   float mx = -INFINITY;
@@ -97,7 +162,7 @@ __global__ void __launch_bounds__(TK_THREADS) topk_partial_kernel(const SearchAr
     keys[i] = 0ull;
     lg[i] = -INFINITY;
     if (v < v1) {
-      lg[i] = masked_logit(a, row, v, first);
+      lg[i] = TS ? ts_masked_logit(a, rule, row, v, first) : masked_logit(a, row, v, first);
       if (lg[i] != -INFINITY) keys[i] = pack_key(lg[i], static_cast<unsigned>(v));
       mx = fmaxf(mx, lg[i]);
     }
@@ -118,16 +183,21 @@ __global__ void __launch_bounds__(TK_THREADS) topk_partial_kernel(const SearchAr
   if (tid == 0) {
     float t = 0.f;
     for (int w = 0; w < TK_THREADS / 32; ++w) t += s_f[w];
-    a.part_max[r * TOPK_CHUNKS + chunk] = mx;
-    a.part_sum[r * TOPK_CHUNKS + chunk] = t;
+    a.part_max[r * NCH + chunk] = mx;
+    a.part_sum[r * NCH + chunk] = t;
   }
-  block_select<TK_PER>(keys, a.n_cand, a.part + (static_cast<long long>(r) * TOPK_CHUNKS + chunk) * MAX_CAND, s_red);
+  block_select<TK_PER>(keys, a.n_cand, a.part + (static_cast<long long>(r) * NCH + chunk) * MAX_CAND, s_red);
 }
 
-// grid (n_utt): merge beam * TOPK_CHUNKS * n_cand partial keys -> sorted candidate list
-constexpr int TM_PER = (MAX_BEAM * TOPK_CHUNKS * MAX_CAND + TK_THREADS - 1) / TK_THREADS;  // 16
+// grid (n_utt): merge beam * NCH * n_cand partial keys -> sorted candidate list
+template <int NCH>
+constexpr int tm_per() { return (MAX_BEAM * NCH * MAX_CAND + TK_THREADS - 1) / TK_THREADS; }  // 16 / 17
 
-__device__ __forceinline__ void topk_merge_body(const SearchArgs& a, unsigned long long* s_red, unsigned long long* s_out, float* s_lse) {
+template <int NCH>
+__device__ __forceinline__ void topk_merge_body(const SearchArgs& a, unsigned long long* s_red, unsigned long long* s_out,
+                                                float* s_lse, int* s_ts_only) {
+  constexpr bool TS = NCH > TOPK_CHUNKS;
+  constexpr int TM_PER = tm_per<NCH>();
   const int u = blockIdx.x;
   const int gen = a.st->gen_step;
   const bool first = gen == 0;
@@ -135,17 +205,28 @@ __device__ __forceinline__ void topk_merge_body(const SearchArgs& a, unsigned lo
   if (threadIdx.x < a.beam) {  // row log-sum-exp from the chunk partials
     const int r = u * a.beam + threadIdx.x;
     float mx = -INFINITY;
-    for (int c = 0; c < TOPK_CHUNKS; ++c) mx = fmaxf(mx, a.part_max[r * TOPK_CHUNKS + c]);
+    for (int c = 0; c < NCH; ++c) mx = fmaxf(mx, a.part_max[r * NCH + c]);
     float t = 0.f;
-    for (int c = 0; c < TOPK_CHUNKS; ++c) {
-      const float pm = a.part_max[r * TOPK_CHUNKS + c];
-      if (pm != -INFINITY) t += a.part_sum[r * TOPK_CHUNKS + c] * __expf(pm - mx);
+    for (int c = 0; c < NCH; ++c) {
+      const float pm = a.part_max[r * NCH + c];
+      if (pm != -INFINITY) t += a.part_sum[r * NCH + c] * __expf(pm - mx);
     }
-    s_lse[threadIdx.x] = mx + logf(t);
-    a.row_lse[r] = s_lse[threadIdx.x];
+    float lse = mx + logf(t);
+    if (TS) {
+      // rule 5: the row's timestamp log-sum-exp against its best text logit (the log-softmax normaliser cancels)
+      float text_max = -INFINITY;
+      for (int c = 0; c < TOPK_CHUNKS; ++c) text_max = fmaxf(text_max, a.part_max[r * NCH + c]);
+      const float pm = a.part_max[r * NCH + TOPK_CHUNKS];
+      const float ts_lse = pm == -INFINITY ? -INFINITY : pm + logf(a.part_sum[r * NCH + TOPK_CHUNKS]);
+      const int ts_only = ts_lse > text_max;
+      s_ts_only[threadIdx.x] = ts_only;
+      if (ts_only) lse = ts_lse;
+    }
+    s_lse[threadIdx.x] = lse;
+    a.row_lse[r] = lse;
   }
   __syncthreads();
-  const int total = a.beam * TOPK_CHUNKS * a.n_cand;
+  const int total = a.beam * NCH * a.n_cand;
   unsigned long long keys[TM_PER];
 #pragma unroll
   for (int i = 0; i < TM_PER; ++i) {
@@ -154,10 +235,11 @@ __device__ __forceinline__ void topk_merge_body(const SearchArgs& a, unsigned lo
     if (j < total) {
       const int c = j % a.n_cand;
       const int rc = j / a.n_cand;       // (beam row, chunk)
-      const int k = rc / TOPK_CHUNKS;    // beam index
-      const unsigned long long pk = a.part[(static_cast<long long>(u * a.beam) * TOPK_CHUNKS + rc) * MAX_CAND + c];
+      const int k = rc / NCH;            // beam index
+      const unsigned long long pk = a.part[(static_cast<long long>(u * a.beam) * NCH + rc) * MAX_CAND + c];
       // at the first step every beam holds the same prefix: only beam 0 counts
-      if (pk != 0ull && !(first && k > 0)) {
+      const bool dropped = TS && s_ts_only[k] && rc % NCH < TOPK_CHUNKS;  // rule 5 turned this row's text off
+      if (pk != 0ull && !(first && k > 0) && !dropped) {
         const float lg = ord2f(static_cast<unsigned>(pk >> 32));
         const unsigned v = ~static_cast<unsigned>(pk & 0xffffffffull);
         const float sc = ((lg - s_lse[k]) + a.cum[u * a.beam + k]) / norm;
@@ -273,16 +355,18 @@ __device__ __forceinline__ void search_bookkeeping_body(const SearchArgs& a, int
 // grid (n_utt) x TK_THREADS: candidate merge, then (warp 0) the bookkeeping of the utterance, then -- by the last CTA to get
 // there -- the step advance (position, generation step, ping-pong flip, per-row positions).  One launch instead of three:
 // the tail of a decoding step is launch-latency bound.
+template <int NCH>
 __global__ void __launch_bounds__(TK_THREADS) search_tail_kernel(const SearchArgs a) {
   __shared__ unsigned long long s_red[32];
   __shared__ unsigned long long s_out[MAX_CAND];
   __shared__ float s_lse[MAX_BEAM];
+  __shared__ int s_ts_only[MAX_BEAM];
   __shared__ int s_pick[MAX_BEAM];
   __shared__ int s_best_k;
   __shared__ int s_finished;
   __shared__ int s_last;
   if (a.st->all_done) return;  // a step enqueued ahead of the host's poll: nothing left to do
-  topk_merge_body(a, s_red, s_out, s_lse);
+  topk_merge_body<NCH>(a, s_red, s_out, s_lse, s_ts_only);
   __syncthreads();  // the candidate list (global) is complete for this CTA's readers
   if (threadIdx.x < 32) search_bookkeeping_body(a, s_pick, s_best_k, s_finished);
   __syncthreads();
@@ -381,8 +465,16 @@ void search_step_run(const SearchArgs& a, cudaStream_t stream) {
   const int R = a.n_utt * a.beam;
   WISB_REQUIRE(a.beam >= 1 && a.beam <= MAX_BEAM && a.n_cand <= MAX_CAND, "search: beam_size must be in [1, 8]");
   WISB_REQUIRE((a.n_vocab + TOPK_CHUNKS - 1) / TOPK_CHUNKS <= TK_THREADS * TK_PER, "search: vocabulary too large");
-  topk_partial_kernel<<<dim3(TOPK_CHUNKS, R), TK_THREADS, 0, stream>>>(a);
-  search_tail_kernel<<<a.n_utt, TK_THREADS, 0, stream>>>(a);
+  if (a.ts) {
+    WISB_REQUIRE(a.ts_begin > a.eot && a.ts_begin < a.n_vocab && a.n_vocab - a.ts_begin <= TK_THREADS * TK_PER &&
+                     a.ts_max_init >= a.ts_begin && a.max_new >= 1,
+                 "search: bad timestamp geometry");
+    topk_partial_kernel<TOPK_CHUNKS + 1><<<dim3(TOPK_CHUNKS + 1, R), TK_THREADS, 0, stream>>>(a);
+    search_tail_kernel<TOPK_CHUNKS + 1><<<a.n_utt, TK_THREADS, 0, stream>>>(a);
+  } else {
+    topk_partial_kernel<TOPK_CHUNKS><<<dim3(TOPK_CHUNKS, R), TK_THREADS, 0, stream>>>(a);
+    search_tail_kernel<TOPK_CHUNKS><<<a.n_utt, TK_THREADS, 0, stream>>>(a);
+  }
   WISB_CUDA(cudaGetLastError());
 }
 

@@ -170,8 +170,16 @@ class Whisper:
                              "(the CTranslate2 defaults WIS uses) are implemented")
         if not suppress_blank or -1 not in suppress_tokens or asynchronous:
             raise ValueError("suppress_blank=True, suppress_tokens containing -1 and asynchronous=False are required")
-        if self._dims["no_timestamps"] not in prompts[0]:
-            raise ValueError("timestamp decoding is not implemented: the prompt must contain <|notimestamps|>")
+        # CTranslate2's rule: a prompt without <|notimestamps|> asks for timestamps (main.py:529, :661 say "Remove this
+        # token to generate timestamps"); the returned ids then hold the timestamp tokens
+        no_ts = self._dims["no_timestamps"]
+        with_ts = {no_ts not in p for p in prompts}
+        if len(with_ts) != 1:
+            raise ValueError("the prompts of one call must all contain <|notimestamps|> or all omit it")
+        timestamps = with_ts.pop()
+        if isinstance(max_initial_timestamp_index, bool) or int(max_initial_timestamp_index) != max_initial_timestamp_index \
+                or max_initial_timestamp_index < 0:
+            raise ValueError("max_initial_timestamp_index must be a non-negative int")
         extra = [int(t) for t in suppress_tokens if t >= 0]
         p = np.asarray(prompts, np.int32)
         parts = self._split(n, mel)
@@ -183,7 +191,8 @@ class Whisper:
 
         def job(i, s, e):
             return lambda: self._handles[i].generate(mel[s:e], p[s:e], beam_size, patience, length_penalty,
-                                                     max_length if ml is None else ml[s:e], extra)
+                                                     max_length if ml is None else ml[s:e], extra, timestamps=timestamps,
+                                                     max_initial_timestamp_index=int(max_initial_timestamp_index))
 
         outs = self._run([job(*pt) for pt in parts])
         results = []

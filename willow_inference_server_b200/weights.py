@@ -199,7 +199,8 @@ def pack_state_dict(sd: dict, dims: WhisperDims) -> dict:
 # seeded synthetic weights (the project ships no real checkpoints)
 # ---------------------------------------------------------------------------
 def synth_state_dict(dims: WhisperDims, seed: int = 0, logit_std: float = 4.0, qk_gain: float = 2.5,
-                     resid_std: float = 8.0, eot_ramp: tuple | None = None, script: tuple | None = None) -> dict:
+                     resid_std: float = 8.0, eot_ramp: tuple | None = None, script: tuple | None = None,
+                     ts_script: tuple | None = None) -> dict:
     """Deterministic random Whisper weights under HF names.
 
     Every GEMM weight is rounded to float16 so oracle (fp32 math) and engine
@@ -218,6 +219,16 @@ def synth_state_dict(dims: WhisperDims, seed: int = 0, logit_std: float = 4.0, q
     candidates are separated by O(rho) deviations instead of the ~0.01-wide near-ties of a flat random model,
     so greedy / beam transcripts are robust to fp16-vs-fp32 rounding.  The share of the residual stream the
     script takes is solved from ``rho`` and d_model, so the same setting works at every model size.
+
+    ``ts_script=(first_pos, period, width)`` (needs ``script``) lifts timestamp tokens the same way, so that timestamp
+    decoding (a prompt without <|notimestamps|>) is steered through every timestamp rule.  Levels are fractions of the
+    top text alternative's lift.  At ``first_pos`` (the first generated step of a 3-token prompt is position 2):
+    timestamp index 8 at 0.8 and index 60 at 0.9, both below the best text token, so the first-step rules and the
+    max-initial-timestamp clamp (index 50) decide; at ``first_pos + 1``: <|notimestamps|> at 1.3.  Every ``period``
+    positions after that a segment boundary: a window of ``width`` increasing timestamps at 0.97 (each below the best
+    text token, their log-sum-exp above it); one position later a lower timestamp at 0.9 and the window again at 0.8 (the
+    non-decreasing rule decides); one more position later the next timestamps at 1.1 (the pair rule turns them off).
+    The windows move up 40 indices per boundary.  ``None`` leaves the model byte-identical to one built without it.
     """
     dims.validate()
     d = dims.d_model
@@ -314,6 +325,8 @@ def synth_state_dict(dims: WhisperDims, seed: int = 0, logit_std: float = 4.0, q
     with ThreadPoolExecutor(max_workers=max(1, min(32, (_os.cpu_count() or 1)))) as ex:
         for k, a in zip(names, ex.map(lambda k: sd[k].fn(), names)):
             sd[k] = a
+    if ts_script is not None and script is None:
+        raise ValueError("ts_script scales its lifts by the text script: pass script too")
     if script is not None:
         n_alt, rho, off = script
         emb = sd[dd + "embed_tokens.weight"]
@@ -337,6 +350,28 @@ def synth_state_dict(dims: WhisperDims, seed: int = 0, logit_std: float = 4.0, q
             for j, t in enumerate(alts):
                 nrm = np.linalg.norm(emb[t])
                 pos[p] += (c[j] * s_eff * logit_std / (nrm * nrm)) * emb[t].astype(np.float64)
+        if ts_script is not None:
+            first_pos, period, width = (int(v) for v in ts_script)
+            ts0 = dims.no_timestamps + 1
+            n_ts = dims.n_vocab - ts0
+
+            def lift(p, tok, level):
+                nrm = np.linalg.norm(emb[tok])
+                pos[p] += (level * c[0] * s_eff * logit_std / (nrm * nrm)) * emb[tok].astype(np.float64)
+
+            lift(first_pos, ts0 + 8, 0.8)
+            lift(first_pos, ts0 + 60, 0.9)
+            lift(first_pos + 1, dims.no_timestamps, 1.3)
+            k = 1
+            while first_pos + k * period + 2 < dims.n_text_ctx and 40 * k + 8 + width + 2 < n_ts:
+                p, base = first_pos + k * period, ts0 + 8 + 40 * k
+                for j in range(width):
+                    lift(p, base + j, 0.97)
+                    lift(p + 1, base + j, 0.8)
+                lift(p + 1, base - 20, 0.9)
+                lift(p + 2, base + width, 1.1)
+                lift(p + 2, base + width + 1, 1.1)
+                k += 1
         sd[dd + "embed_positions.weight"] = pos.astype(np.float32)
     if eot_ramp is not None:
         p0, slope = eot_ramp
