@@ -87,6 +87,23 @@ int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* pro
  * lang_ids_out int32 [B, n_langs], probs_out float32 [B, n_langs]. */
 int wisb_detect_language(wisb_handle* h, const float* mel, int B, int32_t* lang_ids_out, float* probs_out);
 
+/* (5b) Whisper.align: token-to-frame alignment from the cross-attention of the alignment heads (blob tensor
+ * meta.alignment_heads [A, 2] (layer, head); without it every head of layers n_dec_layers / 2 .. n_dec_layers - 1).
+ * mel as in wisb_generate (NULL = the features wisb_logmel kept on the device).  Window b is teacher-forced with
+ * start_seq [start_len] + <|notimestamps|> + text[b, :text_len[b]]; start_seq begins with <|startoftranscript|> and holds
+ * neither <|notimestamps|> nor timestamp ids, text ids are in [0, eot), start_len + 1 + text_len[b] <= n_text_ctx,
+ * num_frames[b] in [2, 3000], median_filter_width odd in [1, 31], path_stride >= text_len[b] + num_frames[b] / 2 + 1 (the longest path: R + F
+ * entries, reached when NaN columns of the filtered matrix, frames whose probabilities are equal in every row, route it
+ * along the last row to frame 0).
+ * Outputs: out_path int32 [B, path_stride, 2] = (text index in [0, text_len], frame in [0, num_frames / 2)) in path order,
+ * out_path_len [B], out_token_probs float32 [B, text_stride] (entry i < text_len[b]: probability of text token i).
+ * A window with text_len 0 gets an empty path and adds no capture, filter or DTW work.  Stage timings in wisb_get_timing:
+ * [1 h2d, 2 encoder + cross K/V, 3 teacher-forced passes (capture and token probabilities included), 4 filter, 5 total,
+ *  6 passes, 7 kernel launches, 13 capture kernels (option "profile" only), 14 DTW]. */
+int wisb_align(wisb_handle* h, const float* mel, int B, const int32_t* start_seq, int start_len, const int32_t* text,
+               const int32_t* text_len, int text_stride, const int32_t* num_frames, int median_filter_width,
+               int32_t* out_path, int path_stride, int32_t* out_path_len, float* out_token_probs);
+
 /* stage timings (ms, CUDA events on the launching stream) of the last wisb_logmel / wisb_generate:
  * [0 logmel, 1 h2d, 2 encoder, 3 cross_kv, 4 decode, 5 total_generate, 6 decode_steps, 7 kernel_launches,
  *  8 sum of GEMM kernels, 9 attention kernels, 10 LayerNorm kernels, 11 conv1, 12 number of GEMM launches, 13-15 0]
@@ -137,6 +154,19 @@ int wisb_debug_read_trace(wisb_handle* h, unsigned long long* out, int n);
 int wisb_debug_encode(wisb_handle* h, const float* mel, int B, float* enc_out, int n_layers);
 /* teacher-forced raw decoder logits (no processors) for utterance 0: float32 [n_tokens, n_vocab] */
 int wisb_debug_forced_logits(wisb_handle* h, const float* mel, const int32_t* tokens, int n_tokens, float* logits_out);
+/* wisb_align's post-processing kernels on caller data for one window: weights float32 [A, R, F] (R = text rows + 1,
+ * 2 <= R <= 449, 1 <= F <= 1500) -> standardise, median filter of odd `width` <= 31, head mean -> matrix_out float32
+ * [R, F] (may be NULL), then DTW -> path_out int32 [R + F, 2], path_len.  dtw_only = 1: weights is the matrix [R, F]
+ * itself (A = 1) and only the DTW runs. */
+/* wisb_align's teacher-forced passes on caller data, returning the raw captured probabilities (before the filter):
+ * cap_out float32 [B, A, n_max + 1, F_max] with n_max / F_max the largest text_len / num_frames / 2 over the windows that
+ * have text; entry [b, a, r, f] (r <= text_len[b], f < num_frames[b] / 2) is alignment head a's softmax over all 1500
+ * frames at row r, other entries are left as they were.  The windows must fit in one group of wisb_align. */
+int wisb_debug_align_capture(wisb_handle* h, const float* mel, int B, const int32_t* start_seq, int start_len,
+                             const int32_t* text, const int32_t* text_len, int text_stride, const int32_t* num_frames,
+                             float* cap_out);
+int wisb_debug_align_post(wisb_handle* h, const float* weights, int A, int R, int F, int width, int dtw_only,
+                          float* matrix_out, int32_t* path_out, int32_t* path_len);
 
 /* ---- (6) FLAC ingest (host code, no handle, no GPU): replaces the decode half of `librosa.load(audio_file, sr=16000)`
  * (main.py:579) for the FLAC files WIS is tested with (client/{3sec,10sec,30sec}.flac).

@@ -40,6 +40,12 @@ _SIGS = {
                                    C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                    C.c_void_p, C.c_void_p]),
     "wisb_detect_language": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "wisb_align": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                             C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "wisb_debug_align_capture": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                           C.c_int, C.c_void_p, C.c_void_p]),
+    "wisb_debug_align_post": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                        C.c_void_p, C.c_void_p]),
     "wisb_get_timing": (C.c_int, [C.c_void_p, C.c_void_p]),
     "wisb_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
     "wisb_debug_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -217,7 +223,73 @@ class Handle:
         check(lib().wisb_detect_language(self._h, ptr(mel), B, ptr(ids), ptr(probs)))
         return ids, probs
 
+    def align(self, mel, start_sequence, text_tokens, num_frames, median_filter_width=7, B=None):
+        """wisb_align -> (paths: list of int32 [len, 2] arrays of (text index, frame), token probs: list of float lists).
+        num_frames: an int or one int per window."""
+        if mel is not None:
+            if mel.dtype != np.float32 or mel.ndim != 3 or mel.shape[1:] != (80, 3000) or not mel.flags["C_CONTIGUOUS"]:
+                raise ValueError("features must be a C-contiguous float32 array of shape [n, 80, 3000]")
+            B = mel.shape[0]
+        if B is None or len(text_tokens) != B:
+            raise ValueError("one text token list per feature window is required")
+        start = np.ascontiguousarray(list(start_sequence), np.int32)
+        lens = np.asarray([len(t) for t in text_tokens], np.int32)
+        stride = max(1, int(lens.max()))
+        text = np.zeros((B, stride), np.int32)
+        for b, t in enumerate(text_tokens):
+            text[b, : len(t)] = t
+        nf = np.ascontiguousarray(np.broadcast_to(np.asarray(num_frames, np.int32), (B,)))
+        path_stride = int((lens + nf // 2).max()) + 1  # the longest DTW path has n + F + 1 entries
+        path = np.zeros((B, path_stride, 2), np.int32)
+        plen = np.zeros(B, np.int32)
+        probs = np.zeros((B, stride), np.float32)
+        check(lib().wisb_align(self._h, ptr(mel), B, ptr(start), start.size, ptr(text), ptr(lens), stride, ptr(nf),
+                               int(median_filter_width), ptr(path), path_stride, ptr(plen), ptr(probs)))
+        return [path[b, : plen[b]].copy() for b in range(B)], [probs[b, : lens[b]].tolist() for b in range(B)]
+
+    def align_timing(self) -> dict:
+        """Stage timings of the last align call (ms; capture_ms needs option "profile")."""
+        out = np.zeros(16, np.float32)
+        check(lib().wisb_get_timing(self._h, ptr(out)))
+        keys = {"h2d_ms": 1, "encoder_ms": 2, "passes_ms": 3, "filter_ms": 4, "align_ms": 5, "passes": 6, "launches": 7,
+                "capture_ms": 13, "dtw_ms": 14}
+        return {k: float(out[i]) for k, i in keys.items()}
+
     # ------------------------------------------------------------------ diagnostics (tests)
+    def debug_align_capture(self, mel, start_sequence, text_tokens, num_frames, n_align_heads: int):
+        """Raw captured probabilities of the model's `n_align_heads` alignment heads in wisb_align -> float32
+        [B, A, n_max + 1, F_max] (zero where a window has no row / frame)."""
+        B = mel.shape[0]
+        start = np.ascontiguousarray(list(start_sequence), np.int32)
+        lens = np.asarray([len(t) for t in text_tokens], np.int32)
+        stride = max(1, int(lens.max()))
+        text = np.zeros((B, stride), np.int32)
+        for b, t in enumerate(text_tokens):
+            text[b, : len(t)] = t
+        nf = np.ascontiguousarray(np.broadcast_to(np.asarray(num_frames, np.int32), (B,)))
+        has = lens > 0
+        A = int(n_align_heads)
+        n_max = int(lens[has].max()) if has.any() else 0
+        f_max = int((nf[has] // 2).max()) if has.any() else 0
+        cap = np.zeros((B, A, n_max + 1, f_max), np.float32)
+        check(lib().wisb_debug_align_capture(self._h, ptr(np.ascontiguousarray(mel, np.float32)), B, ptr(start), start.size,
+                                             ptr(text), ptr(lens), stride, ptr(nf), ptr(cap)))
+        return cap
+
+    def debug_align_post(self, weights, width: int = 7, dtw_only: bool = False):
+        """wisb_debug_align_post on one window: weights float32 [A, R, F] (or the matrix [R, F] with dtw_only) ->
+        (matrix float32 [R, F], path int32 [len, 2])."""
+        w = np.ascontiguousarray(weights, np.float32)
+        if dtw_only:
+            w = w.reshape((1,) + w.shape[-2:])
+        A, R, F = w.shape
+        mat = np.zeros((R, F), np.float32)
+        path = np.zeros((R + F, 2), np.int32)
+        plen = np.zeros(1, np.int32)
+        check(lib().wisb_debug_align_post(self._h, ptr(w), A, R, F, int(width), 1 if dtw_only else 0, ptr(mat), ptr(path),
+                                          ptr(plen)))
+        return mat, path[: plen[0]].copy()
+
     def debug_gemm(self, a16: np.ndarray, w16: np.ndarray, impl: int = 0, bn: int = 0, *, mode: int = EPI_F32,
                    planner: int = 0, bias=None, pos=None, out=None, aux=None, aux2=None, row_slot=None, row_pos=None,
                    a_wrap: int = 0, k_splits: int = 1, m_valid: int = 0, n_valid: int = 0, ldo: int = 0, d_model: int = 0,

@@ -141,9 +141,42 @@ struct BatchArgs {
   // cat 0 GEMM, 1 cross-attention, 2 LayerNorm / embedding, 3 self-attention; begin = 1 / 0
   void (*prof)(void* ctx, int cat, int begin) = nullptr;
   void* prof_ctx = nullptr;
+  // optional per-layer hook, called after the layer's cross-query GEMM (q holds the cross-attention queries); returns the
+  // number of kernels it launched.  Null except in Whisper.align, which captures the alignment heads' attention there.
+  int (*layer_hook)(void* ctx, int layer, cudaStream_t stream) = nullptr;
+  void* hook_ctx = nullptr;
 };
 // returns the number of kernels launched
 int batch_pass_run(const BatchArgs& a, const BatchLayer* layers, int n_layers, cudaStream_t stream);
+
+// ------------------------------------------------------------------ alignment (decoder_batch.cu, align.cu)
+// Cross-attention probabilities of the alignment heads of one layer, captured during a teacher-forced batched prefill pass
+// (rows_per_utt consecutive positions per utterance).  Item = (utterance, head of this layer).  P = softmax over all 1500
+// keys of the fp16-rounded, 1/8-scaled query against the layer's cross K; written for positions s0 + r, 0 <= r <= n_text[u],
+// frames f < n_frames[u] into cap [u][A][n_max + 1][f_max] at head index items[i].
+struct AlignCaptureArgs {
+  const float* q = nullptr;        // [n_utt * rows_per_utt, d] cross-attention queries (no scaling applied yet)
+  const __half* ck = nullptr;      // cross K of this layer, utterance 0 of the pass: [n_utt][H][1536][64]
+  const int* row_pos = nullptr;    // [rows] position of each row
+  const int* items = nullptr;      // [n_items] global alignment-head index (into cap) of this layer's heads
+  const int* head_of = nullptr;    // [A] head (within its layer) of every alignment head
+  const int* n_text = nullptr;     // [n_utt]
+  const int* n_frames = nullptr;   // [n_utt] F = num_frames // 2
+  float* cap = nullptr;
+  int n_items = 0, n_utt = 0, rows_per_utt = 0, d = 0, H = 0, A = 0, s0 = 0, n_max = 0, f_max = 0;
+};
+void align_capture_run(const AlignCaptureArgs& a, cudaStream_t stream);
+// standardise cap over the rows (population std) per (utterance, head, frame), median-filter along frames (reflect
+// padding, odd width <= 31; identity when F <= width / 2), mean over heads in head order -> mat [u][n_max + 1][f_max]
+void align_filter_run(float* cap, float* mat, const int* n_text, const int* n_frames, int n_utt, int A, int n_max, int f_max,
+                      int width, cudaStream_t stream);
+// DTW on -mat per utterance (transformers _dynamic_time_warping, fp32 cost) -> path [u][path_stride][2] (text, time), len [u]
+void align_dtw_run(const float* mat, const int* n_text, const int* n_frames, int n_utt, int n_max, int f_max, int* path,
+                   int path_stride, int* path_len, cudaStream_t stream);
+// text-token probabilities of one pass: for pass row (u, k) at position p = row_pos, i = p - s0 in [0, n_text[u]):
+// probs[u][i] = softmax over ids [0, eot) of the row's logits, at text[u][i]
+void align_token_probs_run(const float* logits, long long ldl, const int* row_pos, const int* text, int text_stride,
+                           const int* n_text, int n_utt, int rows_per_utt, int s0, int eot, float* probs, cudaStream_t stream);
 
 // ------------------------------------------------------------------ persistent decoder pass (decoder_mega.cu)
 struct MegaGemv {

@@ -574,6 +574,113 @@ bd_cross_attn_tc_kernel(const __grid_constant__ CUtensorMap map_kv, const float*
   }
 }
 
+// =====================================================================================================================
+// alignment capture (Whisper.align): one CTA per (alignment head of this layer, utterance).  The item's query rows are
+// rounded to fp16 after the exact 1/8 scale, as bd_cross_attn_tc_kernel feeds them to the tensor core, the scores against
+// all 1500 keys stay in shared memory, and one exact fp32 row maximum / row sum gives the probabilities the decoder itself
+// attends with.  Only rows at positions s0 .. s0 + n_text[u] and frames < n_frames[u] are written.
+// =====================================================================================================================
+constexpr int AC_THREADS = 256;
+constexpr int AC_SMEM = (MAX_BEAM * HEAD_DIM + MAX_BEAM * T_ENC) * 4;  // q [8][64] + scores [8][1500]
+
+__global__ void __launch_bounds__(AC_THREADS)
+bd_align_attn_kernel(const AlignCaptureArgs a) {
+  extern __shared__ float ac_smem[];
+  float* s_q = ac_smem;
+  float* s_p = ac_smem + MAX_BEAM * HEAD_DIM;
+  __shared__ float s_red[AC_THREADS / 32][MAX_BEAM];
+  __shared__ float s_stat[MAX_BEAM];
+  const int u = blockIdx.y, ga = a.items[blockIdx.x];
+  const int h = a.head_of[ga];
+  const int rpu = a.rows_per_utt, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int n = a.n_text[u];
+  const int* rp = a.row_pos + u * rpu;
+  // uniform over the CTA: does any row of this pass land in the captured range?
+  if (rp[rpu - 1] < a.s0 || rp[0] > a.s0 + n || n <= 0) return;
+  for (int i = tid; i < rpu * HEAD_DIM; i += AC_THREADS) {
+    const int k = i / HEAD_DIM, e = i % HEAD_DIM;
+    s_q[i] = __half2float(__float2half_rn(a.q[static_cast<long long>(u * rpu + k) * a.d + h * HEAD_DIM + e] * 0.125f));
+  }
+  __syncthreads();
+  const __half* kb = a.ck + (static_cast<long long>(u) * a.H + h) * T_ENC_PAD * HEAD_DIM;
+  float mx[MAX_BEAM];
+#pragma unroll
+  for (int k = 0; k < MAX_BEAM; ++k) mx[k] = -INFINITY;
+  for (int t = tid; t < T_ENC; t += AC_THREADS) {
+    const uint4* kr = reinterpret_cast<const uint4*>(kb + static_cast<long long>(t) * HEAD_DIM);
+    float acc[MAX_BEAM];
+#pragma unroll
+    for (int k = 0; k < MAX_BEAM; ++k) acc[k] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const uint4 uu = __ldg(kr + i);
+      const __half2* h2 = reinterpret_cast<const __half2*>(&uu);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 f = __half22float2(h2[j]);
+#pragma unroll
+        for (int k = 0; k < MAX_BEAM; ++k)
+          if (k < rpu) {
+            acc[k] = fmaf(s_q[k * HEAD_DIM + 8 * i + 2 * j], f.x, acc[k]);
+            acc[k] = fmaf(s_q[k * HEAD_DIM + 8 * i + 2 * j + 1], f.y, acc[k]);
+          }
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < MAX_BEAM; ++k)
+      if (k < rpu) {
+        s_p[k * T_ENC + t] = acc[k];
+        mx[k] = fmaxf(mx[k], acc[k]);
+      }
+  }
+#pragma unroll
+  for (int k = 0; k < MAX_BEAM; ++k) {
+    const float m = warp_max(mx[k]);
+    if (lane == 0) s_red[warp][k] = m;
+  }
+  __syncthreads();
+  if (tid < rpu) {
+    float m = -INFINITY;
+    for (int w = 0; w < AC_THREADS / 32; ++w) m = fmaxf(m, s_red[w][tid]);
+    s_stat[tid] = m;
+  }
+  __syncthreads();
+  float sum[MAX_BEAM];
+#pragma unroll
+  for (int k = 0; k < MAX_BEAM; ++k) {
+    sum[k] = 0.f;
+    if (k < rpu) {
+      const float m = s_stat[k];
+      for (int t = tid; t < T_ENC; t += AC_THREADS) {
+        const float e = expf(s_p[k * T_ENC + t] - m);
+        s_p[k * T_ENC + t] = e;
+        sum[k] += e;
+      }
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < MAX_BEAM; ++k) {
+    const float v = warp_sum(sum[k]);
+    if (lane == 0) s_red[warp][k] = v;
+  }
+  __syncthreads();
+  if (tid < rpu) {
+    float v = 0.f;
+    for (int w = 0; w < AC_THREADS / 32; ++w) v += s_red[w][tid];
+    s_stat[tid] = v;
+  }
+  __syncthreads();
+  const int F = a.n_frames[u];
+  for (int k = 0; k < rpu; ++k) {
+    const int r = rp[k] - a.s0;
+    if (r < 0 || r > n) continue;
+    const float l = s_stat[k];
+    float* dst = a.cap + ((static_cast<long long>(u) * a.A + ga) * (a.n_max + 1) + r) * a.f_max;
+    for (int f = tid; f < F; f += AC_THREADS) dst[f] = s_p[k * T_ENC + f] / l;
+  }
+}
+
 template <typename Kern, typename... Args>
 void bd_launch(Kern kern, dim3 grid, dim3 block, size_t smem, cudaStream_t stream, bool pdl, Args... args) {
   cudaLaunchConfig_t cfg{};
@@ -647,6 +754,17 @@ void run_gemm_rows(const GemmPlan& plan, int rows, int pdl, cudaStream_t s) {
 
 }  // namespace
 
+void align_capture_run(const AlignCaptureArgs& a, cudaStream_t s) {
+  WISB_REQUIRE(a.rows_per_utt >= 1 && a.rows_per_utt <= MAX_BEAM, "alignment capture: 1..8 rows per utterance");
+  if (a.n_items == 0 || a.n_utt == 0) return;
+  static std::atomic<unsigned long long> once{0};
+  once_per_device(once, [] {
+    WISB_CUDA(cudaFuncSetAttribute(bd_align_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AC_SMEM));
+  });
+  bd_align_attn_kernel<<<dim3(a.n_items, a.n_utt), AC_THREADS, AC_SMEM, s>>>(a);
+  WISB_CUDA(cudaGetLastError());
+}
+
 int batch_pass_run(const BatchArgs& a, const BatchLayer* layers, int n_layers, cudaStream_t s) {
   WISB_REQUIRE(a.R >= 1 && a.R == a.n_utt * a.rows_per_utt, "batched decoder pass: rows must be utterances x rows per utterance");
   WISB_REQUIRE(a.rows_per_utt >= 1 && a.rows_per_utt <= MAX_BEAM, "batched decoder pass: 1..8 rows per utterance");
@@ -688,6 +806,7 @@ int batch_pass_run(const BatchArgs& a, const BatchLayer* layers, int n_layers, c
     gemm(ly.o);
     ln(ly.o.k_splits, ly.ob, ly.ln2g, ly.ln2b);
     gemm(ly.cq);
+    if (a.layer_hook) n += a.layer_hook(a.hook_ctx, i, s);
     {
       Scope t(a, 1);
       cross_attn_launch(a, ly, s);

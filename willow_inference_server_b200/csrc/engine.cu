@@ -163,6 +163,12 @@ struct wisb_handle {
   DevBuf<unsigned> cross_flags;
   DevBuf<float> ln_fold;       // per LN-GEMV: s2[N] and folded bias[N] (qkv, cq, fc1 of every decoder layer, vocab)
   DevBuf<__half> fc2_chunked;  // decoder fc2 weights in chunk-major layout for the persistent pass kernel
+  // wisb_align: alignment heads ordered by layer (al_items = their blob-order index, al_layer_off[l] = first of layer l),
+  // the head of each, and the per-call workspaces
+  std::vector<int> al_layer_off;
+  int al_A = 0;
+  DevBuf<int> al_items, al_head, al_ntext, al_nframes, al_text, al_path, al_len;
+  DevBuf<float> al_cap, al_mat, al_probs;
   DevBuf<unsigned long long> mega_trace;
   int mega_trace_on = 0, mega_trace_cta = 0, mega_trace_layer = 0;
   cudaEvent_t ev_flag[2] = {nullptr, nullptr};  // decode loop: `all_done` copies of the last two steps
@@ -390,6 +396,39 @@ void finish_create(wisb_handle* h) {
     if (id >= 0 && id < d.n_vocab) mask[id] |= 1;
   for (int id : fetch_ids("meta.suppress_ids_begin"))
     if (id >= 0 && id < d.n_vocab) mask[id] |= 2;
+  {
+    // alignment heads: meta.alignment_heads [A, 2] (layer, head), else every head of the upper half of the decoder
+    std::vector<int> lh;
+    auto it = h->tensors.find("meta.alignment_heads");
+    if (it != h->tensors.end()) {
+      const TensorRef& t = it->second;
+      WISB_REQUIRE(t.dtype == 2 && t.ndim == 2 && t.shape[1] == 2 && t.shape[0] >= 1 && t.shape[0] <= 4096,
+                   "bad 'meta.alignment_heads' in the weight blob");
+      lh.resize(static_cast<size_t>(t.numel()));
+      WISB_CUDA(cudaMemcpy(lh.data(), t.ptr, lh.size() * 4, cudaMemcpyDeviceToHost));
+      for (size_t i = 0; i < lh.size(); i += 2)
+        WISB_REQUIRE(lh[i] >= 0 && lh[i] < d.n_dec_layers && lh[i + 1] >= 0 && lh[i + 1] < d.n_heads,
+                     "'meta.alignment_heads' names a head outside the decoder");
+    } else {
+      for (int l = d.n_dec_layers / 2; l < d.n_dec_layers; ++l)
+        for (int hh = 0; hh < d.n_heads; ++hh) lh.insert(lh.end(), {l, hh});
+    }
+    const int A = static_cast<int>(lh.size() / 2);
+    std::vector<int> items, heads(A);
+    h->al_layer_off.assign(d.n_dec_layers + 1, 0);
+    for (int l = 0; l < d.n_dec_layers; ++l) {
+      h->al_layer_off[l] = static_cast<int>(items.size());
+      for (int a = 0; a < A; ++a)
+        if (lh[2 * a] == l) items.push_back(a);
+    }
+    h->al_layer_off[d.n_dec_layers] = A;
+    for (int a = 0; a < A; ++a) heads[a] = lh[2 * a + 1];
+    h->al_A = A;
+    h->al_items.ensure(A);
+    h->al_head.ensure(A);
+    WISB_CUDA(cudaMemcpy(h->al_items.p, items.data(), A * 4, cudaMemcpyHostToDevice));
+    WISB_CUDA(cudaMemcpy(h->al_head.p, heads.data(), A * 4, cudaMemcpyHostToDevice));
+  }
   h->mask_base.ensure(d.n_vocab);
   h->mask_cur.ensure(d.n_vocab);
   WISB_CUDA(cudaMemcpy(h->mask_base.p, mask.data(), mask.size(), cudaMemcpyHostToDevice));
@@ -1290,6 +1329,128 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
   return steps;
 }
 
+// ------------------------------------------------------------------------------------------------- alignment
+// The capture buffer [utterances][A][n_max + 1][F_max] fp32 is the largest workspace of wisb_align (one large-v2 window with
+// the default 320 heads, 449 rows and 1500 frames: 0.86 GB): utterances are grouped so that it stays under this cap.
+constexpr size_t ALIGN_WS_BYTES = 2ull << 30;
+
+struct AlignHook {
+  wisb_handle* h;
+  AlignCaptureArgs a;  // everything but this layer's cross K and heads
+};
+
+int align_hook(void* ctx, int layer, cudaStream_t s) {
+  AlignHook* k = static_cast<AlignHook*>(ctx);
+  wisb_handle* h = k->h;
+  const int i0 = h->al_layer_off[layer], i1 = h->al_layer_off[layer + 1];
+  if (i0 == i1) return 0;
+  AlignCaptureArgs a = k->a;
+  a.items = h->al_items.p + i0;
+  a.n_items = i1 - i0;
+  a.ck = h->bd_layers[layer].ck;
+  h->prof_begin(5);
+  align_capture_run(a, s);
+  h->prof_end();
+  return 1;
+}
+
+// one group of utterances [g0, g0 + n) whose cross K/V are in h->ckv (encoded as a batch of n): teacher-forced passes with
+// the capture hook, token probabilities, filter, DTW, results to the caller's arrays
+void align_group(wisb_handle* h, int g0, int n, const int32_t* start_seq, int S, const int32_t* text, const int32_t* text_len,
+                 int text_stride, const int32_t* num_frames, int width, int n_max, int f_max, int32_t* out_path,
+                 int path_stride, int32_t* out_path_len, float* out_token_probs, float* cap_out) {
+  const Dims& dm = h->dims;
+  cudaStream_t s = h->stream;
+  const int A = h->al_A;
+  int n_grp = 0;
+  for (int u = 0; u < n; ++u) n_grp = std::max(n_grp, static_cast<int>(text_len[g0 + u]));
+  const int total = S + 1 + n_grp;
+  int P = round_up(total, MAX_BEAM);
+  if (P > dm.n_text_ctx) P = dm.n_text_ctx;
+  ensure_batch(h, n * MAX_BEAM, P);
+  const size_t head_block = static_cast<size_t>(dm.n_heads) * T_ENC_PAD * HEAD_DIM;
+  for (int i = 0; i < dm.n_dec_layers; ++i) {
+    h->bd_layers[i].ck = h->ckv.p + static_cast<size_t>(i * 2 + 0) * n * head_block;
+    h->bd_layers[i].cv = h->ckv.p + static_cast<size_t>(i * 2 + 1) * n * head_block;
+  }
+  // teacher-forced tokens [n][P]: start_seq, <|notimestamps|>, text; rows past an utterance's end feed <|endoftext|>
+  // (causal attention keeps the rows before them exact; their outputs are not read)
+  const int ts = std::max(text_stride, 1);
+  std::vector<int> tok(static_cast<size_t>(n) * P, dm.eot), nt(n), nf(n), txt(static_cast<size_t>(n) * ts, 0);
+  for (int u = 0; u < n; ++u) {
+    int* t = tok.data() + static_cast<size_t>(u) * P;
+    std::copy(start_seq, start_seq + S, t);
+    t[S] = dm.no_timestamps;
+    nt[u] = text_len[g0 + u];
+    nf[u] = num_frames[g0 + u] / 2;
+    for (int i = 0; i < nt[u]; ++i) t[S + 1 + i] = txt[static_cast<size_t>(u) * ts + i] = text[static_cast<size_t>(g0 + u) * text_stride + i];
+  }
+  h->al_ntext.ensure(n);
+  h->al_nframes.ensure(n);
+  h->al_text.ensure(static_cast<size_t>(n) * ts);
+  h->al_cap.ensure(static_cast<size_t>(n) * A * (n_max + 1) * f_max);
+  h->al_mat.ensure(static_cast<size_t>(n) * (n_max + 1) * f_max);
+  h->al_probs.ensure(static_cast<size_t>(n) * ts);
+  h->al_path.ensure(static_cast<size_t>(n) * path_stride * 2);
+  h->al_len.ensure(n);
+  WISB_CUDA(cudaMemcpyAsync(h->prompt_dev.p, tok.data(), tok.size() * 4, cudaMemcpyHostToDevice, s));
+  WISB_CUDA(cudaMemcpyAsync(h->al_ntext.p, nt.data(), n * 4, cudaMemcpyHostToDevice, s));
+  WISB_CUDA(cudaMemcpyAsync(h->al_nframes.p, nf.data(), n * 4, cudaMemcpyHostToDevice, s));
+  WISB_CUDA(cudaMemcpyAsync(h->al_text.p, txt.data(), txt.size() * 4, cudaMemcpyHostToDevice, s));
+  WISB_CUDA(cudaMemsetAsync(h->al_probs.p, 0, static_cast<size_t>(n) * ts * 4, s));
+  AlignHook hook{h, AlignCaptureArgs()};
+  hook.a.head_of = h->al_head.p;
+  hook.a.n_text = h->al_ntext.p;
+  hook.a.n_frames = h->al_nframes.p;
+  hook.a.cap = h->al_cap.p;
+  hook.a.q = h->bq.p;
+  hook.a.row_pos = h->row_pos.p;
+  hook.a.n_utt = n;
+  hook.a.d = dm.d_model;
+  hook.a.H = dm.n_heads;
+  hook.a.A = A;
+  hook.a.s0 = S;
+  hook.a.n_max = n_max;
+  hook.a.f_max = f_max;
+  DecodeCfg c{};
+  c.n_utt = n;
+  c.B_total = n;
+  for (int p0 = 0; p0 < P; p0 += MAX_BEAM) {
+    const int chunk = std::min(MAX_BEAM, P - p0);
+    prefill_rows_run(h->tokens.p, h->row_pos.p, h->row_slot.p, h->prompt_dev.p, P, n, p0, chunk, 1, s);
+    BatchArgs a = make_batch_args(h, c);
+    a.R = n * chunk;
+    a.rows_per_utt = chunk;
+    a.prefill = 1;
+    a.with_logits = 1;
+    hook.a.rows_per_utt = chunk;
+    a.layer_hook = align_hook;
+    a.hook_ctx = &hook;
+    h->launches += 2 + batch_pass_run(a, h->bd_layers.data(), dm.n_dec_layers, s);
+    align_token_probs_run(h->blogits.p, dm.n_vocab_pad, h->row_pos.p, h->al_text.p, ts, h->al_ntext.p, n, chunk, S, dm.eot,
+                          h->al_probs.p, s);
+    h->timing[6] += 1.f;
+  }
+  WISB_CUDA(cudaEventRecord(h->ev[4], s));
+  if (cap_out)  // (stream-ordered before the filter standardises the buffer in place)
+    WISB_CUDA(cudaMemcpyAsync(cap_out + static_cast<size_t>(g0) * A * (n_max + 1) * f_max, h->al_cap.p,
+                              static_cast<size_t>(n) * A * (n_max + 1) * f_max * 4, cudaMemcpyDeviceToHost, s));
+  align_filter_run(h->al_cap.p, h->al_mat.p, h->al_ntext.p, h->al_nframes.p, n, A, n_max, f_max, width, s);
+  WISB_CUDA(cudaEventRecord(h->ev[5], s));
+  align_dtw_run(h->al_mat.p, h->al_ntext.p, h->al_nframes.p, n, n_max, f_max, h->al_path.p, path_stride, h->al_len.p, s);
+  WISB_CUDA(cudaEventRecord(h->ev[6], s));
+  h->launches += 3;
+  WISB_CUDA(cudaMemcpyAsync(out_path + static_cast<size_t>(g0) * path_stride * 2, h->al_path.p,
+                            static_cast<size_t>(n) * path_stride * 2 * 4, cudaMemcpyDeviceToHost, s));
+  WISB_CUDA(cudaMemcpyAsync(out_path_len + g0, h->al_len.p, n * 4, cudaMemcpyDeviceToHost, s));
+  if (text_stride > 0)
+    WISB_CUDA(cudaMemcpy2DAsync(out_token_probs + static_cast<size_t>(g0) * text_stride, text_stride * 4, h->al_probs.p, ts * 4,
+                                text_stride * 4, n, cudaMemcpyDeviceToHost, s));
+  WISB_CUDA(cudaStreamSynchronize(s));
+  for (int u = 0; u < n; ++u)
+    if (nt[u] == 0) out_path_len[g0 + u] = 0;
+}
+
 template <typename Fn>
 int guarded(wisb_handle* h, Fn&& fn) {
   try {
@@ -1919,6 +2080,146 @@ int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, const 
     WISB_CUDA(cudaMemcpyAsync(cand_idx, d_ci.p, sizeof(int) * n_utt * MAX_CAND, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaMemcpyAsync(cand_score, d_cs.p, sizeof(float) * n_utt * MAX_CAND, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaMemcpyAsync(row_lse, d_lse.p, sizeof(float) * R, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+// wisb_align's body; cap_out (wisb_debug_align_capture) receives the raw capture buffer [B][A][n_max + 1][F_max]
+static void align_impl(wisb_handle* h, const float* mel, int B, const int32_t* start_seq, int start_len, const int32_t* text,
+                       const int32_t* text_len, int text_stride, const int32_t* num_frames, int median_filter_width,
+                       int32_t* out_path, int path_stride, int32_t* out_path_len, float* out_token_probs, float* cap_out) {
+    const Dims& dm = h->dims;
+    WISB_REQUIRE(h->blob != nullptr, "handle has no model (created by wisb_create_frontend)");
+    WISB_REQUIRE(B >= 1 && B <= 4096, "B out of range");
+    WISB_REQUIRE(start_seq != nullptr && text_len != nullptr && num_frames != nullptr && out_path != nullptr &&
+                 out_path_len != nullptr && out_token_probs != nullptr, "NULL argument");
+    WISB_REQUIRE(start_len >= 1 && start_seq[0] == dm.sot, "start_sequence must begin with <|startoftranscript|>");
+    for (int i = 0; i < start_len; ++i)
+      WISB_REQUIRE(start_seq[i] >= 0 && start_seq[i] < dm.no_timestamps,
+                   "start_sequence must not contain <|notimestamps|> or timestamp tokens");
+    WISB_REQUIRE(median_filter_width >= 1 && median_filter_width <= 31 && median_filter_width % 2 == 1,
+                 "median_filter_width must be odd and in [1, 31]");
+    WISB_REQUIRE(text_stride >= 0 && path_stride >= 0, "negative stride");
+    int n_max = 0, f_max = 0;
+    for (int b = 0; b < B; ++b) {
+      const int n = text_len[b];
+      WISB_REQUIRE(n >= 0 && n <= text_stride && (n == 0 || text != nullptr), "text_len out of range");
+      WISB_REQUIRE(start_len + 1 + n <= dm.n_text_ctx, "start_sequence + <|notimestamps|> + text exceeds n_text_ctx");
+      for (int i = 0; i < n; ++i) {
+        const int t = text[static_cast<size_t>(b) * text_stride + i];
+        WISB_REQUIRE(t >= 0 && t < dm.eot, "text token outside [0, eot)");
+      }
+      WISB_REQUIRE(num_frames[b] >= 2 && num_frames[b] <= N_FRAMES, "num_frames must be in [2, 3000]");
+      if (n > 0) {
+        // a finite matrix gives at most n + F entries; NaN columns (a frame whose probabilities are equal in every row)
+        // can route the path along row n to frame 0 and up: n + F + 1
+        WISB_REQUIRE(path_stride >= n + num_frames[b] / 2 + 1, "path_stride smaller than len(text) + num_frames // 2 + 1");
+        n_max = std::max(n_max, n);
+        f_max = std::max(f_max, num_frames[b] / 2);
+      }
+    }
+    for (int b = 0; b < B; ++b) out_path_len[b] = 0;
+    if (text_stride > 0) std::fill(out_token_probs, out_token_probs + static_cast<size_t>(B) * text_stride, 0.f);
+    for (int i = 1; i <= 7; ++i) h->timing[i] = 0.f;
+    h->timing[13] = h->timing[14] = 0.f;
+    if (n_max == 0) return;  // no text anywhere: nothing to align
+    cudaStream_t s = h->stream;
+    h->launches = 0;
+    WISB_CUDA(cudaEventRecord(h->ev[0], s));
+    bool reuse = upload_mel(h, mel, B);
+    h->ckv_sw = 0;  // the capture and the batched pass read the cross K/V linear
+    WISB_CUDA(cudaEventRecord(h->ev[2], s));
+    WISB_CUDA(cudaEventSynchronize(h->ev[2]));
+    WISB_CUDA(cudaEventElapsedTime(&h->timing[1], h->ev[0], h->ev[2]));
+    const size_t per_utt = static_cast<size_t>(h->al_A) * (n_max + 1) * f_max * sizeof(float);
+    int group = std::min(h->batch_rows / MAX_BEAM, static_cast<int>(std::min<size_t>(ALIGN_WS_BYTES / per_utt, 4096)));
+    if (group < 1) group = 1;
+    if (reuse && group < B) reuse = false;
+    for (int g0 = 0; g0 < B; g0 += group) {
+      const int n = std::min(group, B - g0);
+      WISB_CUDA(cudaEventRecord(h->ev[2], s));
+      if (reuse) {
+        if (h->ckv_is_sw) {  // left chunk-swizzled by a <= 8-row generate: rerun only the cross-K/V GEMM, linear
+          ensure_encoder(h, B);
+          h->plan_ckv.epi.kv_swizzle = 0;
+          gemm_run(h->plan_ckv, s);
+          h->ckv_is_sw = 0;
+          h->launches += 1;
+        }
+      } else {
+        run_encoder(h, n, -1, true, g0);
+        h->enc_valid = h->encoder_cache != 0 && h->mel_cache_B == B && n == B;
+      }
+      WISB_CUDA(cudaEventRecord(h->ev[3], s));
+      align_group(h, g0, n, start_seq, start_len, text, text_len, text_stride, num_frames, median_filter_width, n_max, f_max,
+                  out_path, path_stride, out_path_len, out_token_probs, cap_out);
+      float t;
+      WISB_CUDA(cudaEventElapsedTime(&t, h->ev[2], h->ev[3]));
+      h->timing[2] += t;
+      WISB_CUDA(cudaEventElapsedTime(&t, h->ev[3], h->ev[4]));
+      h->timing[3] += t;
+      WISB_CUDA(cudaEventElapsedTime(&t, h->ev[4], h->ev[5]));
+      h->timing[4] += t;
+      WISB_CUDA(cudaEventElapsedTime(&t, h->ev[5], h->ev[6]));
+      h->timing[14] += t;
+    }
+    WISB_CUDA(cudaEventElapsedTime(&h->timing[5], h->ev[0], h->ev[6]));
+    h->timing[7] = static_cast<float>(h->launches);
+    const float dtw = h->timing[14];
+    h->prof_collect();  // (capture kernels are profile category 5 -> timing[13])
+    h->timing[14] = dtw;
+}
+
+int wisb_align(wisb_handle* h, const float* mel, int B, const int32_t* start_seq, int start_len, const int32_t* text,
+               const int32_t* text_len, int text_stride, const int32_t* num_frames, int median_filter_width,
+               int32_t* out_path, int path_stride, int32_t* out_path_len, float* out_token_probs) {
+  return guarded(h, [&] {
+    align_impl(h, mel, B, start_seq, start_len, text, text_len, text_stride, num_frames, median_filter_width, out_path,
+               path_stride, out_path_len, out_token_probs, nullptr);
+  });
+}
+
+int wisb_debug_align_capture(wisb_handle* h, const float* mel, int B, const int32_t* start_seq, int start_len,
+                             const int32_t* text, const int32_t* text_len, int text_stride, const int32_t* num_frames,
+                             float* cap_out) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(cap_out != nullptr && text_len != nullptr && num_frames != nullptr && B >= 1 && B <= 4096, "bad arguments");
+    int stride = 1;
+    for (int b = 0; b < B; ++b) stride = std::max(stride, text_len[b] + num_frames[b] / 2 + 1);
+    std::vector<int32_t> path(static_cast<size_t>(B) * stride * 2), len(B);
+    std::vector<float> probs(static_cast<size_t>(B) * std::max(text_stride, 1));
+    align_impl(h, mel, B, start_seq, start_len, text, text_len, text_stride, num_frames, 7, path.data(), stride, len.data(),
+               probs.data(), cap_out);
+  });
+}
+
+int wisb_debug_align_post(wisb_handle* h, const float* weights, int A, int R, int F, int width, int dtw_only,
+                          float* matrix_out, int32_t* path_out, int32_t* path_len) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(weights != nullptr && path_out != nullptr && path_len != nullptr, "NULL argument");
+    WISB_REQUIRE(R >= 2 && R <= T_MAX + 1 && F >= 1 && F <= T_ENC && A >= 1 && A <= 4096, "debug_align_post: bad shape");
+    WISB_REQUIRE(!dtw_only || A == 1, "debug_align_post: dtw_only takes one matrix (A = 1)");
+    WISB_REQUIRE(dtw_only || (width >= 1 && width <= 31 && width % 2 == 1), "median filter width must be odd and in [1, 31]");
+    cudaStream_t s = h->stream;
+    const size_t cells = static_cast<size_t>(R) * F;
+    DevBuf<float> cap, mat;
+    DevBuf<int> meta, path;
+    mat.ensure(cells);
+    meta.ensure(3);
+    path.ensure(static_cast<size_t>(R + F) * 2, true);
+    const int nt_nf[2] = {R - 1, F};
+    WISB_CUDA(cudaMemcpyAsync(meta.p, nt_nf, sizeof(nt_nf), cudaMemcpyHostToDevice, s));
+    if (dtw_only) {
+      WISB_CUDA(cudaMemcpyAsync(mat.p, weights, cells * 4, cudaMemcpyHostToDevice, s));
+    } else {
+      cap.ensure(cells * A);
+      WISB_CUDA(cudaMemcpyAsync(cap.p, weights, cells * A * 4, cudaMemcpyHostToDevice, s));
+      align_filter_run(cap.p, mat.p, meta.p, meta.p + 1, 1, A, R - 1, F, width, s);
+    }
+    align_dtw_run(mat.p, meta.p, meta.p + 1, 1, R - 1, F, path.p, R + F, meta.p + 2, s);
+    if (matrix_out) WISB_CUDA(cudaMemcpyAsync(matrix_out, mat.p, cells * 4, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(path_out, path.p, static_cast<size_t>(R + F) * 2 * 4, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(path_len, meta.p + 2, 4, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaStreamSynchronize(s));
   });
 }

@@ -63,6 +63,8 @@ def dims_from_hf_config(cfg: dict, gen_cfg: dict | None = None) -> W.WhisperDims
     beg = gen_cfg.get("begin_suppress_tokens", cfg.get("begin_suppress_tokens"))
     if beg:
         dims.suppress_ids_begin = [int(v) for v in beg]
+    if gen_cfg.get("alignment_heads"):
+        dims.alignment_heads = [[int(a), int(b)] for a, b in gen_cfg["alignment_heads"]]
     dims.validate()
     return dims
 
@@ -276,6 +278,8 @@ def load_ct2_dir(path: str):
         if cfg.get("lang_ids"):
             ids = sorted(int(x) for x in cfg["lang_ids"])
             dims.lang_first, dims.n_langs = ids[0], len(ids)
+        if cfg.get("alignment_heads"):
+            dims.alignment_heads = [[int(a), int(b)] for a, b in cfg["alignment_heads"]]
     dims.validate()
     return dims, W.pack_state_dict(ct2_to_hf_state_dict(variables, aliases, dims), dims)
 

@@ -59,6 +59,12 @@ class WhisperGenerationResult:
         return [[str(t) for t in seq] for seq in self.sequences_ids]
 
 
+@dataclass
+class WhisperAlignmentResult:
+    alignments: list  # list[tuple[int, int]]: (text token index, encoder frame) along the DTW path
+    text_token_probs: list  # list[float]
+
+
 def get_supported_compute_types(device: str, device_index: int = 0):
     """main.py:454 only logs this.  One compute path exists: fp16 weights/activations, fp32 accumulation."""
     if device != "cuda":
@@ -215,6 +221,37 @@ class Whisper:
                 out.append([(f"<|{LANGUAGE_CODES[int(t) - first]}|>" if int(t) - first < len(LANGUAGE_CODES) else f"<|{int(t)}|>",
                              float(pr)) for t, pr in zip(row_ids, row_p)])
         return out
+
+    def align(self, features, start_sequence, text_tokens, num_frames, median_filter_width: int = 7):
+        """ctranslate2.models.Whisper.align: per window, the DTW path from text tokens to encoder frames over the
+        alignment heads' cross-attention, and each text token's probability.  The decoder is teacher-forced with
+        start_sequence + [<|notimestamps|>] + text_tokens[b]; num_frames is an int or one int per window (feature frames,
+        the path covers num_frames // 2 encoder frames).  Word grouping needs a tokenizer and stays with the caller."""
+        mel = _features_array(features)
+        n = mel.shape[0]
+        if len(text_tokens) != n:
+            raise ValueError(f"expected {n} text token lists (one per feature window), got {len(text_tokens)}")
+        if any(isinstance(t, str) for seq in text_tokens for t in seq) or any(isinstance(t, str) for t in start_sequence):
+            raise ValueError("start_sequence and text_tokens must be token ids")
+        if np.isscalar(num_frames):
+            nf = np.full(n, int(num_frames), np.int64)
+        else:
+            nf = np.asarray(num_frames, np.int64)
+            if nf.shape != (n,):
+                raise ValueError("num_frames must be an int or one int per feature window")
+        if (nf < 2).any() or (nf > 3000).any():
+            raise ValueError("num_frames must be in [2, 3000]")
+        text = [list(t) for t in text_tokens]
+        start = list(start_sequence)
+
+        def job(i, s, e):
+            return lambda: self._handles[i].align(mel[s:e], start, text[s:e], nf[s:e], median_filter_width)
+
+        results = []
+        for paths, probs in self._run([job(*pt) for pt in self._split(n, mel)]):
+            for p, pr in zip(paths, probs):
+                results.append(WhisperAlignmentResult([(int(a), int(b)) for a, b in p], [float(v) for v in pr]))
+        return results
 
     def timing(self, replica: int = 0) -> dict:
         return self._handles[replica].timing()

@@ -77,6 +77,9 @@ class WhisperDims:
     n_langs: int = 99
     suppress_ids: list = field(default_factory=lambda: list(NON_SPEECH_TOKENS_MULTI))
     suppress_ids_begin: list = field(default_factory=lambda: [220, 50257])
+    # (layer, head) pairs whose cross-attention Whisper.align uses; None = the engine's default (every head of the upper
+    # half of the decoder) and no blob tensor, so models without named heads serialise exactly as before
+    alignment_heads: list | None = None
 
     @property
     def n_vocab_pad(self) -> int:
@@ -192,6 +195,12 @@ def pack_state_dict(sd: dict, dims: WhisperDims) -> dict:
     out["meta.suppress_ids"] = np.asarray(sorted(set(dims.suppress_ids)), np.int32)
     out["meta.suppress_ids_begin"] = np.asarray(dims.suppress_ids_begin, np.int32)
     out["meta.lang_ids"] = np.asarray(dims.lang_ids, np.int32)
+    if dims.alignment_heads:
+        heads = np.asarray(dims.alignment_heads, np.int32).reshape(-1, 2)
+        if (heads[:, 0] < 0).any() or (heads[:, 0] >= dims.n_dec_layers).any() or (heads[:, 1] < 0).any() \
+                or (heads[:, 1] >= dims.n_heads).any():
+            raise ValueError("alignment_heads names a (layer, head) outside the decoder")
+        out["meta.alignment_heads"] = np.ascontiguousarray(heads)
     return out
 
 
@@ -200,7 +209,7 @@ def pack_state_dict(sd: dict, dims: WhisperDims) -> dict:
 # ---------------------------------------------------------------------------
 def synth_state_dict(dims: WhisperDims, seed: int = 0, logit_std: float = 4.0, qk_gain: float = 2.5,
                      resid_std: float = 8.0, eot_ramp: tuple | None = None, script: tuple | None = None,
-                     ts_script: tuple | None = None) -> dict:
+                     ts_script: tuple | None = None, align_script: tuple | None = None) -> dict:
     """Deterministic random Whisper weights under HF names.
 
     Every GEMM weight is rounded to float16 so oracle (fp32 math) and engine
@@ -229,6 +238,11 @@ def synth_state_dict(dims: WhisperDims, seed: int = 0, logit_std: float = 4.0, q
     text token, their log-sum-exp above it); one position later a lower timestamp at 0.9 and the window again at 0.8 (the
     non-decreasing rule decides); one more position later the next timestamps at 1.1 (the pair rule turns them off).
     The windows move up 40 indices per boundary.  ``None`` leaves the model byte-identical to one built without it.
+
+    ``align_script=(step, gain, amp)`` gives the alignment heads (``dims.alignment_heads``, else every head of the upper
+    half of the decoder) a sharp cross-attention peak at encoder frame ``step * p`` for decoder position p, so that
+    Whisper.align's DTW paths are non-trivial and robust (a random model attends almost uniformly); see ``_align_script``.
+    ``None`` leaves the model byte-identical to one built without it.
     """
     dims.validate()
     d = dims.d_model
@@ -379,7 +393,47 @@ def synth_state_dict(dims: WhisperDims, seed: int = 0, logit_std: float = 4.0, q
         u = emb[dims.eot] / np.linalg.norm(emb[dims.eot])
         ramp = np.maximum(0.0, np.arange(dims.n_text_ctx, dtype=np.float32) - p0) * np.float32(slope)
         sd[dd + "embed_positions.weight"] = (sd[dd + "embed_positions.weight"] + ramp[:, None] * u[None, :]).astype(np.float32)
+    if align_script is not None:
+        _align_script(sd, dims, *align_script)
     return sd
+
+
+def _align_script(sd: dict, dims: WhisperDims, step: float, gain: float, amp: float):
+    """Sharp, monotone cross-attention peaks for the alignment heads (see ``synth_state_dict(align_script=...)``).
+
+    Encoder: channels 0 / 1 of the positional table get ``amp * (sin, cos)(w t)``, w = pi / 1500, so that they dominate
+    the encoder output's LayerNorm and enc_out[:, 0 / 1] ~ sqrt(d) (sin, cos)(w t).  Decoder: channels 0 / 1 of the
+    positional table get ``amp * (sin, cos)(w t*(p))`` with t*(p) = step * p.  Each alignment head's query reads decoder
+    channels 0 / 1 and its key encoder channels 0 / 1 (the head's other 62 query / key rows are zero), so its score is
+    ~ gain * cos(w (t - t*(p))): one peak at frame t*(p), of width ~ 1 / (w sqrt(gain))."""
+    d = dims.d_model
+    w = np.pi / T_ENC
+    e, dd = "model.encoder.", "model.decoder."
+    t = np.arange(T_ENC, dtype=np.float64)
+    ep = sd[e + "embed_positions.weight"].astype(np.float64)
+    ep[:, 0] += amp * np.sin(w * t)
+    ep[:, 1] += amp * np.cos(w * t)
+    sd[e + "embed_positions.weight"] = ep.astype(np.float32)
+    tp = step * np.arange(dims.n_text_ctx, dtype=np.float64)
+    dp = sd[dd + "embed_positions.weight"].astype(np.float64)
+    dp[:, 0] += amp * np.sin(w * tp)
+    dp[:, 1] += amp * np.cos(w * tp)
+    sd[dd + "embed_positions.weight"] = dp.astype(np.float32)
+    # LayerNorm output in the two dominating channels ~ sqrt(d) (sin, cos); score = q . k / 8 = c^2 d cos / 8
+    c = float(np.sqrt(8.0 * gain / d))
+    heads = dims.alignment_heads or [[l, h] for l in range(dims.n_dec_layers // 2, dims.n_dec_layers)
+                                     for h in range(dims.n_heads)]
+    for layer, head in heads:
+        p = f"{dd}layers.{layer}.encoder_attn."
+        rows = slice(64 * head, 64 * head + 64)
+        for name in ("q_proj.weight", "k_proj.weight"):
+            m = sd[p + name].copy()
+            m[rows] = 0.0
+            m[64 * head, 0] = m[64 * head + 1, 1] = np.float32(np.float16(c))
+            sd[p + name] = m
+        b = sd[p + "q_proj.bias"].copy()
+        b[rows] = 0.0
+        sd[p + "q_proj.bias"] = b
 
 
 def synth_engine_tensors(dims: WhisperDims, seed: int = 0, **kw) -> dict:
@@ -457,6 +511,8 @@ def read_blob(src) -> tuple:
     dims = WhisperDims(**hv)
     dims.suppress_ids = [int(v) for v in tensors["meta.suppress_ids"]]
     dims.suppress_ids_begin = [int(v) for v in tensors["meta.suppress_ids_begin"]]
+    if "meta.alignment_heads" in tensors:
+        dims.alignment_heads = [[int(a), int(b)] for a, b in tensors["meta.alignment_heads"]]
     return dims, tensors
 
 
