@@ -143,6 +143,36 @@ int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, const 
 /* encoder self-attention on caller data: qkv [B*1536, 3d] fp16 -> ctx [B*1536, d] fp16, d = 64 H; impl 0 = wgmma with
  * MN-major V, 1 = wgmma with the transposed Vt layout (built from the same qkv), 2 = SIMT check */
 int wisb_debug_enc_attn(wisb_handle* h, const uint16_t* qkv16, int B, int d, int H, int impl, uint16_t* ctx16_out);
+/* The batched decoder pass's own kernels on caller data, launched exactly as the pass launches them (without
+ * programmatic dependent launch).  fp16 arrays are raw uint16.  Outputs are uploaded before the launch and downloaded
+ * after it, so elements the kernel must not write keep what the caller put there.  Every index a kernel can form is
+ * checked against the sizes given here first: a bad argument returns 1 and launches nothing. */
+/* cross-attention.  prm[6] int32: n_utt (1..1024), rows_per_utt (1..8), H (1..32), n_layers, layer, impl (0 = wgmma
+ * kernel through a tensor map over the whole buffer, 1 = SIMT cluster kernel).  d = 64 H.  q float32 [n_utt *
+ * rows_per_utt, d] (unscaled), ckv [n_layers][2 (K, V)][n_utt][H][1536][64] (keys >= 1500 are padding), done int32
+ * [n_utt] or NULL (finished utterances are skipped), ctx [n_utt * rows_per_utt, d] in / out. */
+int wisb_debug_dec_cross_attn(wisb_handle* h, const int32_t* prm, int n_prm, const float* q, const uint16_t* ckv,
+                              const int32_t* done, uint16_t* ctx16);
+/* self-attention over a beam-indirected cache.  prm[8] int32: R, H (1..32), n_slots, t_cap, t_ind (<= 448),
+ * rows_per_utt (1..8, divides R), prefill (0/1), flip (0/1: which indirection table is current).  d = 64 H.  q float32
+ * [R, d], kcache / vcache [n_slots][t_cap][d], row_pos / row_slot int32 [R] (row_pos < min(t_cap, t_ind)), indir0 /
+ * indir1 int32 [R][t_ind] (slots), done int32 [R / rows_per_utt] or NULL, ctx [R, d] in / out.  Row r attends positions
+ * t <= row_pos[r]: slot indir[r][t] for t < row_pos[r], its own slot row_slot[r] at t = row_pos[r] (and at every t with
+ * prefill). */
+int wisb_debug_dec_self_attn(wisb_handle* h, const int32_t* prm, int n_prm, const float* q, const uint16_t* kcache,
+                             const uint16_t* vcache, const int32_t* row_pos, const int32_t* row_slot, const int32_t* indir0,
+                             const int32_t* indir1, const int32_t* done, uint16_t* ctx16);
+/* split-K reduction + bias + residual + LayerNorm: x[r] += ((bias + slab 0) + slab 1) + ..., xn = LN(x) (fp16).
+ * d % 128 == 0, d <= 1536; n_splits 1, 2, 4 or 8 slabs of [R, d] float32 at part + s * split_stride (split_stride % 4
+ * == 0, >= R d when n_splits > 1, part_elems >= (n_splits - 1) split_stride + R d); bias, g, b float32 [d]; x float32
+ * [cap, d] and xn [cap, d] in / out (cap >= R: rows R .. cap - 1 must come back untouched). */
+int wisb_debug_dec_resid_ln(wisb_handle* h, int R, int cap, int d, int n_splits, int64_t split_stride, const float* part,
+                            size_t part_elems, const float* bias, const float* g, const float* b, float* x, uint16_t* xn16);
+/* token + position embedding + LayerNorm: x[r] = float(tok_emb[tokens[r]]) + pos_emb[row_pos[r]], xn = LN(x).  tok_emb
+ * [n_vocab, d] fp16, pos_emb [n_pos, d] float32, g, b float32 [d]; x float32 [cap, d] and xn [cap, d] in / out (cap >= R). */
+int wisb_debug_dec_embed_ln(wisb_handle* h, int R, int cap, int d, int n_vocab, int n_pos, const int32_t* tokens, const int32_t* row_pos,
+                            const uint16_t* tok_emb, const float* pos_emb, const float* g, const float* b, float* x,
+                            uint16_t* xn16);
 /* the wgmma skinny-GEMV building block of the decoder pass on caller data: out[R,N] (float32) = x[R,K] (float32, rounded
  * to fp16 inside) . W[N,K]^T (fp16 as raw uint16) + bias (may be NULL); R <= 8, K % 64 == 0, K <= 5120.  avg_us (may be
  * NULL) receives the average kernel time over `iters` back-to-back launches. */

@@ -9,6 +9,7 @@ and what BASELINE.json configs[2] / configs[3] (batch 64 / 512) measure.
     oracle on every robust case (tests/gpu_common.robust_cases)
   * per-utterance length limits in one shared pass == separate calls
   * row capacity smaller than the batch (groups) == one group
+  * batch_rows = 1024 at beam 1: 520 windows in one shared pass equal the oracle on robust cases
 """
 import numpy as np
 import pytest
@@ -153,6 +154,26 @@ def test_greedy16_both_cross_attention_kernels_match_oracle(pair, prompt):
             h.set_option("cross_tc", 1)
         for i in robust:
             assert ids[i] == res[i].sequences_ids[0], (tc, i)
+
+
+def test_greedy_pass_above_512_utterances(pair):
+    # batch_rows = 1024 at beam 1 puts 520 windows into ONE shared pass (one row each): the cross-attention takes up to
+    # 1024 utterances per launch.  Every copy of a robust window equals the oracle; copies of a window are identical.
+    dims, oracle, h = pair
+    mel16 = mel_inputs(16)
+    res, robust = robust_cases(oracle, mel16, [PROMPT] * 16, 1, n_probe=2, max_length=24)
+    assert len(robust) >= 10, f"only {len(robust)} of 16 oracle transcripts are robust decisions"
+    n = 520
+    mel = np.ascontiguousarray(np.tile(mel16, (n // 16 + 1, 1, 1))[:n])
+    h.set_option("batch_rows", 1024)
+    try:
+        ids, _ = h.generate(mel, np.asarray([PROMPT] * n, np.int32), beam_size=1, max_length=24)
+    finally:
+        h.set_option("batch_rows", 320)
+    for i in range(n):
+        assert ids[i] == ids[i % 16], i
+    for i in robust:
+        assert ids[i] == res[i].sequences_ids[0], i
 
 
 def test_row_capacity_groups(pair):

@@ -54,6 +54,13 @@ _SIGS = {
     "wisb_debug_search_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_enc_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "wisb_debug_dec_cross_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wisb_debug_dec_self_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wisb_debug_dec_resid_ln": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_size_t,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wisb_debug_dec_embed_ln": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_gemv_tc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                       C.c_void_p]),
     "wisb_debug_read_trace": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
@@ -367,6 +374,87 @@ class Handle:
         ctx = np.zeros((B, 1536, d), np.float16)
         check(lib().wisb_debug_enc_attn(self._h, ptr(qkv16), B, d, n_heads, impl, ptr(ctx)))
         return ctx
+
+    # the batched decoder pass's own kernels (csrc/decoder_batch.cu) on caller data.  Output arrays are updated in place:
+    # elements the kernel does not write keep their values.
+    @staticmethod
+    def _inout(a, dtype, shape, name):
+        if not isinstance(a, np.ndarray) or a.dtype != dtype or a.shape != shape or not a.flags["C_CONTIGUOUS"]:
+            raise ValueError(f"{name} must be a C-contiguous {np.dtype(dtype).name} array of shape {shape}")
+        return a
+
+    def debug_dec_cross_attn(self, q, ckv, ctx, *, layer: int, rows_per_utt: int, impl: int = 0, done=None):
+        """Cross-attention: q float32 [n_utt * rows_per_utt, d] (unscaled), ckv float16 [n_layers, 2 (K, V), n_utt, H,
+        1536, 64], ctx float16 [n_utt * rows_per_utt, d] in / out, done int [n_utt] or None.  impl 0 = wgmma, 1 = SIMT
+        cluster kernel."""
+        if not isinstance(ckv, np.ndarray) or ckv.dtype != np.float16 or ckv.ndim != 6 or ckv.shape[1] != 2 \
+                or ckv.shape[4:] != (1536, 64) or not ckv.flags["C_CONTIGUOUS"]:
+            raise ValueError("ckv must be a C-contiguous float16 array [n_layers, 2, n_utt, H, 1536, 64]")
+        L, _, n_utt, H = ckv.shape[:4]
+        shape = (n_utt * rows_per_utt, 64 * H)
+        q = self._inout(np.ascontiguousarray(q, np.float32), np.float32, shape, "q")
+        self._inout(ctx, np.float16, shape, "ctx")
+        done = None if done is None else np.ascontiguousarray(np.asarray(done, np.int32).reshape(n_utt))
+        prm = np.asarray([n_utt, rows_per_utt, H, L, layer, impl], np.int32)
+        check(lib().wisb_debug_dec_cross_attn(self._h, ptr(prm), prm.size, ptr(q), ptr(ckv), ptr(done), ptr(ctx)))
+        return ctx
+
+    def debug_dec_self_attn(self, q, kcache, vcache, row_pos, row_slot, indir0, indir1, ctx, *, rows_per_utt: int,
+                            flip: int, prefill: bool = False, done=None):
+        """Self-attention over the cache: q float32 [R, d], kcache / vcache float16 [n_slots, t_cap, d], row_pos /
+        row_slot int [R], indir0 / indir1 int [R, t_ind], ctx float16 [R, d] in / out, done int [R / rows_per_utt] or
+        None; flip selects indir1."""
+        q = np.ascontiguousarray(q, np.float32)
+        R, d = q.shape
+        n_slots, t_cap = kcache.shape[:2]
+        self._inout(kcache, np.float16, (n_slots, t_cap, d), "kcache")
+        self._inout(vcache, np.float16, (n_slots, t_cap, d), "vcache")
+        self._inout(ctx, np.float16, (R, d), "ctx")
+        if d % 64:
+            raise ValueError("d must be 64 x heads")
+        row_pos, row_slot = (np.ascontiguousarray(np.asarray(v, np.int32).reshape(R)) for v in (row_pos, row_slot))
+        indir0, indir1 = (np.ascontiguousarray(v, np.int32) for v in (indir0, indir1))
+        if indir0.ndim != 2 or indir0.shape[0] != R or indir1.shape != indir0.shape:
+            raise ValueError("indir0 / indir1 must be [R, t_ind]")
+        if R % rows_per_utt:
+            raise ValueError("R must be a multiple of rows_per_utt")
+        done = None if done is None else np.ascontiguousarray(np.asarray(done, np.int32).reshape(R // rows_per_utt))
+        prm = np.asarray([R, d // 64, n_slots, t_cap, indir0.shape[1], rows_per_utt, int(prefill), int(flip)], np.int32)
+        check(lib().wisb_debug_dec_self_attn(self._h, ptr(prm), prm.size, ptr(q), ptr(kcache), ptr(vcache), ptr(row_pos),
+                                             ptr(row_slot), ptr(indir0), ptr(indir1), ptr(done), ptr(ctx)))
+        return ctx
+
+    def debug_dec_resid_ln(self, x, xn, part, bias, g, b, *, n_splits: int, split_stride: int, rows=None):
+        """Split-K reduction + bias + residual + LayerNorm of the first `rows` rows (default all): x float32 [cap, d] and
+        xn float16 [cap, d] in / out; part a C-contiguous float32 array holding slab s at flat offset s * split_stride;
+        bias, g, b float32 [d]."""
+        cap, d = x.shape
+        R = cap if rows is None else int(rows)
+        self._inout(x, np.float32, (cap, d), "x")
+        self._inout(xn, np.float16, (cap, d), "xn")
+        if not isinstance(part, np.ndarray) or part.dtype != np.float32 or not part.flags["C_CONTIGUOUS"]:
+            raise ValueError("part must be a C-contiguous float32 array")
+        vecs = [np.ascontiguousarray(np.asarray(v, np.float32).reshape(d)) for v in (bias, g, b)]
+        check(lib().wisb_debug_dec_resid_ln(self._h, R, cap, d, int(n_splits), int(split_stride), ptr(part), part.size,
+                                            *(ptr(v) for v in vecs), ptr(x), ptr(xn)))
+        return x, xn
+
+    def debug_dec_embed_ln(self, tokens, row_pos, tok_emb, pos_emb, g, b, x, xn):
+        """Embedding + LayerNorm of R = len(tokens) rows: row_pos int [R], tok_emb float16 [n_vocab, d], pos_emb
+        float32 [n_pos, d], g, b float32 [d]; x float32 [cap, d] and xn float16 [cap, d] in / out, cap >= R."""
+        cap, d = x.shape
+        R = len(tokens)
+        self._inout(x, np.float32, (cap, d), "x")
+        self._inout(xn, np.float16, (cap, d), "xn")
+        tokens, row_pos = (np.ascontiguousarray(np.asarray(v, np.int32).reshape(R)) for v in (tokens, row_pos))
+        tok_emb = np.ascontiguousarray(tok_emb, np.float16)
+        pos_emb = np.ascontiguousarray(pos_emb, np.float32)
+        if tok_emb.ndim != 2 or tok_emb.shape[1] != d or pos_emb.ndim != 2 or pos_emb.shape[1] != d:
+            raise ValueError("tok_emb / pos_emb must be [rows, d]")
+        vecs = [np.ascontiguousarray(np.asarray(v, np.float32).reshape(d)) for v in (g, b)]
+        check(lib().wisb_debug_dec_embed_ln(self._h, R, cap, d, tok_emb.shape[0], pos_emb.shape[0], ptr(tokens), ptr(row_pos),
+                                            ptr(tok_emb), ptr(pos_emb), *(ptr(v) for v in vecs), ptr(x), ptr(xn)))
+        return x, xn
 
     def debug_gemv_tc(self, x: np.ndarray, w16: np.ndarray, bias=None, iters: int = 0):
         """wgmma skinny GEMV on caller data -> (out float32 [R, N], average kernel time in us over `iters` launches)."""

@@ -149,6 +149,19 @@ struct BatchArgs {
 // returns the number of kernels launched
 int batch_pass_run(const BatchArgs& a, const BatchLayer* layers, int n_layers, cudaStream_t stream);
 
+// The launchers of the pass's own kernels.  batch_pass_run and the wisb_debug_dec_* entries (engine.cu) both launch
+// through them; they check nothing but what the kernel choice depends on, so callers validate indices first.
+// Utterances one cross-attention launch takes: the largest row capacity of a pass (option batch_rows) at one row each.
+constexpr int BD_CROSS_MAX_UTT = 1024;
+// x = tok_emb[tokens] + pos_emb[row_pos]; xn = LN(x) with gain g, shift b  (a.R rows of a.d <= 1536, a.d % 128 == 0)
+void embed_ln_launch(const BatchArgs& a, const float* g, const float* b, cudaStream_t stream);
+// ctx = self-attention of q over ly.kcache / ly.vcache through row_pos, row_slot, indir0 / indir1 (*flip), done, prefill
+void self_attn_launch(const BatchArgs& a, const BatchLayer& ly, cudaStream_t stream);
+// ctx = cross-attention of q over ly.ck / ly.cv; a.cross_tc picks the wgmma kernel (through a.ckv_map) or the SIMT one
+void cross_attn_launch(const BatchArgs& a, const BatchLayer& ly, cudaStream_t stream);
+// x += bias + the n_splits partial slabs at a.part (stride a.part_stride), in slab order; xn = LN(x)
+void resid_ln_launch(const BatchArgs& a, int n_splits, const float* bias, const float* g, const float* b, cudaStream_t stream);
+
 // ------------------------------------------------------------------ alignment (decoder_batch.cu, align.cu)
 // Cross-attention probabilities of the alignment heads of one layer, captured during a teacher-forced batched prefill pass
 // (rows_per_utt consecutive positions per utterance).  Item = (utterance, head of this layer).  P = softmax over all 1500

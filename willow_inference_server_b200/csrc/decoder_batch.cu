@@ -370,8 +370,11 @@ constexpr int XT_Q_BYTES = XT_NQ * HEAD_DIM * 2;   // 1 KB
 constexpr int XT_OFF_P = XT_STAGES * XT_TILE;
 constexpr int XT_OFF_Q = XT_OFF_P + XT_NT * XT_P_TILE;
 constexpr int XT_OFF_BAR = XT_OFF_Q + 1024;
-constexpr int XT_MAX_UTT = 512;                    // utterances of one pass (row capacity <= 1024, >= 2 ... rows each, or greedy)
-constexpr int XT_SMEM = XT_OFF_BAR + 2048 + 1024;  // + barriers / scratch / live list (1412 B) + alignment slack
+constexpr int XT_OFF_RED = XT_OFF_BAR + 2 * XT_STAGES * 8;         // [2][4 warps][8 rows] fp32: row max, row sum partials
+constexpr int XT_OFF_LIVE = XT_OFF_RED + 2 * 4 * XT_NQ * 4;        // [BD_CROSS_MAX_UTT] unsigned short: live utterances
+constexpr int XT_OFF_NLIVE = XT_OFF_LIVE + BD_CROSS_MAX_UTT * 2;   // int: number of live utterances
+constexpr int XT_SMEM = XT_OFF_NLIVE + 4 + 1024;                   // + slack for the 1024-byte alignment of the base
+static_assert(BD_CROSS_MAX_UTT <= 65536, "cross-attention: the live list holds utterance indices as unsigned short");
 constexpr float XT_LOG2E = 1.4426950408889634f;
 
 __global__ void __launch_bounds__(XT_THREADS, 1)
@@ -387,7 +390,7 @@ bd_cross_attn_tc_kernel(const __grid_constant__ CUtensorMap map_kv, const float*
   const uint32_t bar0 = smem_u32(bars);
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (XT_STAGES + s); };
-  float* s_red = reinterpret_cast<float*>(bars + 2 * XT_STAGES);  // [2][4 warps][8 rows]: row max, row sum partials
+  float* s_red = reinterpret_cast<float*>(smem + XT_OFF_RED);  // [2][4 warps][8 rows]: row max, row sum partials
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   pdl_launch_dependents();
@@ -408,8 +411,8 @@ bd_cross_attn_tc_kernel(const __grid_constant__ CUtensorMap map_kv, const float*
 
   // live utterances, compacted: item k of this CTA is (s_live[idx / H], idx % H) with idx = blockIdx.x + k * gridDim.x, so the
   // CTAs stay balanced whichever utterances have finished
-  unsigned short* s_live = reinterpret_cast<unsigned short*>(s_red + 64);
-  int* s_nlive = reinterpret_cast<int*>(s_live + XT_MAX_UTT);
+  unsigned short* s_live = reinterpret_cast<unsigned short*>(smem + XT_OFF_LIVE);
+  int* s_nlive = reinterpret_cast<int*>(smem + XT_OFF_NLIVE);
   if (threadIdx.x == 0) {
     int n = 0;
     for (int u = 0; u < n_utt; ++u)
@@ -699,7 +702,6 @@ void bd_launch(Kern kern, dim3 grid, dim3 block, size_t smem, cudaStream_t strea
 int bd_ca_smem(int nb) { return 2 * BD_CA_KEYS * HEAD_DIM * 2 + BD_CA_GROUPS * nb * HEAD_DIM * 4; }
 
 void cross_tc_launch(const BatchArgs& a, const BatchLayer& ly, cudaStream_t s) {
-  WISB_REQUIRE(a.n_utt <= XT_MAX_UTT, "cross-attention: more than 512 utterances in one pass");
   static std::atomic<unsigned long long> once{0};
   once_per_device(once, [] {
     WISB_CUDA(cudaFuncSetAttribute(bd_cross_attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XT_SMEM));
@@ -710,7 +712,30 @@ void cross_tc_launch(const BatchArgs& a, const BatchLayer& ly, cudaStream_t s) {
             *a.ckv_map, a.q, row_k0, row_v0, a.done, a.ctx, a.n_utt, a.rows_per_utt, a.d, a.H);
 }
 
+void run_gemm_rows(const GemmPlan& plan, int rows, int pdl, cudaStream_t s) {
+  GemmPlan p = plan;  // the plan is built for the buffer capacity; this pass uses the first `rows` rows
+  p.M = round_up(rows, 128);
+  if (p.M > plan.M) p.M = plan.M;
+  p.epi.m_valid = rows;
+  p.pdl = pdl;
+  gemm_run(p, s);
+}
+
+}  // namespace
+
+void embed_ln_launch(const BatchArgs& a, const float* g, const float* b, cudaStream_t s) {
+  bd_launch(bd_embed_ln_kernel, dim3(cdiv(a.R, BD_LN_WARPS)), dim3(BD_LN_WARPS * 32), 0, s, a.pdl != 0, a.tokens, a.row_pos,
+            a.tok_emb, a.pos_emb, g, b, a.x, a.xn, a.d, a.R);
+}
+
+void self_attn_launch(const BatchArgs& a, const BatchLayer& ly, cudaStream_t s) {
+  bd_launch(bd_self_attn_kernel, dim3(cdiv(a.H, 4), a.R), dim3(128), 0, s, a.pdl != 0, a.q, ly.kcache, ly.vcache, a.row_pos,
+            a.row_slot, a.indir0, a.indir1, a.flip, a.done, a.ctx, a.d, a.H, a.t_cap, a.t_ind, a.rows_per_utt, a.prefill);
+}
+
 void cross_attn_launch(const BatchArgs& a, const BatchLayer& ly, cudaStream_t s) {
+  WISB_REQUIRE(a.n_utt >= 1 && a.n_utt <= BD_CROSS_MAX_UTT,
+               "cross-attention: 1.." + std::to_string(BD_CROSS_MAX_UTT) + " utterances in one pass, got " + std::to_string(a.n_utt));
   if (a.cross_tc) {
     cross_tc_launch(a, ly, s);
     return;
@@ -743,17 +768,6 @@ void resid_ln_launch(const BatchArgs& a, int n_splits, const float* bias, const 
   }
 }
 
-void run_gemm_rows(const GemmPlan& plan, int rows, int pdl, cudaStream_t s) {
-  GemmPlan p = plan;  // the plan is built for the buffer capacity; this pass uses the first `rows` rows
-  p.M = round_up(rows, 128);
-  if (p.M > plan.M) p.M = plan.M;
-  p.epi.m_valid = rows;
-  p.pdl = pdl;
-  gemm_run(p, s);
-}
-
-}  // namespace
-
 void align_capture_run(const AlignCaptureArgs& a, cudaStream_t s) {
   WISB_REQUIRE(a.rows_per_utt >= 1 && a.rows_per_utt <= MAX_BEAM, "alignment capture: 1..8 rows per utterance");
   if (a.n_items == 0 || a.n_utt == 0) return;
@@ -770,7 +784,6 @@ int batch_pass_run(const BatchArgs& a, const BatchLayer* layers, int n_layers, c
   WISB_REQUIRE(a.rows_per_utt >= 1 && a.rows_per_utt <= MAX_BEAM, "batched decoder pass: 1..8 rows per utterance");
   WISB_REQUIRE(a.d % 128 == 0 && a.d <= 128 * BD_LN_MAX, "batched decoder pass: d_model multiple of 128, <= 1536");
   WISB_REQUIRE(a.t_ind <= BD_SA_TMAX, "batched decoder pass: more than 448 text positions");
-  const bool pdl = a.pdl != 0;
   struct Scope {  // brackets one kernel with the optional timing hook
     const BatchArgs& a;
     Scope(const BatchArgs& a_, int cat) : a(a_) {
@@ -783,8 +796,7 @@ int batch_pass_run(const BatchArgs& a, const BatchLayer* layers, int n_layers, c
   int n = 0;
   {
     Scope t(a, 2);
-    bd_launch(bd_embed_ln_kernel, dim3(cdiv(a.R, BD_LN_WARPS)), dim3(BD_LN_WARPS * 32), 0, s, pdl, a.tokens, a.row_pos, a.tok_emb,
-              a.pos_emb, layers[0].ln1g, layers[0].ln1b, a.x, a.xn, a.d, a.R);
+    embed_ln_launch(a, layers[0].ln1g, layers[0].ln1b, s);
   }
   ++n;
   auto gemm = [&](const GemmPlan& p) {
@@ -800,8 +812,7 @@ int batch_pass_run(const BatchArgs& a, const BatchLayer* layers, int n_layers, c
     gemm(ly.qkv);
     {
       Scope t(a, 3);
-      bd_launch(bd_self_attn_kernel, dim3(cdiv(a.H, 4), a.R), dim3(128), 0, s, pdl, a.q, ly.kcache, ly.vcache, a.row_pos,
-                a.row_slot, a.indir0, a.indir1, a.flip, a.done, a.ctx, a.d, a.H, a.t_cap, a.t_ind, a.rows_per_utt, a.prefill);
+      self_attn_launch(a, ly, s);
     }
     gemm(ly.o);
     ln(ly.o.k_splits, ly.ob, ly.ln2g, ly.ln2b);

@@ -1505,6 +1505,14 @@ int create_common(wisb_handle** out, int device, const std::function<void(wisb_h
   }
 }
 
+// `count` elements from the host into a new device buffer (the wisb_debug_dec_* entries)
+template <typename T>
+T* to_device(DevBuf<T>& d, const void* src, size_t count, cudaStream_t s) {
+  d.ensure(count);
+  WISB_CUDA(cudaMemcpyAsync(d.p, src, count * sizeof(T), cudaMemcpyHostToDevice, s));
+  return d.p;
+}
+
 }  // namespace
 
 // ===================================================================================================================== C ABI
@@ -2251,6 +2259,160 @@ int wisb_debug_enc_attn(wisb_handle* h, const uint16_t* qkv16, int B, int d, int
       enc_attn_run(ap, s);
     }
     WISB_CUDA(cudaMemcpyAsync(ctx16_out, dctx.p, sizeof(__half) * rows * d, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+// The batched decoder pass's own kernels on caller data, through the launchers batch_pass_run uses (decoder.cuh), without
+// programmatic dependent launch.  Every index a kernel can form is checked against the caller's sizes first.
+int wisb_debug_dec_cross_attn(wisb_handle* h, const int32_t* prm, int n_prm, const float* q, const uint16_t* ckv,
+                              const int32_t* done, uint16_t* ctx16) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(prm != nullptr && n_prm == 6 && q && ckv && ctx16, "debug_dec_cross_attn: bad arguments");
+    const int n_utt = prm[0], rpu = prm[1], H = prm[2], n_layers = prm[3], layer = prm[4], impl = prm[5];
+    WISB_REQUIRE(n_utt >= 1 && n_utt <= BD_CROSS_MAX_UTT,
+                 "debug_dec_cross_attn: 1.." + std::to_string(BD_CROSS_MAX_UTT) + " utterances in one pass");
+    WISB_REQUIRE(rpu >= 1 && rpu <= MAX_BEAM, "debug_dec_cross_attn: 1..8 rows per utterance");
+    WISB_REQUIRE(H >= 1 && H <= 32 && n_layers >= 1 && layer >= 0 && layer < n_layers && (impl == 0 || impl == 1),
+                 "debug_dec_cross_attn: bad heads / layer / impl");
+    cudaStream_t s = h->stream;
+    const int d = H * HEAD_DIM;
+    const size_t rows = static_cast<size_t>(n_utt) * rpu;
+    const size_t block = static_cast<size_t>(n_utt) * H * T_ENC_PAD * HEAD_DIM;  // one layer's K (or V), all utterances
+    const size_t ckv_elems = static_cast<size_t>(n_layers) * 2 * block;
+    DevBuf<float> dq;
+    DevBuf<__half> dckv, dctx;
+    DevBuf<int> ddone;
+    BatchArgs a;
+    a.R = static_cast<int>(rows);
+    a.d = d;
+    a.H = H;
+    a.n_utt = n_utt;
+    a.rows_per_utt = rpu;
+    a.q = to_device(dq, q, rows * d, s);
+    a.ctx = to_device(dctx, ctx16, rows * d, s);
+    a.done = done ? to_device(ddone, done, n_utt, s) : nullptr;
+    a.cross_tc = impl == 0 ? 1 : 0;
+    a.num_sms = h->num_sms;
+    a.ckv_base = to_device(dckv, ckv, ckv_elems, s);
+    CUtensorMap map;  // as the engine's ckv_map: the whole buffer as rows of one head's 64 values
+    make_tmap_f16_2d(&map, dckv.p, HEAD_DIM, static_cast<long long>(ckv_elems / HEAD_DIM), HEAD_DIM, HEAD_DIM, 128);
+    a.ckv_map = &map;
+    BatchLayer ly;
+    ly.ck = dckv.p + static_cast<size_t>(2 * layer) * block;
+    ly.cv = dckv.p + static_cast<size_t>(2 * layer + 1) * block;
+    cross_attn_launch(a, ly, s);
+    WISB_CUDA(cudaMemcpyAsync(ctx16, dctx.p, sizeof(__half) * rows * d, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+int wisb_debug_dec_self_attn(wisb_handle* h, const int32_t* prm, int n_prm, const float* q, const uint16_t* kcache,
+                             const uint16_t* vcache, const int32_t* row_pos, const int32_t* row_slot, const int32_t* indir0,
+                             const int32_t* indir1, const int32_t* done, uint16_t* ctx16) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(prm != nullptr && n_prm == 8 && q && kcache && vcache && row_pos && row_slot && indir0 && indir1 && ctx16,
+                 "debug_dec_self_attn: bad arguments");
+    const int R = prm[0], H = prm[1], n_slots = prm[2], t_cap = prm[3], t_ind = prm[4], rpu = prm[5], prefill = prm[6],
+              flip = prm[7];
+    WISB_REQUIRE(rpu >= 1 && rpu <= MAX_BEAM && R >= 1 && R <= 65535 && R % rpu == 0,
+                 "debug_dec_self_attn: R = utterances x 1..8 rows per utterance");
+    WISB_REQUIRE(H >= 1 && H <= 32 && n_slots >= 1 && t_cap >= 1 && t_ind >= 1 && t_ind <= T_MAX,
+                 "debug_dec_self_attn: bad heads / slots / t_cap / t_ind (<= 448)");
+    WISB_REQUIRE((prefill == 0 || prefill == 1) && (flip == 0 || flip == 1), "debug_dec_self_attn: prefill and flip are 0 / 1");
+    for (int r = 0; r < R; ++r)
+      WISB_REQUIRE(row_slot[r] >= 0 && row_slot[r] < n_slots && row_pos[r] >= 0 && row_pos[r] < t_cap && row_pos[r] < t_ind,
+                   "debug_dec_self_attn: row slot / position out of range");
+    const size_t n_ind = static_cast<size_t>(R) * t_ind;
+    for (size_t i = 0; i < n_ind; ++i)
+      WISB_REQUIRE(indir0[i] >= 0 && indir0[i] < n_slots && indir1[i] >= 0 && indir1[i] < n_slots,
+                   "debug_dec_self_attn: indirection entry out of range");
+    cudaStream_t s = h->stream;
+    const int d = H * HEAD_DIM;
+    const size_t cache = static_cast<size_t>(n_slots) * t_cap * d;
+    DevBuf<float> dq;
+    DevBuf<__half> dk, dv, dctx;
+    DevBuf<int> dpos, dslot, di0, di1, dflip, ddone;
+    BatchArgs a;
+    a.R = R;
+    a.d = d;
+    a.H = H;
+    a.n_utt = R / rpu;
+    a.rows_per_utt = rpu;
+    a.t_cap = t_cap;
+    a.t_ind = t_ind;
+    a.prefill = prefill;
+    a.q = to_device(dq, q, static_cast<size_t>(R) * d, s);
+    a.ctx = to_device(dctx, ctx16, static_cast<size_t>(R) * d, s);
+    a.row_pos = to_device(dpos, row_pos, R, s);
+    a.row_slot = to_device(dslot, row_slot, R, s);
+    a.indir0 = to_device(di0, indir0, n_ind, s);
+    a.indir1 = to_device(di1, indir1, n_ind, s);
+    a.flip = to_device(dflip, &flip, 1, s);
+    a.done = done ? to_device(ddone, done, R / rpu, s) : nullptr;
+    BatchLayer ly;
+    ly.kcache = to_device(dk, kcache, cache, s);
+    ly.vcache = to_device(dv, vcache, cache, s);
+    self_attn_launch(a, ly, s);
+    WISB_CUDA(cudaMemcpyAsync(ctx16, dctx.p, sizeof(__half) * R * d, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+int wisb_debug_dec_resid_ln(wisb_handle* h, int R, int cap, int d, int n_splits, int64_t split_stride, const float* part,
+                            size_t part_elems, const float* bias, const float* g, const float* b, float* x, uint16_t* xn16) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(part && bias && g && b && x && xn16, "debug_dec_resid_ln: NULL argument");
+    WISB_REQUIRE(R >= 1 && cap >= R && d >= 128 && d % 128 == 0 && d <= 1536, "debug_dec_resid_ln: d_model multiple of 128, <= 1536");
+    WISB_REQUIRE(n_splits == 1 || n_splits == 2 || n_splits == 4 || n_splits == 8, "debug_dec_resid_ln: 1, 2, 4 or 8 slabs");
+    const size_t rd = static_cast<size_t>(R) * d, cd = static_cast<size_t>(cap) * d;
+    WISB_REQUIRE(split_stride % 4 == 0 && (n_splits == 1 || split_stride >= static_cast<int64_t>(rd)) &&
+                     part_elems >= static_cast<size_t>(n_splits - 1) * static_cast<size_t>(split_stride) + rd,
+                 "debug_dec_resid_ln: slabs overlap, are misaligned or exceed the partial buffer");
+    cudaStream_t s = h->stream;
+    DevBuf<float> dx, dpart, dbias, dg, db;
+    DevBuf<__half> dxn;
+    BatchArgs a;
+    a.R = R;
+    a.d = d;
+    a.x = to_device(dx, x, cd, s);
+    a.xn = to_device(dxn, xn16, cd, s);
+    a.part = to_device(dpart, part, part_elems, s);
+    a.part_stride = split_stride;
+    resid_ln_launch(a, n_splits, to_device(dbias, bias, d, s), to_device(dg, g, d, s), to_device(db, b, d, s), s);
+    WISB_CUDA(cudaMemcpyAsync(x, dx.p, sizeof(float) * cd, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(xn16, dxn.p, sizeof(__half) * cd, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+int wisb_debug_dec_embed_ln(wisb_handle* h, int R, int cap, int d, int n_vocab, int n_pos, const int32_t* tokens, const int32_t* row_pos,
+                            const uint16_t* tok_emb, const float* pos_emb, const float* g, const float* b, float* x,
+                            uint16_t* xn16) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(tokens && row_pos && tok_emb && pos_emb && g && b && x && xn16, "debug_dec_embed_ln: NULL argument");
+    WISB_REQUIRE(R >= 1 && cap >= R && d >= 128 && d % 128 == 0 && d <= 1536, "debug_dec_embed_ln: d_model multiple of 128, <= 1536");
+    WISB_REQUIRE(n_vocab >= 1 && n_pos >= 1, "debug_dec_embed_ln: empty embedding table");
+    for (int r = 0; r < R; ++r)
+      WISB_REQUIRE(tokens[r] >= 0 && tokens[r] < n_vocab && row_pos[r] >= 0 && row_pos[r] < n_pos,
+                   "debug_dec_embed_ln: token / position out of range");
+    cudaStream_t s = h->stream;
+    const size_t cd = static_cast<size_t>(cap) * d;
+    DevBuf<float> dx, dpos, dg, db;
+    DevBuf<__half> dxn, demb;
+    DevBuf<int> dtok, drow;
+    BatchArgs a;
+    a.R = R;
+    a.d = d;
+    a.tokens = to_device(dtok, tokens, R, s);
+    a.row_pos = to_device(drow, row_pos, R, s);
+    a.tok_emb = to_device(demb, tok_emb, static_cast<size_t>(n_vocab) * d, s);
+    a.pos_emb = to_device(dpos, pos_emb, static_cast<size_t>(n_pos) * d, s);
+    a.x = to_device(dx, x, cd, s);
+    a.xn = to_device(dxn, xn16, cd, s);
+    embed_ln_launch(a, to_device(dg, g, d, s), to_device(db, b, d, s), s);
+    WISB_CUDA(cudaMemcpyAsync(x, dx.p, sizeof(float) * cd, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(xn16, dxn.p, sizeof(__half) * cd, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaStreamSynchronize(s));
   });
 }
