@@ -110,7 +110,8 @@ int wisb_align(wisb_handle* h, const float* mel, int B, const int32_t* start_seq
  * entries 8-12 are filled only with option "profile" = 1 (per-kernel event pairs; leave it off for timed runs). */
 int wisb_get_timing(wisb_handle* h, float* out16);
 /* options: "use_graphs" (default 1), "attn_v_mn_major" (default 1), "attn_ref" (0), "decode_poll" (1), "profile" (0),
- * "decoder_mega" (1: persistent decoder-pass kernel; 0: the per-op kernel chain kept as a cross-check),
+ * "mega_mma" (for calls of <= 8 rows: 1, the default where d_model <= 1280, the warp-MMA persistent decoder pass; 0 the
+ * SIMT persistent pass, fp32 arithmetic, the only one for d_model > 1280),
  * "encoder_cache" (default 0; 1: consecutive wisb_detect_language / wisb_generate calls on byte-identical host features
  * of <= 2 windows reuse the encoder output and cross K/V already in HBM -- the detect -> transcribe -> translate sequence
  * of main.py:633-644, 514-547 then encodes once instead of three times) */
@@ -173,11 +174,6 @@ int wisb_debug_dec_resid_ln(wisb_handle* h, int R, int cap, int d, int n_splits,
 int wisb_debug_dec_embed_ln(wisb_handle* h, int R, int cap, int d, int n_vocab, int n_pos, const int32_t* tokens, const int32_t* row_pos,
                             const uint16_t* tok_emb, const float* pos_emb, const float* g, const float* b, float* x,
                             uint16_t* xn16);
-/* the wgmma skinny-GEMV building block of the decoder pass on caller data: out[R,N] (float32) = x[R,K] (float32, rounded
- * to fp16 inside) . W[N,K]^T (fp16 as raw uint16) + bias (may be NULL); R <= 8, K % 64 == 0, K <= 5120.  avg_us (may be
- * NULL) receives the average kernel time over `iters` back-to-back launches. */
-int wisb_debug_gemv_tc(wisb_handle* h, const float* x, const uint16_t* w, const float* bias, float* out, int R, int N, int K,
-                       int iters, float* avg_us);
 /* per-phase %globaltimer stamps of the last persistent decoder pass (option "mega_trace" = 1): n <= 2048 values */
 int wisb_debug_read_trace(wisb_handle* h, unsigned long long* out, int n);
 /* encoder output after the final LayerNorm, float32 [B,1500,d_model]; n_layers < 0 = all */

@@ -70,6 +70,9 @@ class WhisperOracle:
         self.suppress = torch.tensor(sorted(set(dims.suppress_ids)), dtype=torch.long)
         self.suppress_begin = torch.tensor(list(dims.suppress_ids_begin), dtype=torch.long)
         self.logit_noise = None
+        # True: cross K/V and every appended self-attention K/V row are rounded through fp16, the two storage roundings
+        # of the engine's SIMT decoder pass (its activations stay fp32), so that pass can be checked to a tight bound
+        self.kv_fp16 = False
 
     @classmethod
     def from_blob(cls, src):
@@ -119,11 +122,14 @@ class WhisperOracle:
         return self._ln(x, "enc.ln_post") if final_ln else x
 
     # ----------------------------------------------------------------- decoder
+    def _kv_store(self, t: torch.Tensor) -> torch.Tensor:
+        return t.half().float() if self.kv_fp16 else t
+
     @torch.no_grad()
     def cross_kv(self, enc: torch.Tensor):
         """enc [1500,d] -> list over layers of (K [1500,d], V [1500,d])."""
         d = self.dims.d_model
-        kv = F.linear(enc, self.w["dec.crosskv.w"], self.w["dec.crosskv.b"])
+        kv = self._kv_store(F.linear(enc, self.w["dec.crosskv.w"], self.w["dec.crosskv.b"]))
         return [(kv[:, i * 2 * d : i * 2 * d + d], kv[:, i * 2 * d + d : (i + 1) * 2 * d])
                 for i in range(self.dims.n_dec_layers)]
 
@@ -143,7 +149,7 @@ class WhisperOracle:
             p = f"dec.{i}."
             xn = self._ln(x, p + "ln1")
             qkv = F.linear(xn, self.w[p + "qkv.w"], self.w[p + "qkv.b"])
-            k_new, v_new = qkv[:, d : 2 * d].unsqueeze(1), qkv[:, 2 * d :].unsqueeze(1)
+            k_new, v_new = self._kv_store(qkv[:, d : 2 * d]).unsqueeze(1), self._kv_store(qkv[:, 2 * d :]).unsqueeze(1)
             if cache is not None:
                 k_all = torch.cat([cache[i][0], k_new], 1)
                 v_all = torch.cat([cache[i][1], v_new], 1)

@@ -51,11 +51,6 @@ def test_mixed_duration_batch_properties(large):
     # greedy and beam agree on the first token whenever the beam result starts with the greedy arg-max path's token
     g = m.generate(feats, [PROMPT] * 5, beam_size=1, max_length=24)
     assert all(len(o.sequences_ids[0]) <= 12 for o in g)
-    # persistent pass kernel vs per-op chain at full size
-    h.set_option("decoder_mega", 0)
-    chain = [o.sequences_ids[0] for o in m.generate(feats, [PROMPT] * 5, beam_size=5, max_length=24)]
-    h.set_option("decoder_mega", 1)
-    assert chain == ids
     langs = m.detect_language(models.StorageView.from_array(mel[:2]))
     assert len(langs) == 2 and abs(sum(p for _, p in langs[0]) - 1.0) < 1e-3
 

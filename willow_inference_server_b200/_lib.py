@@ -61,8 +61,6 @@ _SIGS = {
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_dec_embed_ln": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "wisb_debug_gemv_tc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
-                                      C.c_void_p]),
     "wisb_debug_read_trace": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     "wisb_debug_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     "wisb_debug_forced_logits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
@@ -455,18 +453,6 @@ class Handle:
         check(lib().wisb_debug_dec_embed_ln(self._h, R, cap, d, tok_emb.shape[0], pos_emb.shape[0], ptr(tokens), ptr(row_pos),
                                             ptr(tok_emb), ptr(pos_emb), *(ptr(v) for v in vecs), ptr(x), ptr(xn)))
         return x, xn
-
-    def debug_gemv_tc(self, x: np.ndarray, w16: np.ndarray, bias=None, iters: int = 0):
-        """wgmma skinny GEMV on caller data -> (out float32 [R, N], average kernel time in us over `iters` launches)."""
-        x = np.ascontiguousarray(x, np.float32)
-        w16 = np.ascontiguousarray(w16, np.float16)
-        R, K = x.shape
-        N = w16.shape[0]
-        out = np.zeros((R, N), np.float32)
-        us = C.c_float(0.0)
-        b = None if bias is None else np.ascontiguousarray(bias, np.float32)
-        check(lib().wisb_debug_gemv_tc(self._h, ptr(x), ptr(w16), ptr(b), ptr(out), R, N, K, int(iters), C.byref(us)))
-        return out, float(us.value)
 
     def debug_read_trace(self, n: int = 600) -> np.ndarray:
         out = np.zeros(n, np.uint64)

@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libwisb200.so")
-SOURCES = ["engine.cu", "gemm_tc.cu", "logmel.cu", "encoder.cu", "decoder.cu", "decoder_mega.cu", "decoder_batch.cu", "gemv_tc.cu", "search.cu", "flac.cu", "align.cu"]
+SOURCES = ["engine.cu", "gemm_tc.cu", "logmel.cu", "encoder.cu", "decoder_mega.cu", "decoder_batch.cu", "search.cu", "flac.cu", "align.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC,-O3,-Wall,-Wno-unused-function", "--expt-relaxed-constexpr",

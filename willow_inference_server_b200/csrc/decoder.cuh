@@ -1,4 +1,4 @@
-// Decoder-side kernel interface (decoder.cu / search.cu).  Token loop of ctranslate2.models.Whisper.generate
+// Decoder-side kernel interface (decoder_mega.cu / decoder_batch.cu / search.cu / align.cu).  Token loop of ctranslate2.models.Whisper.generate
 // (main.py:687-692; SURVEY.md section 8a rows A10-A14).
 #pragma once
 #include "common.cuh"
@@ -26,38 +26,6 @@ enum GemvEpi : int {
   GV_GELU = 2,    // out[r, n] = gelu(v)
   GV_QKV = 3,     // n < d: q[r, n] = v ; d <= n < 2d: kcache[slot r][pos][n - d] ; else vcache
 };
-
-struct GemvArgs {
-  const float* x = nullptr;   // [R, K] fp32
-  const float* ln_g = nullptr;  // LayerNorm prologue when non-null
-  const float* ln_b = nullptr;
-  const __half* w = nullptr;  // [N, K] fp16
-  const float* bias = nullptr;
-  float* out = nullptr;       // fp32 [R, ldo]
-  long long ldo = 0;
-  int R = 0, N = 0, K = 0;
-  int epi = GV_STORE;
-  // GV_QKV
-  __half* kcache = nullptr;   // [R_slots][t_max][d]
-  __half* vcache = nullptr;
-  int d_model = 0, t_max = 0;
-  const DecState* st = nullptr;
-};
-void gemv_run(const GemvArgs& a, cudaStream_t stream);
-
-// x[r, :] = tok_emb[token[r], :] + pos_emb[pos, :]
-void dec_embed_run(const int* tokens, const __half* tok_emb, const float* pos_emb, float* x, int R, int d,
-                   const DecState* st, cudaStream_t stream);
-
-// causal self-attention over the cache, with beam indirection: position t of row r lives in slot indir[r][t]
-// (two ping-pong indirection tables; *flip says which one is current)
-void dec_self_attn_run(const float* q /*[R,d]*/, const __half* kcache, const __half* vcache, const int* indir0,
-                       const int* indir1, const int* flip, float* ctx /*[R,d]*/, int R, int d, int H, int t_max,
-                       const DecState* st, cudaStream_t stream);
-
-// cross-attention: rows of utterance u share K/V [H][1536][64]; grid = (H, n_utt) x cluster of 8 CTAs over the keys
-void dec_cross_attn_run(const float* q /*[R,d]*/, const __half* k /*[n_utt_total][H][1536][64]*/, const __half* v,
-                        float* ctx, int n_utt, int beam, int d, int H, cudaStream_t stream);
 
 struct SearchArgs {
   // inputs
@@ -256,10 +224,6 @@ void mega_mma_image(const __half* src, __half* dst, int N, int K, int grid, cuda
 void mega_ln_fold(const __half* w, const float* g, const float* b, const float* bias, float* s2, float* biasf, int N, int K,
                   cudaStream_t stream);
 void dec_pass_run(const MegaArgs& a, int num_sms, cudaStream_t stream);
-
-// wgmma skinny GEMV (gemv_tc.cu), diagnostics entry: returns the average kernel time in microseconds
-float gemv_tc_debug_run(const float* x, const __half* w, const float* bias, float* out, int R, int N, int K, int num_sms,
-                        int iters, cudaStream_t stream);
 
 // language detection head: softmax over lang ids of the logits of row u*beam (one step on <|startoftranscript|>)
 void lang_probs_run(const float* logits, long long ldl, const int* lang_ids, int n_lang, int n_utt, int row_stride,

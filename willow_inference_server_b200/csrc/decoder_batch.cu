@@ -4,7 +4,7 @@
 // (main.py:676-693 of the reference server feeds several windows per call; SURVEY.md section 8a row A10, section 7 step 5:
 // "decoder with M = B x beam rows").  Architecture per [HF] modeling_whisper.py:417-508.
 //
-// Up to 8 rows the persistent SIMT pass (decoder_mega.cu) is the latency path.  Beyond that the pass is a chain of
+// Up to 8 rows the persistent passes (decoder_mega.cu) are the latency path.  Beyond that the pass is a chain of
 //   * wgmma GEMMs (gemm_tc.cu): rows are the M dimension (padded to 128-row tiles), the weight matrix streams through
 //     the TMA ring exactly once per pass whatever the number of rows; narrow tiles (BN = 64) and split-K keep >= ~100 CTAs
 //     streaming even when the weight matrix has only d_model output columns;

@@ -956,8 +956,8 @@ __global__ void __launch_bounds__(MG_THREADS, 1) dec_pass_kernel(const MegaArgs 
 // rows its N, K is split over the 7 consumer warps and their partial tiles are summed through shared memory.
 // Why not wgmma here (it is what the encoder, the batched pass and the cross-attention of the batched pass use): at N = 8
 // a warpgroup MMA is one 64 x 8 x 16 instruction for four warps, and this pass splits K over 7 consumer warps that each
-// work on their own 16-row tiles; the warp MMA fits that split directly (scripts/diag_gemv_tc.py times the wgmma GEMV
-// at the same shapes for comparison).  18 (k-block, m-tile) items of 4 HMMAs each per warp cover the QKV phase.  What disappears against the SIMT pass: the
+// work on their own 16-row tiles; the warp MMA fits that split directly.
+// 18 (k-block, m-tile) items of 4 HMMAs each per warp cover the QKV phase.  What disappears against the SIMT pass: the
 // fp32 FMA loop over the weight stage and the transposing shuffle reductions.  What stays: the
 // producer thread and its static weight schedule (2-D TMA boxes, 128-byte swizzle, straight from the row-major W -- the
 // swizzle is what makes ldmatrix conflict-free), the grid barrier between phases, the attention phases, LayerNorm folded

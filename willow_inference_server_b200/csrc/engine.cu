@@ -77,16 +77,14 @@ struct DecLayerW {
   const __half *qkvw, *ow, *cqw, *cow, *fc1w, *fc2w;
 };
 
+// key of a captured step of the batched decoder pass
 struct GraphKey {
-  int n_utt, beam, prompt_len, max_new, max_hyp, u0, b_total, batched;
+  int n_utt, beam, prompt_len, max_new, max_hyp, u0, b_total, per_utt_max_new;
   int ts, ts_max_init;  // timestamp mode: the step graph bakes SearchArgs in, so a mode never reuses another's graph
   float lp;
   bool operator<(const GraphKey& o) const {
     return memcmp(this, &o, sizeof(GraphKey)) < 0;
   }
-};
-struct DecGraphs {
-  cudaGraphExec_t prefill = nullptr, step = nullptr;
 };
 
 }  // namespace
@@ -108,7 +106,7 @@ struct wisb_handle {
   std::map<std::string, TensorRef> tensors;
   std::vector<DecLayerW> dec_w;
   // options
-  int use_graphs = 1, attn_v_mn = 1, attn_ref = 0, decode_poll = 1, decoder_mega = 1;
+  int use_graphs = 1, attn_v_mn = 1, attn_ref = 0, decode_poll = 1;
   // front end
   DevBuf<float> lm_tables;
   DevBuf<unsigned> lm_max;
@@ -176,7 +174,7 @@ struct wisb_handle {
   PinBuf<int> pin_i;
   PinBuf<float> pin_f;
   PinBuf<uint8_t> pin_b;
-  std::map<GraphKey, DecGraphs> graphs;
+  std::map<GraphKey, cudaGraphExec_t> graphs;
   // timing
   cudaEvent_t ev[8] = {};
   float timing[16] = {};
@@ -322,10 +320,7 @@ void parse_blob(wisb_handle* h, const std::vector<uint8_t>& head) {
 }
 
 void drop_graphs(wisb_handle* h) {
-  for (auto& kv : h->graphs) {
-    if (kv.second.prefill) cudaGraphExecDestroy(kv.second.prefill);
-    if (kv.second.step) cudaGraphExecDestroy(kv.second.step);
-  }
+  for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second);
   h->graphs.clear();
 }
 
@@ -599,7 +594,7 @@ void ensure_encoder(wisb_handle* h, int B) {
 // the persistent warp-MMA pass (<= 8 rows) reads the cross K/V rows chunk-swizzled (ldmatrix without bank conflicts); every
 // other decoder path reads them linear
 bool want_ckv_swizzle(const wisb_handle* h, int rows) {
-  return rows <= DEC_MAX_ROWS && h->decoder_batch != 2 && h->decoder_mega && h->mega_tc;
+  return rows <= DEC_MAX_ROWS && h->decoder_batch != 2 && h->mega_tc;
 }
 
 // mel (device, [B,80,3000]) -> enc_out fp16 [B*1536, d] (+ cross K/V when with_ckv)
@@ -807,7 +802,8 @@ void upload_mega_layers(wisb_handle* h, const DecodeCfg& c) {
                             cudaMemcpyHostToDevice, h->stream));
 }
 
-int enqueue_decoder_forward_mega(wisb_handle* h, const DecodeCfg& c, bool with_logits, bool prefill_pass = false) {
+// one decoder forward for R <= 8 rows at position st->pos: ONE launch of the persistent pass
+void enqueue_decoder_forward(wisb_handle* h, const DecodeCfg& c, bool with_logits, bool prefill_pass = false) {
   const Dims& dm = h->dims;
   MegaArgs a;
   a.layers = h->mega_layers.p;
@@ -875,68 +871,6 @@ int enqueue_decoder_forward_mega(wisb_handle* h, const DecodeCfg& c, bool with_l
     a.trace_cap = h->mega_tc ? 380 : 70;
   }
   dec_pass_run(a, h->num_sms, h->stream);
-  return 1;
-}
-
-// one decoder forward for R rows at position st->pos; returns kernels launched
-int enqueue_decoder_forward(wisb_handle* h, const DecodeCfg& c, bool with_logits) {
-  if (h->decoder_mega) return enqueue_decoder_forward_mega(h, c, with_logits);
-  const Dims& dm = h->dims;
-  const int d = dm.d_model, H = dm.n_heads, R = c.n_utt * c.beam;
-  cudaStream_t s = h->stream;
-  const DecState* st = h->st.p;
-  int n = 0;
-  dec_embed_run(h->tokens.p, h->H("dec.tok_emb"), h->F("dec.pos"), h->dx.p, R, d, st, s);
-  ++n;
-  const size_t layer_cache = static_cast<size_t>(DEC_MAX_ROWS) * T_MAX * d;
-  const size_t head_block = static_cast<size_t>(H) * T_ENC_PAD * HEAD_DIM;  // one utterance, one of K/V
-  for (int i = 0; i < dm.n_dec_layers; ++i) {
-    const DecLayerW& w = h->dec_w[i];
-    GemvArgs g;
-    g.R = R;
-    g.st = st;
-    // LN1 + QKV (+ cache append)
-    g.x = h->dx.p; g.ln_g = w.ln1g; g.ln_b = w.ln1b; g.w = w.qkvw; g.bias = w.qkvb;
-    g.out = h->dq.p; g.ldo = d; g.N = 3 * d; g.K = d; g.epi = GV_QKV;
-    g.kcache = h->kcache.p + i * layer_cache; g.vcache = h->vcache.p + i * layer_cache; g.d_model = d; g.t_max = T_MAX;
-    gemv_run(g, s);
-    dec_self_attn_run(h->dq.p, h->kcache.p + i * layer_cache, h->vcache.p + i * layer_cache, h->ind0.p, h->ind1.p,
-                      h->flip.p, h->dctx.p, R, d, H, T_MAX, st, s);
-    GemvArgs o;
-    o.R = R; o.st = st; o.x = h->dctx.p; o.w = w.ow; o.bias = w.ob; o.out = h->dx.p; o.ldo = d; o.N = d; o.K = d;
-    o.epi = GV_RESID;
-    gemv_run(o, s);
-    // LN2 + cross-attention
-    GemvArgs q;
-    q.R = R; q.st = st; q.x = h->dx.p; q.ln_g = w.ln2g; q.ln_b = w.ln2b; q.w = w.cqw; q.bias = w.cqb; q.out = h->dq.p;
-    q.ldo = d; q.N = d; q.K = d; q.epi = GV_STORE;
-    gemv_run(q, s);
-    const __half* kl = h->ckv.p + (static_cast<size_t>(i * 2 + 0) * c.B_total + c.u0) * head_block;
-    const __half* vl = h->ckv.p + (static_cast<size_t>(i * 2 + 1) * c.B_total + c.u0) * head_block;
-    dec_cross_attn_run(h->dq.p, kl, vl, h->dctx.p, c.n_utt, c.beam, d, H, s);
-    GemvArgs co;
-    co.R = R; co.st = st; co.x = h->dctx.p; co.w = w.cow; co.bias = w.cob; co.out = h->dx.p; co.ldo = d; co.N = d;
-    co.K = d; co.epi = GV_RESID;
-    gemv_run(co, s);
-    // LN3 + MLP
-    GemvArgs f1;
-    f1.R = R; f1.st = st; f1.x = h->dx.p; f1.ln_g = w.ln3g; f1.ln_b = w.ln3b; f1.w = w.fc1w; f1.bias = w.fc1b;
-    f1.out = h->dh.p; f1.ldo = 4 * d; f1.N = 4 * d; f1.K = d; f1.epi = GV_GELU;
-    gemv_run(f1, s);
-    GemvArgs f2;
-    f2.R = R; f2.st = st; f2.x = h->dh.p; f2.w = w.fc2w; f2.bias = w.fc2b; f2.out = h->dx.p; f2.ldo = d; f2.N = d;
-    f2.K = 4 * d; f2.epi = GV_RESID;
-    gemv_run(f2, s);
-    n += 8;
-  }
-  if (with_logits) {
-    GemvArgs v;
-    v.R = R; v.st = st; v.x = h->dx.p; v.ln_g = h->F("dec.ln.g"); v.ln_b = h->F("dec.ln.b"); v.w = h->H("dec.tok_emb");
-    v.out = h->logits.p; v.ldo = dm.n_vocab_pad; v.N = dm.n_vocab; v.K = d; v.epi = GV_STORE;
-    gemv_run(v, s);
-    ++n;
-  }
-  return n;
 }
 
 void enqueue_prefill(wisb_handle* h, const DecodeCfg& c) {
@@ -946,37 +880,6 @@ void enqueue_prefill(wisb_handle* h, const DecodeCfg& c) {
 void enqueue_step(wisb_handle* h, const DecodeCfg& c) {
   enqueue_decoder_forward(h, c, true);
   search_step_run(make_search_args(h, c), h->stream);
-}
-
-DecGraphs& get_graphs(wisb_handle* h, const DecodeCfg& c) {
-  GraphKey key;
-  memset(&key, 0, sizeof(key));
-  key.n_utt = c.n_utt; key.beam = c.beam; key.prompt_len = c.prompt_len; key.max_new = c.max_new;
-  key.max_hyp = c.max_hyp; key.lp = c.lp;
-  key.u0 = c.u0; key.b_total = c.B_total;  // they move the cross-K/V base pointers baked into the graph
-  key.ts = c.ts; key.ts_max_init = c.ts ? c.ts_max_init : 0;
-  auto it = h->graphs.find(key);
-  if (it != h->graphs.end()) return it->second;
-  if (h->graphs.size() > 64) {  // bound the cache
-    for (auto& kv : h->graphs) {
-      if (kv.second.prefill) cudaGraphExecDestroy(kv.second.prefill);
-      if (kv.second.step) cudaGraphExecDestroy(kv.second.step);
-    }
-    h->graphs.clear();
-  }
-  DecGraphs g;
-  cudaGraph_t graph;
-  WISB_CUDA(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-  enqueue_prefill(h, c);
-  WISB_CUDA(cudaStreamEndCapture(h->stream, &graph));
-  WISB_CUDA(cudaGraphInstantiate(&g.prefill, graph, 0));
-  WISB_CUDA(cudaGraphDestroy(graph));
-  WISB_CUDA(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-  enqueue_step(h, c);
-  WISB_CUDA(cudaStreamEndCapture(h->stream, &graph));
-  WISB_CUDA(cudaGraphInstantiate(&g.step, graph, 0));
-  WISB_CUDA(cudaGraphDestroy(graph));
-  return h->graphs[key] = g;
 }
 
 void set_extra_suppress(wisb_handle* h, const int32_t* extra, int n_extra) {
@@ -997,48 +900,70 @@ void set_extra_suppress(wisb_handle* h, const int32_t* extra, int n_extra) {
   h->mask_extra = want;
 }
 
-// decode utterances [u0, u0 + n_utt) of the encoded batch; writes results to the host arrays
+// prompts [n_utt][prompt_len] of utterances [u0, u0 + n_utt) -> h->prompt_dev (staged through the pinned buffer, whose
+// first 4 words hold the decode loop's flags)
+void upload_prompts(wisb_handle* h, const int32_t* prompts, const DecodeCfg& c) {
+  const size_t n = static_cast<size_t>(c.n_utt) * c.prompt_len;
+  memcpy(h->pin_i.p + 4, prompts + static_cast<size_t>(c.u0) * c.prompt_len, sizeof(int) * n);
+  WISB_CUDA(cudaMemcpyAsync(h->prompt_dev.p, h->pin_i.p + 4, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
+}
+
+// best hypothesis of every utterance of the pass (search state) -> the caller's host arrays at utterance u0
+void read_results(wisb_handle* h, const DecodeCfg& c, int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score) {
+  cudaStream_t s = h->stream;
+  int* lens = h->pin_i.p + 4;
+  int* toks = lens + c.n_utt;
+  const int mn = c.max_new > 0 ? c.max_new : 1;
+  WISB_CUDA(cudaMemcpyAsync(lens, h->best_len.p, sizeof(int) * c.n_utt, cudaMemcpyDeviceToHost, s));
+  WISB_CUDA(cudaMemcpyAsync(toks, h->best_tokens.p, sizeof(int) * c.n_utt * mn, cudaMemcpyDeviceToHost, s));
+  WISB_CUDA(cudaMemcpyAsync(h->pin_f.p, h->best_score.p, sizeof(float) * c.n_utt, cudaMemcpyDeviceToHost, s));
+  WISB_CUDA(cudaStreamSynchronize(s));
+  for (int u = 0; u < c.n_utt; ++u) {
+    const int len = c.max_new > 0 ? lens[u] : 0;
+    out_len[c.u0 + u] = len;
+    for (int t = 0; t < len && t < out_stride; ++t) out_ids[static_cast<size_t>(c.u0 + u) * out_stride + t] = toks[u * mn + t];
+    if (out_score) out_score[c.u0 + u] = c.max_new > 0 ? h->pin_f.p[u] : 0.f;
+  }
+}
+
+// decode utterances [u0, u0 + n_utt) of the encoded batch with the persistent pass (<= 8 rows); writes results to the
+// host arrays
 int decode_pass(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, int32_t* out_ids, int out_stride,
                 int32_t* out_len, float* out_score) {
   cudaStream_t s = h->stream;
-  const int R = c.n_utt * c.beam;
   int steps = 0;
-  // prompts for this pass
-  memcpy(h->pin_i.p + 4, prompts + static_cast<size_t>(c.u0) * c.prompt_len, sizeof(int) * c.n_utt * c.prompt_len);
-  WISB_CUDA(cudaMemcpyAsync(h->prompt_dev.p, h->pin_i.p + 4, sizeof(int) * c.n_utt * c.prompt_len, cudaMemcpyHostToDevice, s));
+  upload_prompts(h, prompts, c);
   SearchArgs sa = make_search_args(h, c);
-  // persistent-pass path: forward the prompt prefix of all utterances in one pass when it fits the 8-row kernel
+  // forward the prompt prefix of all utterances in one pass when it fits the 8-row kernel
   const int pf_rows = c.n_utt * (c.prompt_len - 1);
-  const bool one_pass_prefill = h->decoder_mega && c.prompt_len > 1 && pf_rows <= DEC_MAX_ROWS && c.prompt_len - 1 <= MAX_BEAM;
+  const bool one_pass_prefill = c.prompt_len > 1 && pf_rows <= DEC_MAX_ROWS && c.prompt_len - 1 <= MAX_BEAM;
   search_init_run(sa, h->prompt_dev.p, s, one_pass_prefill ? 1 : 0);
-  if (h->decoder_mega) upload_mega_layers(h, c);
+  upload_mega_layers(h, c);
   if (c.max_new > 0) {
-    // the persistent pass kernel is a handful of launches per step: no graph needed (and it is a cooperative launch)
-    DecGraphs* g = (h->use_graphs && !h->decoder_mega) ? &get_graphs(h, c) : nullptr;
+    // the persistent pass is one cooperative launch per step: no graph needed
     if (one_pass_prefill) {
-      enqueue_decoder_forward_mega(h, c, false, true);
+      enqueue_decoder_forward(h, c, false, true);
       ++steps;
     } else {
       for (int p = 0; p + 1 < c.prompt_len; ++p) {
-        if (g) WISB_CUDA(cudaGraphLaunch(g->prefill, s)); else enqueue_prefill(h, c);
+        enqueue_prefill(h, c);
         ++steps;
       }
     }
-    const int fwd = h->decoder_mega ? 1 : 1 + 8 * h->dims.n_dec_layers + 1;
-    const int per_step = fwd + 2;
-    h->launches += (c.prompt_len - 1) * (fwd + 1);
+    const int per_step = 1 + 2;  // the pass + the two kernels of the search step
+    h->launches += (c.prompt_len - 1) * 2;
     volatile int* flag = h->pin_i.p;
     flag[0] = flag[1] = 0;
-    // persistent-pass path with a poll every step: step gs + 1 is enqueued BEFORE the host waits for step gs's `all_done`
-    // word (the kernels of a step that turns out to be superfluous leave at once on the device flag), so neither the
-    // launch latency of the cooperative kernel nor the host's wake-up sits between two steps
-    const bool ahead = h->decoder_mega && h->decode_poll == 1;
+    // with a poll every step, step gs + 1 is enqueued BEFORE the host waits for step gs's `all_done` word (the kernels of
+    // a step that turns out to be superfluous leave at once on the device flag), so neither the launch latency of the
+    // cooperative kernel nor the host's wake-up sits between two steps
+    const bool ahead = h->decode_poll == 1;
     if (ahead && h->ev_flag[0] == nullptr) {
       WISB_CUDA(cudaEventCreateWithFlags(&h->ev_flag[0], cudaEventDisableTiming));
       WISB_CUDA(cudaEventCreateWithFlags(&h->ev_flag[1], cudaEventDisableTiming));
     }
     for (int gs = 0; gs < c.max_new; ++gs) {
-      if (g) WISB_CUDA(cudaGraphLaunch(g->step, s)); else enqueue_step(h, c);
+      enqueue_step(h, c);
       ++steps;
       h->launches += per_step;
       if (ahead) {
@@ -1061,20 +986,7 @@ int decode_pass(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, int3
       }
     }
   }
-  // results
-  int* lens = h->pin_i.p + 4;
-  int* toks = lens + DEC_MAX_ROWS;
-  WISB_CUDA(cudaMemcpyAsync(lens, h->best_len.p, sizeof(int) * c.n_utt, cudaMemcpyDeviceToHost, s));
-  WISB_CUDA(cudaMemcpyAsync(toks, h->best_tokens.p, sizeof(int) * c.n_utt * (c.max_new > 0 ? c.max_new : 1), cudaMemcpyDeviceToHost, s));
-  WISB_CUDA(cudaMemcpyAsync(h->pin_f.p, h->best_score.p, sizeof(float) * c.n_utt, cudaMemcpyDeviceToHost, s));
-  WISB_CUDA(cudaStreamSynchronize(s));
-  for (int u = 0; u < c.n_utt; ++u) {
-    const int len = c.max_new > 0 ? lens[u] : 0;
-    out_len[c.u0 + u] = len;
-    for (int t = 0; t < len && t < out_stride; ++t) out_ids[static_cast<size_t>(c.u0 + u) * out_stride + t] = toks[u * c.max_new + t];
-    if (out_score) out_score[c.u0 + u] = c.max_new > 0 ? h->pin_f.p[u] : 0.f;
-  }
-  (void)R;
+  read_results(h, c, out_ids, out_stride, out_len, out_score);
   return steps;
 }
 
@@ -1249,10 +1161,8 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
     h->bd_layers[i].cv = h->ckv.p + (static_cast<size_t>(i * 2 + 1) * c.B_total + c.u0) * head_block;
   }
   int steps = 0;
-  int* pin = h->pin_i.p + 4;
-  memcpy(pin, prompts + static_cast<size_t>(c.u0) * c.prompt_len, sizeof(int) * c.n_utt * c.prompt_len);
-  WISB_CUDA(cudaMemcpyAsync(h->prompt_dev.p, pin, sizeof(int) * c.n_utt * c.prompt_len, cudaMemcpyHostToDevice, s));
-  int* pin_mx = pin + static_cast<size_t>(c.n_utt) * c.prompt_len;
+  upload_prompts(h, prompts, c);
+  int* pin_mx = h->pin_i.p + 4 + static_cast<size_t>(c.n_utt) * c.prompt_len;
   if (c.per_utt_max_new) {
     memcpy(pin_mx, max_new_host, sizeof(int) * c.n_utt);
     WISB_CUDA(cudaMemcpyAsync(h->max_new_u.p, pin_mx, sizeof(int) * c.n_utt, cudaMemcpyHostToDevice, s));
@@ -1276,32 +1186,32 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
     }
     SearchArgs sa = make_batch_search_args(h, c);
     search_init_run(sa, h->prompt_dev.p, s, 1);
-    DecGraphs* g = nullptr;
+    cudaGraphExec_t g = nullptr;
     if (h->use_graphs && !h->profile) {  // (the per-kernel timing hook needs eager launches)
       GraphKey key;
       memset(&key, 0, sizeof(key));
       key.n_utt = c.n_utt; key.beam = c.beam; key.prompt_len = c.prompt_len; key.max_new = c.max_new;
       key.max_hyp = c.max_hyp; key.lp = c.lp; key.u0 = c.u0; key.b_total = c.B_total;
-      key.batched = 1 + c.per_utt_max_new;
+      key.per_utt_max_new = c.per_utt_max_new;
       key.ts = c.ts; key.ts_max_init = c.ts ? c.ts_max_init : 0;
       auto it = h->graphs.find(key);
       if (it == h->graphs.end()) {
         if (h->graphs.size() > 64) drop_graphs(h);
-        DecGraphs ng;
         cudaGraph_t graph;
+        cudaGraphExec_t exec;
         WISB_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
         enqueue_batch_step(h, c);
         WISB_CUDA(cudaStreamEndCapture(s, &graph));
-        WISB_CUDA(cudaGraphInstantiate(&ng.step, graph, 0));
+        WISB_CUDA(cudaGraphInstantiate(&exec, graph, 0));
         WISB_CUDA(cudaGraphDestroy(graph));
-        it = h->graphs.emplace(key, ng).first;
+        it = h->graphs.emplace(key, exec).first;
       }
-      g = &it->second;
+      g = it->second;
     }
     volatile int* flag = h->pin_i.p;
     *flag = 0;
     for (int gs = 0; gs < c.max_new; ++gs) {
-      if (g) WISB_CUDA(cudaGraphLaunch(g->step, s)); else enqueue_batch_step(h, c);
+      if (g) WISB_CUDA(cudaGraphLaunch(g, s)); else enqueue_batch_step(h, c);
       ++steps;
       h->launches += h->bd_launches_step;
       const bool poll = ((gs + 1) % h->decode_poll == 0) || gs + 1 == c.max_new;
@@ -1312,20 +1222,7 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
       }
     }
   }
-  // results
-  int* lens = h->pin_i.p + 4;
-  int* toks = lens + c.n_utt;
-  const int mn = c.max_new > 0 ? c.max_new : 1;
-  WISB_CUDA(cudaMemcpyAsync(lens, h->best_len.p, sizeof(int) * c.n_utt, cudaMemcpyDeviceToHost, s));
-  WISB_CUDA(cudaMemcpyAsync(toks, h->best_tokens.p, sizeof(int) * c.n_utt * mn, cudaMemcpyDeviceToHost, s));
-  WISB_CUDA(cudaMemcpyAsync(h->pin_f.p, h->best_score.p, sizeof(float) * c.n_utt, cudaMemcpyDeviceToHost, s));
-  WISB_CUDA(cudaStreamSynchronize(s));
-  for (int u = 0; u < c.n_utt; ++u) {
-    const int len = c.max_new > 0 ? lens[u] : 0;
-    out_len[c.u0 + u] = len;
-    for (int t = 0; t < len && t < out_stride; ++t) out_ids[static_cast<size_t>(c.u0 + u) * out_stride + t] = toks[u * mn + t];
-    if (out_score) out_score[c.u0 + u] = c.max_new > 0 ? h->pin_f.p[u] : 0.f;
-  }
+  read_results(h, c, out_ids, out_stride, out_len, out_score);
   return steps;
 }
 
@@ -1586,10 +1483,7 @@ int wisb_destroy(wisb_handle* h) {
   if (h == nullptr) return 0;
   cudaSetDevice(h->device);
   if (h->stream) cudaStreamSynchronize(h->stream);
-  for (auto& kv : h->graphs) {
-    if (kv.second.prefill) cudaGraphExecDestroy(kv.second.prefill);
-    if (kv.second.step) cudaGraphExecDestroy(kv.second.step);
-  }
+  drop_graphs(h);
   for (auto& e : h->ev)
     if (e) cudaEventDestroy(e);
   for (auto& e : h->prof_ev) cudaEventDestroy(e);
@@ -1617,7 +1511,6 @@ int wisb_set_option(wisb_handle* h, const char* key, int value) {
     else if (k == "attn_ref") h->attn_ref = value;
     else if (k == "decode_poll") h->decode_poll = value < 1 ? 1 : value;
     else if (k == "profile") h->profile = value;
-    else if (k == "decoder_mega") h->decoder_mega = value;
     else if (k == "encoder_cache") {
       h->encoder_cache = value ? 1 : 0;
       h->enc_valid = false;
@@ -1833,7 +1726,7 @@ int wisb_detect_language(wisb_handle* h, const float* mel, int B, int32_t* lang_
     WISB_REQUIRE(lang_ids_out != nullptr && probs_out != nullptr, "output pointer is NULL");
     cudaStream_t s = h->stream;
     bool reuse = upload_mel(h, mel, B);
-    h->ckv_sw = (h->decoder_mega && h->mega_tc) ? 1 : 0;  // language detection always runs the <= 8-row pass
+    h->ckv_sw = h->mega_tc;  // language detection always runs the <= 8-row pass
     if (reuse && h->ckv_is_sw != h->ckv_sw) reuse = false;
     encode_for_decode(h, B, reuse);
     const int nl = dm.n_langs;
@@ -1842,7 +1735,7 @@ int wisb_detect_language(wisb_handle* h, const float* mel, int B, int32_t* lang_
     for (int i = 0; i < nl; ++i) ids[i] = dm.lang_first + i;
     WISB_CUDA(cudaMemcpyAsync(h->lang_ids.p, ids.data(), sizeof(int) * nl, cudaMemcpyHostToDevice, s));
     WISB_CUDA(cudaStreamSynchronize(s));
-    std::vector<int32_t> sot(DEC_MAX_ROWS, dm.sot);
+    const std::vector<int32_t> sot(B, dm.sot);
     for (int u0 = 0; u0 < B; u0 += DEC_MAX_ROWS) {
       DecodeCfg c;
       c.u0 = u0;
@@ -1853,10 +1746,9 @@ int wisb_detect_language(wisb_handle* h, const float* mel, int B, int32_t* lang_
       c.max_new = 1;
       c.max_hyp = 1;
       c.lp = 1.f;
-      memcpy(h->pin_i.p + 4, sot.data(), sizeof(int) * c.n_utt);
-      WISB_CUDA(cudaMemcpyAsync(h->prompt_dev.p, h->pin_i.p + 4, sizeof(int) * c.n_utt, cudaMemcpyHostToDevice, s));
+      upload_prompts(h, sot.data(), c);
       search_init_run(make_search_args(h, c), h->prompt_dev.p, s);
-      if (h->decoder_mega) upload_mega_layers(h, c);
+      upload_mega_layers(h, c);
       enqueue_decoder_forward(h, c, true);
       lang_probs_run(h->logits.p, dm.n_vocab_pad, h->lang_ids.p, nl, c.n_utt, 1, h->lang_probs.p, s);
       WISB_CUDA(cudaMemcpyAsync(h->pin_f.p, h->lang_probs.p, sizeof(float) * c.n_utt * nl, cudaMemcpyDeviceToHost, s));
@@ -2417,27 +2309,6 @@ int wisb_debug_dec_embed_ln(wisb_handle* h, int R, int cap, int d, int n_vocab, 
   });
 }
 
-int wisb_debug_gemv_tc(wisb_handle* h, const float* x, const uint16_t* w, const float* bias, float* out, int R, int N, int K,
-                       int iters, float* avg_us) {
-  return guarded(h, [&] {
-    WISB_REQUIRE(x && w && out, "NULL pointer");
-    cudaStream_t s = h->stream;
-    DevBuf<float> dx, db, dout;
-    DevBuf<__half> dw;
-    dx.ensure(static_cast<size_t>(R) * K);
-    dw.ensure(static_cast<size_t>(N) * K);
-    db.ensure(static_cast<size_t>(N));
-    dout.ensure(static_cast<size_t>(R) * N, true);
-    WISB_CUDA(cudaMemcpyAsync(dx.p, x, sizeof(float) * R * K, cudaMemcpyHostToDevice, s));
-    WISB_CUDA(cudaMemcpyAsync(dw.p, w, sizeof(__half) * static_cast<size_t>(N) * K, cudaMemcpyHostToDevice, s));
-    if (bias) WISB_CUDA(cudaMemcpyAsync(db.p, bias, sizeof(float) * N, cudaMemcpyHostToDevice, s));
-    const float us = gemv_tc_debug_run(dx.p, dw.p, bias ? db.p : nullptr, dout.p, R, N, K, h->num_sms, iters, s);
-    if (avg_us) *avg_us = us;
-    WISB_CUDA(cudaMemcpyAsync(out, dout.p, sizeof(float) * R * N, cudaMemcpyDeviceToHost, s));
-    WISB_CUDA(cudaStreamSynchronize(s));
-  });
-}
-
 int wisb_debug_read_trace(wisb_handle* h, unsigned long long* out, int n) {
   return guarded(h, [&] {
     WISB_REQUIRE(out != nullptr && n > 0 && n <= 2048 + 160 * 264, "trace: at most 2048 + 160 * 264 words");
@@ -2473,8 +2344,7 @@ int wisb_debug_forced_logits(wisb_handle* h, const float* mel, const int32_t* to
     run_encoder(h, 1, -1, true);
     DecodeCfg c;
     c.u0 = 0; c.n_utt = 1; c.B_total = 1; c.beam = 1; c.prompt_len = n_tokens; c.max_new = 1; c.max_hyp = 1; c.lp = 1.f;
-    memcpy(h->pin_i.p + 4, tokens, sizeof(int) * n_tokens);
-    WISB_CUDA(cudaMemcpyAsync(h->prompt_dev.p, h->pin_i.p + 4, sizeof(int) * n_tokens, cudaMemcpyHostToDevice, s));
+    upload_prompts(h, tokens, c);
     if (h->decoder_batch == 2) {  // the batched pass, one row: position p of the token list per pass
       ensure_batch(h, MAX_BEAM, n_tokens);
       const size_t head_block = static_cast<size_t>(dm.n_heads) * T_ENC_PAD * HEAD_DIM;
@@ -2501,7 +2371,7 @@ int wisb_debug_forced_logits(wisb_handle* h, const float* mel, const int32_t* to
       return;
     }
     search_init_run(make_search_args(h, c), h->prompt_dev.p, s);
-    if (h->decoder_mega) upload_mega_layers(h, c);
+    upload_mega_layers(h, c);
     for (int p = 0; p < n_tokens; ++p) {
       enqueue_decoder_forward(h, c, true);
       WISB_CUDA(cudaMemcpyAsync(logits_out + static_cast<size_t>(p) * dm.n_vocab, h->logits.p, sizeof(float) * dm.n_vocab, cudaMemcpyDeviceToHost, s));
