@@ -109,12 +109,13 @@ int wisb_align(wisb_handle* h, const float* mel, int B, const int32_t* start_seq
  *  8 sum of GEMM kernels, 9 attention kernels, 10 LayerNorm kernels, 11 conv1, 12 number of GEMM launches, 13-15 0]
  * entries 8-12 are filled only with option "profile" = 1 (per-kernel event pairs; leave it off for timed runs). */
 int wisb_get_timing(wisb_handle* h, float* out16);
-/* options: "use_graphs" (default 1), "attn_v_mn_major" (default 1), "attn_ref" (0), "decode_poll" (1), "profile" (0),
+/* options: "use_graphs" (default 1), "attn_v_mn_major" (default 1), "attn_ref" (0), "profile" (0),
  * "mega_mma" (for calls of <= 8 rows: 1, the default where d_model <= 1280, the warp-MMA persistent decoder pass; 0 the
  * SIMT persistent pass, fp32 arithmetic, the only one for d_model > 1280),
- * "encoder_cache" (default 0; 1: consecutive wisb_detect_language / wisb_generate calls on byte-identical host features
- * of <= 2 windows reuse the encoder output and cross K/V already in HBM -- the detect -> transcribe -> translate sequence
- * of main.py:633-644, 514-547 then encodes once instead of three times) */
+ * "encoder_cache" (default 0; 1: consecutive wisb_detect_language / wisb_generate / wisb_align calls on byte-identical
+ * host features of <= 2 windows reuse the encoder output and cross K/V already in HBM when the call encodes all its
+ * windows in one group -- the detect -> transcribe -> translate sequence of main.py:633-644, 514-547 then encodes once
+ * instead of three times; cached cross K/V in the other decoder pass's layout is rewritten by the cross-K/V GEMM alone) */
 int wisb_set_option(wisb_handle* h, const char* key, int value);
 
 /* ---- diagnostics used by tests/ (run the product kernels on caller data) ---- */

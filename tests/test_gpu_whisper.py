@@ -12,7 +12,7 @@ import torch
 
 from oracle.whisper_ref import WhisperOracle
 from tests.gpu_common import LOGIT_TOL, PROMPT, make_blob, mel_inputs, model_pair, robust_cases
-from willow_inference_server_b200 import models
+from willow_inference_server_b200 import _lib, models
 
 pytestmark = pytest.mark.gpu
 ENC_TOL = 3e-2
@@ -253,6 +253,43 @@ def test_encoder_cache_detect_then_generate(pair):
         assert again == want and m2.timing()["encoder_ms"] > 0.05   # different features in between: re-encoded
     finally:
         h.set_option("encoder_cache", 0)
+
+
+def test_encoder_cache_needs_one_group(pair):
+    # a cache that holds two windows encoded as one batch must not serve a call that decodes them in two groups: each
+    # group would read the cross K/V at the offsets of a batch of one, and the second group would read the first window's
+    dims = pair[0]
+    mel = np.ascontiguousarray(mel_inputs(4)[:2])
+    prompts = np.asarray([PROMPT] * 2, np.int32)
+    plain = _lib.Handle.from_host(make_blob(dims), 0)
+    plain.set_option("batch_rows", 8)
+    want = plain.generate(mel, prompts, beam_size=5)
+    h = _lib.Handle.from_host(make_blob(dims), 0)
+    h.set_option("encoder_cache", 1)
+    h.generate(mel, prompts, beam_size=5)  # 10 rows, one group of 2 windows: the cache now holds both
+    h.set_option("batch_rows", 8)          # 8 // 5 = 1 window per group
+    assert h.generate(mel, prompts, beam_size=5) == want
+    assert h.timing()["launches"] == plain.timing()["launches"]  # both groups were encoded again
+
+
+def test_encoder_cache_layout_rerun(pair):
+    # detect_language leaves the cross K/V chunk-swizzled (<= 8 rows: the warp-MMA persistent pass); a generate at beam 5
+    # on the same 2 windows (10 rows: the batched pass) reads it linear and reruns only the cross-K/V GEMM
+    dims = pair[0]
+    mel = np.ascontiguousarray(mel_inputs(4)[:2])
+    prompts = np.asarray([PROMPT] * 2, np.int32)
+    plain = _lib.Handle.from_host(make_blob(dims), 0)
+    want = plain.generate(mel, prompts, beam_size=5)
+    t_plain = plain.timing()
+    h = _lib.Handle.from_host(make_blob(dims), 0)
+    h.set_option("encoder_cache", 1)
+    h.detect_language(mel)
+    got = h.generate(mel, prompts, beam_size=5)
+    t = h.timing()
+    assert got == want
+    assert t["decode_steps"] == t_plain["decode_steps"]
+    # no encoder: conv1, conv2, 7 per layer, ln_post are gone; the cross-K/V GEMM reran once (linear layout)
+    assert t["launches"] == t_plain["launches"] - (3 + 7 * dims.n_enc_layers)
 
 
 def test_batcher_over_the_real_engine(pair):

@@ -106,7 +106,7 @@ struct wisb_handle {
   std::map<std::string, TensorRef> tensors;
   std::vector<DecLayerW> dec_w;
   // options
-  int use_graphs = 1, attn_v_mn = 1, attn_ref = 0, decode_poll = 1;
+  int use_graphs = 1, attn_v_mn = 1, attn_ref = 0;
   // front end
   DevBuf<float> lm_tables;
   DevBuf<unsigned> lm_max;
@@ -156,7 +156,7 @@ struct wisb_handle {
   std::vector<float> mel_cache;
   int mel_cache_B = 0;
   bool enc_valid = false;
-  int ckv_sw = 0, ckv_is_sw = 0;  // cross K/V layout wanted by the decoder pass of this call / layout of what is in HBM
+  int ckv_is_sw = 0;  // layout of the cross K/V in HBM (1: chunk-swizzled, see ckv_layout)
   DevBuf<float> cross_part;
   DevBuf<unsigned> cross_flags;
   DevBuf<float> ln_fold;       // per LN-GEMV: s2[N] and folded bias[N] (qkv, cq, fc1 of every decoder layer, vocab)
@@ -591,14 +591,20 @@ void ensure_encoder(wisb_handle* h, int B) {
   h->plans_vmn = h->attn_v_mn;
 }
 
-// the persistent warp-MMA pass (<= 8 rows) reads the cross K/V rows chunk-swizzled (ldmatrix without bank conflicts); every
-// other decoder path reads them linear
-bool want_ckv_swizzle(const wisb_handle* h, int rows) {
-  return rows <= DEC_MAX_ROWS && h->decoder_batch != 2 && h->mega_tc;
+// decoder pass of a call on `rows` rows (utterances x beams): the persistent pass for <= 8 rows unless option
+// "decoder_batch" = 2 forces the batched pass
+bool use_persistent_pass(const wisb_handle* h, int rows) {
+  return rows <= DEC_MAX_ROWS && h->decoder_batch != 2;
 }
 
-// mel (device, [B,80,3000]) -> enc_out fp16 [B*1536, d] (+ cross K/V when with_ckv)
-void run_encoder(wisb_handle* h, int B, int n_layers, bool with_ckv, int mel_first = 0) {
+// cross-K/V layout the decoder pass reads: chunk-swizzled (1) for the persistent warp-MMA pass (ldmatrix without bank
+// conflicts), linear (0) for the SIMT persistent pass, the batched pass and the alignment capture
+int ckv_layout(const wisb_handle* h, bool persistent_pass) {
+  return persistent_pass && h->mega_tc ? 1 : 0;
+}
+
+// mel (device, [B,80,3000]) -> enc_out fp16 [B*1536, d]
+void run_encoder(wisb_handle* h, int B, int n_layers, int mel_first = 0) {
   const Dims& dm = h->dims;
   const int d = dm.d_model;
   const int M = B * T_ENC_PAD;
@@ -644,15 +650,6 @@ void run_encoder(wisb_handle* h, int B, int n_layers, bool with_ckv, int mel_fir
   layernorm_f32_to_f16_run(h->x.p, h->F("enc.ln_post.g"), h->F("enc.ln_post.b"), h->enc_out.p, M, d, s, h->enc_pdl != 0);
   h->prof_end();
   h->launches += 2 + 7 * nl + 1;
-  if (with_ckv) {
-    WISB_CUDA(cudaEventRecord(h->ev[3], s));
-    h->prof_begin(0);
-    h->plan_ckv.epi.kv_swizzle = h->ckv_sw;
-    gemm_run(h->plan_ckv, s);
-    h->ckv_is_sw = h->ckv_sw;
-    h->prof_end();
-    h->launches += 1;
-  }
 }
 
 // Places the features of this call in h->mel.  Returns true when the encoder output and cross K/V already in HBM belong
@@ -680,14 +677,51 @@ bool upload_mel(wisb_handle* h, const float* mel, int B) {
   return false;
 }
 
-// encoder + cross K/V for the features placed by upload_mel, unless they are already there
-void encode_for_decode(wisb_handle* h, int B, bool reuse) {
-  if (reuse) {
-    WISB_CUDA(cudaEventRecord(h->ev[3], h->stream));  // keeps the stage timings well defined (both read ~0)
-    return;
+// Encoder stage of a call on the B windows placed by upload_mel: leaves the encoder output and the cross K/V of windows
+// [g0, g0 + n) in HBM, the cross K/V in layout `ckv_sw` (ckv_layout).  What is already there is reused only when
+// upload_mel reported a hit (`cached`) and this group is the whole call (the cache holds a batch of B windows); cached
+// cross K/V in the other layout is rewritten by the cross-K/V GEMM alone.  Records the stage events ev[2] (start), ev[3]
+// (encoder done) and ev[4] (cross K/V done).
+void encode_stage(wisb_handle* h, bool cached, int B, int g0, int n, int ckv_sw) {
+  cudaStream_t s = h->stream;
+  const bool reuse = cached && n == B;
+  WISB_CUDA(cudaEventRecord(h->ev[2], s));
+  if (!reuse) run_encoder(h, n, -1, g0);
+  WISB_CUDA(cudaEventRecord(h->ev[3], s));
+  if (!reuse || h->ckv_is_sw != ckv_sw) {
+    ensure_encoder(h, n);
+    h->prof_begin(0);
+    h->plan_ckv.epi.kv_swizzle = ckv_sw;
+    gemm_run(h->plan_ckv, s);
+    h->prof_end();
+    h->ckv_is_sw = ckv_sw;
+    h->launches += 1;
   }
-  run_encoder(h, B, -1, true);
-  h->enc_valid = h->encoder_cache != 0 && h->mel_cache_B == B;
+  if (!reuse) h->enc_valid = h->encoder_cache != 0 && h->mel_cache_B == B && n == B;
+  WISB_CUDA(cudaEventRecord(h->ev[4], s));
+}
+
+// Stage timings of wisb_generate / wisb_align (slots as documented in wisb200.h).  ev[0] opens the call, ev[1] closes its
+// host-to-device stage, and ev[2], ev[3], ... delimit the stages of one group of utterances (encode_stage records ev[2]
+// to ev[4], the caller the rest).
+void time_h2d(wisb_handle* h) {
+  WISB_CUDA(cudaEventRecord(h->ev[1], h->stream));
+  WISB_CUDA(cudaEventSynchronize(h->ev[1]));
+  WISB_CUDA(cudaEventElapsedTime(&h->timing[1], h->ev[0], h->ev[1]));
+}
+
+// after the last stage of a group: adds the time from ev[2 + k] to ev[3 + k] to timing[slots[k]] and sets timing[5], the
+// call's total so far (ev[0] to the group's last event)
+void time_group(wisb_handle* h, std::initializer_list<int> slots) {
+  const cudaEvent_t* e = h->ev + 2;
+  WISB_CUDA(cudaEventSynchronize(e[slots.size()]));
+  for (int slot : slots) {
+    float t;
+    WISB_CUDA(cudaEventElapsedTime(&t, e[0], e[1]));
+    h->timing[slot] += t;
+    ++e;
+  }
+  WISB_CUDA(cudaEventElapsedTime(&h->timing[5], h->ev[0], *e));
 }
 
 struct DecodeCfg {
@@ -745,12 +779,20 @@ SearchArgs make_search_args(wisb_handle* h, const DecodeCfg& c) {
   return a;
 }
 
+// points a layer descriptor (MegaLayer / BatchLayer) at the cross K and V of decoder layer `layer` for utterance u0 of a
+// batch of B_total encoded windows (h->ckv: [layer][K | V][B_total][H][1536][64])
+template <typename Layer>
+void bind_cross_kv(const wisb_handle* h, Layer& l, int layer, int u0, int B_total) {
+  const size_t head_block = static_cast<size_t>(h->dims.n_heads) * T_ENC_PAD * HEAD_DIM;
+  l.ck = h->ckv.p + (static_cast<size_t>(layer * 2 + 0) * B_total + u0) * head_block;
+  l.cv = h->ckv.p + (static_cast<size_t>(layer * 2 + 1) * B_total + u0) * head_block;
+}
+
 // descriptors of the persistent decoder pass for this batch slice (device array of per-layer pointers)
 void upload_mega_layers(wisb_handle* h, const DecodeCfg& c) {
   const Dims& dm = h->dims;
-  const int d = dm.d_model, H = dm.n_heads;
+  const int d = dm.d_model;
   const size_t layer_cache = static_cast<size_t>(DEC_MAX_ROWS) * T_MAX * d;
-  const size_t head_block = static_cast<size_t>(H) * T_ENC_PAD * HEAD_DIM;
   for (int i = 0; i < dm.n_dec_layers; ++i) {
     const DecLayerW& w = h->dec_w[i];
     MegaLayer& m = h->mega_layers_host.p[i];
@@ -792,9 +834,7 @@ void upload_mega_layers(wisb_handle* h, const DecodeCfg& c) {
       m.fc1.w = img + 6 * dd * dd;
       m.fc2.w = img + 10 * dd * dd;
     }
-    const int ikv = (h->mega_dbg & 1) ? 0 : i;
-    m.ck = h->ckv.p + (static_cast<size_t>(ikv * 2 + 0) * c.B_total + c.u0) * head_block;
-    m.cv = h->ckv.p + (static_cast<size_t>(ikv * 2 + 1) * c.B_total + c.u0) * head_block;
+    bind_cross_kv(h, m, (h->mega_dbg & 1) ? 0 : i, c.u0, c.B_total);
     m.kcache = h->kcache.p + i * layer_cache;
     m.vcache = h->vcache.p + i * layer_cache;
   }
@@ -900,12 +940,19 @@ void set_extra_suppress(wisb_handle* h, const int32_t* extra, int n_extra) {
   h->mask_extra = want;
 }
 
-// prompts [n_utt][prompt_len] of utterances [u0, u0 + n_utt) -> h->prompt_dev (staged through the pinned buffer, whose
-// first 4 words hold the decode loop's flags)
-void upload_prompts(wisb_handle* h, const int32_t* prompts, const DecodeCfg& c) {
+// prompts [n_utt][prompt_len] of utterances [u0, u0 + n_utt) -> h->prompt_dev and, when c.per_utt_max_new, their caps on
+// new tokens (max_new_host[u0 + u]) -> h->max_new_u.  Both are staged through the pinned buffer, whose first 4 words hold
+// the step loop's flags: the host may rewrite it only after the stream sync that ends the previous group, because these
+// asynchronous copies read from it.
+void upload_prompts(wisb_handle* h, const int32_t* prompts, const int* max_new_host, const DecodeCfg& c) {
   const size_t n = static_cast<size_t>(c.n_utt) * c.prompt_len;
-  memcpy(h->pin_i.p + 4, prompts + static_cast<size_t>(c.u0) * c.prompt_len, sizeof(int) * n);
-  WISB_CUDA(cudaMemcpyAsync(h->prompt_dev.p, h->pin_i.p + 4, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
+  int* pin = h->pin_i.p + 4;
+  memcpy(pin, prompts + static_cast<size_t>(c.u0) * c.prompt_len, sizeof(int) * n);
+  WISB_CUDA(cudaMemcpyAsync(h->prompt_dev.p, pin, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
+  if (c.per_utt_max_new) {
+    memcpy(pin + n, max_new_host + c.u0, sizeof(int) * c.n_utt);
+    WISB_CUDA(cudaMemcpyAsync(h->max_new_u.p, pin + n, sizeof(int) * c.n_utt, cudaMemcpyHostToDevice, h->stream));
+  }
 }
 
 // best hypothesis of every utterance of the pass (search state) -> the caller's host arrays at utterance u0
@@ -926,19 +973,58 @@ void read_results(wisb_handle* h, const DecodeCfg& c, int32_t* out_ids, int out_
   }
 }
 
+// setup of the persistent pass for this batch slice: prompts (and caps), search state, layer descriptors
+void persistent_setup(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, const int* max_new_host,
+                      int shared_prefix = 0) {
+  upload_prompts(h, prompts, max_new_host, c);
+  search_init_run(make_search_args(h, c), h->prompt_dev.p, h->stream, shared_prefix);
+  upload_mega_layers(h, c);
+}
+
+// Generated-token loop of both decoder passes: enqueue() issues one step and returns its kernel launches; the loop ends at
+// the first step whose `all_done` word reads 1.  With look_ahead (the persistent pass) step gs + 1 is enqueued BEFORE the
+// host waits for step gs's word (the kernels of a step that turns out to be superfluous leave at once on the device flag),
+// so neither the launch latency of the cooperative kernel nor the host's wake-up sits between two steps.  The batched
+// pass polls after every step instead: its GEMMs do not exit early.  Returns the steps that did work.
+int step_loop(wisb_handle* h, int max_new, bool look_ahead, const std::function<int()>& enqueue) {
+  cudaStream_t s = h->stream;
+  volatile int* flag = h->pin_i.p;
+  flag[0] = flag[1] = 0;
+  if (look_ahead && h->ev_flag[0] == nullptr) {
+    WISB_CUDA(cudaEventCreateWithFlags(&h->ev_flag[0], cudaEventDisableTiming));
+    WISB_CUDA(cudaEventCreateWithFlags(&h->ev_flag[1], cudaEventDisableTiming));
+  }
+  int steps = 0;
+  for (int gs = 0; gs < max_new; ++gs) {
+    h->launches += enqueue();
+    ++steps;
+    WISB_CUDA(cudaMemcpyAsync(const_cast<int*>(flag) + (gs & 1), &h->st.p->all_done, sizeof(int), cudaMemcpyDeviceToHost, s));
+    if (!look_ahead) {
+      WISB_CUDA(cudaStreamSynchronize(s));
+      if (flag[gs & 1]) break;
+      continue;
+    }
+    WISB_CUDA(cudaEventRecord(h->ev_flag[gs & 1], s));
+    if (gs >= 1) {
+      WISB_CUDA(cudaEventSynchronize(h->ev_flag[(gs - 1) & 1]));
+      if (flag[(gs - 1) & 1]) {
+        --steps;  // the step just enqueued does nothing
+        break;
+      }
+    }
+  }
+  return steps;
+}
+
 // decode utterances [u0, u0 + n_utt) of the encoded batch with the persistent pass (<= 8 rows); writes results to the
 // host arrays
-int decode_pass(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, int32_t* out_ids, int out_stride,
-                int32_t* out_len, float* out_score) {
-  cudaStream_t s = h->stream;
+int decode_pass(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, const int* max_new_host, int32_t* out_ids,
+                int out_stride, int32_t* out_len, float* out_score) {
   int steps = 0;
-  upload_prompts(h, prompts, c);
-  SearchArgs sa = make_search_args(h, c);
   // forward the prompt prefix of all utterances in one pass when it fits the 8-row kernel
   const int pf_rows = c.n_utt * (c.prompt_len - 1);
   const bool one_pass_prefill = c.prompt_len > 1 && pf_rows <= DEC_MAX_ROWS && c.prompt_len - 1 <= MAX_BEAM;
-  search_init_run(sa, h->prompt_dev.p, s, one_pass_prefill ? 1 : 0);
-  upload_mega_layers(h, c);
+  persistent_setup(h, c, prompts, max_new_host, one_pass_prefill ? 1 : 0);
   if (c.max_new > 0) {
     // the persistent pass is one cooperative launch per step: no graph needed
     if (one_pass_prefill) {
@@ -950,41 +1036,11 @@ int decode_pass(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, int3
         ++steps;
       }
     }
-    const int per_step = 1 + 2;  // the pass + the two kernels of the search step
     h->launches += (c.prompt_len - 1) * 2;
-    volatile int* flag = h->pin_i.p;
-    flag[0] = flag[1] = 0;
-    // with a poll every step, step gs + 1 is enqueued BEFORE the host waits for step gs's `all_done` word (the kernels of
-    // a step that turns out to be superfluous leave at once on the device flag), so neither the launch latency of the
-    // cooperative kernel nor the host's wake-up sits between two steps
-    const bool ahead = h->decode_poll == 1;
-    if (ahead && h->ev_flag[0] == nullptr) {
-      WISB_CUDA(cudaEventCreateWithFlags(&h->ev_flag[0], cudaEventDisableTiming));
-      WISB_CUDA(cudaEventCreateWithFlags(&h->ev_flag[1], cudaEventDisableTiming));
-    }
-    for (int gs = 0; gs < c.max_new; ++gs) {
+    steps += step_loop(h, c.max_new, true, [&] {
       enqueue_step(h, c);
-      ++steps;
-      h->launches += per_step;
-      if (ahead) {
-        WISB_CUDA(cudaMemcpyAsync(const_cast<int*>(flag) + (gs & 1), &h->st.p->all_done, sizeof(int), cudaMemcpyDeviceToHost, s));
-        WISB_CUDA(cudaEventRecord(h->ev_flag[gs & 1], s));
-        if (gs >= 1) {
-          WISB_CUDA(cudaEventSynchronize(h->ev_flag[(gs - 1) & 1]));
-          if (flag[(gs - 1) & 1]) {
-            --steps;  // the step just enqueued does nothing
-            break;
-          }
-        }
-        continue;
-      }
-      const bool poll = ((gs + 1) % h->decode_poll == 0) || gs + 1 == c.max_new;
-      if (poll) {
-        WISB_CUDA(cudaMemcpyAsync(const_cast<int*>(flag), &h->st.p->all_done, sizeof(int), cudaMemcpyDeviceToHost, s));
-        WISB_CUDA(cudaStreamSynchronize(s));
-        if (*flag) break;
-      }
-    }
+      return 1 + 2;  // the pass + the two kernels of the search step
+    });
   }
   read_results(h, c, out_ids, out_stride, out_len, out_score);
   return steps;
@@ -1146,46 +1202,60 @@ void enqueue_batch_step(wisb_handle* h, const DecodeCfg& c) {
   search_step_run(make_batch_search_args(h, c), h->stream);
 }
 
+// Batched prefill: positions [0, n_pos) of the token matrix in h->prompt_dev ([c.n_utt][tok_stride]) as the rows of
+// shared passes of at most chunk_max positions per utterance, K/V into cache slot u * slot_stride.  layer_hook(layer,
+// chunk), if given, runs after every layer's cross-query GEMM and returns its launches; after_pass(p0, chunk), if given,
+// runs after every pass.  Returns the number of passes.
+int batch_prefill(wisb_handle* h, const DecodeCfg& c, int tok_stride, int n_pos, int chunk_max, int slot_stride,
+                  bool with_logits, const std::function<int(int layer, int chunk)>& layer_hook = nullptr,
+                  const std::function<void(int p0, int chunk)>& after_pass = nullptr) {
+  struct Hook {
+    const std::function<int(int, int)>* fn;
+    int chunk;
+  } hook{&layer_hook, 0};
+  int passes = 0;
+  for (int p0 = 0; p0 < n_pos; p0 += chunk_max, ++passes) {
+    const int chunk = std::min(chunk_max, n_pos - p0);
+    prefill_rows_run(h->tokens.p, h->row_pos.p, h->row_slot.p, h->prompt_dev.p, tok_stride, c.n_utt, p0, chunk, slot_stride,
+                     h->stream);
+    BatchArgs a = make_batch_args(h, c);
+    a.R = c.n_utt * chunk;
+    a.rows_per_utt = chunk;
+    a.prefill = 1;
+    a.with_logits = with_logits ? 1 : 0;
+    if (layer_hook) {
+      hook.chunk = chunk;
+      a.layer_hook = [](void* ctx, int layer, cudaStream_t) {
+        const Hook* k = static_cast<const Hook*>(ctx);
+        return (*k->fn)(layer, k->chunk);
+      };
+      a.hook_ctx = &hook;
+    }
+    h->launches += 1 + batch_pass_run(a, h->bd_layers.data(), h->dims.n_dec_layers, h->stream);
+    if (after_pass) after_pass(p0, chunk);
+  }
+  return passes;
+}
+
+// cross K/V of utterance u0 of a batch of B_total encoded windows for every layer of the batched pass
+void bind_batch_cross_kv(wisb_handle* h, int u0, int B_total) {
+  for (int i = 0; i < h->dims.n_dec_layers; ++i) bind_cross_kv(h, h->bd_layers[i], i, u0, B_total);
+}
+
 // decode utterances [u0, u0 + n_utt) of the encoded batch with ONE shared decoder pass per generated token
 int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, const int* max_new_host, int32_t* out_ids,
                  int out_stride, int32_t* out_len, float* out_score) {
-  const Dims& dm = h->dims;
   cudaStream_t s = h->stream;
-  const int R = c.n_utt * c.beam;
-  const int H = dm.n_heads;
-  ensure_batch(h, R, c.prompt_len + c.max_new);
-  // cross K/V of the utterances of this pass
-  const size_t head_block = static_cast<size_t>(H) * T_ENC_PAD * HEAD_DIM;
-  for (int i = 0; i < dm.n_dec_layers; ++i) {
-    h->bd_layers[i].ck = h->ckv.p + (static_cast<size_t>(i * 2 + 0) * c.B_total + c.u0) * head_block;
-    h->bd_layers[i].cv = h->ckv.p + (static_cast<size_t>(i * 2 + 1) * c.B_total + c.u0) * head_block;
-  }
+  ensure_batch(h, c.n_utt * c.beam, c.prompt_len + c.max_new);
+  bind_batch_cross_kv(h, c.u0, c.B_total);
   int steps = 0;
-  upload_prompts(h, prompts, c);
-  int* pin_mx = h->pin_i.p + 4 + static_cast<size_t>(c.n_utt) * c.prompt_len;
-  if (c.per_utt_max_new) {
-    memcpy(pin_mx, max_new_host, sizeof(int) * c.n_utt);
-    WISB_CUDA(cudaMemcpyAsync(h->max_new_u.p, pin_mx, sizeof(int) * c.n_utt, cudaMemcpyHostToDevice, s));
-  }
+  upload_prompts(h, prompts, max_new_host, c);
   if (c.max_new > 0) {
     // ---- prompt prefix: every utterance's positions [0, prompt_len - 1) as rows of shared passes (<= 8 positions and
     //      <= the row capacity per pass), K/V into the slot of the utterance's first beam
-    const int pf_len = c.prompt_len - 1;
-    int chunk_max = h->bd_rows / c.n_utt;
-    if (chunk_max > MAX_BEAM) chunk_max = MAX_BEAM;
-    if (chunk_max < 1) chunk_max = 1;
-    for (int p0 = 0; p0 < pf_len; p0 += chunk_max) {
-      const int chunk = pf_len - p0 < chunk_max ? pf_len - p0 : chunk_max;
-      prefill_rows_run(h->tokens.p, h->row_pos.p, h->row_slot.p, h->prompt_dev.p, c.prompt_len, c.n_utt, p0, chunk, c.beam, s);
-      BatchArgs a = make_batch_args(h, c);
-      a.R = c.n_utt * chunk;
-      a.rows_per_utt = chunk;
-      a.prefill = 1;
-      h->launches += 1 + batch_pass_run(a, h->bd_layers.data(), dm.n_dec_layers, s);
-      ++steps;
-    }
-    SearchArgs sa = make_batch_search_args(h, c);
-    search_init_run(sa, h->prompt_dev.p, s, 1);
+    const int chunk_max = std::max(1, std::min(h->bd_rows / c.n_utt, MAX_BEAM));
+    steps += batch_prefill(h, c, c.prompt_len, c.prompt_len - 1, chunk_max, c.beam, false);
+    search_init_run(make_batch_search_args(h, c), h->prompt_dev.p, s, 1);
     cudaGraphExec_t g = nullptr;
     if (h->use_graphs && !h->profile) {  // (the per-kernel timing hook needs eager launches)
       GraphKey key;
@@ -1208,19 +1278,10 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
       }
       g = it->second;
     }
-    volatile int* flag = h->pin_i.p;
-    *flag = 0;
-    for (int gs = 0; gs < c.max_new; ++gs) {
+    steps += step_loop(h, c.max_new, false, [&] {
       if (g) WISB_CUDA(cudaGraphLaunch(g, s)); else enqueue_batch_step(h, c);
-      ++steps;
-      h->launches += h->bd_launches_step;
-      const bool poll = ((gs + 1) % h->decode_poll == 0) || gs + 1 == c.max_new;
-      if (poll) {
-        WISB_CUDA(cudaMemcpyAsync(const_cast<int*>(flag), &h->st.p->all_done, sizeof(int), cudaMemcpyDeviceToHost, s));
-        WISB_CUDA(cudaStreamSynchronize(s));
-        if (*flag) break;
-      }
-    }
+      return h->bd_launches_step;
+    });
   }
   read_results(h, c, out_ids, out_stride, out_len, out_score);
   return steps;
@@ -1231,28 +1292,9 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
 // the default 320 heads, 449 rows and 1500 frames: 0.86 GB): utterances are grouped so that it stays under this cap.
 constexpr size_t ALIGN_WS_BYTES = 2ull << 30;
 
-struct AlignHook {
-  wisb_handle* h;
-  AlignCaptureArgs a;  // everything but this layer's cross K and heads
-};
-
-int align_hook(void* ctx, int layer, cudaStream_t s) {
-  AlignHook* k = static_cast<AlignHook*>(ctx);
-  wisb_handle* h = k->h;
-  const int i0 = h->al_layer_off[layer], i1 = h->al_layer_off[layer + 1];
-  if (i0 == i1) return 0;
-  AlignCaptureArgs a = k->a;
-  a.items = h->al_items.p + i0;
-  a.n_items = i1 - i0;
-  a.ck = h->bd_layers[layer].ck;
-  h->prof_begin(5);
-  align_capture_run(a, s);
-  h->prof_end();
-  return 1;
-}
-
 // one group of utterances [g0, g0 + n) whose cross K/V are in h->ckv (encoded as a batch of n): teacher-forced passes with
-// the capture hook, token probabilities, filter, DTW, results to the caller's arrays
+// the capture hook, token probabilities, filter, DTW, results to the caller's arrays; records the stage events ev[5]
+// (passes done), ev[6] (filter done) and ev[7] (DTW done)
 void align_group(wisb_handle* h, int g0, int n, const int32_t* start_seq, int S, const int32_t* text, const int32_t* text_len,
                  int text_stride, const int32_t* num_frames, int width, int n_max, int f_max, int32_t* out_path,
                  int path_stride, int32_t* out_path_len, float* out_token_probs, float* cap_out) {
@@ -1265,11 +1307,7 @@ void align_group(wisb_handle* h, int g0, int n, const int32_t* start_seq, int S,
   int P = round_up(total, MAX_BEAM);
   if (P > dm.n_text_ctx) P = dm.n_text_ctx;
   ensure_batch(h, n * MAX_BEAM, P);
-  const size_t head_block = static_cast<size_t>(dm.n_heads) * T_ENC_PAD * HEAD_DIM;
-  for (int i = 0; i < dm.n_dec_layers; ++i) {
-    h->bd_layers[i].ck = h->ckv.p + static_cast<size_t>(i * 2 + 0) * n * head_block;
-    h->bd_layers[i].cv = h->ckv.p + static_cast<size_t>(i * 2 + 1) * n * head_block;
-  }
+  bind_batch_cross_kv(h, 0, n);
   // teacher-forced tokens [n][P]: start_seq, <|notimestamps|>, text; rows past an utterance's end feed <|endoftext|>
   // (causal attention keeps the rows before them exact; their outputs are not read)
   const int ts = std::max(text_stride, 1);
@@ -1295,47 +1333,49 @@ void align_group(wisb_handle* h, int g0, int n, const int32_t* start_seq, int S,
   WISB_CUDA(cudaMemcpyAsync(h->al_nframes.p, nf.data(), n * 4, cudaMemcpyHostToDevice, s));
   WISB_CUDA(cudaMemcpyAsync(h->al_text.p, txt.data(), txt.size() * 4, cudaMemcpyHostToDevice, s));
   WISB_CUDA(cudaMemsetAsync(h->al_probs.p, 0, static_cast<size_t>(n) * ts * 4, s));
-  AlignHook hook{h, AlignCaptureArgs()};
-  hook.a.head_of = h->al_head.p;
-  hook.a.n_text = h->al_ntext.p;
-  hook.a.n_frames = h->al_nframes.p;
-  hook.a.cap = h->al_cap.p;
-  hook.a.q = h->bq.p;
-  hook.a.row_pos = h->row_pos.p;
-  hook.a.n_utt = n;
-  hook.a.d = dm.d_model;
-  hook.a.H = dm.n_heads;
-  hook.a.A = A;
-  hook.a.s0 = S;
-  hook.a.n_max = n_max;
-  hook.a.f_max = f_max;
-  DecodeCfg c{};
-  c.n_utt = n;
-  c.B_total = n;
-  for (int p0 = 0; p0 < P; p0 += MAX_BEAM) {
-    const int chunk = std::min(MAX_BEAM, P - p0);
-    prefill_rows_run(h->tokens.p, h->row_pos.p, h->row_slot.p, h->prompt_dev.p, P, n, p0, chunk, 1, s);
-    BatchArgs a = make_batch_args(h, c);
-    a.R = n * chunk;
+  AlignCaptureArgs cap;  // everything but the layer's cross K, heads and rows per utterance
+  cap.head_of = h->al_head.p;
+  cap.n_text = h->al_ntext.p;
+  cap.n_frames = h->al_nframes.p;
+  cap.cap = h->al_cap.p;
+  cap.q = h->bq.p;
+  cap.row_pos = h->row_pos.p;
+  cap.n_utt = n;
+  cap.d = dm.d_model;
+  cap.H = dm.n_heads;
+  cap.A = A;
+  cap.s0 = S;
+  cap.n_max = n_max;
+  cap.f_max = f_max;
+  auto capture = [&](int layer, int chunk) {
+    const int i0 = h->al_layer_off[layer], i1 = h->al_layer_off[layer + 1];
+    if (i0 == i1) return 0;
+    AlignCaptureArgs a = cap;
+    a.items = h->al_items.p + i0;
+    a.n_items = i1 - i0;
+    a.ck = h->bd_layers[layer].ck;
     a.rows_per_utt = chunk;
-    a.prefill = 1;
-    a.with_logits = 1;
-    hook.a.rows_per_utt = chunk;
-    a.layer_hook = align_hook;
-    a.hook_ctx = &hook;
-    h->launches += 2 + batch_pass_run(a, h->bd_layers.data(), dm.n_dec_layers, s);
+    h->prof_begin(5);
+    align_capture_run(a, s);
+    h->prof_end();
+    return 1;
+  };
+  auto token_probs = [&](int, int chunk) {
     align_token_probs_run(h->blogits.p, dm.n_vocab_pad, h->row_pos.p, h->al_text.p, ts, h->al_ntext.p, n, chunk, S, dm.eot,
                           h->al_probs.p, s);
-    h->timing[6] += 1.f;
-  }
-  WISB_CUDA(cudaEventRecord(h->ev[4], s));
+    h->launches += 1;
+  };
+  DecodeCfg c{};
+  c.n_utt = n;
+  h->timing[6] += static_cast<float>(batch_prefill(h, c, P, P, MAX_BEAM, 1, true, capture, token_probs));
+  WISB_CUDA(cudaEventRecord(h->ev[5], s));
   if (cap_out)  // (stream-ordered before the filter standardises the buffer in place)
     WISB_CUDA(cudaMemcpyAsync(cap_out + static_cast<size_t>(g0) * A * (n_max + 1) * f_max, h->al_cap.p,
                               static_cast<size_t>(n) * A * (n_max + 1) * f_max * 4, cudaMemcpyDeviceToHost, s));
   align_filter_run(h->al_cap.p, h->al_mat.p, h->al_ntext.p, h->al_nframes.p, n, A, n_max, f_max, width, s);
-  WISB_CUDA(cudaEventRecord(h->ev[5], s));
-  align_dtw_run(h->al_mat.p, h->al_ntext.p, h->al_nframes.p, n, n_max, f_max, h->al_path.p, path_stride, h->al_len.p, s);
   WISB_CUDA(cudaEventRecord(h->ev[6], s));
+  align_dtw_run(h->al_mat.p, h->al_ntext.p, h->al_nframes.p, n, n_max, f_max, h->al_path.p, path_stride, h->al_len.p, s);
+  WISB_CUDA(cudaEventRecord(h->ev[7], s));
   h->launches += 3;
   WISB_CUDA(cudaMemcpyAsync(out_path + static_cast<size_t>(g0) * path_stride * 2, h->al_path.p,
                             static_cast<size_t>(n) * path_stride * 2 * 4, cudaMemcpyDeviceToHost, s));
@@ -1509,7 +1549,6 @@ int wisb_set_option(wisb_handle* h, const char* key, int value) {
     if (k == "use_graphs") h->use_graphs = value;
     else if (k == "attn_v_mn_major") h->attn_v_mn = value;
     else if (k == "attn_ref") h->attn_ref = value;
-    else if (k == "decode_poll") h->decode_poll = value < 1 ? 1 : value;
     else if (k == "profile") h->profile = value;
     else if (k == "encoder_cache") {
       h->encoder_cache = value ? 1 : 0;
@@ -1631,13 +1670,9 @@ int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* pro
     h->launches = 0;
     for (int i = 1; i <= 5; ++i) h->timing[i] = 0.f;
     WISB_CUDA(cudaEventRecord(h->ev[0], s));
-    bool reuse = upload_mel(h, mel, B);
-    h->ckv_sw = want_ckv_swizzle(h, B * beam_size) ? 1 : 0;
-    if (reuse && h->ckv_is_sw != h->ckv_sw) reuse = false;  // cached cross K/V is in the other pass's layout (the features are still on the device)
+    const bool cached = upload_mel(h, mel, B);
     set_extra_suppress(h, extra_suppress, n_extra);
-    WISB_CUDA(cudaEventRecord(h->ev[2], s));
-    WISB_CUDA(cudaEventSynchronize(h->ev[2]));
-    WISB_CUDA(cudaEventElapsedTime(&h->timing[1], h->ev[0], h->ev[2]));
+    time_h2d(h);
     DecodeCfg c;
     c.beam = beam_size;
     c.prompt_len = prompt_len;
@@ -1649,20 +1684,13 @@ int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* pro
     // Utterances are encoded and decoded in groups that share every decoder pass: the group's rows (utterances x beams)
     // are the M dimension of the batched pass, so the decoder weights stream once per generated token for the whole
     // group.  The group size only bounds the workspaces (cross K/V: 252 MB per large-v2 utterance).
-    const bool mega = B * beam_size <= DEC_MAX_ROWS && h->decoder_batch != 2;
-    int group = mega ? B : h->batch_rows / beam_size;
+    const bool persistent = use_persistent_pass(h, B * beam_size);
+    int group = persistent ? B : h->batch_rows / beam_size;
     if (group < 1) group = 1;
     int steps = 0;
     for (int g0 = 0; g0 < B; g0 += group) {
       const int n = B - g0 < group ? B - g0 : group;
-      WISB_CUDA(cudaEventRecord(h->ev[2], s));
-      if (reuse) {
-        WISB_CUDA(cudaEventRecord(h->ev[3], s));
-      } else {
-        run_encoder(h, n, -1, true, g0);
-        h->enc_valid = h->encoder_cache != 0 && h->mel_cache_B == B && n == B;
-      }
-      WISB_CUDA(cudaEventRecord(h->ev[4], s));
+      encode_stage(h, cached, B, g0, n, ckv_layout(h, persistent));
       c.u0 = 0;
       c.n_utt = n;
       c.B_total = n;
@@ -1674,29 +1702,14 @@ int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* pro
         for (int u = 0; u < n; ++u) c.max_new = per_utt[g0 + u] > c.max_new ? per_utt[g0 + u] : c.max_new;
       }
       const int32_t* gp = prompts + static_cast<size_t>(g0) * prompt_len;
+      const int* gmx = per_utt.empty() ? nullptr : per_utt.data() + g0;
       int32_t* gi = out_ids + static_cast<size_t>(g0) * out_stride;
-      if (mega) {
-        WISB_REQUIRE(per_utt.empty() || c.max_new == max_new, "internal: per-utterance limits on the small path");
-        if (!per_utt.empty()) {  // small path: the search kernels read the per-utterance caps from the same buffer
-          WISB_CUDA(cudaMemcpyAsync(h->max_new_u.p, per_utt.data() + g0, sizeof(int) * n, cudaMemcpyHostToDevice, s));
-          WISB_CUDA(cudaStreamSynchronize(s));
-        }
-        steps += decode_pass(h, c, gp, gi, out_stride, out_len + g0, out_score ? out_score + g0 : nullptr);
-      } else {
-        steps += decode_batch(h, c, gp, per_utt.empty() ? nullptr : per_utt.data() + g0, gi, out_stride, out_len + g0,
-                              out_score ? out_score + g0 : nullptr);
-      }
+      float* gs = out_score ? out_score + g0 : nullptr;
+      steps += persistent ? decode_pass(h, c, gp, gmx, gi, out_stride, out_len + g0, gs)
+                          : decode_batch(h, c, gp, gmx, gi, out_stride, out_len + g0, gs);
       WISB_CUDA(cudaEventRecord(h->ev[5], s));
-      WISB_CUDA(cudaStreamSynchronize(s));
-      float t;
-      WISB_CUDA(cudaEventElapsedTime(&t, h->ev[2], h->ev[3]));
-      h->timing[2] += t;
-      WISB_CUDA(cudaEventElapsedTime(&t, h->ev[3], h->ev[4]));
-      h->timing[3] += t;
-      WISB_CUDA(cudaEventElapsedTime(&t, h->ev[4], h->ev[5]));
-      h->timing[4] += t;
+      time_group(h, {2, 3, 4});  // encoder, cross K/V, decode
     }
-    WISB_CUDA(cudaEventElapsedTime(&h->timing[5], h->ev[0], h->ev[5]));
     h->timing[6] = static_cast<float>(steps);
     h->timing[7] = static_cast<float>(h->launches);
     h->prof_collect();
@@ -1725,10 +1738,8 @@ int wisb_detect_language(wisb_handle* h, const float* mel, int B, int32_t* lang_
     WISB_REQUIRE(B >= 1 && B <= 4096, "B out of range");
     WISB_REQUIRE(lang_ids_out != nullptr && probs_out != nullptr, "output pointer is NULL");
     cudaStream_t s = h->stream;
-    bool reuse = upload_mel(h, mel, B);
-    h->ckv_sw = h->mega_tc;  // language detection always runs the <= 8-row pass
-    if (reuse && h->ckv_is_sw != h->ckv_sw) reuse = false;
-    encode_for_decode(h, B, reuse);
+    const bool cached = upload_mel(h, mel, B);
+    encode_stage(h, cached, B, 0, B, ckv_layout(h, true));  // language detection always runs the persistent pass
     const int nl = dm.n_langs;
     h->lang_ids.ensure(nl);
     std::vector<int> ids(nl);
@@ -1746,9 +1757,7 @@ int wisb_detect_language(wisb_handle* h, const float* mel, int B, int32_t* lang_
       c.max_new = 1;
       c.max_hyp = 1;
       c.lp = 1.f;
-      upload_prompts(h, sot.data(), c);
-      search_init_run(make_search_args(h, c), h->prompt_dev.p, s);
-      upload_mega_layers(h, c);
+      persistent_setup(h, c, sot.data(), nullptr);
       enqueue_decoder_forward(h, c, true);
       lang_probs_run(h->logits.p, dm.n_vocab_pad, h->lang_ids.p, nl, c.n_utt, 1, h->lang_probs.p, s);
       WISB_CUDA(cudaMemcpyAsync(h->pin_f.p, h->lang_probs.p, sizeof(float) * c.n_utt * nl, cudaMemcpyDeviceToHost, s));
@@ -2026,44 +2035,18 @@ static void align_impl(wisb_handle* h, const float* mel, int B, const int32_t* s
     cudaStream_t s = h->stream;
     h->launches = 0;
     WISB_CUDA(cudaEventRecord(h->ev[0], s));
-    bool reuse = upload_mel(h, mel, B);
-    h->ckv_sw = 0;  // the capture and the batched pass read the cross K/V linear
-    WISB_CUDA(cudaEventRecord(h->ev[2], s));
-    WISB_CUDA(cudaEventSynchronize(h->ev[2]));
-    WISB_CUDA(cudaEventElapsedTime(&h->timing[1], h->ev[0], h->ev[2]));
+    const bool cached = upload_mel(h, mel, B);
+    time_h2d(h);
     const size_t per_utt = static_cast<size_t>(h->al_A) * (n_max + 1) * f_max * sizeof(float);
     int group = std::min(h->batch_rows / MAX_BEAM, static_cast<int>(std::min<size_t>(ALIGN_WS_BYTES / per_utt, 4096)));
     if (group < 1) group = 1;
-    if (reuse && group < B) reuse = false;
     for (int g0 = 0; g0 < B; g0 += group) {
       const int n = std::min(group, B - g0);
-      WISB_CUDA(cudaEventRecord(h->ev[2], s));
-      if (reuse) {
-        if (h->ckv_is_sw) {  // left chunk-swizzled by a <= 8-row generate: rerun only the cross-K/V GEMM, linear
-          ensure_encoder(h, B);
-          h->plan_ckv.epi.kv_swizzle = 0;
-          gemm_run(h->plan_ckv, s);
-          h->ckv_is_sw = 0;
-          h->launches += 1;
-        }
-      } else {
-        run_encoder(h, n, -1, true, g0);
-        h->enc_valid = h->encoder_cache != 0 && h->mel_cache_B == B && n == B;
-      }
-      WISB_CUDA(cudaEventRecord(h->ev[3], s));
+      encode_stage(h, cached, B, g0, n, ckv_layout(h, false));  // the capture and the batched pass read linear cross K/V
       align_group(h, g0, n, start_seq, start_len, text, text_len, text_stride, num_frames, median_filter_width, n_max, f_max,
                   out_path, path_stride, out_path_len, out_token_probs, cap_out);
-      float t;
-      WISB_CUDA(cudaEventElapsedTime(&t, h->ev[2], h->ev[3]));
-      h->timing[2] += t;
-      WISB_CUDA(cudaEventElapsedTime(&t, h->ev[3], h->ev[4]));
-      h->timing[3] += t;
-      WISB_CUDA(cudaEventElapsedTime(&t, h->ev[4], h->ev[5]));
-      h->timing[4] += t;
-      WISB_CUDA(cudaEventElapsedTime(&t, h->ev[5], h->ev[6]));
-      h->timing[14] += t;
+      time_group(h, {2, 2, 3, 4, 14});  // encoder + cross K/V, passes, filter, DTW
     }
-    WISB_CUDA(cudaEventElapsedTime(&h->timing[5], h->ev[0], h->ev[6]));
     h->timing[7] = static_cast<float>(h->launches);
     const float dtw = h->timing[14];
     h->prof_collect();  // (capture kernels are profile category 5 -> timing[13])
@@ -2323,7 +2306,7 @@ int wisb_debug_encode(wisb_handle* h, const float* mel, int B, float* enc_out, i
     const int d = h->dims.d_model;
     cudaStream_t s = h->stream;
     upload_mel(h, mel, B);
-    run_encoder(h, B, n_layers, false);
+    run_encoder(h, B, n_layers);
     std::vector<__half> tmp(static_cast<size_t>(B) * T_ENC_PAD * d);
     WISB_CUDA(cudaMemcpyAsync(tmp.data(), h->enc_out.p, tmp.size() * sizeof(__half), cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaStreamSynchronize(s));
@@ -2339,39 +2322,25 @@ int wisb_debug_forced_logits(wisb_handle* h, const float* mel, const int32_t* to
     const Dims& dm = h->dims;
     WISB_REQUIRE(h->blob != nullptr && tokens != nullptr && logits_out != nullptr && n_tokens >= 1 && n_tokens <= dm.n_text_ctx, "bad arguments");
     cudaStream_t s = h->stream;
-    upload_mel(h, mel, 1);
-    h->ckv_sw = want_ckv_swizzle(h, 1) ? 1 : 0;
-    run_encoder(h, 1, -1, true);
+    const bool batched = h->decoder_batch == 2;
+    encode_stage(h, upload_mel(h, mel, 1), 1, 0, 1, ckv_layout(h, !batched));
     DecodeCfg c;
     c.u0 = 0; c.n_utt = 1; c.B_total = 1; c.beam = 1; c.prompt_len = n_tokens; c.max_new = 1; c.max_hyp = 1; c.lp = 1.f;
-    upload_prompts(h, tokens, c);
-    if (h->decoder_batch == 2) {  // the batched pass, one row: position p of the token list per pass
+    if (batched) {  // the batched pass, one row: position p of the token list per pass
       ensure_batch(h, MAX_BEAM, n_tokens);
-      const size_t head_block = static_cast<size_t>(dm.n_heads) * T_ENC_PAD * HEAD_DIM;
-      for (int i = 0; i < dm.n_dec_layers; ++i) {
-        h->bd_layers[i].ck = h->ckv.p + static_cast<size_t>(i * 2 + 0) * head_block;
-        h->bd_layers[i].cv = h->ckv.p + static_cast<size_t>(i * 2 + 1) * head_block;
-      }
+      bind_batch_cross_kv(h, 0, 1);
+      upload_prompts(h, tokens, nullptr, c);
       // `debug_chunk` positions per pass (1..8): > 1 feeds consecutive positions as rows of one pass, the way the prompt
       // prefix is prefilled (exercises the multi-row paths of the attention kernels under teacher forcing)
-      const int chunk_max = h->debug_chunk < 1 ? 1 : (h->debug_chunk > MAX_BEAM ? MAX_BEAM : h->debug_chunk);
-      for (int p = 0; p < n_tokens; p += chunk_max) {
-        const int chunk = n_tokens - p < chunk_max ? n_tokens - p : chunk_max;
-        prefill_rows_run(h->tokens.p, h->row_pos.p, h->row_slot.p, h->prompt_dev.p, n_tokens, 1, p, chunk, 1, s);
-        BatchArgs a = make_batch_args(h, c);
-        a.R = chunk;
-        a.rows_per_utt = chunk;
-        a.prefill = 1;
-        a.with_logits = 1;
-        batch_pass_run(a, h->bd_layers.data(), dm.n_dec_layers, s);
+      const int chunk_max = std::max(1, std::min(h->debug_chunk, MAX_BEAM));
+      batch_prefill(h, c, n_tokens, n_tokens, chunk_max, 1, true, nullptr, [&](int p, int chunk) {
         WISB_CUDA(cudaMemcpy2DAsync(logits_out + static_cast<size_t>(p) * dm.n_vocab, sizeof(float) * dm.n_vocab, h->blogits.p,
                                     sizeof(float) * dm.n_vocab_pad, sizeof(float) * dm.n_vocab, chunk, cudaMemcpyDeviceToHost, s));
-      }
+      });
       WISB_CUDA(cudaStreamSynchronize(s));
       return;
     }
-    search_init_run(make_search_args(h, c), h->prompt_dev.p, s);
-    upload_mega_layers(h, c);
+    persistent_setup(h, c, tokens, nullptr);
     for (int p = 0; p < n_tokens; ++p) {
       enqueue_decoder_forward(h, c, true);
       WISB_CUDA(cudaMemcpyAsync(logits_out + static_cast<size_t>(p) * dm.n_vocab, h->logits.p, sizeof(float) * dm.n_vocab, cudaMemcpyDeviceToHost, s));
