@@ -175,6 +175,18 @@ int wisb_debug_dec_resid_ln(wisb_handle* h, int R, int cap, int d, int n_splits,
 int wisb_debug_dec_embed_ln(wisb_handle* h, int R, int cap, int d, int n_vocab, int n_pos, const int32_t* tokens, const int32_t* row_pos,
                             const uint16_t* tok_emb, const float* pos_emb, const float* g, const float* b, float* x,
                             uint16_t* xn16);
+/* ONE persistent decoder pass on caller state, launched exactly as decoding launches it.  prm = {impl (1 warp-MMA,
+ * 0 SIMT), n_utt, beam, pf_len, pos, flip, with_logits}.  Decoding step (pf_len 0): R = n_utt * beam <= 8 rows at
+ * position pos (0..447), tokens[R], cache indirection indir0 / indir1 int32 [R][448] (flip picks indir1).  One-pass
+ * prompt prefill (pf_len >= 1): R = n_utt * pf_len <= 8 rows, row u * pf_len + p = prompt position p of utterance u,
+ * written to cache slot u * beam; pos, flip and indir are unused.  enc16: fp16 encoder rows [n_utt][1536][d] (padding
+ * rows included) -> the cross K/V through the cross-K/V GEMM; ckv_out receives it in the plain layout, [L][2][n_utt][H]
+ * [1536][64] fp16.  kcache / vcache: fp16 [L][8][448][d] in / out; x: float32 [8][d] in / out (rows < R are the
+ * pass's residual stream); logits: float32 [8][n_vocab_pad] in / out (rows < R, columns < n_vocab written when
+ * with_logits).  Invalidates the cached encoder output. */
+int wisb_debug_dec_pass(wisb_handle* h, const int32_t* prm, int n_prm, const int32_t* tokens, const int32_t* indir0,
+                        const int32_t* indir1, const uint16_t* enc16, uint16_t* ckv_out, uint16_t* kcache, uint16_t* vcache,
+                        float* x, float* logits);
 /* per-phase %globaltimer stamps of the last persistent decoder pass (option "mega_trace" = 1): n <= 2048 values */
 int wisb_debug_read_trace(wisb_handle* h, unsigned long long* out, int n);
 /* encoder output after the final LayerNorm, float32 [B,1500,d_model]; n_layers < 0 = all */

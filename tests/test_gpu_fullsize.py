@@ -127,20 +127,24 @@ def test_large_v2_numeric_parity_against_the_oracle():
     enc_err = float(np.abs(got_enc - enc.numpy()).max())
     toks = PROMPT + [1000, 2000, 30000, 41000, 12, 50000]
     want = oracle.forced_logits(enc[0], toks).numpy()
-    got = h.debug_forced_logits(mel[:1], toks)           # persistent SIMT pass (fp32 activations)
+    h.set_option("mega_mma", 1)
+    got_mma = h.debug_forced_logits(mel[:1], toks)       # persistent warp-MMA pass (fp16 activations, the default)
+    h.set_option("mega_mma", 0)
+    got_simt = h.debug_forced_logits(mel[:1], toks)      # persistent SIMT pass (fp32 activations)
+    h.set_option("mega_mma", 1)
     h.set_option("decoder_batch", 2)
     got_b = h.debug_forced_logits(mel[:1], toks)         # batched pass (fp16 GEMM operands, wgmma)
     h.set_option("decoder_batch", 1)
-    err, err_b = float(np.abs(got - want).max()), float(np.abs(got_b - want).max())
-    print(f"large-v2: encoder max abs err {enc_err:.4f}; logits err {err:.4f} (SIMT pass) {err_b:.4f} (batched pass); "
-          f"logit range [{want.min():.1f}, {want.max():.1f}]")
+    err_mma, err_simt, err_b = (float(np.abs(g - want).max()) for g in (got_mma, got_simt, got_b))
+    print(f"large-v2: encoder max abs err {enc_err:.4f}; logits err {err_mma:.4f} (warp-MMA pass) {err_simt:.4f} (SIMT "
+          f"pass) {err_b:.4f} (batched pass); logit range [{want.min():.1f}, {want.max():.1f}]")
     assert enc_err <= 6e-2
-    assert err <= 2.5e-1 and err_b <= 2.5e-1
+    assert err_mma <= 2.5e-1 and err_simt <= 2.5e-1 and err_b <= 2.5e-1
     # beam-5 decode, hypotheses finish through the <|endoftext|> ramp (finished pool, early stop, length normalisation)
     base = oracle.generate(mel, [PROMPT] * 2, beam_size=5, enc=enc)
     probe = oracle.generate(mel, [PROMPT] * 2, beam_size=5, enc=enc, logit_noise=(LOGIT_TOL, 77))
     m = models.Whisper(None, device="cuda", _handles=[h])
-    # one utterance per call: 5 rows, the persistent SIMT pass
+    # one utterance per call: 5 rows, the persistent warp-MMA pass
     out = [m.generate(models.StorageView.from_array(mel[i : i + 1]), [PROMPT], beam_size=5, return_scores=True)[0] for i in range(2)]
     robust = [i for i in range(2) if base[i].sequences_ids == probe[i].sequences_ids]
     assert robust, "neither full-size oracle transcript is a robust decision"

@@ -61,6 +61,8 @@ _SIGS = {
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_dec_embed_ln": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wisb_debug_dec_pass": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_read_trace": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     "wisb_debug_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     "wisb_debug_forced_logits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
@@ -453,6 +455,35 @@ class Handle:
         check(lib().wisb_debug_dec_embed_ln(self._h, R, cap, d, tok_emb.shape[0], pos_emb.shape[0], ptr(tokens), ptr(row_pos),
                                             ptr(tok_emb), ptr(pos_emb), *(ptr(v) for v in vecs), ptr(x), ptr(xn)))
         return x, xn
+
+    def debug_dec_pass(self, impl: int, tokens, enc16, kcache, vcache, x, logits, *, n_utt: int, beam: int = 1,
+                       pf_len: int = 0, pos: int = 0, flip: int = 0, indir0=None, indir1=None, with_logits: bool = True):
+        """One persistent decoder pass (impl 1 warp-MMA, 0 SIMT) on caller state (wisb_debug_dec_pass).  tokens int
+        [R] (R = n_utt * beam, or n_utt * pf_len for the one-pass prefill), enc16 float16 [n_utt, 1536, d], indir0 /
+        indir1 int [R, 448] (decoding steps).  In / out: kcache / vcache float16 [L, 8, 448, d], x float32 [8, d],
+        logits float32 [8, n_vocab_pad].  -> the cross K/V the pass read, float16 [L, 2, n_utt, H, 1536, 64]."""
+        dm = self.dims()
+        d, L, H = dm["d_model"], dm["n_dec_layers"], dm["n_heads"]
+        self._inout(kcache, np.float16, (L, 8, 448, d), "kcache")
+        self._inout(vcache, np.float16, (L, 8, 448, d), "vcache")
+        self._inout(x, np.float32, (8, d), "x")
+        self._inout(logits, np.float32, (8, dm["n_vocab_pad"]), "logits")
+        enc16 = self._inout(np.ascontiguousarray(enc16, np.float16), np.float16, (n_utt, 1536, d), "enc16")
+        R = n_utt * (pf_len if pf_len > 0 else beam)
+        tokens = np.ascontiguousarray(np.asarray(tokens, np.int32).reshape(-1))
+        if tokens.size != R:
+            raise ValueError(f"tokens must have {R} entries")
+        ind = [None, None]
+        if pf_len == 0:
+            if indir0 is None or indir1 is None:
+                raise ValueError("a decoding step needs indir0 and indir1")
+            ind = [self._inout(np.ascontiguousarray(v, np.int32), np.int32, (R, 448), n) for v, n in
+                   ((indir0, "indir0"), (indir1, "indir1"))]
+        ckv = np.zeros((L, 2, n_utt, H, 1536, 64), np.float16)
+        prm = np.asarray([impl, n_utt, beam, pf_len, pos, flip, int(with_logits)], np.int32)
+        check(lib().wisb_debug_dec_pass(self._h, ptr(prm), prm.size, ptr(tokens), ptr(ind[0]), ptr(ind[1]), ptr(enc16),
+                                        ptr(ckv), ptr(kcache), ptr(vcache), ptr(x), ptr(logits)))
+        return ckv
 
     def debug_read_trace(self, n: int = 600) -> np.ndarray:
         out = np.zeros(n, np.uint64)

@@ -2350,4 +2350,87 @@ int wisb_debug_forced_logits(wisb_handle* h, const float* mel, const int32_t* to
   });
 }
 
+int wisb_debug_dec_pass(wisb_handle* h, const int32_t* prm, int n_prm, const int32_t* tokens, const int32_t* indir0,
+                        const int32_t* indir1, const uint16_t* enc16, uint16_t* ckv_out, uint16_t* kcache, uint16_t* vcache,
+                        float* x, float* logits) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(h->blob != nullptr && prm != nullptr && n_prm == 7 && tokens && enc16 && ckv_out && kcache && vcache && x && logits,
+                 "debug_dec_pass: bad arguments");
+    const Dims& dm = h->dims;
+    const int impl = prm[0], n_utt = prm[1], beam = prm[2], pf_len = prm[3], pos = prm[4], flip = prm[5], with_logits = prm[6];
+    WISB_REQUIRE(impl == 0 || impl == 1, "debug_dec_pass: impl is 0 (SIMT) or 1 (warp-MMA)");
+    WISB_REQUIRE(impl == 0 || h->mega_img.p != nullptr, "debug_dec_pass: the warp-MMA pass needs d_model <= 1280");
+    WISB_REQUIRE(n_utt >= 1 && beam >= 1 && n_utt * beam <= DEC_MAX_ROWS, "debug_dec_pass: n_utt x beam must be 1..8");
+    WISB_REQUIRE(pf_len >= 0 && pf_len <= MAX_BEAM && n_utt * pf_len <= DEC_MAX_ROWS, "debug_dec_pass: n_utt x pf_len must be <= 8");
+    WISB_REQUIRE((flip == 0 || flip == 1) && (with_logits == 0 || with_logits == 1), "debug_dec_pass: flip and with_logits are 0 / 1");
+    const int R = pf_len > 0 ? n_utt * pf_len : n_utt * beam;
+    WISB_REQUIRE(pf_len > 0 || (pos >= 0 && pos < T_MAX), "debug_dec_pass: position outside 0..447");
+    for (int r = 0; r < R; ++r)
+      WISB_REQUIRE(tokens[r] >= 0 && tokens[r] < dm.n_vocab, "debug_dec_pass: token outside the vocabulary");
+    if (pf_len == 0) {
+      WISB_REQUIRE(indir0 != nullptr && indir1 != nullptr, "debug_dec_pass: a decoding step needs indir0 / indir1");
+      for (int r = 0; r < R; ++r)
+        for (int t = 0; t < pos; ++t)
+          WISB_REQUIRE(indir0[r * T_MAX + t] >= 0 && indir0[r * T_MAX + t] < DEC_MAX_ROWS && indir1[r * T_MAX + t] >= 0 &&
+                           indir1[r * T_MAX + t] < DEC_MAX_ROWS,
+                       "debug_dec_pass: indirection entry outside the 8 cache slots");
+    }
+    cudaStream_t s = h->stream;
+    const int d = dm.d_model, L = dm.n_dec_layers;
+    // encoder rows -> enc_out -> cross K/V: first in the plain layout (returned), then in the layout the pass reads
+    ensure_encoder(h, n_utt);
+    h->enc_valid = false;  // these rows belong to no features: a later call must not reuse them
+    h->mel_cache_B = 0;
+    const size_t enc_elems = static_cast<size_t>(n_utt) * T_ENC_PAD * d;
+    WISB_CUDA(cudaMemcpyAsync(h->enc_out.p, enc16, enc_elems * sizeof(__half), cudaMemcpyHostToDevice, s));
+    const size_t ckv_elems = static_cast<size_t>(L) * 2 * enc_elems;
+    h->plan_ckv.epi.kv_swizzle = 0;
+    gemm_run(h->plan_ckv, s);
+    WISB_CUDA(cudaMemcpyAsync(ckv_out, h->ckv.p, ckv_elems * sizeof(__half), cudaMemcpyDeviceToHost, s));
+    const int saved_tc = h->mega_tc;
+    h->mega_tc = impl;
+    const int sw = ckv_layout(h, true);
+    if (sw != 0) {
+      h->plan_ckv.epi.kv_swizzle = sw;
+      gemm_run(h->plan_ckv, s);
+    }
+    h->ckv_is_sw = sw;
+    // the step's device state: position, indirection, tokens (prefill: the prompt rows), caches, sentinel outputs
+    DecodeCfg c;
+    c.u0 = 0; c.n_utt = n_utt; c.B_total = n_utt; c.beam = beam; c.prompt_len = pf_len + 1; c.max_new = 1; c.max_hyp = 1; c.lp = 1.f;
+    const DecState st{pf_len > 0 ? 0 : pos, 0, 0, 0, 0};
+    WISB_CUDA(cudaMemcpyAsync(h->st.p, &st, sizeof(DecState), cudaMemcpyHostToDevice, s));
+    WISB_CUDA(cudaMemcpyAsync(h->flip.p, &flip, sizeof(int), cudaMemcpyHostToDevice, s));
+    std::vector<int> prompt;
+    if (pf_len > 0) {
+      prompt.assign(static_cast<size_t>(n_utt) * c.prompt_len, 0);
+      for (int r = 0; r < R; ++r) prompt[(r / pf_len) * c.prompt_len + r % pf_len] = tokens[r];
+      WISB_CUDA(cudaMemcpyAsync(h->prompt_dev.p, prompt.data(), prompt.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    } else {
+      WISB_CUDA(cudaMemcpyAsync(h->tokens.p, tokens, R * sizeof(int), cudaMemcpyHostToDevice, s));
+      WISB_CUDA(cudaMemcpyAsync(h->ind0.p, indir0, static_cast<size_t>(R) * T_MAX * sizeof(int), cudaMemcpyHostToDevice, s));
+      WISB_CUDA(cudaMemcpyAsync(h->ind1.p, indir1, static_cast<size_t>(R) * T_MAX * sizeof(int), cudaMemcpyHostToDevice, s));
+    }
+    const size_t cache = static_cast<size_t>(L) * DEC_MAX_ROWS * T_MAX * d;
+    const size_t xs = static_cast<size_t>(DEC_MAX_ROWS) * d, ls = static_cast<size_t>(DEC_MAX_ROWS) * dm.n_vocab_pad;
+    WISB_CUDA(cudaMemcpyAsync(h->kcache.p, kcache, cache * sizeof(__half), cudaMemcpyHostToDevice, s));
+    WISB_CUDA(cudaMemcpyAsync(h->vcache.p, vcache, cache * sizeof(__half), cudaMemcpyHostToDevice, s));
+    WISB_CUDA(cudaMemcpyAsync(h->dx.p, x, xs * sizeof(float), cudaMemcpyHostToDevice, s));
+    WISB_CUDA(cudaMemcpyAsync(h->logits.p, logits, ls * sizeof(float), cudaMemcpyHostToDevice, s));
+    try {
+      upload_mega_layers(h, c);
+      enqueue_decoder_forward(h, c, with_logits != 0, pf_len > 0);
+    } catch (...) {
+      h->mega_tc = saved_tc;
+      throw;
+    }
+    h->mega_tc = saved_tc;
+    WISB_CUDA(cudaMemcpyAsync(kcache, h->kcache.p, cache * sizeof(__half), cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(vcache, h->vcache.p, cache * sizeof(__half), cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(x, h->dx.p, xs * sizeof(float), cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(logits, h->logits.p, ls * sizeof(float), cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
 }  // extern "C"
