@@ -132,16 +132,21 @@ int wisb_set_option(wisb_handle* h, const char* key, int value);
 int wisb_debug_gemm(wisb_handle* h, const int32_t* prm, int n_prm, const uint16_t* a, const uint16_t* w, const float* bias,
                     const float* pos, const int32_t* row_slot, const int32_t* row_pos, void* out, size_t out_bytes, void* aux,
                     size_t aux_bytes, void* aux2, size_t aux2_bytes, int32_t* plan_out);
-/* ONE production token-search step (wisb_generate's processors, top-k and beam bookkeeping) on caller data.
- * prm[8] int32: n_utt, beam, gen (index of the token being generated), V, eot, no_timestamps, timestamps (0/1),
- * max_initial_timestamp_index.  logits float32 [n_utt*beam, V]; hist int32 [n_utt*beam, gen] each row's generated
- * tokens (may be NULL at gen 0); mask uint8 [V] (bit 0: suppressed every step, bit 1: suppressed at gen 0); cum float32
- * [n_utt*beam] cumulative beam scores (NULL = 0); done int32 [n_utt] finished utterances (NULL = none).  Length penalty 1.
+/* ONE production token-search step (wisb_generate's processors, top-k, beam bookkeeping and step advance) on caller
+ * search state, which it returns.  prm[13] int32: n_utt, beam, V, ldl (>= V), eot, no_timestamps, timestamps (0/1),
+ * max_initial_timestamp_index, max_new (1..448), max_hyp (>= 1), t_max (1..448), init (0: the state as given; 1 / 2:
+ * search initialisation from `prompt` first, with shared_prefix 0 / 1), prompt_len.  n_utt * beam <= 1024.
+ * logits float32 [n_utt*beam, ldl] (columns >= V are never read); mask uint8 [V] (bit 0: suppressed every step, bit 1:
+ * at the first generated step); max_new_u int32 [n_utt] per-utterance caps in [0, max_new] or NULL; prompt int32
+ * [n_utt, prompt_len] (init only).  state_i int32 in / out: DecState {pos, gen_step, n_done, all_done, ticket (0)},
+ * flip, seq [2][R][max_new], indir [2][R][t_max], tokens [R], row_pos [R], done [n_utt], n_hyp [n_utt], best_len
+ * [n_utt], best_tokens [n_utt][max_new]; state_f float32 in / out: cum [R], best_score [n_utt]  (R = n_utt * beam).
  * Outputs: cand_idx int32 [n_utt, 16] (beam * V + token, -1 = none) and cand_score float32 [n_utt, 16], the first
- * 2*beam entries used; row_lse float32 [n_utt*beam], the log-softmax normaliser of each fully processed row. */
-int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, const float* logits, const int32_t* hist,
-                           const uint8_t* mask, const float* cum, const int32_t* done, int32_t* cand_idx, float* cand_score,
-                           float* row_lse);
+ * 2*beam entries used; row_lse float32 [n_utt*beam].  Sizes, the current history tokens and indirection entries are
+ * checked before anything is launched. */
+int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, float length_penalty, const float* logits,
+                           const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
+                           float* state_f, int32_t* cand_idx, float* cand_score, float* row_lse);
 /* encoder self-attention on caller data: qkv [B*1536, 3d] fp16 -> ctx [B*1536, d] fp16, d = 64 H; impl 0 = wgmma with
  * MN-major V, 1 = wgmma with the transposed Vt layout (built from the same qkv), 2 = SIMT check */
 int wisb_debug_enc_attn(wisb_handle* h, const uint16_t* qkv16, int B, int d, int H, int impl, uint16_t* ctx16_out);

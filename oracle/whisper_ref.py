@@ -38,7 +38,7 @@ golden transcript ships with the reference server.
 from __future__ import annotations
 
 import math
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 
 import numpy as np
 import torch
@@ -59,6 +59,163 @@ def _t(a):
     return torch.from_numpy(np.ascontiguousarray(a)).float()
 
 
+# ------------------------------------------------------------------------------------------------------------ search
+def max_hypotheses(beam: int, patience: float) -> int:
+    """Finished hypotheses that end an utterance's search: beam * patience rounded half up, in fp32 as the engine
+    computes it, and at least 1.  UNPINNED: CTranslate2 is C++ and presumably rounds with std::round (half away from
+    zero, the same for positive values); Python's round() would round half to even (beam 5 x patience 0.5 -> 2)."""
+    return max(1, int(np.float32(beam) * np.float32(patience) + np.float32(0.5)))
+
+
+def length_norm(gen: int, length_penalty: float) -> float:
+    """Divisor of the cumulative log-prob at generated-token index ``gen``."""
+    return math.pow(gen + 1, length_penalty) if length_penalty != 0 else 1.0
+
+
+@dataclass
+class BeamState:
+    """One utterance's search state between two steps, as the engine keeps it.  Every list over rows has ``beam``
+    entries.  A row whose candidate does not exist is dead: it feeds eot, its cum is -inf and it never becomes a
+    hypothesis."""
+    seqs: list                                  # generated tokens of every row
+    cum: list                                   # cumulative log-prob of every row (fp32 values)
+    tokens: list = None                         # token every row feeds next (None before the first step)
+    parents: list = None                        # row of the previous step every row continues
+    hyps: list = field(default_factory=list)    # (normalised score, tokens) of every finished hypothesis, in order
+    best: int = -1                              # index into hyps of the best one, -1 = none
+    finished: bool = False
+    picks: list = None                          # candidate rank every row took at the last step
+
+    @property
+    def best_score(self) -> float:
+        return self.hyps[self.best][0] if self.best >= 0 else NEG_INF
+
+    @property
+    def best_tokens(self) -> list:
+        return self.hyps[self.best][1] if self.best >= 0 else []
+
+
+BEAM_STEP_DEFECTS = ("secondary_from_0", "best_ge", "is_last_early", "invalid_hyps")
+
+
+def beam_step(state: BeamState, cand_ids, cand_scores, *, V: int, eot: int, gen: int, cap: int, max_hyp: int,
+              norm: float, defect=None) -> BeamState:
+    """The bookkeeping of one step of one utterance.
+
+    cand_ids: the 2 * beam candidates, best first, as flat ids row * V + token, -1 where no candidate exists;
+    cand_scores: their normalised scores (fp32 values).  gen: index of the token being generated; cap: the utterance's
+    limit on generated tokens (gen + 1 == cap is its last step, and with gen >= cap it finishes with no hypothesis);
+    norm: the step's length normalisation.  Rules: each of the first ``beam`` candidates that exists and ends in eot (or
+    any, at the last step) becomes a hypothesis, the first best one wins ties, and its row continues with the next
+    unused non-eot candidate after rank beam - 1 (or keeps its own candidate when none is left); a row without a
+    candidate is dead; the new cum is the fp32 product score * norm.  ``defect`` (comparator tests only) injects one
+    of BEAM_STEP_DEFECTS."""
+    beam, n_cand = len(state.seqs), len(cand_ids)
+    is_last = gen + (2 if defect == "is_last_early" else 1) >= cap
+    capped = gen >= cap
+    hyps, best = list(state.hyps), state.best
+    best_score = state.best_score
+    picks = []
+    secondary = 0 if defect == "secondary_from_0" else beam
+    for k in range(beam):
+        pick = k
+        idx = cand_ids[k]
+        tok = idx % V if idx >= 0 else eot
+        if not capped and (idx >= 0 or defect == "invalid_hyps") and (tok == eot or is_last):
+            row = idx // V if idx >= 0 else k
+            hyps.append((cand_scores[k], state.seqs[row] + ([] if tok == eot else [tok])))
+            if cand_scores[k] > best_score or (defect == "best_ge" and cand_scores[k] == best_score):
+                best, best_score = len(hyps) - 1, cand_scores[k]
+            for j in range(secondary, n_cand):
+                if cand_ids[j] >= 0 and cand_ids[j] % V != eot:
+                    pick, secondary = j, j + 1
+                    break
+        picks.append(pick)
+    seqs, cum, tokens, parents = [], [], [], []
+    for k, j in enumerate(picks):
+        idx = cand_ids[j]
+        parent, tok = (idx // V, idx % V) if idx >= 0 else (k, eot)
+        seqs.append(state.seqs[parent] + [tok])
+        cum.append(float(np.float32(cand_scores[j]) * np.float32(norm)) if idx >= 0 else NEG_INF)
+        tokens.append(tok)
+        parents.append(parent)
+    return BeamState(seqs, cum, tokens, parents, hyps, best, is_last or len(hyps) >= max_hyp, picks)
+
+
+def beam_candidates(logp: torch.Tensor, cum: torch.Tensor, norm: float, n_cand: int, first: bool):
+    """logp [rows, V] processed log-probs, cum [rows] (fp32) -> (flat ids, scores) of the n_cand best
+    (logp + cum) / norm, ties to the lowest flat id.  Only row 0 counts at the first step (every row holds the prompt);
+    a token whose processed logit is -inf is no candidate, and missing candidates are id -1 with score -inf."""
+    V = logp.shape[1]
+    flat = ((logp + cum[:, None]) / norm).reshape(-1)
+    valid = torch.isfinite(logp).reshape(-1)
+    if first:
+        valid[V:] = False
+    idx = torch.nonzero(valid).flatten()
+    order = idx[torch.argsort(-flat[idx], stable=True)[:n_cand]]
+    pad = n_cand - order.numel()
+    return order.tolist() + [-1] * pad, flat[order].tolist() + [NEG_INF] * pad
+
+
+def beam_search(logits_fn, process, *, beam: int, V: int, eot: int, max_new: int, max_hyp: int, length_penalty: float,
+                trace=None) -> BeamState:
+    """The search loop around ``beam_step`` for one utterance.
+
+    logits_fn(s, tokens, parents) -> raw logits of step s: [1, V] or [beam, V] at s = 0 (every row holds the prompt),
+    [beam, V] after, row k fed tokens[k] and continuing row parents[k] of the previous step.  process(logits, hists, s)
+    -> processed logits (hists: the rows' generated tokens).  trace, if a list, receives every step's smallest
+    decision-relevant gap (``beam_margin``)."""
+    st = BeamState([[] for _ in range(beam)], [0.0] * beam)
+    rows = beam
+    for s in range(max_new):
+        logits = logits_fn(s, st.tokens, None if st.parents is None else ([0] * beam if rows == 1 else st.parents))
+        rows = logits.shape[0]
+        logp = torch.log_softmax(process(logits, st.seqs[:rows], s), dim=-1)
+        norm = length_norm(s, length_penalty)
+        ids, scores = beam_candidates(logp, torch.tensor(st.cum[:rows], dtype=torch.float32), norm, 2 * beam, s == 0)
+        st = beam_step(st, ids, scores, V=V, eot=eot, gen=s, cap=max_new, max_hyp=max_hyp, norm=norm)
+        if trace is not None:
+            toks = [i % V if i >= 0 else -1 for i in ids]
+            trace.append(beam_margin(scores, toks, st.picks, beam, eot, norm, st.finished, s + 1 == max_new))
+        if st.finished:
+            break
+    return st
+
+
+def beam_margin(cs, cand_tok, nxt, beam, eot, norm, finishing, is_last):
+    """Smallest DECISION-RELEVANT gap of one beam-search step, in cumulative log-prob units (normalised gap x norm).
+
+    A step decides (a) which candidates form the top-``beam`` set -- those ending in eot (all of them at the last
+    step) become hypotheses -- and (b) which later non-eot candidates replace them as alive beams.  The order of two
+    alive non-eot candidates inside the used set changes nothing (it only permutes rows), so only two boundaries
+    count: rank beam-1 vs rank beam, and the last used candidate vs the next one that could be used instead.  When
+    the search ends at this step the alive set no longer matters, only the hypothesis set does."""
+    gaps = []
+
+    def gap(a, b):
+        if b < len(cs) and math.isfinite(cs[a]):
+            gaps.append((cs[a] - cs[b]) if math.isfinite(cs[b]) else 1e9)
+
+    a, b = beam - 1, beam
+    both_plain = cand_tok[a] != eot and cand_tok[b] != eot
+    if finishing:
+        if is_last or not both_plain:
+            gap(a, b)
+    else:
+        if not (both_plain and b in nxt):
+            gap(a, b)
+        m = max(nxt)
+        if m >= beam:
+            c = next((j for j in range(m + 1, len(cs)) if cand_tok[j] != eot), None)
+            if c is not None:
+                gap(m, c)
+            elif m + 1 < len(cs):
+                gap(m, len(cs) - 1)  # the real competitor is below the candidate list: a lower bound of the gap
+            else:
+                gaps.append(0.0)     # cannot tell how close the next candidate was
+    return (min(gaps) if gaps else 1e9) * norm
+
+
 class WhisperOracle:
     def __init__(self, dims: WhisperDims, tensors: dict):
         self.dims = dims
@@ -73,6 +230,7 @@ class WhisperOracle:
         # True: cross K/V and every appended self-attention K/V row are rounded through fp16, the two storage roundings
         # of the engine's SIMT decoder pass (its activations stay fp32), so that pass can be checked to a tight bound
         self.kv_fp16 = False
+        self._call_search = (1.0, 1.0)   # (patience, length penalty) of the generate call in progress
 
     @classmethod
     def from_blob(cls, src):
@@ -203,118 +361,51 @@ class WhisperOracle:
         return torch.stack(out)
 
     # ------------------------------------------------------------------ search
+    def _processors(self, prompt, extra_suppress):
+        """-> process(logits, hists, gen): the logits processors of one utterance's search (hists: the rows' generated
+        tokens; the timestamp oracle adds its rules here)."""
+        return lambda logits, hists, gen: self._process(logits, gen, extra_suppress)
+
+    # The two per-utterance entry points (a subclass may override either); both run the one search loop.
     @torch.no_grad()
     def _greedy(self, enc_row, prompt, max_length, extra_suppress, trace):
-        ckv = self.cross_kv(enc_row)
-        cache = self._prefill(prompt, ckv)
-        start = len(prompt) - 1
-        last = prompt[-1]
-        out, cum = [], 0.0
-        for s in range(self.max_new_tokens(len(prompt), max_length)):
-            logits, cache = self.decode_rows([last], start + s, cache, ckv)
-            logits = self._process(logits, s, extra_suppress)
-            tok = int(torch.argmax(logits[0]))  # first (lowest id) maximum
-            if trace is not None:
-                top2 = torch.topk(logits[0], 2).values
-                trace.append(float(top2[0] - top2[1]))
-            cum += float(torch.log_softmax(logits[0], -1)[tok])
-            if tok == self.dims.eot:
-                break
-            out.append(tok)
-            last = tok
-        return GenerationResult([out], [cum])
+        """beam 1: the beam procedure with 2 candidates (greedy arg-max decoding), at the call's patience and length
+        penalty as the engine runs it."""
+        patience, length_penalty = self._call_search
+        return self._search(enc_row, prompt, 1, max_length, patience, length_penalty, extra_suppress, trace)
 
     @torch.no_grad()
     def _beam(self, enc_row, prompt, beam, max_length, patience, length_penalty, extra_suppress, trace):
-        V = self.dims.n_vocab
-        eot = self.dims.eot
+        return self._search(enc_row, prompt, beam, max_length, patience, length_penalty, extra_suppress, trace)
+
+    _beam_margin = staticmethod(beam_margin)
+
+    @torch.no_grad()
+    def _search(self, enc_row, prompt, beam, max_length, patience, length_penalty, extra_suppress, trace):
+        """One utterance through ``beam_search``."""
         ckv = self.cross_kv(enc_row)
         cache = self._prefill(prompt, ckv)
         start = len(prompt) - 1
-        n_cand = 2 * beam
-        max_hyp = int(round(beam * patience))
-        max_new = self.max_new_tokens(len(prompt), max_length)
-        alive_tokens = [[]]  # generated tokens per alive beam
-        alive_scores = torch.zeros(1)
-        last = [prompt[-1]]
-        hyps = []  # (normalised score, tokens)
-        for s in range(max_new):
-            is_last = s + 1 == max_new
-            logits, cache = self.decode_rows(last, start + s, cache, ckv)
-            logp = torch.log_softmax(self._process(logits, s, extra_suppress), dim=-1)
-            total = logp + alive_scores[:, None]  # [rows, V] cumulative
-            norm = math.pow(s + 1, length_penalty) if length_penalty != 0 else 1.0
-            flat = (total / norm).reshape(-1)
-            # descending, ties -> lowest flat index (stable sort on the negated values)
-            order = torch.argsort(-flat, stable=True)[:n_cand]
-            cand_scores = flat[order]
-            cand_beam = (order // V).tolist()
-            cand_tok = (order % V).tolist()
-            nxt = []  # indices into the candidate list that stay alive
-            secondary = beam
-            for k in range(beam):
-                pick = k
-                if cand_tok[k] == eot or is_last:
-                    toks = alive_tokens[cand_beam[k]] + ([] if cand_tok[k] == eot else [cand_tok[k]])
-                    hyps.append((float(cand_scores[k]), toks))
-                    for j in range(secondary, n_cand):
-                        if cand_tok[j] != eot:
-                            pick = j
-                            secondary = j + 1
-                            break
-                nxt.append(pick)
-            if trace is not None:
-                trace.append(self._beam_margin(cand_scores.tolist(), cand_tok, nxt, beam, eot, norm,
-                                               is_last or len(hyps) >= max_hyp, is_last))
-            if is_last or len(hyps) >= max_hyp:
-                break
-            parents = [cand_beam[j] for j in nxt]
-            alive_tokens = [alive_tokens[cand_beam[j]] + [cand_tok[j]] for j in nxt]
-            alive_scores = torch.stack([cand_scores[j] for j in nxt]) * norm
-            last = [cand_tok[j] for j in nxt]
-            pidx = torch.tensor(parents, dtype=torch.long)
-            cache = [(k_[pidx], v_[pidx]) for k_, v_ in cache]
-        if not hyps:
+
+        def logits_fn(s, tokens, parents):
+            nonlocal cache
+            if s == 0:
+                tokens = [prompt[-1]]
+            else:
+                pidx = torch.tensor(parents, dtype=torch.long)
+                cache = [(k_[pidx], v_[pidx]) for k_, v_ in cache]
+            logits, cache = self.decode_rows(tokens, start + s, cache, ckv)
+            return logits
+
+        st = beam_search(logits_fn, self._processors(prompt, extra_suppress), beam=beam, V=self.dims.n_vocab,
+                         eot=self.dims.eot, max_new=self.max_new_tokens(len(prompt), max_length),
+                         max_hyp=max_hypotheses(beam, patience), length_penalty=length_penalty, trace=trace)
+        if not st.hyps:
             return GenerationResult([[]], [0.0])
         if trace is not None:  # last entry: gap between the two best finished hypotheses (normalised scores)
-            hs = sorted((h_[0] for h_ in hyps), reverse=True)
+            hs = sorted((h_[0] for h_ in st.hyps), reverse=True)
             trace.append(("final", hs[0] - hs[1] if len(hs) > 1 else 1e9))
-        best = max(range(len(hyps)), key=lambda i: (hyps[i][0], -i))  # first best on ties
-        return GenerationResult([hyps[best][1]], [hyps[best][0]])
-
-    @staticmethod
-    def _beam_margin(cs, cand_tok, nxt, beam, eot, norm, finishing, is_last):
-        """Smallest DECISION-RELEVANT gap of one beam-search step, in cumulative log-prob units (normalised gap x norm).
-
-        A step decides (a) which candidates form the top-``beam`` set -- those ending in eot (all of them at the last
-        step) become hypotheses -- and (b) which later non-eot candidates replace them as alive beams.  The order of two
-        alive non-eot candidates inside the used set changes nothing (it only permutes rows), so only two boundaries
-        count: rank beam-1 vs rank beam, and the last used candidate vs the next one that could be used instead.  When
-        the search ends at this step the alive set no longer matters, only the hypothesis set does."""
-        gaps = []
-
-        def gap(a, b):
-            if b < len(cs) and math.isfinite(cs[a]):
-                gaps.append((cs[a] - cs[b]) if math.isfinite(cs[b]) else 1e9)
-
-        a, b = beam - 1, beam
-        both_plain = cand_tok[a] != eot and cand_tok[b] != eot
-        if finishing:
-            if is_last or not both_plain:
-                gap(a, b)
-        else:
-            if not (both_plain and b in nxt):
-                gap(a, b)
-            m = max(nxt)
-            if m >= beam:
-                c = next((j for j in range(m + 1, len(cs)) if cand_tok[j] != eot), None)
-                if c is not None:
-                    gap(m, c)
-                elif m + 1 < len(cs):
-                    gap(m, len(cs) - 1)  # the real competitor is below the candidate list: a lower bound of the gap
-                else:
-                    gaps.append(0.0)     # cannot tell how close the next candidate was
-        return (min(gaps) if gaps else 1e9) * norm
+        return GenerationResult([st.best_tokens], [st.best_score])
 
     @torch.no_grad()
     def generate(self, features, prompts, beam_size: int = 5, patience: float = 1.0, length_penalty: float = 1.0,
@@ -326,6 +417,7 @@ class WhisperOracle:
         tests use it to find out whether a transcript is a ROBUST decision of the reference algorithm (unchanged under
         perturbations of the size of the documented fp16-vs-fp32 logit tolerance) or hangs on a near-tie."""
         self.logit_noise = None
+        self._call_search = (patience, length_penalty)
         if logit_noise is not None:
             g = torch.Generator()
             g.manual_seed(int(logit_noise[1]))
@@ -335,6 +427,7 @@ class WhisperOracle:
                                   trace, enc)
         finally:
             self.logit_noise = None
+            self._call_search = (1.0, 1.0)
 
     def _generate(self, features, prompts, beam_size, patience, length_penalty, max_length, suppress_tokens, trace, enc):
         extra = [t for t in suppress_tokens if t >= 0]

@@ -87,6 +87,14 @@ def test_per_utterance_max_length_in_one_pass(pair):
     assert all(len(g) <= min(ml // 2, ml - 4) for g, ml in zip(got2, limits))
     with pytest.raises(ValueError):
         h.generate(mel, [PROMPT] * 6, beam_size=5, max_length=np.asarray([16, 30], np.int32))
+    # limits at the prompt length (no new token) and one above it (one token), beside a longer one: on the persistent
+    # pass (beam 2: 6 rows) and on the batched pass (beam 5: 15 rows), like the same limits given alone
+    for beam in (2, 5):
+        ids, sc = h.generate(mel[:3], [PROMPT] * 3, beam_size=beam, max_length=np.asarray([4, 5, 16], np.int32))
+        assert ids[0] == [] and sc[0] == 0.0, (beam, ids[0], sc[0])
+        assert len(ids[1]) == 1 and ids[1] == h.generate(mel[1:2], [PROMPT], beam_size=beam, max_length=5)[0][0], beam
+        assert ids[2] == h.generate(mel[2:3], [PROMPT], beam_size=beam, max_length=16)[0][0], beam
+        assert h.generate(mel[:1], [PROMPT], beam_size=beam, max_length=4) == ([[]], [0.0])
 
 
 def test_cross_attention_tensor_core_vs_simt(pair):

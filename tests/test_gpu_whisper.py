@@ -74,14 +74,56 @@ def test_generate_matches_oracle(pair, beam):
     assert len(robust) >= 4, f"only {len(robust)} of {n} oracle transcripts are robust decisions"
     m = models.Whisper(None, device="cuda", _handles=[h])
     out = m.generate(models.StorageView.from_array(mel), [PROMPT] * n, beam_size=beam, return_scores=True)
-    for i in robust:  # exact token parity, no tolerated mismatch
+    for i in robust:  # exact token parity, no tolerated mismatch; the length-normalised score at every beam size
         assert out[i].sequences_ids[0] == res[i].sequences_ids[0], (beam, i)
-        if beam > 1:
-            assert abs(out[i].scores[0] - res[i].scores[0]) < 5e-2
+        assert abs(out[i].scores[0] - res[i].scores[0]) < 5e-2, (beam, i)
     assert len({tuple(res[i].sequences_ids[0]) for i in robust}) >= 3  # the transcripts depend on the audio
     for o in out:
         assert dims.eot not in o.sequences_ids[0]
         assert not set(o.sequences_ids[0]) & set(dims.suppress_ids)
+
+
+SEARCH_CONFIGS = [(5, 0.5, 1.0), (5, 2.0, 1.0), (2, 1.25, 1.0), (5, 1.0, 0.0), (2, 1.0, 0.6)]   # beam, patience, lp
+
+
+@pytest.mark.parametrize("beam,patience,lp", SEARCH_CONFIGS)
+def test_patience_and_length_penalty_match_oracle(pair, beam, patience, lp):
+    # max_hyp = beam * patience rounded half up (5 x 0.5 -> 3, 2 x 1.25 -> 3) and the length penalty, on the batched
+    # pass (6 utterances: 12 or 30 rows) and on the <= 8-row persistent pass (one utterance per call)
+    dims, oracle, h = pair
+    mel = mel_inputs(6)
+    n = mel.shape[0]
+    kw = dict(patience=patience, length_penalty=lp)
+    res, robust = robust_cases(oracle, mel, [PROMPT] * n, beam, **kw)
+    kw["beam_size"] = beam
+    assert len(robust) >= 3, f"only {len(robust)} of {n} oracle transcripts are robust decisions"
+    batched = h.generate(mel, [PROMPT] * n, **kw)
+    solo = [h.generate(mel[i : i + 1], [PROMPT], **kw) for i in range(n)]
+    for i in robust:
+        for where, ids, sc in (("batched", batched[0][i], batched[1][i]), ("solo", solo[i][0][0], solo[i][1][0])):
+            assert ids == res[i].sequences_ids[0], (where, beam, patience, lp, i)
+            assert abs(sc - res[i].scores[0]) < 5e-2, (where, beam, patience, lp, i)
+
+
+def test_search_settings_do_not_share_a_graph(pair):
+    # back-to-back batched calls that differ only in patience or length penalty each decode what they decode alone
+    dims = pair[0]
+    mel = mel_inputs(6)
+    calls = [dict(patience=1.0, length_penalty=1.0), dict(patience=2.0, length_penalty=1.0),
+             dict(patience=2.0, length_penalty=0.0), dict(patience=1.0, length_penalty=1.0)]
+    h = _lib.Handle.from_host(make_blob(dims), 0)
+    try:
+        mixed = [h.generate(mel, [PROMPT] * 6, beam_size=5, **c) for c in calls]
+    finally:
+        h.close()
+    for c, got in zip(calls, mixed):
+        alone = _lib.Handle.from_host(make_blob(dims), 0)
+        try:
+            want = alone.generate(mel, [PROMPT] * 6, beam_size=5, **c)
+        finally:
+            alone.close()
+        assert got[0] == want[0] and np.array_equal(np.float32(got[1]), np.float32(want[1])), c
+    assert mixed[0] == mixed[3] and mixed[2][1] != mixed[1][1]   # the length penalty really changed the call
 
 
 def test_graphs_and_eager_agree(pair):

@@ -4,7 +4,8 @@
 ``WhisperTimeStampLogitsProcessor`` (pinned against that class by ``tests/golden/timestamp_rules_hf.npz``, written by
 ``scripts/gen_golden_timestamp_rules_hf.py``).  ``TimestampOracle`` is ``oracle.whisper_ref.WhisperOracle`` with the
 rules applied after the logit-noise probe and the suppress masks whenever the prompt lacks <|notimestamps|>
-(CTranslate2's switch), in greedy and in beam search alike.  Every rule can be switched off (``disable``) so the tests
+(CTranslate2's switch), in greedy and in beam search alike: it supplies only the rules to
+``oracle.whisper_ref.beam_search``, the one search loop.  Every rule can be switched off (``disable``) so the tests
 can show that each one changes something.
 
 Rules (ts_begin = no_timestamps + 1, gen = index of the token being generated, hist = the row's generated tokens):
@@ -16,11 +17,9 @@ Rules (ts_begin = no_timestamps + 1, gen = index of the token being generated, h
 """
 from __future__ import annotations
 
-import math
-
 import torch
 
-from oracle.whisper_ref import GenerationResult, WhisperOracle
+from oracle.whisper_ref import WhisperOracle
 
 NEG_INF = float("-inf")
 RULES = (1, 2, 3, 4, 5)
@@ -75,82 +74,11 @@ class TimestampOracle(WhisperOracle):
     def _wants_ts(self, prompt):
         return self.dims.no_timestamps not in prompt
 
-    @torch.no_grad()
-    def _greedy(self, enc_row, prompt, max_length, extra_suppress, trace):
+    def _processors(self, prompt, extra_suppress):
+        base = super()._processors(prompt, extra_suppress)
         if not self._wants_ts(prompt):
-            return super()._greedy(enc_row, prompt, max_length, extra_suppress, trace)
-        ckv = self.cross_kv(enc_row)
-        cache = self._prefill(prompt, ckv)
-        start = len(prompt) - 1
-        last = prompt[-1]
-        out, cum = [], 0.0
-        for s in range(self.max_new_tokens(len(prompt), max_length)):
-            logits, cache = self.decode_rows([last], start + s, cache, ckv)
-            logits = self._rules(self._process(logits, s, extra_suppress), [out], s)
-            tok = int(torch.argmax(logits[0]))
-            cum += float(torch.log_softmax(logits[0], -1)[tok])
-            if tok == self.dims.eot:
-                break
-            out.append(tok)
-            last = tok
-        return GenerationResult([out], [cum])
-
-    @torch.no_grad()
-    def _beam(self, enc_row, prompt, beam, max_length, patience, length_penalty, extra_suppress, trace):
-        if not self._wants_ts(prompt):
-            return super()._beam(enc_row, prompt, beam, max_length, patience, length_penalty, extra_suppress, trace)
-        V, eot = self.dims.n_vocab, self.dims.eot
-        ckv = self.cross_kv(enc_row)
-        cache = self._prefill(prompt, ckv)
-        start = len(prompt) - 1
-        n_cand = 2 * beam
-        max_hyp = int(round(beam * patience))
-        max_new = self.max_new_tokens(len(prompt), max_length)
-        alive_tokens = [[]]
-        alive_scores = torch.zeros(1)
-        last = [prompt[-1]]
-        hyps = []
-        for s in range(max_new):
-            is_last = s + 1 == max_new
-            logits, cache = self.decode_rows(last, start + s, cache, ckv)
-            logp = torch.log_softmax(self._rules(self._process(logits, s, extra_suppress), alive_tokens, s), dim=-1)
-            norm = math.pow(s + 1, length_penalty) if length_penalty != 0 else 1.0
-            flat = ((logp + alive_scores[:, None]) / norm).reshape(-1)
-            order = torch.argsort(-flat, stable=True)[:n_cand]
-            cand_scores = flat[order]
-            cand_beam = (order // V).tolist()
-            cand_tok = (order % V).tolist()
-            nxt = []
-            secondary = beam
-            for k in range(beam):
-                pick = k
-                if cand_tok[k] == eot or is_last:
-                    toks = alive_tokens[cand_beam[k]] + ([] if cand_tok[k] == eot else [cand_tok[k]])
-                    hyps.append((float(cand_scores[k]), toks))
-                    for j in range(secondary, n_cand):
-                        if cand_tok[j] != eot:
-                            pick = j
-                            secondary = j + 1
-                            break
-                nxt.append(pick)
-            if trace is not None:  # the step's smallest decision-relevant gap (WhisperOracle._beam_margin)
-                trace.append(self._beam_margin(cand_scores.tolist(), cand_tok, nxt, beam, eot, norm,
-                                               is_last or len(hyps) >= max_hyp, is_last))
-            if is_last or len(hyps) >= max_hyp:
-                break
-            parents = [cand_beam[j] for j in nxt]
-            alive_tokens = [alive_tokens[cand_beam[j]] + [cand_tok[j]] for j in nxt]
-            alive_scores = torch.stack([cand_scores[j] for j in nxt]) * norm
-            last = [cand_tok[j] for j in nxt]
-            pidx = torch.tensor(parents, dtype=torch.long)
-            cache = [(k_[pidx], v_[pidx]) for k_, v_ in cache]
-        if not hyps:
-            return GenerationResult([[]], [0.0])
-        if trace is not None:  # last entry: gap between the two best finished hypotheses (normalised scores)
-            hs = sorted((h_[0] for h_ in hyps), reverse=True)
-            trace.append(("final", hs[0] - hs[1] if len(hs) > 1 else 1e9))
-        best = max(range(len(hyps)), key=lambda i: (hyps[i][0], -i))
-        return GenerationResult([hyps[best][1]], [hyps[best][0]])
+            return base
+        return lambda logits, hists, gen: self._rules(base(logits, hists, gen), hists, gen)
 
 
 def check_invariants(seq, dims, max_initial_timestamp_index: int = 50):

@@ -51,8 +51,8 @@ _SIGS = {
     "wisb_debug_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
                                   C.c_void_p]),
-    "wisb_debug_search_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wisb_debug_search_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_enc_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "wisb_debug_dec_cross_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_dec_self_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -338,30 +338,89 @@ class Handle:
             return out, dict(zip(("bn", "mcast", "k_splits", "grid"), (int(v) for v in plan)))
         return out
 
+    @staticmethod
+    def search_state(n_utt: int, beam: int, max_new: int, t_max: int) -> dict:
+        """A zeroed search state for debug_search_step_state (best_score -inf): name -> array, in the entry's order."""
+        R = n_utt * beam
+        return {"st": np.zeros(5, np.int32), "flip": np.zeros(1, np.int32),   # DecState: pos, gen_step, n_done, all_done, ticket
+                "seq": np.zeros((2, R, max_new), np.int32), "indir": np.zeros((2, R, t_max), np.int32),
+                "tokens": np.zeros(R, np.int32), "row_pos": np.zeros(R, np.int32), "done": np.zeros(n_utt, np.int32),
+                "n_hyp": np.zeros(n_utt, np.int32), "best_len": np.zeros(n_utt, np.int32),
+                "best_tokens": np.zeros((n_utt, max_new), np.int32),
+                "cum": np.zeros(R, np.float32), "best_score": np.full(n_utt, -np.inf, np.float32)}
+
+    _STATE_F = ("cum", "best_score")
+
     def debug_search_step(self, logits, hist, mask, *, beam: int, gen: int, eot: int, no_timestamps: int,
                           timestamps: bool, max_initial_timestamp_index: int = 50, cum=None, done=None):
-        """One production search step on caller data.  logits float32 [n_utt*beam, V]; hist int [n_utt*beam, gen];
-        mask uint8 [V] (bit 0 every step, bit 1 at gen 0).  -> (cand_idx int32 [n_utt, 2*beam] = beam*V + token,
-        cand_score float32 [n_utt, 2*beam], row_lse float32 [n_utt*beam])."""
+        """The candidates of one production search step on fresh hypotheses (max_hyp = beam, length penalty 1).
+        logits float32 [n_utt*beam, V]; hist int [n_utt*beam, gen] the rows' generated tokens; mask uint8 [V] (bit 0
+        every step, bit 1 at gen 0); cum [n_utt*beam] (None = 0); done [n_utt] finished utterances (None = none).
+        -> (cand_idx int32 [n_utt, 2*beam] = beam*V + token, cand_score float32 [n_utt, 2*beam], row_lse float32
+        [n_utt*beam]).  The whole search state: debug_search_step_state."""
         logits = np.ascontiguousarray(logits, np.float32)
-        R, V = logits.shape
+        R = logits.shape[0]
         if R % beam:
             raise ValueError("logits rows must be n_utt * beam")
         n_utt = R // beam
-        hist = np.ascontiguousarray(np.asarray(hist, np.int32).reshape(R, gen))
+        st = self.search_state(n_utt, beam, gen + 2, 1)
+        st["st"][1] = gen
+        if gen:
+            st["seq"][0, :, :gen] = np.asarray(hist, np.int32).reshape(R, gen)
+        if cum is not None:
+            st["cum"][:] = np.asarray(cum, np.float32).reshape(R)
+        if done is not None:
+            st["done"][:] = np.asarray(done, np.int32).reshape(n_utt)
+            st["st"][2] = int((st["done"] != 0).sum())
+            if st["st"][2] == n_utt:
+                raise ValueError("every utterance is finished")
+        _, ci, cs, lse = self.debug_search_step_state(logits, mask, st, beam=beam, max_hyp=beam, eot=eot,
+                                                      no_timestamps=no_timestamps, timestamps=timestamps,
+                                                      max_initial_timestamp_index=max_initial_timestamp_index)
+        return ci, cs, lse
+
+    def debug_search_step_state(self, logits, mask, state, *, beam: int, max_hyp: int, eot: int, V: int = 0, no_timestamps: int = 0,
+                          timestamps: bool = False, max_initial_timestamp_index: int = 50, length_penalty: float = 1.0,
+                          max_new_u=None, prompt=None, shared_prefix: int = 0):
+        """One production search step on caller state.  logits float32 [n_utt*beam, ldl] (only columns < V are read; V
+        = ldl by default); mask uint8 [V] (bit 0 every step, bit 1 at the first generated step); state as made by
+        search_state (its shapes give max_new and t_max); prompt int [n_utt, prompt_len]: run the search initialisation
+        (with shared_prefix) first.  -> (new state, cand_idx int32 [n_utt, 2*beam] = beam*V + token or -1, cand_score
+        float32 [n_utt, 2*beam], row_lse float32 [n_utt*beam])."""
+        logits = np.ascontiguousarray(logits, np.float32)
+        R, ldl = logits.shape
+        V = V or ldl
+        if R % beam:
+            raise ValueError("logits rows must be n_utt * beam")
+        n_utt = R // beam
         mask = np.ascontiguousarray(mask, np.uint8)
         if mask.shape != (V,):
             raise ValueError("mask must have V entries")
-        cum = None if cum is None else np.ascontiguousarray(cum, np.float32).reshape(R)
-        done = None if done is None else np.ascontiguousarray(done, np.int32).reshape(n_utt)
-        prm = np.asarray([n_utt, beam, gen, V, eot, no_timestamps, 1 if timestamps else 0, max_initial_timestamp_index],
-                         np.int32)
+        _, _, max_new = state["seq"].shape
+        t_max = state["indir"].shape[2]
+        want = self.search_state(n_utt, beam, max_new, t_max)
+        for k, v in want.items():
+            if np.shape(state[k]) != v.shape:
+                raise ValueError(f"state[{k!r}] must have shape {v.shape}")
+        si = np.concatenate([np.asarray(state[k], np.int32).ravel() for k in want if k not in self._STATE_F])
+        sf = np.concatenate([np.asarray(state[k], np.float32).ravel() for k in self._STATE_F])
+        caps = None if max_new_u is None else np.ascontiguousarray(max_new_u, np.int32).reshape(n_utt)
+        pr = None if prompt is None else np.ascontiguousarray(prompt, np.int32).reshape(n_utt, -1)
+        init = 0 if pr is None else 1 + int(shared_prefix)
+        prm = np.asarray([n_utt, beam, V, ldl, eot, no_timestamps, 1 if timestamps else 0, max_initial_timestamp_index,
+                          max_new, max_hyp, t_max, init, 0 if pr is None else pr.shape[1]], np.int32)
         ci = np.zeros((n_utt, 16), np.int32)
         cs = np.zeros((n_utt, 16), np.float32)
         lse = np.zeros(R, np.float32)
-        check(lib().wisb_debug_search_step(self._h, ptr(prm), prm.size, ptr(logits), ptr(hist) if gen else None, ptr(mask),
-                                           ptr(cum), ptr(done), ptr(ci), ptr(cs), ptr(lse)))
-        return ci[:, : 2 * beam], cs[:, : 2 * beam], lse
+        check(lib().wisb_debug_search_step(self._h, ptr(prm), prm.size, float(length_penalty), ptr(logits), ptr(mask),
+                                           ptr(caps), ptr(pr), ptr(si), ptr(sf), ptr(ci), ptr(cs), ptr(lse)))
+        out, oi, of = {}, 0, 0
+        for k, v in want.items():
+            if k in self._STATE_F:
+                out[k], of = sf[of : of + v.size].reshape(v.shape).copy(), of + v.size
+            else:
+                out[k], oi = si[oi : oi + v.size].reshape(v.shape).copy(), oi + v.size
+        return out, ci[:, : 2 * beam], cs[:, : 2 * beam], lse
 
     def debug_enc_attn(self, qkv16: np.ndarray, n_heads: int, impl: int = 0) -> np.ndarray:
         """Encoder self-attention on qkv fp16 [B, 1536, 3d] -> ctx fp16 [B, 1536, d]; impl 0 = wgmma (MN-major V),

@@ -955,8 +955,10 @@ void upload_prompts(wisb_handle* h, const int32_t* prompts, const int* max_new_h
   }
 }
 
-// best hypothesis of every utterance of the pass (search state) -> the caller's host arrays at utterance u0
-void read_results(wisb_handle* h, const DecodeCfg& c, int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score) {
+// best hypothesis of every utterance of the pass (search state) -> the caller's host arrays at utterance u0.  An
+// utterance capped at 0 new tokens (c.max_new or its max_new_host entry) returns no tokens and score 0.
+void read_results(wisb_handle* h, const DecodeCfg& c, const int* max_new_host, int32_t* out_ids, int out_stride,
+                  int32_t* out_len, float* out_score) {
   cudaStream_t s = h->stream;
   int* lens = h->pin_i.p + 4;
   int* toks = lens + c.n_utt;
@@ -966,10 +968,11 @@ void read_results(wisb_handle* h, const DecodeCfg& c, int32_t* out_ids, int out_
   WISB_CUDA(cudaMemcpyAsync(h->pin_f.p, h->best_score.p, sizeof(float) * c.n_utt, cudaMemcpyDeviceToHost, s));
   WISB_CUDA(cudaStreamSynchronize(s));
   for (int u = 0; u < c.n_utt; ++u) {
-    const int len = c.max_new > 0 ? lens[u] : 0;
+    const int cap = c.per_utt_max_new ? max_new_host[c.u0 + u] : c.max_new;
+    const int len = cap > 0 ? lens[u] : 0;
     out_len[c.u0 + u] = len;
     for (int t = 0; t < len && t < out_stride; ++t) out_ids[static_cast<size_t>(c.u0 + u) * out_stride + t] = toks[u * mn + t];
-    if (out_score) out_score[c.u0 + u] = c.max_new > 0 ? h->pin_f.p[u] : 0.f;
+    if (out_score) out_score[c.u0 + u] = cap > 0 ? h->pin_f.p[u] : 0.f;
   }
 }
 
@@ -1042,7 +1045,7 @@ int decode_pass(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, cons
       return 1 + 2;  // the pass + the two kernels of the search step
     });
   }
-  read_results(h, c, out_ids, out_stride, out_len, out_score);
+  read_results(h, c, max_new_host, out_ids, out_stride, out_len, out_score);
   return steps;
 }
 
@@ -1283,7 +1286,7 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
       return h->bd_launches_step;
     });
   }
-  read_results(h, c, out_ids, out_stride, out_len, out_score);
+  read_results(h, c, max_new_host, out_ids, out_stride, out_len, out_score);
   return steps;
 }
 
@@ -1895,71 +1898,94 @@ int wisb_debug_gemm(wisb_handle* h, const int32_t* prm, int n_prm, const uint16_
   });
 }
 
-int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, const float* logits, const int32_t* hist,
-                           const uint8_t* mask, const float* cum, const int32_t* done, int32_t* cand_idx, float* cand_score,
-                           float* row_lse) {
+int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, float length_penalty, const float* logits,
+                           const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
+                           float* state_f, int32_t* cand_idx, float* cand_score, float* row_lse) {
   return guarded(h, [&] {
-    WISB_REQUIRE(prm != nullptr && n_prm == 8 && logits && mask && cand_idx && cand_score && row_lse, "debug_search_step: bad arguments");
-    const int n_utt = prm[0], beam = prm[1], gen = prm[2], V = prm[3], eot = prm[4], no_ts = prm[5], ts = prm[6], max_init = prm[7];
-    WISB_REQUIRE(n_utt >= 1 && n_utt <= 64 && beam >= 1 && beam <= MAX_BEAM && gen >= 0 && gen + 2 <= T_MAX && V >= 2 &&
-                     eot >= 0 && eot < V && (ts == 0 || ts == 1) && max_init >= 0 && (gen == 0 || hist != nullptr),
+    WISB_REQUIRE(prm != nullptr && n_prm == 13 && logits && mask && state_i && state_f && cand_idx && cand_score && row_lse,
+                 "debug_search_step: bad arguments");
+    const int n_utt = prm[0], beam = prm[1], V = prm[2], ldl = prm[3], eot = prm[4], no_ts = prm[5], ts = prm[6];
+    const int max_init = prm[7], max_new = prm[8], max_hyp = prm[9], t_max = prm[10], init = prm[11], prompt_len = prm[12];
+    WISB_REQUIRE(n_utt >= 1 && beam >= 1 && beam <= MAX_BEAM && n_utt * beam <= 1024 && V >= 2 && V <= TOPK_CHUNKS * 2048 &&
+                     ldl >= V && eot >= 0 && eot < V && (ts == 0 || ts == 1) && max_init >= 0 && max_new >= 1 &&
+                     max_new <= T_MAX && max_hyp >= 1 && t_max >= 1 && t_max <= T_MAX && init >= 0 && init <= 2,
                  "debug_search_step: bad scalar parameters");
-    WISB_REQUIRE(!ts || (no_ts > eot && no_ts + 1 < V), "debug_search_step: bad timestamp geometry");
+    WISB_REQUIRE(!ts || (no_ts > eot && no_ts + 1 < V && V - no_ts - 1 <= 2048), "debug_search_step: bad timestamp geometry");
+    const int R = n_utt * beam;
+    // state_i: DecState (5) | flip | seq [2][R][max_new] | indir [2][R][t_max] | tokens [R] | row_pos [R] | done [n_utt] |
+    // n_hyp [n_utt] | best_len [n_utt] | best_tokens [n_utt][max_new];  state_f: cum [R] | best_score [n_utt]
+    const size_t o_seq = 6, o_ind = o_seq + 2ull * R * max_new, o_tok = o_ind + 2ull * R * t_max, o_rpos = o_tok + R;
+    const size_t o_done = o_rpos + R, o_nhyp = o_done + n_utt, o_blen = o_nhyp + n_utt, o_btok = o_blen + n_utt;
+    const size_t n_i = o_btok + static_cast<size_t>(n_utt) * max_new, n_f = static_cast<size_t>(R) + n_utt;
+    if (init) {
+      WISB_REQUIRE(prompt != nullptr && prompt_len >= 1 && prompt_len <= t_max, "debug_search_step: bad prompt");
+      for (long long i = 0; i < static_cast<long long>(n_utt) * prompt_len; ++i)
+        WISB_REQUIRE(prompt[i] >= 0 && prompt[i] < V, "debug_search_step: prompt token outside the vocabulary");
+    } else {
+      const int pos = state_i[0], gen = state_i[1], n_done = state_i[2], all_done = state_i[3], flip = state_i[5];
+      // (a finished search may sit at gen_step == max_new: its step launches nothing)
+      WISB_REQUIRE(pos >= 0 && pos < t_max && gen >= 0 && (gen < max_new || (all_done == 1 && gen == max_new)) &&
+                       n_done >= 0 && n_done <= n_utt &&
+                       (all_done == 0 || all_done == 1) && state_i[4] == 0 && (flip == 0 || flip == 1),
+                   "debug_search_step: bad DecState or flip");
+      const int32_t* seq = state_i + o_seq + static_cast<size_t>(flip) * R * max_new;
+      const int32_t* ind = state_i + o_ind + static_cast<size_t>(flip) * R * t_max;
+      for (int r = 0; r < R; ++r) {
+        for (int t = 0; t < gen; ++t)
+          WISB_REQUIRE(seq[static_cast<size_t>(r) * max_new + t] >= 0 && seq[static_cast<size_t>(r) * max_new + t] < V,
+                       "debug_search_step: history token outside the vocabulary");
+        for (int t = 0; t < pos; ++t)
+          WISB_REQUIRE(ind[static_cast<size_t>(r) * t_max + t] >= 0 && ind[static_cast<size_t>(r) * t_max + t] < R,
+                       "debug_search_step: indirection entry outside [0, R)");
+      }
+      for (int u = 0; u < n_utt; ++u)
+        WISB_REQUIRE(state_i[o_done + u] == 0 || state_i[o_done + u] == 1, "debug_search_step: done must be 0 or 1");
+    }
+    if (max_new_u)
+      for (int u = 0; u < n_utt; ++u)
+        WISB_REQUIRE(max_new_u[u] >= 0 && max_new_u[u] <= max_new, "debug_search_step: per-utterance cap outside [0, max_new]");
     cudaStream_t s = h->stream;
-    const int R = n_utt * beam, max_new = gen + 2;
-    DevBuf<float> d_logits, d_lse, d_pmax, d_psum, d_cum, d_cs, d_best;
+    DevBuf<float> d_logits, d_lse, d_pmax, d_psum, d_f, d_cs;
     DevBuf<unsigned long long> d_part;
     DevBuf<uint8_t> d_mask;
-    DevBuf<int> d_ci, d_tok, d_seq, d_ind, d_flip, d_done, d_nhyp, d_blen, d_btok;
-    DevBuf<DecState> d_st;
-    d_logits.ensure(static_cast<size_t>(R) * V);
+    DevBuf<int> d_i, d_ci, d_cap, d_prompt, d_slot;
+    d_logits.ensure(static_cast<size_t>(R) * ldl);
     d_mask.ensure(V);
-    d_lse.ensure(R);
     d_pmax.ensure(static_cast<size_t>(R) * (TOPK_CHUNKS + 1));
     d_psum.ensure(static_cast<size_t>(R) * (TOPK_CHUNKS + 1));
     d_part.ensure(static_cast<size_t>(R) * (TOPK_CHUNKS + 1) * MAX_CAND);
-    d_cum.ensure(R, true);
-    d_cs.ensure(static_cast<size_t>(n_utt) * MAX_CAND);
-    d_ci.ensure(static_cast<size_t>(n_utt) * MAX_CAND);
-    d_tok.ensure(R);
-    d_seq.ensure(2ull * R * max_new, true);
-    d_ind.ensure(2ull * R, true);
-    d_flip.ensure(1, true);
-    d_done.ensure(n_utt, true);
-    d_nhyp.ensure(n_utt, true);
-    d_best.ensure(n_utt);
-    d_blen.ensure(n_utt, true);
-    d_btok.ensure(static_cast<size_t>(n_utt) * max_new, true);
-    d_st.ensure(1);
-    WISB_CUDA(cudaMemcpyAsync(d_logits.p, logits, sizeof(float) * R * V, cudaMemcpyHostToDevice, s));
+    d_cs.ensure(static_cast<size_t>(n_utt) * MAX_CAND, true);  // (zero when a finished search launches nothing)
+    d_ci.ensure(static_cast<size_t>(n_utt) * MAX_CAND, true);
+    d_lse.ensure(R, true);
+    d_i.ensure(n_i);
+    d_f.ensure(n_f);
+    d_slot.ensure(R);
+    WISB_CUDA(cudaMemcpyAsync(d_logits.p, logits, sizeof(float) * R * ldl, cudaMemcpyHostToDevice, s));
     WISB_CUDA(cudaMemcpyAsync(d_mask.p, mask, V, cudaMemcpyHostToDevice, s));
-    if (cum) WISB_CUDA(cudaMemcpyAsync(d_cum.p, cum, sizeof(float) * R, cudaMemcpyHostToDevice, s));
-    if (done) WISB_CUDA(cudaMemcpyAsync(d_done.p, done, sizeof(int) * n_utt, cudaMemcpyHostToDevice, s));
-    std::vector<int> seq(static_cast<size_t>(R) * max_new, 0);
-    for (int r = 0; r < R; ++r)
-      for (int t = 0; t < gen; ++t) seq[static_cast<size_t>(r) * max_new + t] = hist[static_cast<size_t>(r) * gen + t];
-    WISB_CUDA(cudaMemcpyAsync(d_seq.p, seq.data(), sizeof(int) * seq.size(), cudaMemcpyHostToDevice, s));
-    std::vector<float> best(n_utt, -INFINITY);
-    WISB_CUDA(cudaMemcpyAsync(d_best.p, best.data(), sizeof(float) * n_utt, cudaMemcpyHostToDevice, s));
-    int n_done = 0;
-    for (int u = 0; u < n_utt && done; ++u) n_done += done[u] != 0;
-    WISB_REQUIRE(n_done < n_utt, "debug_search_step: every utterance is finished");
-    DecState st{0, gen, n_done, 0, 0};
-    WISB_CUDA(cudaMemcpyAsync(d_st.p, &st, sizeof(st), cudaMemcpyHostToDevice, s));
+    WISB_CUDA(cudaMemcpyAsync(d_i.p, state_i, sizeof(int) * n_i, cudaMemcpyHostToDevice, s));
+    WISB_CUDA(cudaMemcpyAsync(d_f.p, state_f, sizeof(float) * n_f, cudaMemcpyHostToDevice, s));
+    if (max_new_u) {
+      d_cap.ensure(n_utt);
+      WISB_CUDA(cudaMemcpyAsync(d_cap.p, max_new_u, sizeof(int) * n_utt, cudaMemcpyHostToDevice, s));
+    }
+    if (init) {
+      d_prompt.ensure(static_cast<size_t>(n_utt) * prompt_len);
+      WISB_CUDA(cudaMemcpyAsync(d_prompt.p, prompt, sizeof(int) * n_utt * prompt_len, cudaMemcpyHostToDevice, s));
+    }
     SearchArgs a;
     a.logits = d_logits.p;
-    a.ldl = V;
+    a.ldl = ldl;
     a.n_vocab = V;
     a.mask = d_mask.p;
     a.n_utt = n_utt;
     a.beam = beam;
     a.n_cand = 2 * beam;
     a.max_new = max_new;
-    a.max_hyp = beam;
+    a.max_hyp = max_hyp;
     a.eot = eot;
-    a.t_max = 1;
-    a.prompt_len = 1;
-    a.length_penalty = 1.f;
+    a.t_max = t_max;
+    a.prompt_len = init ? prompt_len : 1;
+    a.length_penalty = length_penalty;
     if (ts) {
       a.ts = 1;
       a.no_ts = no_ts;
@@ -1969,23 +1995,30 @@ int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, const 
     a.row_lse = d_lse.p;
     a.part_max = d_pmax.p;
     a.part_sum = d_psum.p;
-    a.cum = d_cum.p;
     a.part = d_part.p;
     a.cand_score = d_cs.p;
     a.cand_idx = d_ci.p;
-    a.tokens = d_tok.p;
-    a.seq[0] = d_seq.p;
-    a.seq[1] = d_seq.p + static_cast<size_t>(R) * max_new;
-    a.indir[0] = d_ind.p;
-    a.indir[1] = d_ind.p + R;
-    a.flip = d_flip.p;
-    a.done = d_done.p;
-    a.n_hyp = d_nhyp.p;
-    a.best_score = d_best.p;
-    a.best_len = d_blen.p;
-    a.best_tokens = d_btok.p;
-    a.st = d_st.p;
-    search_step_run(a, s);  // the production step: processors, top-k partials, merge and the beam bookkeeping
+    a.st = reinterpret_cast<DecState*>(d_i.p);
+    a.flip = d_i.p + 5;
+    a.seq[0] = d_i.p + o_seq;
+    a.seq[1] = d_i.p + o_seq + static_cast<size_t>(R) * max_new;
+    a.indir[0] = d_i.p + o_ind;
+    a.indir[1] = d_i.p + o_ind + static_cast<size_t>(R) * t_max;
+    a.tokens = d_i.p + o_tok;
+    a.row_pos = d_i.p + o_rpos;
+    a.row_slot = d_slot.p;
+    a.done = d_i.p + o_done;
+    a.n_hyp = d_i.p + o_nhyp;
+    a.best_len = d_i.p + o_blen;
+    a.best_tokens = d_i.p + o_btok;
+    a.cum = d_f.p;
+    a.best_score = d_f.p + R;
+    a.max_new_u = max_new_u ? d_cap.p : nullptr;
+    static_assert(sizeof(DecState) == 5 * sizeof(int), "DecState is five ints");
+    if (init) search_init_run(a, d_prompt.p, s, init - 1);
+    search_step_run(a, s);  // the production step: processors, top-k partials, merge, bookkeeping and step advance
+    WISB_CUDA(cudaMemcpyAsync(state_i, d_i.p, sizeof(int) * n_i, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(state_f, d_f.p, sizeof(float) * n_f, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaMemcpyAsync(cand_idx, d_ci.p, sizeof(int) * n_utt * MAX_CAND, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaMemcpyAsync(cand_score, d_cs.p, sizeof(float) * n_utt * MAX_CAND, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaMemcpyAsync(row_lse, d_lse.p, sizeof(float) * R, cudaMemcpyDeviceToHost, s));

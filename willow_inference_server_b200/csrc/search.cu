@@ -9,6 +9,7 @@
 //   * candidates: top 2*beam of beam*V (ties: lowest flat index); at step 0 only beam 0 is live
 //   * the first `beam` candidates that end in eot (or any at the last step) become hypotheses and are replaced by the
 //     next non-eot candidates; an utterance is finished once round(beam*patience) hypotheses exist or at the last step
+//     (a cap of 0 new tokens: at once, with no hypothesis); a row left without a candidate is dead (eot, cum -inf)
 //   * result: best normalised score, first one on ties; eot itself is not part of the output
 //   * beam_size == 1 is the same procedure with 2 candidates, i.e. greedy arg-max decoding
 // Timestamp mode (SearchArgs::ts, prompt without <|notimestamps|>) adds Whisper's timestamp rules after those processors
@@ -280,7 +281,9 @@ __device__ __forceinline__ void search_bookkeeping_body(const SearchArgs& a, int
   }
   const float* cs = a.cand_score + u * MAX_CAND;
   const int* ci = a.cand_idx + u * MAX_CAND;
-  const bool is_last = (gen + 1 >= (a.max_new_u != nullptr ? a.max_new_u[u] : a.max_new));
+  const int cap = a.max_new_u != nullptr ? a.max_new_u[u] : a.max_new;
+  const bool is_last = gen + 1 >= cap;
+  const bool capped = gen >= cap;  // a cap of 0 new tokens: the utterance finishes without a hypothesis
   const float norm = (a.length_penalty != 0.f) ? powf(static_cast<float>(gen + 1), a.length_penalty) : 1.f;
   if (lane == 0) {
     int n_hyp = a.n_hyp[u];
@@ -291,7 +294,7 @@ __device__ __forceinline__ void search_bookkeeping_body(const SearchArgs& a, int
       int pick = k;
       const int idx = ci[k];
       const int tok = idx < 0 ? a.eot : idx % V;
-      if (idx >= 0 && (tok == a.eot || is_last)) {
+      if (!capped && idx >= 0 && (tok == a.eot || is_last)) {
         ++n_hyp;
         if (cs[k] > best) {  // strict: the first best hypothesis wins ties
           best = cs[k];
@@ -314,8 +317,7 @@ __device__ __forceinline__ void search_bookkeeping_body(const SearchArgs& a, int
     s_finished = fin;
     if (fin) {
       a.done[u] = 1;
-      const int nd = atomicAdd(&a.st->n_done, 1) + 1;
-      if (nd == gridDim.x) a.st->all_done = 1;
+      atomicAdd(&a.st->n_done, 1);  // all_done follows in the step advance, once every CTA has taken its ticket
     }
   }
   __syncwarp();
@@ -378,6 +380,9 @@ __global__ void __launch_bounds__(TK_THREADS) search_tail_kernel(const SearchArg
   __syncthreads();
   if (s_last) {  // every utterance has read this step's position / generation step / flip
     if (threadIdx.x == 0) {
+      // set here, not by the CTA that finishes the last utterance: a CTA of this launch that starts after that one
+      // must still take its ticket, or the advance below is skipped
+      if (atomicAdd(&a.st->n_done, 0) == a.n_utt) a.st->all_done = 1;
       a.st->ticket = 0;
       a.st->pos += 1;
       a.st->gen_step += 1;
