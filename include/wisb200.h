@@ -196,6 +196,24 @@ int wisb_debug_dec_pass(wisb_handle* h, const int32_t* prm, int n_prm, const int
 int wisb_debug_read_trace(wisb_handle* h, unsigned long long* out, int n);
 /* encoder output after the final LayerNorm, float32 [B,1500,d_model]; n_layers < 0 = all */
 int wisb_debug_encode(wisb_handle* h, const float* mel, int B, float* enc_out, int n_layers);
+/* The encoder one stage at a time, through the functions the encoder itself runs.  Sizes and indices are checked before
+ * anything is launched (a bad argument returns 1); each entry invalidates the cached encoder output.  fp16 as raw uint16.
+ * stem: conv1 + the conv2 GEMM on log-mel float32 [B,80,3000] (1 <= B <= 4096) -> h1_out fp16 [B * 3072 + 8, d] (conv1
+ * output, all of it: window b's frame f at row b * 3072 + 1 + f, zero rows 0 and 3001..3071 of each window, 8 tail rows)
+ * and x_out float32 [B * 1536, d] (conv2 + positions; rows 1500..1535 of each window are padding). */
+int wisb_debug_enc_stem(wisb_handle* h, const float* mel, int B, uint16_t* h1_out, float* x_out);
+/* the encoder LayerNorm on caller data: x float32 [rows, d] (d a multiple of 128, <= 1536), g, b float32 [d], pdl 0 / 1
+ * (launch with programmatic dependent launch) -> y fp16 [round_up(rows, 8), d] in / out: rows >= `rows` of the kernel's
+ * last 8-row block come back as the caller put them. */
+int wisb_debug_enc_ln(wisb_handle* h, const float* x, int rows, int d, const float* g, const float* b, int pdl, uint16_t* y);
+/* the seven launches of encoder layer `layer` on the residual x_in float32 [B * 1536, d] (padding rows included) ->
+ * x_out float32 [B * 1536, d].  stages_out (may be NULL) receives the output of every launch, at byte offsets in units
+ * of md = B * 1536 * d: 0 xn1 fp16 [md], 2 qkv fp16 [B * 1536, 3 d], 8 vt fp16 [B, H, 64, 1536] (as the QKV epilogue
+ * leaves it: written only under attn_v_mn_major = 0, when qkv's V columns are not), 10 ctx fp16 [md], 12 x after the
+ * o-projection float32 [md], 16 xn2 fp16 [md], 18 fc1 output fp16 [B * 1536, 4 d]; 26 md bytes in all.  Taking the
+ * snapshots serialises the chain; without them it runs as the encoder does (options enc_pdl, attn_v_mn_major, attn_ref).
+ * plan_out (may be NULL) int32 [4][4]: BN, multicast, K splits and grid of the qkv, o, fc1 and fc2 GEMMs. */
+int wisb_debug_enc_layer(wisb_handle* h, int layer, int B, const float* x_in, float* x_out, void* stages_out, int32_t* plan_out);
 /* teacher-forced raw decoder logits (no processors) for utterance 0: float32 [n_tokens, n_vocab] */
 int wisb_debug_forced_logits(wisb_handle* h, const float* mel, const int32_t* tokens, int n_tokens, float* logits_out);
 /* wisb_align's post-processing kernels on caller data for one window: weights float32 [A, R, F] (R = text rows + 1,

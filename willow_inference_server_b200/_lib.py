@@ -65,6 +65,9 @@ _SIGS = {
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_read_trace": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     "wisb_debug_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
+    "wisb_debug_enc_stem": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "wisb_debug_enc_ln": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "wisb_debug_enc_layer": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_forced_logits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "wisb_flac_last_error": (C.c_char_p, []),
     "wisb_flac_info": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -554,6 +557,58 @@ class Handle:
         out = np.zeros((mel.shape[0], 1500, self.dims()["d_model"]), np.float32)
         check(lib().wisb_debug_encode(self._h, ptr(mel), mel.shape[0], ptr(out), n_layers))
         return out
+
+    # the encoder one stage at a time (wisb_debug_enc_*)
+    def debug_enc_stem(self, mel: np.ndarray):
+        """conv1 + conv2 on log-mel float32 [B, 80, 3000] -> (h1 float16 [B * 3072 + 8, d], x float32 [B, 1536, d])"""
+        mel = np.ascontiguousarray(mel, np.float32)
+        if mel.ndim != 3 or mel.shape[1:] != (80, 3000):
+            raise ValueError("mel must be [B, 80, 3000]")
+        B, d = mel.shape[0], self.dims()["d_model"]
+        h1 = np.zeros((B * 3072 + 8, d), np.float16)
+        x = np.zeros((B, 1536, d), np.float32)
+        check(lib().wisb_debug_enc_stem(self._h, ptr(mel), B, ptr(h1), ptr(x)))
+        return h1, x
+
+    def debug_enc_ln(self, x, g, b, y, *, pdl: bool = False):
+        """The encoder LayerNorm of x float32 [rows, d] with g, b float32 [d] into y float16 [round_up(rows, 8), d] (in
+        / out: rows >= `rows` keep their values)."""
+        x = np.ascontiguousarray(x, np.float32)
+        rows, d = x.shape
+        self._inout(y, np.float16, ((rows + 7) // 8 * 8, d), "y")
+        g, b = (np.ascontiguousarray(np.asarray(v, np.float32).reshape(d)) for v in (g, b))
+        check(lib().wisb_debug_enc_ln(self._h, ptr(x), rows, d, ptr(g), ptr(b), int(bool(pdl)), ptr(y)))
+        return y
+
+    ENC_STAGES = (("xn1", np.float16, 1), ("qkv", np.float16, 3), ("vt", np.float16, 1), ("ctx", np.float16, 1),
+                  ("x_o", np.float32, 1), ("xn2", np.float16, 1), ("fc1", np.float16, 4))
+
+    def debug_enc_layer(self, layer: int, x_in, *, stages: bool = False):
+        """Encoder layer `layer` on the residual x_in float32 [B, 1536, d] -> (x_out float32 [B, 1536, d], stages,
+        plans).  stages (with stages=True, else None): the output of every launch, name -> array [B, 1536, width]
+        (xn1, qkv, ctx, x_o after the o-projection, xn2, fc1), and vt [B, H, 64, 1536].  plans: {"qkv" | "o" | "fc1" |
+        "fc2": (BN, multicast, K splits, grid)}."""
+        dm = self.dims()
+        d, H = dm["d_model"], dm["n_heads"]
+        x_in = np.ascontiguousarray(x_in, np.float32)
+        if x_in.ndim != 3 or x_in.shape[1:] != (1536, d):
+            raise ValueError(f"x_in must be [B, 1536, {d}]")
+        B = x_in.shape[0]
+        md = B * 1536 * d
+        x_out = np.zeros_like(x_in)
+        buf = np.zeros(26 * md, np.uint8) if stages else None
+        plan = np.zeros(16, np.int32)
+        check(lib().wisb_debug_enc_layer(self._h, int(layer), B, ptr(x_in), ptr(x_out), ptr(buf), ptr(plan)))
+        plans = {k: tuple(int(v) for v in plan[4 * i: 4 * i + 4]) for i, k in enumerate(("qkv", "o", "fc1", "fc2"))}
+        if not stages:
+            return x_out, None, plans
+        out, at = {}, 0
+        for name, dt, w in self.ENC_STAGES:
+            n = np.dtype(dt).itemsize * w * md
+            a = buf[at: at + n].view(dt)
+            out[name] = a.reshape(B, H, 64, 1536) if name == "vt" else a.reshape(B, 1536, w * d)
+            at += n
+        return x_out, out, plans
 
     def debug_forced_logits(self, mel: np.ndarray, tokens) -> np.ndarray:
         mel = np.ascontiguousarray(mel, np.float32)

@@ -528,7 +528,10 @@ void ensure_encoder(wisb_handle* h, int B) {
     make_tmap_f16_2d(&h->ckv_map, h->ckv.p, HEAD_DIM, static_cast<long long>(h->ckv.n / HEAD_DIM), HEAD_DIM, HEAD_DIM, 128);
     h->enc_cap = B;
   }
-  if (h->plans_B == B && h->plans_vmn == h->attn_v_mn && h->plans_pdl == h->enc_pdl) return;
+  // V stays in qkv (MN-major) unless the wgmma attention reads the transposed Vt: the SIMT attention (option
+  // "attn_ref") reads V from qkv, which the Vt epilogue does not write
+  const int vmn = h->attn_v_mn || h->attn_ref ? 1 : 0;
+  if (h->plans_B == B && h->plans_vmn == vmn && h->plans_pdl == h->enc_pdl) return;
   const int Mi = static_cast<int>(M);
   {
     GemmEpi e;
@@ -544,7 +547,7 @@ void ensure_encoder(wisb_handle* h, int B) {
     const std::string p = "enc." + std::to_string(i) + ".";
     EncLayerPlans& pl = h->enc_plans[i];
     GemmEpi e;
-    e.mode = h->attn_v_mn ? EPI_F16 : EPI_QKV_VT;
+    e.mode = vmn ? EPI_F16 : EPI_QKV_VT;
     e.bias = h->F(p + "qkv.b");
     e.out = h->qkv.p;
     e.ldo = 3 * d;
@@ -582,13 +585,13 @@ void ensure_encoder(wisb_handle* h, int B) {
     e.batch = B;
     gemm_plan(h->plan_ckv, h->enc_out.p, d, h->H("dec.crosskv.w"), Mi, dm.n_dec_layers * 2 * d, d, e, h->num_sms);
   }
-  enc_attn_plan(h->attn_plan, h->qkv.p, h->vt.p, h->ctx.p, B, d, H, h->attn_v_mn != 0);
+  enc_attn_plan(h->attn_plan, h->qkv.p, h->vt.p, h->ctx.p, B, d, H, vmn != 0);
   h->attn_plan.pdl = h->enc_pdl != 0;
   h->plan_conv2.pdl = h->plan_ckv.pdl = h->enc_pdl;
   for (EncLayerPlans& pl : h->enc_plans) pl.qkv.pdl = pl.o.pdl = pl.fc1.pdl = pl.fc2.pdl = h->enc_pdl;
   h->plans_pdl = h->enc_pdl;
   h->plans_B = B;
-  h->plans_vmn = h->attn_v_mn;
+  h->plans_vmn = vmn;
 }
 
 // decoder pass of a call on `rows` rows (utterances x beams): the persistent pass for <= 8 rows unless option
@@ -603,53 +606,79 @@ int ckv_layout(const wisb_handle* h, bool persistent_pass) {
   return persistent_pass && h->mega_tc ? 1 : 0;
 }
 
-// mel (device, [B,80,3000]) -> enc_out fp16 [B*1536, d]
-void run_encoder(wisb_handle* h, int B, int n_layers, int mel_first = 0) {
-  const Dims& dm = h->dims;
-  const int d = dm.d_model;
-  const int M = B * T_ENC_PAD;
+// Encoder stem on the plans ensure_encoder(h, B) bound: conv1 of windows [mel_first, mel_first + B) of h->mel into h1
+// (rows 1..3000 of each window; row 0 and rows 3001.. stay zero from the allocation), then the conv2 GEMM into x.
+void enc_stem_run(wisb_handle* h, int B, int mel_first) {
   cudaStream_t s = h->stream;
-  ensure_encoder(h, B);
-  h->enc_valid = false;  // callers that want the result cached re-validate it after a full encode
   h->prof_begin(3);
-  conv1_gelu_run(h->mel.p + static_cast<size_t>(mel_first) * N_MELS * N_FRAMES, h->H("enc.conv1.w"), h->F("enc.conv1.b"), h->h1.p, B, d, s);
+  conv1_gelu_run(h->mel.p + static_cast<size_t>(mel_first) * N_MELS * N_FRAMES, h->H("enc.conv1.w"), h->F("enc.conv1.b"), h->h1.p, B,
+                 h->dims.d_model, s);
   h->prof_end();
   h->prof_begin(0);
   gemm_run(h->plan_conv2, s);
   h->prof_end();
-  const int nl = (n_layers < 0 || n_layers > dm.n_enc_layers) ? dm.n_enc_layers : n_layers;
-  for (int i = 0; i < nl; ++i) {
-    const std::string p = "enc." + std::to_string(i) + ".";
-    EncLayerPlans& pl = h->enc_plans[i];
-    h->prof_begin(2);
-    layernorm_f32_to_f16_run(h->x.p, h->F(p + "ln1.g"), h->F(p + "ln1.b"), h->xn.p, M, d, s, h->enc_pdl != 0);
-    h->prof_end();
-    h->prof_begin(0);
-    gemm_run(pl.qkv, s);
-    h->prof_end();
-    h->prof_begin(1);
-    if (h->attn_ref)
-      enc_attn_ref_run(h->qkv.p, h->ctx.p, B, d, dm.n_heads, s);
-    else
-      enc_attn_run(h->attn_plan, s);
-    h->prof_end();
-    h->prof_begin(0);
-    gemm_run(pl.o, s);
-    h->prof_end();
-    h->prof_begin(2);
-    layernorm_f32_to_f16_run(h->x.p, h->F(p + "ln2.g"), h->F(p + "ln2.b"), h->xn.p, M, d, s, h->enc_pdl != 0);
-    h->prof_end();
-    h->prof_begin(0);
-    gemm_run(pl.fc1, s);
-    h->prof_end();
-    h->prof_begin(0);
-    gemm_run(pl.fc2, s);
-    h->prof_end();
-  }
+  h->launches += 2;
+}
+
+// The seven launches of encoder layer i on M = B * 1536 rows of x (plans of ensure_encoder(h, B)).  snap (debug entry
+// only), if given, runs after launch k = 0..6 (LN1, QKV, attention, o-proj, LN2, fc1, fc2) and may read its output.
+void enc_layer_run(wisb_handle* h, int i, int M, const std::function<void(int)>* snap) {
+  const Dims& dm = h->dims;
+  const int d = dm.d_model;
+  cudaStream_t s = h->stream;
+  const std::string p = "enc." + std::to_string(i) + ".";
+  EncLayerPlans& pl = h->enc_plans[i];
+  auto after = [&](int k) {
+    if (snap) (*snap)(k);
+  };
   h->prof_begin(2);
-  layernorm_f32_to_f16_run(h->x.p, h->F("enc.ln_post.g"), h->F("enc.ln_post.b"), h->enc_out.p, M, d, s, h->enc_pdl != 0);
+  layernorm_f32_to_f16_run(h->x.p, h->F(p + "ln1.g"), h->F(p + "ln1.b"), h->xn.p, M, d, s, h->enc_pdl != 0);
   h->prof_end();
-  h->launches += 2 + 7 * nl + 1;
+  after(0);
+  h->prof_begin(0);
+  gemm_run(pl.qkv, s);
+  h->prof_end();
+  after(1);
+  h->prof_begin(1);
+  if (h->attn_ref)
+    enc_attn_ref_run(h->qkv.p, h->ctx.p, M / T_ENC_PAD, d, dm.n_heads, s);
+  else
+    enc_attn_run(h->attn_plan, s);
+  h->prof_end();
+  after(2);
+  h->prof_begin(0);
+  gemm_run(pl.o, s);
+  h->prof_end();
+  after(3);
+  h->prof_begin(2);
+  layernorm_f32_to_f16_run(h->x.p, h->F(p + "ln2.g"), h->F(p + "ln2.b"), h->xn.p, M, d, s, h->enc_pdl != 0);
+  h->prof_end();
+  after(4);
+  h->prof_begin(0);
+  gemm_run(pl.fc1, s);
+  h->prof_end();
+  after(5);
+  h->prof_begin(0);
+  gemm_run(pl.fc2, s);
+  h->prof_end();
+  after(6);
+  h->launches += 7;
+}
+
+// mel (device, [B,80,3000]) -> enc_out fp16 [B*1536, d]
+void run_encoder(wisb_handle* h, int B, int n_layers, int mel_first = 0) {
+  const Dims& dm = h->dims;
+  const int M = B * T_ENC_PAD;
+  ensure_encoder(h, B);
+  h->enc_valid = false;  // callers that want the result cached re-validate it after a full encode
+  enc_stem_run(h, B, mel_first);
+  const int nl = (n_layers < 0 || n_layers > dm.n_enc_layers) ? dm.n_enc_layers : n_layers;
+  for (int i = 0; i < nl; ++i) enc_layer_run(h, i, M, nullptr);
+  h->prof_begin(2);
+  layernorm_f32_to_f16_run(h->x.p, h->F("enc.ln_post.g"), h->F("enc.ln_post.b"), h->enc_out.p, M, dm.d_model, h->stream,
+                           h->enc_pdl != 0);
+  h->prof_end();
+  h->launches += 1;
 }
 
 // Places the features of this call in h->mel.  Returns true when the encoder output and cross K/V already in HBM belong
@@ -2347,6 +2376,86 @@ int wisb_debug_encode(wisb_handle* h, const float* mel, int B, float* enc_out, i
       for (int t = 0; t < T_ENC; ++t)
         for (int e = 0; e < d; ++e)
           enc_out[(static_cast<size_t>(b) * T_ENC + t) * d + e] = __half2float(tmp[(static_cast<size_t>(b) * T_ENC_PAD + t) * d + e]);
+  });
+}
+
+int wisb_debug_enc_stem(wisb_handle* h, const float* mel, int B, uint16_t* h1_out, float* x_out) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(h->blob != nullptr && mel && h1_out && x_out, "debug_enc_stem: bad arguments");
+    WISB_REQUIRE(B >= 1 && B <= 4096, "debug_enc_stem: B out of range");
+    const int d = h->dims.d_model;
+    cudaStream_t s = h->stream;
+    upload_mel(h, mel, B);
+    ensure_encoder(h, B);
+    h->enc_valid = false;
+    h->mel_cache_B = 0;
+    enc_stem_run(h, B, 0);
+    const size_t n1 = (static_cast<size_t>(B) * H1_ROWS + 8) * d, nx = static_cast<size_t>(B) * T_ENC_PAD * d;
+    WISB_CUDA(cudaMemcpyAsync(h1_out, h->h1.p, n1 * sizeof(__half), cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(x_out, h->x.p, nx * sizeof(float), cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+int wisb_debug_enc_ln(wisb_handle* h, const float* x, int rows, int d, const float* g, const float* b, int pdl, uint16_t* y) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(x && g && b && y, "debug_enc_ln: NULL argument");
+    WISB_REQUIRE(rows >= 1 && rows <= 4096 * T_ENC_PAD, "debug_enc_ln: rows out of range");
+    WISB_REQUIRE(d >= 128 && d % 128 == 0 && d <= 1536 && (pdl == 0 || pdl == 1),
+                 "debug_enc_ln: d_model a multiple of 128, <= 1536; pdl 0 / 1");
+    h->enc_valid = false;
+    cudaStream_t s = h->stream;
+    const size_t rd = static_cast<size_t>(rows) * d, cap = static_cast<size_t>(round_up(rows, 8)) * d;
+    DevBuf<float> dx, dg, db;
+    DevBuf<__half> dy;
+    layernorm_f32_to_f16_run(to_device(dx, x, rd, s), to_device(dg, g, d, s), to_device(db, b, d, s), to_device(dy, y, cap, s),
+                             rows, d, s, pdl != 0);
+    WISB_CUDA(cudaMemcpyAsync(y, dy.p, cap * sizeof(__half), cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+int wisb_debug_enc_layer(wisb_handle* h, int layer, int B, const float* x_in, float* x_out, void* stages_out, int32_t* plan_out) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(h->blob != nullptr && x_in && x_out, "debug_enc_layer: bad arguments");
+    WISB_REQUIRE(layer >= 0 && layer < h->dims.n_enc_layers, "debug_enc_layer: layer out of range");
+    WISB_REQUIRE(B >= 1 && B <= 4096, "debug_enc_layer: B out of range");
+    const int d = h->dims.d_model;
+    const size_t md = static_cast<size_t>(B) * T_ENC_PAD * d;
+    cudaStream_t s = h->stream;
+    ensure_encoder(h, B);
+    h->enc_valid = false;  // x now holds no features' rows
+    h->mel_cache_B = 0;
+    WISB_CUDA(cudaMemcpyAsync(h->x.p, x_in, md * sizeof(float), cudaMemcpyHostToDevice, s));
+    // snapshots at byte offsets (units of md): xn1 0, qkv 2, vt 8, ctx 10, x after o-proj 12, xn2 16, fc1 output 18
+    uint8_t* o = static_cast<uint8_t*>(stages_out);
+    auto save = [&](size_t at, const void* src, size_t bytes) {
+      WISB_CUDA(cudaMemcpyAsync(o + at * md, src, bytes, cudaMemcpyDeviceToHost, s));
+    };
+    const std::function<void(int)> snap = [&](int k) {
+      switch (k) {
+        case 0: save(0, h->xn.p, md * 2); break;
+        case 1: save(2, h->qkv.p, md * 6); save(8, h->vt.p, md * 2); break;
+        case 2: save(10, h->ctx.p, md * 2); break;
+        case 3: save(12, h->x.p, md * 4); break;
+        case 4: save(16, h->xn.p, md * 2); break;
+        case 5: save(18, h->hbuf.p, md * 8); break;
+        default: break;
+      }
+    };
+    enc_layer_run(h, layer, B * T_ENC_PAD, o ? &snap : nullptr);
+    WISB_CUDA(cudaMemcpyAsync(x_out, h->x.p, md * sizeof(float), cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+    if (plan_out) {
+      const EncLayerPlans& pl = h->enc_plans[layer];
+      const GemmPlan* ps[4] = {&pl.qkv, &pl.o, &pl.fc1, &pl.fc2};
+      for (int i = 0; i < 4; ++i) {
+        plan_out[4 * i] = ps[i]->BN;
+        plan_out[4 * i + 1] = ps[i]->mcast;
+        plan_out[4 * i + 2] = ps[i]->k_splits;
+        plan_out[4 * i + 3] = ps[i]->grid;
+      }
+    }
   });
 }
 
