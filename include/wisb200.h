@@ -38,21 +38,25 @@ const char* wisb_last_error(void);
 int wisb_create(const char* weights_path, int device, wisb_handle** out);
 int wisb_create_from_host(const void* blob, size_t nbytes, int device, wisb_handle** out);
 int wisb_create_from_device(const void* device_blob, size_t nbytes, int device, wisb_handle** out);
-/* a handle without a model: only wisb_logmel works on it (wis.audio.log_mel_spectrogram is a free function) */
+/* a handle without a model: only wisb_logmel works on it (wis.audio.log_mel_spectrogram is a free function).
+ * wisb_create_frontend computes 80-bin features; wisb_create_frontend_mels takes the bin count, 80 or 128 (the
+ * large-v3 family), and returns 1 for any other.  A model handle's front end has its model's n_mels. */
 int wisb_create_frontend(int device, wisb_handle** out);
+int wisb_create_frontend_mels(int device, int n_mels, wisb_handle** out);
 int wisb_destroy(wisb_handle* h);
 /* d_model, n_heads, n_enc_layers, n_dec_layers, n_vocab, n_vocab_pad, n_text_ctx, n_mels, n_audio_ctx, sot, eot,
  * transcribe, translate, no_timestamps, sot_prev, sot_lm, no_speech, blank, lang_first, n_langs */
 int wisb_get_dims(wisb_handle* h, int32_t* dims /* [WISB_N_DIMS] */);
 
 /* (1) batched log-mel.  Utterance b is n_samples[b] samples starting at pcm + offsets[b] (in samples); padding with
- * zeros / trimming to 480000 samples is fused.  pcm_on_device != 0: `pcm` is a device pointer.
- * mel_out (host, float32 [B,80,3000]) may be NULL; keep_on_device != 0 keeps the features in HBM for the next
+ * zeros / trimming to 480000 samples is fused.  pcm_on_device != 0: `pcm` is a device pointer.  n_mels below is the
+ * handle's (wisb_get_dims entry 7): 80, or 128 for the large-v3 family; a blob with any other value is refused (code 1).
+ * mel_out (host, float32 [B,n_mels,3000]) may be NULL; keep_on_device != 0 keeps the features in HBM for the next
  * wisb_generate / wisb_detect_language call that passes mel == NULL. */
 int wisb_logmel(wisb_handle* h, const void* pcm, int pcm_dtype, int pcm_on_device, const int64_t* offsets,
                 const int32_t* n_samples, int B, float* mel_out, int keep_on_device);
 
-/* (3)+(4) features [B,80,3000] float32 host (or NULL: use the features kept by wisb_logmel) -> token ids.
+/* (3)+(4) features [B,n_mels,3000] float32 host (or NULL: use the features kept by wisb_logmel) -> token ids.
  * prompts: int32 [B, prompt_len] (WIS passes the same 4-token prompt for every window, main.py:689).  This entry always
  * decodes without timestamp rules; wisb_generate_ts switches them on.
  * beam_size 1 = greedy.  patience / length_penalty / max_length: CTranslate2 defaults 1, 1, 448.
@@ -198,7 +202,7 @@ int wisb_debug_read_trace(wisb_handle* h, unsigned long long* out, int n);
 int wisb_debug_encode(wisb_handle* h, const float* mel, int B, float* enc_out, int n_layers);
 /* The encoder one stage at a time, through the functions the encoder itself runs.  Sizes and indices are checked before
  * anything is launched (a bad argument returns 1); each entry invalidates the cached encoder output.  fp16 as raw uint16.
- * stem: conv1 + the conv2 GEMM on log-mel float32 [B,80,3000] (1 <= B <= 4096) -> h1_out fp16 [B * 3072 + 8, d] (conv1
+ * stem: conv1 + the conv2 GEMM on log-mel float32 [B,n_mels,3000] (1 <= B <= 4096) -> h1_out fp16 [B * 3072 + 8, d] (conv1
  * output, all of it: window b's frame f at row b * 3072 + 1 + f, zero rows 0 and 3001..3071 of each window, 8 tail rows)
  * and x_out float32 [B * 1536, d] (conv2 + positions; rows 1500..1535 of each window are padding). */
 int wisb_debug_enc_stem(wisb_handle* h, const float* mel, int B, uint16_t* h1_out, float* x_out);

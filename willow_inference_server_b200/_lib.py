@@ -29,6 +29,7 @@ _SIGS = {
     "wisb_create_from_host": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int, C.POINTER(C.c_void_p)]),
     "wisb_create_from_device": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int, C.POINTER(C.c_void_p)]),
     "wisb_create_frontend": (C.c_int, [C.c_int, C.POINTER(C.c_void_p)]),
+    "wisb_create_frontend_mels": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     "wisb_destroy": (C.c_int, [C.c_void_p]),
     "wisb_get_dims": (C.c_int, [C.c_void_p, C.c_void_p]),
     "wisb_logmel": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
@@ -136,9 +137,10 @@ class Handle:
         return cls(h, keepalive)
 
     @classmethod
-    def frontend(cls, device: int = 0):
+    def frontend(cls, device: int = 0, n_mels: int = 80):
+        """a handle without a model that computes n_mels-bin (80 or 128) log-mel features"""
         h = C.c_void_p()
-        check(lib().wisb_create_frontend(device, C.byref(h)))
+        check(lib().wisb_create_frontend_mels(device, int(n_mels), C.byref(h)))
         return cls(h)
 
     def close(self):
@@ -157,6 +159,17 @@ class Handle:
         out = np.zeros(N_DIMS, np.int32)
         check(lib().wisb_get_dims(self._h, ptr(out)))
         return dict(zip(DIM_NAMES, (int(v) for v in out)))
+
+    @property
+    def n_mels(self) -> int:
+        """log-mel bins of this handle's features: 80, or 128 for the large-v3 family"""
+        if getattr(self, "_n_mels", None) is None:
+            self._n_mels = self.dims()["n_mels"]
+        return self._n_mels
+
+    def _check_features(self, mel):
+        if mel.dtype != np.float32 or mel.ndim != 3 or mel.shape[1:] != (self.n_mels, 3000) or not mel.flags["C_CONTIGUOUS"]:
+            raise ValueError(f"features must be a C-contiguous float32 array of shape [n, {self.n_mels}, 3000]")
 
     def set_option(self, key: str, value: int):
         check(lib().wisb_set_option(self._h, key.encode(), int(value)))
@@ -183,7 +196,7 @@ class Handle:
                 raise ValueError("pcm must be float32 or int16")
             pcm = np.ascontiguousarray(pcm)
             p = ptr(pcm)
-        out = np.empty((B, 80, 3000), np.float32) if to_host else None
+        out = np.empty((B, self.n_mels, 3000), np.float32) if to_host else None
         check(lib().wisb_logmel(self._h, p, dt, 1 if pcm_on_device else 0, ptr(offsets), ptr(n_samples), B, ptr(out),
                                 1 if keep else 0))
         return out
@@ -196,8 +209,7 @@ class Handle:
         if prompts.ndim != 2:
             raise ValueError("prompts must be [B, prompt_len]")
         if mel is not None:
-            if mel.dtype != np.float32 or mel.ndim != 3 or mel.shape[1:] != (80, 3000) or not mel.flags["C_CONTIGUOUS"]:
-                raise ValueError("features must be a C-contiguous float32 array of shape [n, 80, 3000]")
+            self._check_features(mel)
             B = mel.shape[0]
         if B is None or prompts.shape[0] != B:
             raise ValueError("one prompt per feature window is required")
@@ -226,6 +238,7 @@ class Handle:
 
     def detect_language(self, mel, B=None):
         if mel is not None:
+            self._check_features(mel)
             B = mel.shape[0]
         nl = self.dims()["n_langs"]
         ids = np.zeros((B, nl), np.int32)
@@ -237,8 +250,7 @@ class Handle:
         """wisb_align -> (paths: list of int32 [len, 2] arrays of (text index, frame), token probs: list of float lists).
         num_frames: an int or one int per window."""
         if mel is not None:
-            if mel.dtype != np.float32 or mel.ndim != 3 or mel.shape[1:] != (80, 3000) or not mel.flags["C_CONTIGUOUS"]:
-                raise ValueError("features must be a C-contiguous float32 array of shape [n, 80, 3000]")
+            self._check_features(mel)
             B = mel.shape[0]
         if B is None or len(text_tokens) != B:
             raise ValueError("one text token list per feature window is required")
@@ -560,10 +572,10 @@ class Handle:
 
     # the encoder one stage at a time (wisb_debug_enc_*)
     def debug_enc_stem(self, mel: np.ndarray):
-        """conv1 + conv2 on log-mel float32 [B, 80, 3000] -> (h1 float16 [B * 3072 + 8, d], x float32 [B, 1536, d])"""
+        """conv1 + conv2 on log-mel float32 [B, n_mels, 3000] -> (h1 float16 [B * 3072 + 8, d], x float32 [B, 1536, d])"""
         mel = np.ascontiguousarray(mel, np.float32)
-        if mel.ndim != 3 or mel.shape[1:] != (80, 3000):
-            raise ValueError("mel must be [B, 80, 3000]")
+        if mel.ndim != 3 or mel.shape[1:] != (self.n_mels, 3000):
+            raise ValueError(f"mel must be [B, {self.n_mels}, 3000]")
         B, d = mel.shape[0], self.dims()["d_model"]
         h1 = np.zeros((B * 3072 + 8, d), np.float16)
         x = np.zeros((B, 1536, d), np.float32)

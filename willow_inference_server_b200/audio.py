@@ -4,7 +4,8 @@
         log_mel_spectrogram, pad_or_trim, chunk_iter, find_longest_common_sequence)
 
 * ``log_mel_spectrogram`` replaces wis/audio.py:72-103: same argument (float32 numpy PCM), returns an
-  object with ``.numpy()`` -> float32 [80, n_frames] exactly as the call sites use it (main.py:608,614).  The STFT /
+  object with ``.numpy()`` -> float32 [n_mels, n_frames] exactly as the call sites use it (main.py:608,614).  n_mels is
+  80 (openai-whisper's default) or 128, what the large-v3 family needs (``models.Whisper.n_mels``).  The STFT /
   mel / log pipeline runs in the CUDA kernel csrc/logmel.cu; there is no CPU path.
 * ``pad_or_trim`` (wis/audio.py:28-51) is kept for API compatibility; the kernel fuses padding/trimming, so calling
   it first is allowed but not required (``log_mel_spectrogram`` accepts the unpadded utterance too).
@@ -23,6 +24,7 @@ from . import _lib
 SAMPLE_RATE = 16000
 N_FFT = 400
 N_MELS = 80
+MEL_BINS = (80, 128)
 HOP_LENGTH = 160
 CHUNK_LENGTH = 30
 N_SAMPLES = CHUNK_LENGTH * SAMPLE_RATE
@@ -34,16 +36,28 @@ chunk_len = chunk_length_s * SAMPLE_RATE
 stride_left = stride_length_s[0] * SAMPLE_RATE
 stride_right = stride_length_s[1] * SAMPLE_RATE
 
-_frontend = None
+_frontends = {}  # n_mels -> front-end handle, made on first use
 _frontend_lock = threading.Lock()
 
 
-def _get_frontend() -> "_lib.Handle":
-    global _frontend
+def _get_frontend(n_mels: int = N_MELS) -> "_lib.Handle":
     with _frontend_lock:
-        if _frontend is None:
-            _frontend = _lib.Handle.frontend(int(os.environ.get("WISB_DEVICE", "0")))
-        return _frontend
+        if n_mels not in _frontends:
+            _frontends[n_mels] = _lib.Handle.frontend(int(os.environ.get("WISB_DEVICE", "0")), n_mels)
+        return _frontends[n_mels]
+
+
+def _handle_for(handle, n_mels):
+    """the handle a front-end call runs on: `handle` (its own n_mels; a different explicit n_mels is an error) or the
+    cached front end for n_mels (default 80)"""
+    if handle is None:
+        n = N_MELS if n_mels is None else int(n_mels)
+        if n not in MEL_BINS:
+            raise ValueError(f"n_mels must be 80 or 128, not {n_mels}")
+        return _get_frontend(n)
+    if n_mels is not None and int(n_mels) != handle.n_mels:
+        raise ValueError(f"n_mels = {n_mels} but the handle computes {handle.n_mels}-bin features")
+    return handle
 
 
 class MelFeatures:
@@ -76,7 +90,7 @@ def pad_or_trim(array, length: int = N_SAMPLES, *, axis: int = -1):
 
 
 def log_mel_spectrogram(audio, n_mels: int = N_MELS) -> MelFeatures:
-    if n_mels != N_MELS:
+    if n_mels not in MEL_BINS:
         raise AssertionError(f"Unsupported n_mels: {n_mels}")
     if isinstance(audio, str):
         raise TypeError("log_mel_spectrogram takes PCM samples (numpy), not a path")
@@ -85,13 +99,14 @@ def log_mel_spectrogram(audio, n_mels: int = N_MELS) -> MelFeatures:
         pcm = pcm.astype(np.float32)
     if pcm.ndim != 1:
         raise ValueError("audio must be a 1-D array of 16 kHz samples")
-    mel = _get_frontend().logmel(pcm, [0], [pcm.shape[0]])
+    mel = _get_frontend(n_mels).logmel(pcm, [0], [pcm.shape[0]])
     return MelFeatures(mel[0])
 
 
-def log_mel_batch(pcm_list, handle=None) -> np.ndarray:
-    """Batched form used by the engine-side tests/bench: list of 1-D arrays -> float32 [B, 80, 3000]."""
-    h = handle or _get_frontend()
+def log_mel_batch(pcm_list, handle=None, n_mels=None) -> np.ndarray:
+    """Batched form used by the engine-side tests/bench: list of 1-D arrays -> float32 [B, n_mels, 3000], n_mels the
+    handle's (a model handle computes its model's) or, without a handle, the argument's (default 80)."""
+    h = _handle_for(handle, n_mels)
     dt = np.int16 if all(np.asarray(p).dtype == np.int16 for p in pcm_list) else np.float32
     arrs = [np.ascontiguousarray(p, dt) for p in pcm_list]
     n = np.array([a.shape[0] for a in arrs], np.int32)
@@ -132,11 +147,13 @@ def chunk_table(total: int):
     return np.asarray(offs, np.int64), np.asarray(lens, np.int32), strides
 
 
-def log_mel_chunks(audio, handle=None):
+def log_mel_chunks(audio, handle=None, n_mels=None):
     """Long-audio front end (main.py:603-611 does ``[log_mel_spectrogram(pad_or_trim(c)) for c in chunk_iter(audio)]``):
     every 22-s window is framed by the log-mel kernel straight out of the one PCM buffer (offset + length per window,
     zero padding to 30 s fused), so neither the padded copies nor a [N, 480000] batch is ever materialised.
-    Returns (float32 [N, 80, 3000], strides) with the strides ``chunk_iter`` would have produced."""
+    Returns (float32 [N, n_mels, 3000], strides) with the strides ``chunk_iter`` would have produced; n_mels as in
+    ``log_mel_batch``."""
+    h = _handle_for(handle, n_mels)
     pcm = np.asarray(audio)
     if pcm.dtype not in (np.float32, np.int16):
         pcm = pcm.astype(np.float32)
@@ -144,18 +161,20 @@ def log_mel_chunks(audio, handle=None):
         raise ValueError("audio must be a 1-D array of 16 kHz samples")
     offs, lens, strides = chunk_table(pcm.shape[0])
     if not strides:
-        return np.zeros((0, N_MELS, N_FRAMES), np.float32), strides
-    return (handle or _get_frontend()).logmel(np.ascontiguousarray(pcm), offs, lens), strides
+        return np.zeros((0, h.n_mels, N_FRAMES), np.float32), strides
+    return h.logmel(np.ascontiguousarray(pcm), offs, lens), strides
 
 
-def log_mel_window(audio, handle=None):
-    """One utterance of at most 30 s -> float32 [1, 80, 3000] (zero padding to the window fused in the kernel): what
-    ``log_mel_spectrogram(pad_or_trim(audio)).numpy()[None]`` yields in main.py:612-617."""
+def log_mel_window(audio, handle=None, n_mels=None):
+    """One utterance of at most 30 s -> float32 [1, n_mels, 3000] (zero padding to the window fused in the kernel): what
+    ``log_mel_spectrogram(pad_or_trim(audio), n_mels).numpy()[None]`` yields in main.py:612-617; n_mels as in
+    ``log_mel_batch``."""
+    h = _handle_for(handle, n_mels)
     pcm = np.asarray(audio)
     if pcm.dtype not in (np.float32, np.int16):
         pcm = pcm.astype(np.float32)
     n = min(int(pcm.shape[0]), N_SAMPLES)
-    return (handle or _get_frontend()).logmel(np.ascontiguousarray(pcm[:n]), [0], [n])
+    return h.logmel(np.ascontiguousarray(pcm[:n]), [0], [n])
 
 
 def transcribe_long(model, audio, prompt, tokenizer, *, beam_size: int = 5, batcher=None, max_windows_per_call: int = 64,
@@ -163,7 +182,8 @@ def transcribe_long(model, audio, prompt, tokenizer, *, beam_size: int = 5, batc
     """The long-audio path of ``do_whisper`` (main.py:582-617, 676-714) on top of the pieces above: window the
     utterance, decode all windows as batch rows (the reference goes two at a time, ``concurrent_gpu_chunks``), stitch
     the token lists with ``find_longest_common_sequence``.  ``model`` is a ``models.Whisper`` (or anything with its
-    ``generate``); with ``batcher`` (a ``TranscribeBatcher``) the windows join other requests' batches.
+    ``generate``); with ``batcher`` (a ``TranscribeBatcher``) the windows join other requests' batches.  The windows
+    are framed with the model's ``n_mels`` (80 for a model without that property).
     Returns the merged token ids (numpy int array), ready for ``whisper_processor.decode``.
 
     A timestamp prompt (one without <|notimestamps|>) works for audio of one window only: the overlap merge matches
@@ -171,13 +191,15 @@ def transcribe_long(model, audio, prompt, tokenizer, *, beam_size: int = 5, batc
     timestamp prompt raises ``ValueError``."""
     from .models import StorageView
 
+    n_mels = int(getattr(model, "n_mels", N_MELS))
+    frame = {} if n_mels == N_MELS else {"n_mels": n_mels}  # (80 bins: the front-end functions' default)
     pcm = np.asarray(audio)
     if pcm.ndim == 1 and pcm.shape[0] <= N_SAMPLES:
         # <= 30 s: the reference does not window at all (main.py:587-617), it decodes one zero-padded 30-s window
-        mel = log_mel_window(pcm)
+        mel = log_mel_window(pcm, **frame)
         strides = [(pcm.shape[0], 0, 0)]
     else:
-        mel, strides = log_mel_chunks(audio)
+        mel, strides = log_mel_chunks(audio, **frame)
     if not strides:
         return np.zeros(0, np.int64)
     if mel.shape[0] > 1:

@@ -57,6 +57,9 @@ class TranscribeBatcher:
         if max_batch < 1:
             raise ValueError("max_batch must be >= 1")
         self._model = model
+        # features are checked at submit against the model's bin count (CTranslate2's Whisper.n_mels); an engine
+        # without that property takes the 80-bin features of every Whisper model before large-v3
+        self._n_mels = int(getattr(model, "n_mels", 80))
         self.max_batch = int(max_batch)
         self.max_wait = float(max_wait_ms) / 1e3
         self.max_queue_windows = int(max_queue_windows)
@@ -70,11 +73,13 @@ class TranscribeBatcher:
 
     # ------------------------------------------------------------------------------------------------ producers
     def submit(self, features, prompt, **generate_options) -> Future:
-        """features: float32 [n, 80, 3000] (or a StorageView); prompt: the n windows' common prompt ids.
+        """features: float32 [n, n_mels, 3000] (or a StorageView), n_mels the model's (80, or 128 for the large-v3
+        family); prompt: the n windows' common prompt ids.
         Returns a Future of the list of n results ``Whisper.generate`` would have returned for this request alone."""
         arr = features.array if isinstance(features, StorageView) else np.asarray(features)
-        if arr.ndim != 3 or arr.dtype != np.float32:
-            raise ValueError("features must be float32 [n, 80, 3000]")
+        if arr.ndim != 3 or arr.dtype != np.float32 or tuple(arr.shape[1:]) != (self._n_mels, 3000):
+            raise ValueError(f"features must be float32 [n, {self._n_mels}, 3000] for this model, got {arr.dtype} "
+                             f"{tuple(arr.shape)}")
         if prompt and isinstance(prompt[0], (list, tuple)):
             if any(list(p) != list(prompt[0]) for p in prompt) or len(prompt) != arr.shape[0]:
                 raise ValueError("one request carries one prompt for all of its windows (as main.py:689 builds it)")

@@ -13,7 +13,6 @@ namespace wisb {
 
 constexpr int T_ENC = 1500;      // encoder positions per 30-s window
 constexpr int T_ENC_PAD = 1536;  // rows per window in every encoder activation (12 x 128)
-constexpr int N_MELS = 80;
 constexpr int N_FRAMES = 3000;
 constexpr int N_SAMPLES = 480000;
 constexpr int HEAD_DIM = 64;

@@ -16,27 +16,30 @@ void make_tmap_f16_2d(CUtensorMap* map, const void* ptr, long long cols, long lo
 namespace {
 
 // =====================================================================================================================
-// conv1: Conv1d(80 -> d, k=3, pad=1) + GELU.  1.8 GFLOP per window (0.1 % of the encoder): fp32 FMA, smem tiled.
+// conv1: Conv1d(NM -> d, k=3, pad=1) + GELU, NM = 80 or 128 mel bins.  1.8 GFLOP per window at 80 bins, 2.95 at 128
+// (d = 1280; 0.1 % of the encoder): fp32 FMA, smem tiled.  At 128 bins the tiles take 133,632 B: one CTA per SM.
 // Output row layout (fp16 [B, 3072, d]): row 0 = zeros (left pad), rows 1..3000 = frames, rows 3001.. = zeros, so that
 // conv2 (k=3, stride 2, pad 1) is a plain GEMM whose A row t' is the 3*d contiguous values starting at row 2*t'.
 // =====================================================================================================================
 constexpr int C1_FT = 64;   // frames per CTA
 constexpr int C1_CT = 64;   // output channels per CTA
-constexpr int C1_K = 3 * N_MELS;
-constexpr int C1_SMEM = (N_MELS * (C1_FT + 2) + C1_K * (C1_CT + 1)) * 4;
+template <int NM>
+constexpr int c1_smem_bytes() { return (NM * (C1_FT + 2) + 3 * NM * (C1_CT + 1)) * 4; }
 
+template <int NM>
 __global__ void __launch_bounds__(256)
 conv1_gelu_kernel(const float* __restrict__ mel, const __half* __restrict__ w, const float* __restrict__ bias,
                   __half* __restrict__ h1, int d) {
+  constexpr int C1_K = 3 * NM;
   extern __shared__ float c1_smem[];
   float (*xm)[C1_FT + 2] = reinterpret_cast<float (*)[C1_FT + 2]>(c1_smem);
-  float (*wt)[C1_CT + 1] = reinterpret_cast<float (*)[C1_CT + 1]>(c1_smem + N_MELS * (C1_FT + 2));
+  float (*wt)[C1_CT + 1] = reinterpret_cast<float (*)[C1_CT + 1]>(c1_smem + NM * (C1_FT + 2));
   const int b = blockIdx.z;
   const int f0 = blockIdx.x * C1_FT;
   const int c0 = blockIdx.y * C1_CT;
   const int tid = threadIdx.x;
-  const float* melb = mel + static_cast<long long>(b) * N_MELS * N_FRAMES;
-  for (int i = tid; i < N_MELS * (C1_FT + 2); i += 256) {
+  const float* melb = mel + static_cast<long long>(b) * NM * N_FRAMES;
+  for (int i = tid; i < NM * (C1_FT + 2); i += 256) {
     const int ci = i / (C1_FT + 2), fl = i % (C1_FT + 2);
     const int f = f0 + fl - 1;
     xm[ci][fl] = (f >= 0 && f < N_FRAMES) ? melb[ci * N_FRAMES + f] : 0.f;
@@ -54,7 +57,7 @@ conv1_gelu_kernel(const float* __restrict__ mel, const __half* __restrict__ w, c
 #pragma unroll
     for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
   for (int kk = 0; kk < C1_K; ++kk) {
-    const int k = kk / N_MELS, ci = kk - k * N_MELS;
+    const int k = kk / NM, ci = kk - k * NM;
     float a[4], bb[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) a[i] = xm[ci][tf * 4 + i + k];
@@ -321,14 +324,20 @@ enc_attn_ref_kernel(const __half* __restrict__ qkv, __half* __restrict__ ctx, in
 
 }  // namespace
 
-void conv1_gelu_run(const float* mel, const __half* w, const float* bias, __half* h1, int B, int d, cudaStream_t stream) {
+void conv1_gelu_run(const float* mel, const __half* w, const float* bias, __half* h1, int B, int d, int n_mels,
+                    cudaStream_t stream) {
   WISB_REQUIRE(d % C1_CT == 0, "conv1: d_model must be a multiple of 64");
+  WISB_REQUIRE(n_mels == 80 || n_mels == 128, "conv1: n_mels must be 80 or 128");
   static std::atomic<unsigned long long> once{0};
   once_per_device(once, [] {
-    WISB_CUDA(cudaFuncSetAttribute(conv1_gelu_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C1_SMEM));
+    WISB_CUDA(cudaFuncSetAttribute(conv1_gelu_kernel<80>, cudaFuncAttributeMaxDynamicSharedMemorySize, c1_smem_bytes<80>()));
+    WISB_CUDA(cudaFuncSetAttribute(conv1_gelu_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, c1_smem_bytes<128>()));
   });
   dim3 grid(cdiv(N_FRAMES, C1_FT), d / C1_CT, B);
-  conv1_gelu_kernel<<<grid, 256, C1_SMEM, stream>>>(mel, w, bias, h1, d);
+  if (n_mels == 80)
+    conv1_gelu_kernel<80><<<grid, 256, c1_smem_bytes<80>(), stream>>>(mel, w, bias, h1, d);
+  else
+    conv1_gelu_kernel<128><<<grid, 256, c1_smem_bytes<128>(), stream>>>(mel, w, bias, h1, d);
   WISB_CUDA(cudaGetLastError());
 }
 

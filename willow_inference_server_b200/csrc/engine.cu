@@ -113,7 +113,7 @@ struct wisb_handle {
   DevBuf<uint8_t> pcm_dev;
   DevBuf<long long> pcm_off;
   DevBuf<int> pcm_n;
-  DevBuf<float> mel;  // [B,80,3000]
+  DevBuf<float> mel;  // [B,n_mels,3000]
   int mel_B = 0;      // utterances currently held in `mel`
   // encoder workspaces (capacity enc_cap utterances)
   int enc_cap = 0;
@@ -268,7 +268,8 @@ void parse_blob(wisb_handle* h, const std::vector<uint8_t>& head) {
   const Dims& d = h->dims;
   WISB_REQUIRE(d.d_model % 128 == 0 && d.d_model == 64 * d.n_heads && d.d_model <= 1536,
                "engine requires head_dim 64 and d_model a multiple of 128 (<= 1536)");
-  WISB_REQUIRE(d.n_mels == N_MELS && d.n_audio_ctx == T_ENC, "engine is built for 80 mels x 1500 positions");
+  WISB_REQUIRE((d.n_mels == 80 || d.n_mels == 128) && d.n_audio_ctx == T_ENC,
+               "engine runs 80- or 128-bin log-mel features x 1500 positions");
   WISB_REQUIRE(d.n_text_ctx <= T_MAX, "n_text_ctx > 448");
   WISB_REQUIRE(d.n_langs <= 128, "more than 128 languages");
   WISB_REQUIRE(d.n_vocab > 0 && d.n_vocab_pad >= d.n_vocab && d.n_vocab_pad % 128 == 0 && d.n_enc_layers > 0 && d.n_dec_layers > 0,
@@ -359,7 +360,7 @@ void finish_create(wisb_handle* h) {
   WISB_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
   for (auto& e : h->ev) WISB_CUDA(cudaEventCreate(&e));
   h->lm_tables.ensure(logmel_table_floats());
-  logmel_init_tables(h->lm_tables.p, h->stream);
+  logmel_init_tables(h->lm_tables.p, d.n_mels, h->stream);
   if (!has_model) {  // front-end-only handle (wisb_create_frontend)
     WISB_CUDA(cudaStreamSynchronize(h->stream));
     return;
@@ -497,10 +498,13 @@ void finish_create(wisb_handle* h) {
   WISB_CUDA(cudaStreamSynchronize(h->stream));
 }
 
-// feature buffer [B,80,3000] (+ the per-utterance maxima of the log-mel kernel); growing it drops what it held
+// floats of the features of B windows: [B, n_mels, 3000]
+size_t mel_floats(const wisb_handle* h, int B) { return static_cast<size_t>(B) * h->dims.n_mels * N_FRAMES; }
+
+// feature buffer [B,n_mels,3000] (+ the per-utterance maxima of the log-mel kernel); growing it drops what it held
 void ensure_mel(wisb_handle* h, int B) {
   h->lm_max.ensure(B);
-  const size_t n = static_cast<size_t>(B) * N_MELS * N_FRAMES;
+  const size_t n = mel_floats(h, B);
   if (n <= h->mel.n) return;
   h->mel.ensure(n);
   h->mel_B = 0;
@@ -611,8 +615,8 @@ int ckv_layout(const wisb_handle* h, bool persistent_pass) {
 void enc_stem_run(wisb_handle* h, int B, int mel_first) {
   cudaStream_t s = h->stream;
   h->prof_begin(3);
-  conv1_gelu_run(h->mel.p + static_cast<size_t>(mel_first) * N_MELS * N_FRAMES, h->H("enc.conv1.w"), h->F("enc.conv1.b"), h->h1.p, B,
-                 h->dims.d_model, s);
+  conv1_gelu_run(h->mel.p + mel_floats(h, mel_first), h->H("enc.conv1.w"), h->F("enc.conv1.b"), h->h1.p, B,
+                 h->dims.d_model, h->dims.n_mels, s);
   h->prof_end();
   h->prof_begin(0);
   gemm_run(h->plan_conv2, s);
@@ -665,7 +669,7 @@ void enc_layer_run(wisb_handle* h, int i, int M, const std::function<void(int)>*
   h->launches += 7;
 }
 
-// mel (device, [B,80,3000]) -> enc_out fp16 [B*1536, d]
+// mel (device, [B,n_mels,3000]) -> enc_out fp16 [B*1536, d]
 void run_encoder(wisb_handle* h, int B, int n_layers, int mel_first = 0) {
   const Dims& dm = h->dims;
   const int M = B * T_ENC_PAD;
@@ -692,7 +696,7 @@ bool upload_mel(wisb_handle* h, const float* mel, int B) {
     h->mel_cache_B = 0;
     return false;
   }
-  const size_t n = static_cast<size_t>(B) * N_MELS * N_FRAMES;
+  const size_t n = mel_floats(h, B);
   if (h->encoder_cache && B <= 2) {
     if (h->enc_valid && h->mel_cache_B == B && memcmp(h->mel_cache.data(), mel, n * sizeof(float)) == 0) return true;
     h->mel_cache.assign(mel, mel + n);
@@ -1547,8 +1551,14 @@ int wisb_create_from_device(const void* device_blob, size_t nbytes, int device, 
   });
 }
 
-int wisb_create_frontend(int device, wisb_handle** out) {
-  return create_common(out, device, [&](wisb_handle*) {});
+int wisb_create_frontend(int device, wisb_handle** out) { return wisb_create_frontend_mels(device, 80, out); }
+
+int wisb_create_frontend_mels(int device, int n_mels, wisb_handle** out) {
+  if (n_mels != 80 && n_mels != 128) {
+    g_last_error = "n_mels must be 80 or 128";
+    return 1;
+  }
+  return create_common(out, device, [&](wisb_handle* h) { h->dims.n_mels = n_mels; });
 }
 
 int wisb_destroy(wisb_handle* h) {
@@ -1645,9 +1655,10 @@ int wisb_logmel(wisb_handle* h, const void* pcm, int pcm_dtype, int pcm_on_devic
     static_assert(sizeof(long long) == sizeof(int64_t), "offset type");
     WISB_CUDA(cudaMemcpyAsync(h->pcm_off.p, offsets, sizeof(int64_t) * B, cudaMemcpyHostToDevice, s));
     WISB_CUDA(cudaMemcpyAsync(h->pcm_n.p, n_samples, sizeof(int32_t) * B, cudaMemcpyHostToDevice, s));
-    logmel_run(pcm_d, pcm_dtype == WISB_PCM_S16, h->pcm_off.p, h->pcm_n.p, B, h->lm_tables.p, h->mel.p, h->lm_max.p, s);
+    logmel_run(pcm_d, pcm_dtype == WISB_PCM_S16, h->pcm_off.p, h->pcm_n.p, B, h->dims.n_mels, h->lm_tables.p, h->mel.p,
+               h->lm_max.p, s);
     if (mel_out != nullptr)
-      WISB_CUDA(cudaMemcpyAsync(mel_out, h->mel.p, static_cast<size_t>(B) * N_MELS * N_FRAMES * sizeof(float), cudaMemcpyDeviceToHost, s));
+      WISB_CUDA(cudaMemcpyAsync(mel_out, h->mel.p, mel_floats(h, B) * sizeof(float), cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaEventRecord(h->ev[1], s));
     WISB_CUDA(cudaStreamSynchronize(s));
     WISB_CUDA(cudaEventElapsedTime(&h->timing[0], h->ev[0], h->ev[1]));

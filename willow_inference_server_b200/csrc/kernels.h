@@ -59,16 +59,18 @@ void make_tmap_f16_2d(CUtensorMap* map, const void* ptr, long long cols, long lo
 
 // ------------------------------------------------------------------ log-mel front end (logmel.cu)
 // pcm: B utterances, f32 or s16, utterance b starts at pcm + offsets[b] (elements) and has n_samples[b] samples
-// (unpadded; padding / trimming to 480000 is fused).  mel: [B, 80, 3000] f32 on device.
+// (unpadded; padding / trimming to 480000 is fused).  mel: [B, n_mels, 3000] f32 on device, n_mels 80 or 128 (the
+// filterbank logmel_init_tables uploaded for that bin count).
 size_t logmel_table_floats();
-void logmel_init_tables(float* tables_dev, cudaStream_t stream);
+void logmel_init_tables(float* tables_dev, int n_mels, cudaStream_t stream);
 void logmel_run(const void* pcm, int pcm_is_s16, const long long* offsets_dev, const int* n_samples_dev, int B,
-                const float* tables_dev, float* mel, unsigned* max_ws /* [B] */, cudaStream_t stream);
+                int n_mels, const float* tables_dev, float* mel, unsigned* max_ws /* [B] */, cudaStream_t stream);
 
 // ------------------------------------------------------------------ encoder pieces (encoder.cu)
-// conv1 (80 -> d, k=3, pad 1) + GELU, writes h1 [B, 3072, d] fp16 with the row layout conv2's strided view needs
-void conv1_gelu_run(const float* mel, const __half* w /*[d,240]*/, const float* bias, __half* h1, int B, int d,
-                    cudaStream_t stream);
+// conv1 (n_mels -> d, k=3, pad 1) + GELU, writes h1 [B, 3072, d] fp16 with the row layout conv2's strided view needs;
+// n_mels 80 or 128
+void conv1_gelu_run(const float* mel, const __half* w /*[d, 3 n_mels]*/, const float* bias, __half* h1, int B, int d,
+                    int n_mels, cudaStream_t stream);
 // LayerNorm over rows of fp32 x [rows, d] -> fp16 y [rows, d]
 void layernorm_f32_to_f16_run(const float* x, const float* g, const float* b, __half* y, int rows, int d,
                               cudaStream_t stream, bool pdl = false);

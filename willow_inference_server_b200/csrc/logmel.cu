@@ -1,19 +1,21 @@
 // Batched log-mel front end for sm_90a.
 //
 // Replaces wis/audio.py:28-51 (pad_or_trim) and :72-103 (log_mel_spectrogram):
-//   hann(400) periodic, STFT n_fft=400 hop=160 center/reflect, |.|^2 of the first 3000 frames, 80x201 Slaney mel
-//   filterbank, log10(clamp 1e-10), max(x, utterance_max - 8), (x + 4) / 4.
+//   hann(400) periodic, STFT n_fft=400 hop=160 center/reflect, |.|^2 of the first 3000 frames, NMx201 Slaney mel
+//   filterbank (NM = 80, or 128 for the large-v3 family), log10(clamp 1e-10), max(x, utterance_max - 8), (x + 4) / 4.
 // Differences in HOW (not what): zero-padding / trimming to 480000 samples and the optional s16 -> f32 conversion are
 // fused into the frame gather (the padded PCM is never materialised); the 400-point real DFT is evaluated directly in
 // fp32 FMA using the even/odd symmetry of the windowed frame (201 x 200 MACs per frame instead of an FFT -- single-pass
 // TF32 tensor cores miss the 1e-4 parity bar, see BASELINE.md section 2); frames that lie wholly in the zero padding
-// skip the DFT.  HBM traffic per window: <= 1.92 MB PCM in, 0.96 MB out (+0.96 MB re-read/write for the clamp pass).
+// skip the DFT.  HBM traffic per window: <= 1.92 MB PCM in, 0.96 MB out at 80 bins / 1.54 MB at 128 (+ the same again
+// re-read/written by the clamp pass).
 #include <math.h>
 
 #include <vector>
 
 #include "kernels.h"
 #include "mel_filters_table.inc"
+#include "mel_filters_table128.inc"
 
 namespace wisb {
 
@@ -29,9 +31,28 @@ constexpr int KQ = 52;
 constexpr int LM_THREADS = 224;  // 208 workers (52 bin-quads x 4 frame groups) + 16 helpers
 constexpr int P_LD = BINS_PAD + 1;
 
+// each bin count has its own tables, so front ends of both kinds can run in one process
 __constant__ int c_mel_start[80];
 __constant__ int c_mel_len[80];
 __constant__ float c_mel_w[80][MEL_MAXNZ];
+__constant__ int c_mel128_start[128];
+__constant__ int c_mel128_len[128];
+__constant__ float c_mel128_w[128][MEL_MAXNZ];
+
+template <int NM>
+struct MelTables;
+template <>
+struct MelTables<80> {
+  static __device__ __forceinline__ int start(int m) { return c_mel_start[m]; }
+  static __device__ __forceinline__ int len(int m) { return c_mel_len[m]; }
+  static __device__ __forceinline__ float w(int m, int q) { return c_mel_w[m][q]; }
+};
+template <>
+struct MelTables<128> {
+  static __device__ __forceinline__ int start(int m) { return c_mel128_start[m]; }
+  static __device__ __forceinline__ int len(int m) { return c_mel128_len[m]; }
+  static __device__ __forceinline__ float w(int m, int q) { return c_mel128_w[m][q]; }
+};
 
 __device__ __forceinline__ unsigned f2ord(float f) {
   unsigned u = __float_as_uint(f);
@@ -52,7 +73,7 @@ __device__ __forceinline__ float load_sample(const void* pcm, long long off, int
 }
 
 // twiddle tables: tw[n][k] = hann[n] * cos(2 pi k n / 400), ts[n][k] = hann[n] * sin(2 pi k n / 400), n in [0,200]
-template <bool S16>
+template <int NM, bool S16>
 __global__ void __launch_bounds__(LM_THREADS)
 logmel_power_kernel(const void* __restrict__ pcm, const long long* __restrict__ offsets, const int* __restrict__ n_samples,
                     const float* __restrict__ tw, const float* __restrict__ ts, float* __restrict__ mel,
@@ -66,13 +87,13 @@ logmel_power_kernel(const void* __restrict__ pcm, const long long* __restrict__ 
   const int n_eff = min(n_samples[b], N_SAMPLES);
   const long long off = offsets[b];
   const long long s0 = static_cast<long long>(f0) * HOP - N_FFT / 2;  // first padded-window index this CTA touches
-  float* out = mel + static_cast<long long>(b) * N_MELS * N_FRAMES;
+  float* out = mel + static_cast<long long>(b) * NM * N_FRAMES;
 
   // frames wholly inside the zero padding: power == 0 -> log10(clamp) == -10 exactly
   const bool all_zero = (s0 >= n_eff) && (s0 + SPAN <= N_SAMPLES);
   float local_max = -10.0f;
   if (all_zero) {
-    for (int i = tid; i < N_MELS * FT; i += LM_THREADS) {
+    for (int i = tid; i < NM * FT; i += LM_THREADS) {
       const int m = i / FT, f = f0 + (i % FT);
       if (f < N_FRAMES) out[m * N_FRAMES + f] = -10.0f;
     }
@@ -114,12 +135,12 @@ logmel_power_kernel(const void* __restrict__ pcm, const long long* __restrict__ 
         for (int f = 0; f < 8; ++f) pw[fg * 8 + f][kq + KQ * j] = re[j][f] * re[j][f] + im[j][f] * im[j][f];
     }
     __syncthreads();
-    for (int i = tid; i < N_MELS * FT; i += LM_THREADS) {
+    for (int i = tid; i < NM * FT; i += LM_THREADS) {
       const int m = i / FT, fl = i % FT;
       const int f = f0 + fl;
-      const int st = c_mel_start[m], ln = c_mel_len[m];
+      const int st = MelTables<NM>::start(m), ln = MelTables<NM>::len(m);
       float acc = 0.f;
-      for (int q = 0; q < ln; ++q) acc = fmaf(c_mel_w[m][q], pw[fl][st + q], acc);
+      for (int q = 0; q < ln; ++q) acc = fmaf(MelTables<NM>::w(m, q), pw[fl][st + q], acc);
       const float lg = log10f(fmaxf(acc, 1e-10f));
       if (f < N_FRAMES) {
         out[m * N_FRAMES + f] = lg;
@@ -155,8 +176,9 @@ __global__ void logmel_finalize_kernel(float* __restrict__ mel, const unsigned* 
 
 size_t logmel_table_floats() { return 2ull * (N_FFT / 2 + 1) * BINS_PAD; }
 
-// tables_dev: [2][201][208] f32 (hann-weighted cos / sin); uploads the mel filterbank to __constant__ memory too
-void logmel_init_tables(float* tables_dev, cudaStream_t stream) {
+// tables_dev: [2][201][208] f32 (hann-weighted cos / sin); uploads the n_mels-bin filterbank to __constant__ memory too
+void logmel_init_tables(float* tables_dev, int n_mels, cudaStream_t stream) {
+  WISB_REQUIRE(n_mels == 80 || n_mels == 128, "log-mel: n_mels must be 80 or 128");
   const int rows = N_FFT / 2 + 1;
   std::vector<float> h(2ull * rows * BINS_PAD, 0.f);
   for (int n = 0; n < rows; ++n) {
@@ -169,25 +191,31 @@ void logmel_init_tables(float* tables_dev, cudaStream_t stream) {
     }
   }
   WISB_CUDA(cudaMemcpyAsync(tables_dev, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice, stream));
-  WISB_CUDA(cudaMemcpyToSymbolAsync(c_mel_start, kMelStart, sizeof(kMelStart), 0, cudaMemcpyHostToDevice, stream));
-  WISB_CUDA(cudaMemcpyToSymbolAsync(c_mel_len, kMelLen, sizeof(kMelLen), 0, cudaMemcpyHostToDevice, stream));
-  WISB_CUDA(cudaMemcpyToSymbolAsync(c_mel_w, kMelW, sizeof(kMelW), 0, cudaMemcpyHostToDevice, stream));
+  if (n_mels == 80) {
+    WISB_CUDA(cudaMemcpyToSymbolAsync(c_mel_start, kMelStart, sizeof(kMelStart), 0, cudaMemcpyHostToDevice, stream));
+    WISB_CUDA(cudaMemcpyToSymbolAsync(c_mel_len, kMelLen, sizeof(kMelLen), 0, cudaMemcpyHostToDevice, stream));
+    WISB_CUDA(cudaMemcpyToSymbolAsync(c_mel_w, kMelW, sizeof(kMelW), 0, cudaMemcpyHostToDevice, stream));
+  } else {
+    WISB_CUDA(cudaMemcpyToSymbolAsync(c_mel128_start, kMel128Start, sizeof(kMel128Start), 0, cudaMemcpyHostToDevice, stream));
+    WISB_CUDA(cudaMemcpyToSymbolAsync(c_mel128_len, kMel128Len, sizeof(kMel128Len), 0, cudaMemcpyHostToDevice, stream));
+    WISB_CUDA(cudaMemcpyToSymbolAsync(c_mel128_w, kMel128W, sizeof(kMel128W), 0, cudaMemcpyHostToDevice, stream));
+  }
   WISB_CUDA(cudaStreamSynchronize(stream));  // h goes out of scope
 }
 
 void logmel_run(const void* pcm, int pcm_is_s16, const long long* offsets_dev, const int* n_samples_dev, int B,
-                const float* tables_dev, float* mel, unsigned* max_ws, cudaStream_t stream) {
+                int n_mels, const float* tables_dev, float* mel, unsigned* max_ws, cudaStream_t stream) {
+  WISB_REQUIRE(n_mels == 80 || n_mels == 128, "log-mel: n_mels must be 80 or 128");
   const int rows = N_FFT / 2 + 1;
   WISB_CUDA(cudaMemsetAsync(max_ws, 0, sizeof(unsigned) * B, stream));
   dim3 grid(cdiv(N_FRAMES, FT), B);
   const float* tw = tables_dev;
   const float* ts = tables_dev + static_cast<size_t>(rows) * BINS_PAD;
-  if (pcm_is_s16)
-    logmel_power_kernel<true><<<grid, LM_THREADS, 0, stream>>>(pcm, offsets_dev, n_samples_dev, tw, ts, mel, max_ws);
-  else
-    logmel_power_kernel<false><<<grid, LM_THREADS, 0, stream>>>(pcm, offsets_dev, n_samples_dev, tw, ts, mel, max_ws);
+  auto kernel = n_mels == 80 ? (pcm_is_s16 ? logmel_power_kernel<80, true> : logmel_power_kernel<80, false>)
+                             : (pcm_is_s16 ? logmel_power_kernel<128, true> : logmel_power_kernel<128, false>);
+  kernel<<<grid, LM_THREADS, 0, stream>>>(pcm, offsets_dev, n_samples_dev, tw, ts, mel, max_ws);
   WISB_CUDA(cudaGetLastError());
-  const int per_utt4 = N_MELS * N_FRAMES / 4;
+  const int per_utt4 = n_mels * N_FRAMES / 4;
   dim3 g2(cdiv(per_utt4, 256 * 4), B);
   logmel_finalize_kernel<<<g2, 256, 0, stream>>>(mel, max_ws, per_utt4);
   WISB_CUDA(cudaGetLastError());

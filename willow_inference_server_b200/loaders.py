@@ -28,7 +28,10 @@ from . import weights as W
 
 
 def dims_from_hf_config(cfg: dict, gen_cfg: dict | None = None) -> W.WhisperDims:
-    """HF ``config.json`` (+ optional ``generation_config.json``) -> WhisperDims.  [HF] configuration_whisper.py."""
+    """HF ``config.json`` (+ optional ``generation_config.json``) -> WhisperDims.  [HF] configuration_whisper.py.
+
+    Special ids start from the vocabulary's own layout (``weights.vocab_layout``: 51865 -> 99 languages, 51866 -> 100),
+    then ``generation_config.json`` overrides what it names."""
     gen_cfg = gen_cfg or {}
     if cfg.get("encoder_layers") is None or cfg.get("d_model") is None:
         raise ValueError("not a Whisper config.json (encoder_layers / d_model missing)")
@@ -56,6 +59,8 @@ def dims_from_hf_config(cfg: dict, gen_cfg: dict | None = None) -> W.WhisperDims
         dims.lang_first, dims.n_langs = ids[0], len(ids)
     if "no_timestamps_token_id" in gen_cfg:
         dims.no_timestamps = int(gen_cfg["no_timestamps_token_id"])
+    if "prev_sot_token_id" in gen_cfg:
+        dims.sot_prev = int(gen_cfg["prev_sot_token_id"])
     sup = gen_cfg.get("suppress_tokens", cfg.get("suppress_tokens"))
     if sup:
         # CTranslate2's converter stores HF suppress_tokens as config.json:suppress_ids (SURVEY 8a row A11)
@@ -266,8 +271,12 @@ def load_ct2_dir(path: str):
     d = int(emb.shape[1])
     n_layers = lambda side: 1 + max(int(k.split("/")[1][6:]) for k in variables if k.startswith(side + "/layer_") and
                                     k.split("/")[1][6:].isdigit())  # noqa: E731
+    # conv1 weight [d, n_mels, 3]: 80 bins up to large-v2, 128 for the large-v3 family (CT2's config.json has no n_mels;
+    # without the tensor the conversion below fails anyway)
+    conv1 = variables.get("encoder/conv1/weight")
     dims = W.WhisperDims(d_model=d, n_heads=d // 64, n_enc_layers=n_layers("encoder"), n_dec_layers=n_layers("decoder"),
-                         n_vocab=int(emb.shape[0]), n_text_ctx=int(variables["decoder/position_encodings/encodings"].shape[0]))
+                         n_vocab=int(emb.shape[0]), n_text_ctx=int(variables["decoder/position_encodings/encodings"].shape[0]),
+                         n_mels=int(conv1.shape[1]) if conv1 is not None else W.N_MELS)
     cfg_path = os.path.join(path, "config.json")
     if os.path.exists(cfg_path):
         cfg = json.load(open(cfg_path))

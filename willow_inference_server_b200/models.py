@@ -72,10 +72,10 @@ def get_supported_compute_types(device: str, device_index: int = 0):
     return {"float16"}
 
 
-def _features_array(features) -> np.ndarray:
+def _features_array(features, n_mels: int) -> np.ndarray:
     a = features.array if isinstance(features, StorageView) else np.asarray(features)
-    if a.dtype != np.float32 or a.ndim != 3 or tuple(a.shape[1:]) != (80, 3000):
-        raise ValueError(f"features must be float32 [n, 80, 3000], got {a.dtype} {tuple(a.shape)}")
+    if a.dtype != np.float32 or a.ndim != 3 or tuple(a.shape[1:]) != (n_mels, 3000):
+        raise ValueError(f"features must be float32 [n, {n_mels}, 3000] for this model, got {a.dtype} {tuple(a.shape)}")
     return np.ascontiguousarray(a)
 
 
@@ -134,6 +134,11 @@ class Whisper:
         return self._dims["n_langs"]
 
     @property
+    def n_mels(self) -> int:
+        """log-mel bins the model's features must have: 80, or 128 for the large-v3 family"""
+        return self._dims.get("n_mels", 80)  # (a stand-in handle that reports no bin count serves 80-bin features)
+
+    @property
     def dims(self) -> dict:
         return dict(self._dims)
 
@@ -162,7 +167,7 @@ class Whisper:
                  suppress_blank: bool = True, suppress_tokens=(-1,), sampling_topk: int = 1,
                  sampling_temperature: float = 1):
         """ctranslate2.models.Whisper.generate for the options WIS relies on (SURVEY.md section 8b defaults)."""
-        mel = _features_array(features)
+        mel = _features_array(features, self.n_mels)
         n = mel.shape[0]
         if len(prompts) != n:
             raise ValueError(f"expected {n} prompts (one per feature window), got {len(prompts)}")
@@ -208,7 +213,7 @@ class Whisper:
         return results
 
     def detect_language(self, features):
-        mel = _features_array(features)
+        mel = _features_array(features, self.n_mels)
         parts = self._split(mel.shape[0], mel)
 
         def job(i, s, e):
@@ -227,7 +232,7 @@ class Whisper:
         alignment heads' cross-attention, and each text token's probability.  The decoder is teacher-forced with
         start_sequence + [<|notimestamps|>] + text_tokens[b]; num_frames is an int or one int per window (feature frames,
         the path covers num_frames // 2 encoder frames).  Word grouping needs a tokenizer and stays with the caller."""
-        mel = _features_array(features)
+        mel = _features_array(features, self.n_mels)
         n = mel.shape[0]
         if len(text_tokens) != n:
             raise ValueError(f"expected {n} text token lists (one per feature window), got {len(text_tokens)}")

@@ -32,6 +32,7 @@ ENTRY_BYTES = 96
 ALIGN = 256
 T_ENC = 1500  # encoder positions per 30-s window
 N_MELS = 80
+MEL_BINS = (80, 128)  # log-mel bin counts the engine runs: 80 (tiny .. large-v2), 128 (the large-v3 family)
 N_FRAMES = 3000
 
 # [HF] configuration_whisper.py NON_SPEECH_TOKENS_MULTI, plus the task/sot tokens CTranslate2
@@ -44,14 +45,38 @@ NON_SPEECH_TOKENS_MULTI = [
     42863, 47425, 49870, 50254, 50258, 50358, 50359, 50360, 50361, 50362,
 ]
 
-SIZES = {  # name -> (d_model, layers, heads)   SURVEY.md section 8
-    "tiny": (384, 4, 6),
-    "base": (512, 6, 8),
-    "small": (768, 12, 12),
-    "medium": (1024, 24, 16),
-    "large-v2": (1280, 32, 20),
-    "large": (1280, 32, 20),
+SIZES = {  # name -> (d_model, encoder layers, decoder layers, heads, n_mels, n_vocab)   SURVEY.md section 8
+    "tiny": (384, 4, 4, 6, 80, 51865),
+    "base": (512, 6, 6, 8, 80, 51865),
+    "small": (768, 12, 12, 12, 80, 51865),
+    "medium": (1024, 24, 24, 16, 80, 51865),
+    "large-v2": (1280, 32, 32, 20, 80, 51865),
+    "large": (1280, 32, 32, 20, 80, 51865),
+    "large-v3": (1280, 32, 32, 20, 128, 51866),
+    "large-v3-turbo": (1280, 32, 4, 20, 128, 51866),
+    "distil-large-v3": (1280, 32, 2, 20, 128, 51866),
 }
+
+_SPECIAL_FIELDS = ("sot", "eot", "transcribe", "translate", "no_timestamps", "sot_prev", "sot_lm", "no_speech", "blank",
+                   "lang_first", "n_langs")
+
+
+def vocab_layout(n_vocab: int) -> dict:
+    """Special token ids and default suppress lists of a multilingual Whisper vocabulary.
+
+    51866 (the large-v3 family) has 100 languages (<|yue|> = 50358), which moves every special token after the languages
+    up by one from the 99-language layout of 51865 (tiny .. large-v2).  Any other size gets the 99-language layout.
+    suppress_ids are the text ids of NON_SPEECH_TOKENS_MULTI plus <|startoftranscript|> and the post-language specials
+    (translate, transcribe, startoflm, startofprev, nospeech) at their positions in this vocabulary."""
+    n_langs = 100 if n_vocab == 51866 else 99
+    sot, eot, lang_first = 50258, 50257, 50259
+    t = lang_first + n_langs  # first id after the languages
+    ids = dict(sot=sot, eot=eot, translate=t, transcribe=t + 1, sot_lm=t + 2, sot_prev=t + 3, no_speech=t + 4,
+               no_timestamps=t + 5, blank=220, lang_first=lang_first, n_langs=n_langs)
+    text = [v for v in NON_SPEECH_TOKENS_MULTI if v < eot]
+    ids["suppress_ids"] = text + [sot] + [ids[k] for k in ("translate", "transcribe", "sot_lm", "sot_prev", "no_speech")]
+    ids["suppress_ids_begin"] = [ids["blank"], eot]
+    return ids
 
 
 @dataclass
@@ -64,22 +89,30 @@ class WhisperDims:
     n_text_ctx: int = 448
     n_mels: int = N_MELS
     n_audio_ctx: int = T_ENC
-    sot: int = 50258
-    eot: int = 50257
-    transcribe: int = 50359
-    translate: int = 50358
-    no_timestamps: int = 50363
-    sot_prev: int = 50361
-    sot_lm: int = 50360
-    no_speech: int = 50362
-    blank: int = 220
-    lang_first: int = 50259  # <|en|>
-    n_langs: int = 99
-    suppress_ids: list = field(default_factory=lambda: list(NON_SPEECH_TOKENS_MULTI))
-    suppress_ids_begin: list = field(default_factory=lambda: [220, 50257])
+    # special ids and suppress lists: None = vocab_layout(n_vocab)'s (51865: transcribe 50359, no_timestamps 50363,
+    # 99 languages from <|en|> = 50259; 51866: every id after the languages one higher, 100 languages)
+    sot: int | None = None
+    eot: int | None = None
+    transcribe: int | None = None
+    translate: int | None = None
+    no_timestamps: int | None = None
+    sot_prev: int | None = None
+    sot_lm: int | None = None
+    no_speech: int | None = None
+    blank: int | None = None
+    lang_first: int | None = None
+    n_langs: int | None = None
+    suppress_ids: list | None = None
+    suppress_ids_begin: list | None = None
     # (layer, head) pairs whose cross-attention Whisper.align uses; None = the engine's default (every head of the upper
     # half of the decoder) and no blob tensor, so models without named heads serialise exactly as before
     alignment_heads: list | None = None
+
+    def __post_init__(self):
+        layout = vocab_layout(self.n_vocab)
+        for k in _SPECIAL_FIELDS + ("suppress_ids", "suppress_ids_begin"):
+            if getattr(self, k) is None:
+                setattr(self, k, layout[k])
 
     @property
     def n_vocab_pad(self) -> int:
@@ -91,14 +124,17 @@ class WhisperDims:
 
     @staticmethod
     def for_size(name: str, **kw) -> "WhisperDims":
-        d, layers, heads = SIZES[name]
-        return WhisperDims(d_model=d, n_heads=heads, n_enc_layers=layers, n_dec_layers=layers, **kw)
+        d, enc_layers, dec_layers, heads, n_mels, n_vocab = SIZES[name]
+        return WhisperDims(**{"d_model": d, "n_heads": heads, "n_enc_layers": enc_layers, "n_dec_layers": dec_layers,
+                              "n_mels": n_mels, "n_vocab": n_vocab, **kw})
 
     def validate(self):
         if self.d_model % 64 or self.d_model != 64 * self.n_heads:
             raise ValueError("engine requires head_dim == 64 (true for every Whisper size)")
-        if self.n_mels != N_MELS or self.n_audio_ctx != T_ENC:
-            raise ValueError("engine is built for 80 mels x 1500 encoder positions")
+        if self.n_mels not in MEL_BINS:
+            raise ValueError(f"engine runs 80- or 128-bin log-mel features, not n_mels = {self.n_mels}")
+        if self.n_audio_ctx != T_ENC:
+            raise ValueError("engine is built for 1500 encoder positions")
         if not (0 <= self.eot < self.n_vocab and 0 <= self.sot < self.n_vocab):
             raise ValueError("special ids outside the vocabulary")
 
