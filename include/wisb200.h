@@ -87,6 +87,17 @@ int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* pro
                      const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
                      int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score);
 
+/* Same call with the history processors of CTranslate2's Whisper.generate: repetition_penalty (finite, > 0; 1 = off)
+ * divides a positive logit and multiplies a negative one of every distinct token the hypothesis has generated so far;
+ * no_repeat_ngram_size (in [0, n_text_ctx]; 0 = off) bans every token that would complete an n-gram the hypothesis
+ * already holds.  History = the hypothesis's generated tokens (timestamp tokens included, prompt tokens not).  They
+ * apply before the suppress masks and the timestamp rules.  wisb_generate_ts is this call with (1, 0). */
+int wisb_generate_proc(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
+                       float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
+                       const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
+                       float repetition_penalty, int no_repeat_ngram_size, int32_t* out_ids, int out_stride,
+                       int32_t* out_len, float* out_score);
+
 /* (5) per utterance: language token ids sorted by probability (descending) and the probabilities.
  * lang_ids_out int32 [B, n_langs], probs_out float32 [B, n_langs]. */
 int wisb_detect_language(wisb_handle* h, const float* mel, int B, int32_t* lang_ids_out, float* probs_out);
@@ -139,7 +150,9 @@ int wisb_debug_gemm(wisb_handle* h, const int32_t* prm, int n_prm, const uint16_
 /* ONE production token-search step (wisb_generate's processors, top-k, beam bookkeeping and step advance) on caller
  * search state, which it returns.  prm[13] int32: n_utt, beam, V, ldl (>= V), eot, no_timestamps, timestamps (0/1),
  * max_initial_timestamp_index, max_new (1..448), max_hyp (>= 1), t_max (1..448), init (0: the state as given; 1 / 2:
- * search initialisation from `prompt` first, with shared_prefix 0 / 1), prompt_len.  n_utt * beam <= 1024.
+ * search initialisation from `prompt` first, with shared_prefix 0 / 1), prompt_len; n_prm == 15 adds the history
+ * processors of wisb_generate_proc: prm[13] = repetition_penalty's float32 bit pattern, prm[14] = no_repeat_ngram_size
+ * (n_prm == 13: both off).  n_utt * beam <= 1024.
  * logits float32 [n_utt*beam, ldl] (columns >= V are never read); mask uint8 [V] (bit 0: suppressed every step, bit 1:
  * at the first generated step); max_new_u int32 [n_utt] per-utterance caps in [0, max_new] or NULL; prompt int32
  * [n_utt, prompt_len] (init only).  state_i int32 in / out: DecState {pos, gen_step, n_done, all_done, ticket (0)},

@@ -40,6 +40,9 @@ _SIGS = {
     "wisb_generate_ts": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
                                    C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                    C.c_void_p, C.c_void_p]),
+    "wisb_generate_proc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
+                                     C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int,
+                                     C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_detect_language": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_align": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                              C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
@@ -202,9 +205,10 @@ class Handle:
         return out
 
     def generate(self, mel, prompts, beam_size=5, patience=1.0, length_penalty=1.0, max_length=448, extra_suppress=(),
-                 B=None, timestamps=False, max_initial_timestamp_index=50):
+                 B=None, timestamps=False, max_initial_timestamp_index=50, repetition_penalty=1.0, no_repeat_ngram_size=0):
         """-> (token ids per utterance, length-normalised scores).  timestamps=True applies Whisper's timestamp rules
-        (wisb_generate_ts); the prompt must then contain neither <|notimestamps|> nor timestamp tokens."""
+        (wisb_generate_ts); the prompt must then contain neither <|notimestamps|> nor timestamp tokens.
+        repetition_penalty != 1 or no_repeat_ngram_size > 0 switches on the history processors (wisb_generate_proc)."""
         prompts = np.ascontiguousarray(prompts, np.int32)
         if prompts.ndim != 2:
             raise ValueError("prompts must be [B, prompt_len]")
@@ -224,7 +228,13 @@ class Handle:
         lens = np.zeros(B, np.int32)
         scores = np.zeros(B, np.float32)
         extra = np.ascontiguousarray(list(extra_suppress), np.int32)
-        if timestamps or max_initial_timestamp_index != 50:
+        if repetition_penalty != 1 or no_repeat_ngram_size != 0:
+            check(lib().wisb_generate_proc(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], int(beam_size),
+                                           float(patience), float(length_penalty), int(max_length), ptr(per_utt),
+                                           ptr(extra) if extra.size else None, extra.size, 1 if timestamps else 0,
+                                           int(max_initial_timestamp_index), float(repetition_penalty),
+                                           int(no_repeat_ngram_size), ptr(ids), stride, ptr(lens), ptr(scores)))
+        elif timestamps or max_initial_timestamp_index != 50:
             check(lib().wisb_generate_ts(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], int(beam_size),
                                          float(patience), float(length_penalty), int(max_length), ptr(per_utt),
                                          ptr(extra) if extra.size else None, extra.size, 1 if timestamps else 0,
@@ -367,7 +377,8 @@ class Handle:
     _STATE_F = ("cum", "best_score")
 
     def debug_search_step(self, logits, hist, mask, *, beam: int, gen: int, eot: int, no_timestamps: int,
-                          timestamps: bool, max_initial_timestamp_index: int = 50, cum=None, done=None):
+                          timestamps: bool, max_initial_timestamp_index: int = 50, cum=None, done=None,
+                          repetition_penalty=None, no_repeat_ngram_size=None):
         """The candidates of one production search step on fresh hypotheses (max_hyp = beam, length penalty 1).
         logits float32 [n_utt*beam, V]; hist int [n_utt*beam, gen] the rows' generated tokens; mask uint8 [V] (bit 0
         every step, bit 1 at gen 0); cum [n_utt*beam] (None = 0); done [n_utt] finished utterances (None = none).
@@ -391,16 +402,21 @@ class Handle:
                 raise ValueError("every utterance is finished")
         _, ci, cs, lse = self.debug_search_step_state(logits, mask, st, beam=beam, max_hyp=beam, eot=eot,
                                                       no_timestamps=no_timestamps, timestamps=timestamps,
-                                                      max_initial_timestamp_index=max_initial_timestamp_index)
+                                                      max_initial_timestamp_index=max_initial_timestamp_index,
+                                                      repetition_penalty=repetition_penalty,
+                                                      no_repeat_ngram_size=no_repeat_ngram_size)
         return ci, cs, lse
 
     def debug_search_step_state(self, logits, mask, state, *, beam: int, max_hyp: int, eot: int, V: int = 0, no_timestamps: int = 0,
                           timestamps: bool = False, max_initial_timestamp_index: int = 50, length_penalty: float = 1.0,
-                          max_new_u=None, prompt=None, shared_prefix: int = 0):
+                          max_new_u=None, prompt=None, shared_prefix: int = 0, repetition_penalty=None,
+                          no_repeat_ngram_size=None):
         """One production search step on caller state.  logits float32 [n_utt*beam, ldl] (only columns < V are read; V
         = ldl by default); mask uint8 [V] (bit 0 every step, bit 1 at the first generated step); state as made by
         search_state (its shapes give max_new and t_max); prompt int [n_utt, prompt_len]: run the search initialisation
-        (with shared_prefix) first.  -> (new state, cand_idx int32 [n_utt, 2*beam] = beam*V + token or -1, cand_score
+        (with shared_prefix) first; repetition_penalty / no_repeat_ngram_size: the history processors (either one
+        given: the 15-parameter form, the other one off; neither: the 13-parameter form).
+        -> (new state, cand_idx int32 [n_utt, 2*beam] = beam*V + token or -1, cand_score
         float32 [n_utt, 2*beam], row_lse float32 [n_utt*beam])."""
         logits = np.ascontiguousarray(logits, np.float32)
         R, ldl = logits.shape
@@ -424,6 +440,9 @@ class Handle:
         init = 0 if pr is None else 1 + int(shared_prefix)
         prm = np.asarray([n_utt, beam, V, ldl, eot, no_timestamps, 1 if timestamps else 0, max_initial_timestamp_index,
                           max_new, max_hyp, t_max, init, 0 if pr is None else pr.shape[1]], np.int32)
+        if repetition_penalty is not None or no_repeat_ngram_size is not None:
+            rp = np.float32(1.0 if repetition_penalty is None else repetition_penalty)
+            prm = np.concatenate([prm, [rp.view(np.int32), int(no_repeat_ngram_size or 0)]]).astype(np.int32)
         ci = np.zeros((n_utt, 16), np.int32)
         cs = np.zeros((n_utt, 16), np.float32)
         lse = np.zeros(R, np.float32)

@@ -60,6 +60,9 @@ struct SearchArgs {
   int* row_pos = nullptr;         // [R] position fed by every row this step (batched pass); advanced with st->pos
   int* row_slot = nullptr;        // [R] cache slot every row writes this step's K/V to (= its own row)
   const int* max_new_u = nullptr; // optional [n_utt]: per-utterance cap on generated tokens (<= max_new)
+  // history processors on every row's generated tokens (search.cu): 1 / 0 = off
+  float rep_penalty = 1.f;        // repetition_penalty, finite and > 0
+  int no_repeat_ngram = 0;        // no_repeat_ngram_size, >= 0
 };
 void search_step_run(const SearchArgs& a, cudaStream_t stream);
 // prompt prefill: no search, just feed the next prompt token and advance the position

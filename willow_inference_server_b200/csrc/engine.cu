@@ -4,6 +4,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <functional>
 #include <map>
 #include <memory>
@@ -82,6 +83,8 @@ struct GraphKey {
   int n_utt, beam, prompt_len, max_new, max_hyp, u0, b_total, per_utt_max_new;
   int ts, ts_max_init;  // timestamp mode: the step graph bakes SearchArgs in, so a mode never reuses another's graph
   float lp;
+  float rep_penalty;    // history processors (baked in too)
+  int no_repeat_ngram;
   bool operator<(const GraphKey& o) const {
     return memcmp(this, &o, sizeof(GraphKey)) < 0;
   }
@@ -763,6 +766,8 @@ struct DecodeCfg {
   int per_utt_max_new = 0;  // h->max_new_u holds a per-utterance cap (<= max_new)
   int ts = 0;               // timestamp rules on (the prompt has no <|notimestamps|>)
   int ts_max_init = 0;      // max_initial_timestamp_index
+  float rep_penalty = 1.f;  // repetition_penalty (1 = off)
+  int no_repeat_ngram = 0;  // no_repeat_ngram_size (0 = off)
 };
 
 SearchArgs make_search_args(wisb_handle* h, const DecodeCfg& c) {
@@ -803,6 +808,8 @@ SearchArgs make_search_args(wisb_handle* h, const DecodeCfg& c) {
   a.row_pos = h->row_pos.p;
   a.row_slot = h->row_slot.p;
   a.max_new_u = c.per_utt_max_new ? h->max_new_u.p : nullptr;
+  a.rep_penalty = c.rep_penalty;
+  a.no_repeat_ngram = c.no_repeat_ngram;
   if (c.ts) {
     a.ts = 1;
     a.no_ts = dm.no_timestamps;
@@ -1300,6 +1307,7 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
       key.max_hyp = c.max_hyp; key.lp = c.lp; key.u0 = c.u0; key.b_total = c.B_total;
       key.per_utt_max_new = c.per_utt_max_new;
       key.ts = c.ts; key.ts_max_init = c.ts ? c.ts_max_init : 0;
+      key.rep_penalty = c.rep_penalty; key.no_repeat_ngram = c.no_repeat_ngram;
       auto it = h->graphs.find(key);
       if (it == h->graphs.end()) {
         if (h->graphs.size() > 64) drop_graphs(h);
@@ -1668,10 +1676,11 @@ int wisb_logmel(wisb_handle* h, const void* pcm, int pcm_dtype, int pcm_on_devic
   });
 }
 
-int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
-                     float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                     const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
-                     int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score) {
+int wisb_generate_proc(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
+                       float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
+                       const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
+                       float repetition_penalty, int no_repeat_ngram_size, int32_t* out_ids, int out_stride,
+                       int32_t* out_len, float* out_score) {
   return guarded(h, [&] {
     const Dims& dm = h->dims;
     WISB_REQUIRE(h->blob != nullptr, "handle has no model (created by wisb_create_frontend)");
@@ -1686,6 +1695,9 @@ int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* pro
       WISB_REQUIRE(prompts[i] >= 0 && prompts[i] < dm.n_vocab, "prompt token outside the vocabulary");
     WISB_REQUIRE(timestamps == 0 || timestamps == 1, "timestamps must be 0 or 1");
     WISB_REQUIRE(max_initial_timestamp_index >= 0, "max_initial_timestamp_index must be >= 0");
+    WISB_REQUIRE(std::isfinite(repetition_penalty) && repetition_penalty > 0.f, "repetition_penalty must be finite and > 0");
+    WISB_REQUIRE(no_repeat_ngram_size >= 0 && no_repeat_ngram_size <= dm.n_text_ctx,
+                 "no_repeat_ngram_size must be in [0, n_text_ctx]");
     if (timestamps) {
       WISB_REQUIRE(dm.no_timestamps > dm.eot && dm.no_timestamps + 1 < dm.n_vocab, "this vocabulary has no timestamp tokens");
       for (long long i = 0; i < static_cast<long long>(B) * prompt_len; ++i) {
@@ -1724,6 +1736,8 @@ int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* pro
     c.lp = length_penalty;
     c.ts = timestamps;
     c.ts_max_init = max_initial_timestamp_index;
+    c.rep_penalty = repetition_penalty;
+    c.no_repeat_ngram = no_repeat_ngram_size;
     // Utterances are encoded and decoded in groups that share every decoder pass: the group's rows (utterances x beams)
     // are the M dimension of the batched pass, so the decoder weights stream once per generated token for the whole
     // group.  The group size only bounds the workspaces (cross K/V: 252 MB per large-v2 utterance).
@@ -1757,6 +1771,15 @@ int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* pro
     h->timing[7] = static_cast<float>(h->launches);
     h->prof_collect();
   });
+}
+
+int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
+                     float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
+                     const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
+                     int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score) {
+  return wisb_generate_proc(h, mel, B, prompts, prompt_len, beam_size, patience, length_penalty, max_length,
+                            max_length_per_utt, extra_suppress, n_extra, timestamps, max_initial_timestamp_index, 1.f, 0,
+                            out_ids, out_stride, out_len, out_score);
 }
 
 int wisb_generate_ex(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
@@ -1942,7 +1965,7 @@ int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, float 
                            const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
                            float* state_f, int32_t* cand_idx, float* cand_score, float* row_lse) {
   return guarded(h, [&] {
-    WISB_REQUIRE(prm != nullptr && n_prm == 13 && logits && mask && state_i && state_f && cand_idx && cand_score && row_lse,
+    WISB_REQUIRE(prm != nullptr && (n_prm == 13 || n_prm == 15) && logits && mask && state_i && state_f && cand_idx && cand_score && row_lse,
                  "debug_search_step: bad arguments");
     const int n_utt = prm[0], beam = prm[1], V = prm[2], ldl = prm[3], eot = prm[4], no_ts = prm[5], ts = prm[6];
     const int max_init = prm[7], max_new = prm[8], max_hyp = prm[9], t_max = prm[10], init = prm[11], prompt_len = prm[12];
@@ -1951,6 +1974,11 @@ int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, float 
                      max_new <= T_MAX && max_hyp >= 1 && t_max >= 1 && t_max <= T_MAX && init >= 0 && init <= 2,
                  "debug_search_step: bad scalar parameters");
     WISB_REQUIRE(!ts || (no_ts > eot && no_ts + 1 < V && V - no_ts - 1 <= 2048), "debug_search_step: bad timestamp geometry");
+    float rep_penalty = 1.f;  // prm[13]: the float's bit pattern
+    const int no_repeat_ngram = n_prm == 15 ? prm[14] : 0;
+    if (n_prm == 15) memcpy(&rep_penalty, &prm[13], sizeof(float));
+    WISB_REQUIRE(std::isfinite(rep_penalty) && rep_penalty > 0.f && no_repeat_ngram >= 0 && no_repeat_ngram <= T_MAX,
+                 "debug_search_step: bad history processor arguments");
     const int R = n_utt * beam;
     // state_i: DecState (5) | flip | seq [2][R][max_new] | indir [2][R][t_max] | tokens [R] | row_pos [R] | done [n_utt] |
     // n_hyp [n_utt] | best_len [n_utt] | best_tokens [n_utt][max_new];  state_f: cum [R] | best_score [n_utt]
@@ -2054,6 +2082,8 @@ int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, float 
     a.cum = d_f.p;
     a.best_score = d_f.p + R;
     a.max_new_u = max_new_u ? d_cap.p : nullptr;
+    a.rep_penalty = rep_penalty;
+    a.no_repeat_ngram = no_repeat_ngram;
     static_assert(sizeof(DecState) == 5 * sizeof(int), "DecState is five ints");
     if (init) search_init_run(a, d_prompt.p, s, init - 1);
     search_step_run(a, s);  // the production step: processors, top-k partials, merge, bookkeeping and step advance

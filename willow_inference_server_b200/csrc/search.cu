@@ -17,6 +17,20 @@
 // timestamps above ts_max_init off; after a timestamp pair timestamps off, after a lone timestamp text (< eot) off;
 // timestamps below the last one off (at or below it unless it opened a pair); and text off in a row whose timestamp
 // log-sum-exp exceeds its best text logit.  The vocabulary is then split as 32 text chunks + one timestamp chunk.
+//
+// History processors (SearchArgs::rep_penalty != 1 or no_repeat_ngram > 0; CTranslate2's repetition_penalty and
+// no_repeat_ngram_size).  hist = the row's generated tokens seq[*flip][r][0, gen), after beam reordering: timestamp
+// tokens count, prompt tokens do not.  Pinned to transformers' RepetitionPenaltyLogitsProcessor and
+// NoRepeatNGramLogitsProcessor with input_ids = hist (tests/golden/history_processors_hf.npz); CTranslate2's own
+// implementation is UNPINNED (it probably also counts the last prompt token, from which its search starts).
+//   * repetition_penalty p: every distinct id in hist gets l < 0 ? l * p : l / p, once however often it occurs
+//   * no_repeat_ngram_size n: if gen + 1 >= n, every hist[i + n - 1] with hist[i .. i + n - 2] == hist[gen - n + 1 ..
+//     gen - 1], 0 <= i <= gen - n, is -inf (n = 1: every id in hist)
+//   * order: penalty on the raw logits, n-gram ban, the suppress masks, then the timestamp rules (rule 5 sees the
+//     penalised logits), then log-softmax and top-k as above.  Each processor is one fp32 IEEE operation, so the result
+//     is bit-exact; an id the masks turn off is -inf whatever the processors did.
+// They run in the topk_partial_kernel<NCH, true> instantiation, picked only when one is on: each (chunk, row) block
+// stages hist in shared memory and flags its chunk's ids before it reads the logits.
 #include "decoder.cuh"
 
 namespace wisb {
@@ -117,8 +131,43 @@ __device__ void block_select(unsigned long long (&keys)[PER], int n_cand, unsign
 // NCH = TOPK_CHUNKS + 1 (timestamp mode): chunks 0..31 split the text ids [0, ts_begin), chunk 32 holds the timestamps.
 constexpr int TK_THREADS = 256;
 constexpr int TK_PER = 8;  // 256 * 8 = 2048 >= ceil(51865 / 32) = 1621 and >= the 1501 timestamps
+constexpr int HIST_MAX = 448;  // generated tokens a row can hold (T_MAX): gen <= max_new - 1 < HIST_MAX
 
-template <int NCH>
+// History flags of the chunk [v0, v1) of row r (every thread of the block): pen[v - v0] = 1 for ids in hist (when the
+// penalty is on), ban[v - v0] = 1 for ids the n-gram rule bans.  Ends with a block barrier.
+__device__ void hist_flags(const SearchArgs& a, int r, int v0, int v1, int* s_hist, unsigned char* pen, unsigned char* ban) {
+  const int tid = threadIdx.x;
+  const int gen = a.st->gen_step;
+  const int* hist = a.seq[*a.flip] + static_cast<long long>(r) * a.max_new;
+  for (int t = tid; t < gen; t += TK_THREADS) s_hist[t] = hist[t];
+  for (int i = tid; i < TK_THREADS * TK_PER / 16; i += TK_THREADS) {
+    reinterpret_cast<uint4*>(pen)[i] = make_uint4(0u, 0u, 0u, 0u);
+    reinterpret_cast<uint4*>(ban)[i] = make_uint4(0u, 0u, 0u, 0u);
+  }
+  __syncthreads();
+  if (a.rep_penalty != 1.f)
+    for (int t = tid; t < gen; t += TK_THREADS) {
+      const int v = s_hist[t];
+      if (v >= v0 && v < v1) pen[v - v0] = 1;  // duplicates store the same byte: penalised once
+    }
+  const int n = a.no_repeat_ngram;
+  if (n > 0)  // (no n-gram is complete while gen < n: the loop is empty, which covers transformers' gen + 1 < n guard)
+    for (int i = tid; i <= gen - n; i += TK_THREADS) {
+      bool same = true;
+      for (int j = 0; j < n - 1 && same; ++j) same = s_hist[i + j] == s_hist[gen - n + 1 + j];
+      const int v = s_hist[i + n - 1];
+      if (same && v >= v0 && v < v1) ban[v - v0] = 1;
+    }
+  __syncthreads();
+}
+
+// the history processors on a logit that already went through the masks (a masked id stays -inf)
+__device__ __forceinline__ float hist_logit(const SearchArgs& a, float x, unsigned char pen, unsigned char ban) {
+  if (pen) x = x < 0.f ? x * a.rep_penalty : x / a.rep_penalty;
+  return ban ? -INFINITY : x;
+}
+
+template <int NCH, bool HIST>
 __global__ void __launch_bounds__(TK_THREADS) topk_partial_kernel(const SearchArgs a) {
   // Within one row the ranking by processed logit equals the ranking by score, so the per-chunk stage needs no
   // log-sum-exp: it emits the chunk's top-n_cand logits plus (max, sum exp) partials; the merge stage turns them into
@@ -145,6 +194,16 @@ __global__ void __launch_bounds__(TK_THREADS) topk_partial_kernel(const SearchAr
     v1 = a.n_vocab;
   }
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const unsigned char* pen = nullptr;
+  const unsigned char* ban = nullptr;
+  if constexpr (HIST) {
+    __shared__ int s_hist[HIST_MAX];
+    __shared__ __align__(16) unsigned char s_pen[TK_THREADS * TK_PER];
+    __shared__ __align__(16) unsigned char s_ban[TK_THREADS * TK_PER];
+    hist_flags(a, r, v0, v1, s_hist, s_pen, s_ban);
+    pen = s_pen;
+    ban = s_ban;
+  }
   TsRule rule;
   if (TS) {
     if (warp == 0) {
@@ -164,6 +223,7 @@ __global__ void __launch_bounds__(TK_THREADS) topk_partial_kernel(const SearchAr
     lg[i] = -INFINITY;
     if (v < v1) {
       lg[i] = TS ? ts_masked_logit(a, rule, row, v, first) : masked_logit(a, row, v, first);
+      if constexpr (HIST) lg[i] = hist_logit(a, lg[i], pen[v - v0], ban[v - v0]);
       if (lg[i] != -INFINITY) keys[i] = pack_key(lg[i], static_cast<unsigned>(v));
       mx = fmaxf(mx, lg[i]);
     }
@@ -470,14 +530,24 @@ void search_step_run(const SearchArgs& a, cudaStream_t stream) {
   const int R = a.n_utt * a.beam;
   WISB_REQUIRE(a.beam >= 1 && a.beam <= MAX_BEAM && a.n_cand <= MAX_CAND, "search: beam_size must be in [1, 8]");
   WISB_REQUIRE((a.n_vocab + TOPK_CHUNKS - 1) / TOPK_CHUNKS <= TK_THREADS * TK_PER, "search: vocabulary too large");
-  if (a.ts) {
+  if (a.ts)
     WISB_REQUIRE(a.ts_begin > a.eot && a.ts_begin < a.n_vocab && a.n_vocab - a.ts_begin <= TK_THREADS * TK_PER &&
                      a.ts_max_init >= a.ts_begin && a.max_new >= 1,
                  "search: bad timestamp geometry");
-    topk_partial_kernel<TOPK_CHUNKS + 1><<<dim3(TOPK_CHUNKS + 1, R), TK_THREADS, 0, stream>>>(a);
+  const bool hist = a.rep_penalty != 1.f || a.no_repeat_ngram > 0;
+  WISB_REQUIRE(!hist || (a.max_new <= HIST_MAX && a.rep_penalty > 0.f && a.no_repeat_ngram >= 0),
+               "search: bad history processor arguments");
+  if (a.ts) {
+    if (hist)
+      topk_partial_kernel<TOPK_CHUNKS + 1, true><<<dim3(TOPK_CHUNKS + 1, R), TK_THREADS, 0, stream>>>(a);
+    else
+      topk_partial_kernel<TOPK_CHUNKS + 1, false><<<dim3(TOPK_CHUNKS + 1, R), TK_THREADS, 0, stream>>>(a);
     search_tail_kernel<TOPK_CHUNKS + 1><<<a.n_utt, TK_THREADS, 0, stream>>>(a);
   } else {
-    topk_partial_kernel<TOPK_CHUNKS><<<dim3(TOPK_CHUNKS, R), TK_THREADS, 0, stream>>>(a);
+    if (hist)
+      topk_partial_kernel<TOPK_CHUNKS, true><<<dim3(TOPK_CHUNKS, R), TK_THREADS, 0, stream>>>(a);
+    else
+      topk_partial_kernel<TOPK_CHUNKS, false><<<dim3(TOPK_CHUNKS, R), TK_THREADS, 0, stream>>>(a);
     search_tail_kernel<TOPK_CHUNKS><<<a.n_utt, TK_THREADS, 0, stream>>>(a);
   }
   WISB_CUDA(cudaGetLastError());

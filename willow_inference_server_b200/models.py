@@ -176,9 +176,15 @@ class Whisper:
             raise ValueError("all prompts must be non-empty and of the same length")
         if isinstance(prompts[0][0], str):
             raise ValueError("prompts must be token ids (WIS builds them with convert_tokens_to_ids, main.py:656-663)")
-        if num_hypotheses != 1 or repetition_penalty != 1 or no_repeat_ngram_size != 0 or sampling_topk != 1:
-            raise ValueError("only num_hypotheses=1, repetition_penalty=1, no_repeat_ngram_size=0, sampling_topk=1 "
-                             "(the CTranslate2 defaults WIS uses) are implemented")
+        if num_hypotheses != 1 or sampling_topk != 1:
+            raise ValueError("only num_hypotheses=1 and sampling_topk=1 (the CTranslate2 defaults WIS uses) are implemented")
+        # history processors on each hypothesis's generated tokens (csrc/search.cu)
+        if isinstance(repetition_penalty, (bool, np.bool_)) or not isinstance(repetition_penalty, (int, float, np.number)) \
+                or not np.isfinite(repetition_penalty) or repetition_penalty <= 0:
+            raise ValueError("repetition_penalty must be a finite number > 0")
+        if isinstance(no_repeat_ngram_size, (bool, np.bool_)) or not isinstance(no_repeat_ngram_size, (int, np.integer)) \
+                or not 0 <= no_repeat_ngram_size <= self._dims.get("n_text_ctx", 448):
+            raise ValueError("no_repeat_ngram_size must be an int in [0, n_text_ctx]")
         if not suppress_blank or -1 not in suppress_tokens or asynchronous:
             raise ValueError("suppress_blank=True, suppress_tokens containing -1 and asynchronous=False are required")
         # CTranslate2's rule: a prompt without <|notimestamps|> asks for timestamps (main.py:529, :661 say "Remove this
@@ -200,10 +206,14 @@ class Whisper:
         if ml is not None and ml.shape != (n,):
             raise ValueError("max_length must be an int or one int per feature window")
 
+        proc = {}
+        if repetition_penalty != 1 or no_repeat_ngram_size != 0:
+            proc = dict(repetition_penalty=float(repetition_penalty), no_repeat_ngram_size=int(no_repeat_ngram_size))
+
         def job(i, s, e):
             return lambda: self._handles[i].generate(mel[s:e], p[s:e], beam_size, patience, length_penalty,
                                                      max_length if ml is None else ml[s:e], extra, timestamps=timestamps,
-                                                     max_initial_timestamp_index=int(max_initial_timestamp_index))
+                                                     max_initial_timestamp_index=int(max_initial_timestamp_index), **proc)
 
         outs = self._run([job(*pt) for pt in parts])
         results = []

@@ -245,7 +245,8 @@ def pack_state_dict(sd: dict, dims: WhisperDims) -> dict:
 # ---------------------------------------------------------------------------
 def synth_state_dict(dims: WhisperDims, seed: int = 0, logit_std: float = 4.0, qk_gain: float = 2.5,
                      resid_std: float = 8.0, eot_ramp: tuple | None = None, script: tuple | None = None,
-                     ts_script: tuple | None = None, align_script: tuple | None = None) -> dict:
+                     ts_script: tuple | None = None, align_script: tuple | None = None,
+                     loop_pool: int | None = None) -> dict:
     """Deterministic random Whisper weights under HF names.
 
     Every GEMM weight is rounded to float16 so oracle (fp32 math) and engine
@@ -274,6 +275,10 @@ def synth_state_dict(dims: WhisperDims, seed: int = 0, logit_std: float = 4.0, q
     text token, their log-sum-exp above it); one position later a lower timestamp at 0.9 and the window again at 0.8 (the
     non-decreasing rule decides); one more position later the next timestamps at 1.1 (the pair rule turns them off).
     The windows move up 40 indices per boundary.  ``None`` leaves the model byte-identical to one built without it.
+
+    ``loop_pool=k`` (needs ``script``) draws every position's alternatives from one seeded pool of ``k`` ordinary text
+    tokens instead of the whole text range, so that transcripts repeat tokens and n-grams the way a decode stuck in a
+    loop does (the history processors' test model).  ``None`` leaves the model byte-identical to one built without it.
 
     ``align_script=(step, gain, amp)`` gives the alignment heads (``dims.alignment_heads``, else every head of the upper
     half of the decoder) a sharp cross-attention peak at encoder frame ``step * p`` for decoder position p, so that
@@ -375,8 +380,8 @@ def synth_state_dict(dims: WhisperDims, seed: int = 0, logit_std: float = 4.0, q
     with ThreadPoolExecutor(max_workers=max(1, min(32, (_os.cpu_count() or 1)))) as ex:
         for k, a in zip(names, ex.map(lambda k: sd[k].fn(), names)):
             sd[k] = a
-    if ts_script is not None and script is None:
-        raise ValueError("ts_script scales its lifts by the text script: pass script too")
+    if (ts_script is not None or loop_pool is not None) and script is None:
+        raise ValueError("ts_script and loop_pool shape the text script: pass script too")
     if script is not None:
         n_alt, rho, off = script
         emb = sd[dd + "embed_tokens.weight"]
@@ -390,11 +395,19 @@ def synth_state_dict(dims: WhisperDims, seed: int = 0, logit_std: float = 4.0, q
         s_eff = resid_std / np.sqrt(1.0 - frac)  # residual-stream std once the scripted components are in it
         banned = set(dims.suppress_ids) | set(dims.suppress_ids_begin)
         rng = np.random.default_rng(np.random.SeedSequence(entropy=ss.entropy, spawn_key=(10 ** 6,)))
+        pool = None
+        if loop_pool is not None:
+            if int(loop_pool) < int(n_alt):
+                raise ValueError("loop_pool must hold at least n_alt tokens")
+            prng = np.random.default_rng(np.random.SeedSequence(entropy=ss.entropy, spawn_key=(10 ** 6 + 1,)))
+            cand = np.asarray([t for t in range(300, dims.eot) if t not in banned])
+            pool = [int(t) for t in prng.choice(cand, int(loop_pool), replace=False)]
         pos = sd[dd + "embed_positions.weight"].astype(np.float64)
         for p in range(dims.n_text_ctx):
             alts = []
             while len(alts) < int(n_alt):
-                t = int(rng.integers(300, dims.eot))  # ordinary text tokens only
+                # ordinary text tokens only
+                t = int(rng.integers(300, dims.eot)) if pool is None else pool[int(rng.integers(len(pool)))]
                 if t not in banned and t not in alts:
                     alts.append(t)
             for j, t in enumerate(alts):
