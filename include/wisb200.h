@@ -209,8 +209,6 @@ int wisb_debug_dec_embed_ln(wisb_handle* h, int R, int cap, int d, int n_vocab, 
 int wisb_debug_dec_pass(wisb_handle* h, const int32_t* prm, int n_prm, const int32_t* tokens, const int32_t* indir0,
                         const int32_t* indir1, const uint16_t* enc16, uint16_t* ckv_out, uint16_t* kcache, uint16_t* vcache,
                         float* x, float* logits);
-/* per-phase %globaltimer stamps of the last persistent decoder pass (option "mega_trace" = 1): n <= 2048 values */
-int wisb_debug_read_trace(wisb_handle* h, unsigned long long* out, int n);
 /* encoder output after the final LayerNorm, float32 [B,1500,d_model]; n_layers < 0 = all */
 int wisb_debug_encode(wisb_handle* h, const float* mel, int B, float* enc_out, int n_layers);
 /* The encoder one stage at a time, through the functions the encoder itself runs.  Sizes and indices are checked before

@@ -14,18 +14,18 @@ for cfg in ((128, 2, 2, 11), (256, 4, 3, 7)):
     mel = mel_inputs(6)
     toks = PROMPT + [100, 2000, 30000, 41000, 12, 50000, 7, 999]
     want = oracle.forced_logits(oracle.encode(mel[:1])[0], toks).numpy()
-    for tc in (0, 1):
-        h.set_option("mega_tc", tc)
+    for mma in (0, 1):
+        h.set_option("mega_mma", mma)
         got = h.debug_forced_logits(mel[:1], toks)
-        print("d", cfg[0], "mega_tc", tc, "logit err per position:", " ".join("%.3f" % e for e in np.abs(got - want).max(axis=1)), flush=True)
+        print("d", cfg[0], "mega_mma", mma, "logit err per position:", " ".join("%.3f" % e for e in np.abs(got - want).max(axis=1)), flush=True)
     for beam in (1, 5):
         res, robust = robust_cases(oracle, mel, [PROMPT] * 6, beam, n_probe=2)
-        for tc in (0, 1):
-            h.set_option("mega_tc", tc)
+        for mma in (0, 1):
+            h.set_option("mega_mma", mma)
             got = [h.generate(mel[i : i + 1], [PROMPT], beam_size=beam)[0][0] for i in range(6)]
             bad = [i for i in robust if got[i] != res[i].sequences_ids[0]]
-            print("d", cfg[0], "beam", beam, "mega_tc", tc, "robust", robust, "mismatches", bad, flush=True)
-    h.set_option("mega_tc", 1)
+            print("d", cfg[0], "beam", beam, "mega_mma", mma, "robust", robust, "mismatches", bad, flush=True)
+    h.set_option("mega_mma", 1)
 
 import bench  # noqa: E402
 from willow_inference_server_b200 import _lib, weights as W  # noqa: E402
@@ -38,11 +38,11 @@ pcm = bench.synth_utterance(bench.AUDIO_SAMPLES, 1234)
 mel = h.logmel(pcm, [0], [len(pcm)])
 P = np.asarray([bench.PROMPT], np.int32)
 ids = {}
-for tc in (0, 1, 0, 1):
-    h.set_option("mega_tc", tc)
+for mma in (0, 1, 0, 1):
+    h.set_option("mega_mma", mma)
     for _ in range(3):
         out, _ = h.generate(mel, P, bench.BEAM, 1.0, 1.0, bench.MAX_LENGTH, [dims.eot])
     t = h.timing()
-    ids[tc] = out[0]
-    print("large-v2 mega_tc", tc, "decode_ms %.3f" % t["decode_ms"], "generate_ms %.3f" % t["generate_ms"], "tokens", out[0][:6], flush=True)
+    ids[mma] = out[0]
+    print("large-v2 mega_mma", mma, "decode_ms %.3f" % t["decode_ms"], "generate_ms %.3f" % t["generate_ms"], "tokens", out[0][:6], flush=True)
 print("large-v2 tokens equal between the two passes:", ids[0] == ids[1])

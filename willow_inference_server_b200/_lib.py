@@ -67,7 +67,6 @@ _SIGS = {
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_dec_pass": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "wisb_debug_read_trace": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     "wisb_debug_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     "wisb_debug_enc_stem": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_debug_enc_ln": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
@@ -577,11 +576,6 @@ class Handle:
         check(lib().wisb_debug_dec_pass(self._h, ptr(prm), prm.size, ptr(tokens), ptr(ind[0]), ptr(ind[1]), ptr(enc16),
                                         ptr(ckv), ptr(kcache), ptr(vcache), ptr(x), ptr(logits)))
         return ckv
-
-    def debug_read_trace(self, n: int = 600) -> np.ndarray:
-        out = np.zeros(n, np.uint64)
-        check(lib().wisb_debug_read_trace(self._h, ptr(out), n))
-        return out
 
     def debug_encode(self, mel: np.ndarray, n_layers: int = -1) -> np.ndarray:
         mel = np.ascontiguousarray(mel, np.float32)

@@ -210,13 +210,8 @@ struct MegaArgs {
   const DecState* st = nullptr;
   float* cross_part = nullptr;   // [n_utt][H][S<=16][MAX_BEAM][68] (64 acc, m, l, pad)
   unsigned* cross_flags = nullptr;  // [n_utt * H][16] epoch-tagged 'partial written' flags, one 128-byte line each
-  unsigned* flags = nullptr;     // grid-barrier epoch flags, one 128-byte line per CTA
-  unsigned* epoch_base = nullptr;
-  int barrier_mode = 0;          // 0: per-CTA epoch flags, 1: shared counter (red.release + spin)
+  unsigned* epoch_base = nullptr;  // [mega_flags_words()]: [0] epoch the last pass ended at, [8] grid-barrier counter
   int tc = 0;                    // 1: GEMV phases on the warp-level tensor path (dec_pass_mma_kernel)
-  int dbg = 0;                   // diagnostics (timing experiments, results are garbage): bit 1 = stream a quarter of every weight unit
-  int trace_cta = 0, trace_layer = 0, trace_cap = 0;  // event trace: which CTA, which layer opens the window, events kept
-  unsigned long long* trace = nullptr;  // optional: [2*k] = time phase k starts, [2*k+1] = time CTA 0 reached barrier k
 };
 size_t mega_flags_words();
 int mega_k_chunks(int K);

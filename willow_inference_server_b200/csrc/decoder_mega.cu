@@ -1,25 +1,28 @@
-// Persistent decoder-pass kernel ("megakernel"): one cooperative launch runs a whole decoder forward pass
+// Persistent decoder-pass kernels ("megakernel"): one cooperative launch runs a whole decoder forward pass
 // (embedding, L x {LN+QKV, self-attention, out-proj, LN+cross-Q, cross-attention, out-proj, LN+fc1+GELU, fc2},
 // final LN + vocabulary projection) for <= 8 rows, instead of ~260 dependent kernel launches.
 //
 // Why: at <= 8 rows the pass is bound by streaming 1.8 GB of fp16 decoder weights (SURVEY.md section 8d), but a chain
-// of per-op kernels exposes launch + HBM latency ~260 times per pass, even with PDL.  Here
+// of per-op kernels exposes launch + HBM latency ~260 times per pass, even with PDL.  Both passes below share the plan:
 //   * one CTA per SM, every CTA owns a fixed column slice of every weight matrix;
-//   * a dedicated producer thread per CTA walks the (static) list of weight chunks of ALL phases and streams them into a
-//     2-stage shared-memory ring with cp.async.bulk (TMA, L2 evict-first) + mbarrier complete_tx -- it never waits for
-//     activations, so the HBM stream keeps running across phase boundaries.  (Two stages on purpose: with 5 stages the
-//     180 KB of bulk copies in flight per SM queued every demand load -- activation reloads, K/V rows -- behind them.)
-//   * consumer warps wait only on (a) the ring and (b) a flag-based grid barrier between phases (per-CTA epoch flags,
-//     no atomics), and read activations with L1-bypassing loads;
-//   * activations stay fp32; LayerNorm (single-pass sum / sum-of-squares statistics in fp32) is applied in registers while staging x.
-// Mapping inside a GEMV phase: thread = one 16-byte K-slice (8 elements) of the CTA's columns; it keeps x[r][8] of all
-// rows in registers and streams the CTA's <= 12 columns through them (weights from the ring), then a transposing warp
-// reduction + one shared-memory hop produce the outputs.
+//   * a dedicated producer thread per CTA walks the (static) list of weight units of ALL phases and streams them into a
+//     shared-memory ring with cp.async.bulk (TMA, L2 evict-first) + mbarrier complete_tx -- it never waits for
+//     activations, so the HBM stream keeps running across phase boundaries;
+//   * consumer warps wait only on (a) the ring and (b) a grid barrier between phases: one release-add per CTA on a
+//     shared counter, thread 0 spins on it with acquire loads.
+// Two passes:
+//   * dec_pass_mma_kernel, the default for d_model <= 1280: the GEMV phases on the warp-level tensor path (mma.sync,
+//     fp16 activation images, see the section "Warp-MMA variant" below);
+//   * dec_pass_kernel, the SIMT pass: the only pass for d_model > 1280 and the fp32 pass the warp-MMA pass is checked
+//     against.  A 2-stage ring (with 5 stages the 180 KB of bulk copies in flight per SM queued every demand load --
+//     activation reloads, K/V rows -- behind them); activations stay fp32 and are read with L1-bypassing loads;
+//     LayerNorm (single-pass sum / sum-of-squares statistics in fp32) is applied in registers while staging x.
+//     Mapping inside a GEMV phase: thread = one 16-byte K-slice (8 elements) of the CTA's columns; it keeps x[r][8] of
+//     all rows in registers and streams the CTA's <= 12 columns through them (weights from the ring), then a
+//     transposing warp reduction + one shared-memory hop produce the outputs.
 //
 // Reference semantics: decoder step of ctranslate2.models.Whisper.generate (main.py:687-692);
 // architecture [HF] modeling_whisper.py:417-508, :650-700, :966-971.
-#include <cooperative_groups.h>
-
 #include "decoder.cuh"
 #include "ptx.cuh"
 
@@ -185,8 +188,7 @@ __device__ __forceinline__ CrossGeom cross_geom(int n_utt, int H) {
   return c;
 }
 
-template <int NS = MG_NSTAGE>
-__device__ __forceinline__ void produce_cross_impl(Ring& rg, const MegaArgs& A, const MegaLayer& ly) {
+__device__ __noinline__ void produce_cross(Ring& rg, const MegaArgs& A, const MegaLayer& ly) {
   const CrossGeom cg = cross_geom(A.n_utt, A.H);
   const uint64_t pol = l2_policy_evict_first();
   for (int task = blockIdx.x; task < cg.n_tasks; task += gridDim.x) {
@@ -197,46 +199,14 @@ __device__ __forceinline__ void produce_cross_impl(Ring& rg, const MegaArgs& A, 
     const int nk = max(0, min(cg.KS, T_ENC_PAD - t0));
     const long long off = (static_cast<long long>(uh) * T_ENC_PAD + t0) * HEAD_DIM;
     for (int kv = 0; kv < 2; ++kv) {
-      const int st = rg.unit % NS;
-      mbar_wait(rg.empty(st), ((rg.unit / NS) & 1u) ^ 1u);
+      const int st = rg.unit % MG_NSTAGE;
+      mbar_wait(rg.empty(st), ((rg.unit / MG_NSTAGE) & 1u) ^ 1u);
       mbar_arrive_expect_tx(rg.full(st), static_cast<uint32_t>(nk * HEAD_DIM * 2));
       if (nk > 0)
         bulk_load_1d_hint(rg.data0 + st * MG_STAGE_BYTES, (kv == 0 ? ly.ck : ly.cv) + off,
                           static_cast<uint32_t>(nk * HEAD_DIM * 2), rg.full(st), pol);
       ++rg.unit;
     }
-  }
-}
-
-__device__ __noinline__ void produce_cross(Ring& rg, const MegaArgs& A, const MegaLayer& ly) { produce_cross_impl<MG_NSTAGE>(rg, A, ly); }
-
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
-
-// fine-grained event trace of thread 0 of ONE CTA over one layer (debug): (event id, SM clock) pairs collected in shared
-// memory -- a clock read and two shared stores per event, far cheaper than a globaltimer read plus global stores -- and
-// copied to trace[1024..] when the kernel ends.  s_tr[0] = events so far, < 0 while the window is closed.
-__device__ __forceinline__ void trace_ev(const MegaArgs& A, int ctid, int* s_tr, int id) {
-  if (A.trace != nullptr && ctid == 0) {
-    const int i = s_tr[0];
-    if (i >= 0 && i < A.trace_cap) {
-      s_tr[1 + 2 * i] = id;
-      s_tr[2 + 2 * i] = static_cast<int>(clock());
-      s_tr[0] = i + 1;
-    }
-  }
-}
-__device__ __forceinline__ void trace_open(const MegaArgs& A, int ctid, int* s_tr, int layer) {
-  if (A.trace != nullptr && ctid == 0 && static_cast<int>(blockIdx.x) == A.trace_cta && layer == A.trace_layer) s_tr[0] = 0;
-}
-__device__ __forceinline__ void trace_dump(const MegaArgs& A, int ctid, const int* s_tr) {
-  if (A.trace != nullptr && ctid == 0 && static_cast<int>(blockIdx.x) == A.trace_cta) {
-    const int n = s_tr[0] < 0 ? 0 : s_tr[0];
-    A.trace[1024] = static_cast<unsigned long long>(n);
-    for (int i = 0; i < 2 * n; ++i) A.trace[1025 + i] = static_cast<unsigned long long>(static_cast<unsigned>(s_tr[1 + i]));
   }
 }
 
@@ -249,35 +219,26 @@ __device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
   return v;
 }
 
-// Flag barrier: bar.sync orders the CTA's writes before thread 0's release store (cumulativity); every CTA publishes its
-// epoch in its own 128-byte line and thread i polls CTA i's line with acquire loads -- no atomics, no all-thread fences.
-__device__ __forceinline__ void grid_barrier(const MegaArgs& A, unsigned& epoch, int ctid, unsigned epoch0) {
-  if (A.trace != nullptr && ctid == 0) {
-    const unsigned long long t = globaltimer_ns();
-    if (blockIdx.x == 0) A.trace[2 * (epoch - epoch0) + 1] = t;
-    if (epoch - epoch0 < 264u) A.trace[2048 + blockIdx.x * 264 + (epoch - epoch0)] = t;  // arrival of every CTA at every barrier
-  }
+// Grid barrier of both passes, to be called by every consumer thread: bar.sync orders the CTA's writes before thread 0's
+// release-add on the shared counter (cumulativity), then thread 0 spins with acquire loads until the counter reaches
+// epoch * gridDim.x, i.e. every CTA has passed barrier `epoch`.  `on_open` runs in thread 0 as soon as the barrier opens,
+// before the closing sync: the warp-MMA pass issues the next phase's activation reload there.
+template <typename OnOpen>
+__device__ __forceinline__ void grid_barrier(const MegaArgs& A, unsigned& epoch, int ctid, OnOpen on_open) {
   cons_sync();
   ++epoch;
-  if (A.barrier_mode == 1) {
-    // one release-add per CTA on a shared counter, thread 0 spins on it (barrier_mode 0: the flag barrier); the counter equals epoch * gridDim.x whenever all CTAs have passed barrier `epoch`
-    if (ctid == 0) {
-      unsigned* counter = A.epoch_base + 8;
-      asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
-      const unsigned target = epoch * gridDim.x;
-      while (static_cast<int>(ld_acquire_gpu(counter) - target) < 0) {
-      }
+  if (ctid == 0) {
+    unsigned* counter = A.epoch_base + 8;
+    asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
+    const unsigned target = epoch * gridDim.x;
+    while (static_cast<int>(ld_acquire_gpu(counter) - target) < 0) {
     }
-  } else {
-    if (ctid == 0) st_release_gpu(A.flags + blockIdx.x * 32, epoch);
-    if (ctid < static_cast<int>(gridDim.x)) {
-      const unsigned* f = A.flags + ctid * 32;
-      while (static_cast<int>(ld_acquire_gpu(f) - epoch) < 0) {
-      }
-    }
+    on_open();
   }
   cons_sync();
-  if (A.trace != nullptr && blockIdx.x == 0 && ctid == 0) A.trace[2 * (epoch - epoch0)] = globaltimer_ns();
+}
+__device__ __forceinline__ void grid_barrier(const MegaArgs& A, unsigned& epoch, int ctid) {
+  grid_barrier(A, epoch, ctid, [] {});
 }
 
 // ------------------------------------------------------------------ consumer: one GEMV phase
@@ -306,8 +267,6 @@ __device__ __noinline__ void consume_gemv(Ring& rg, const MegaArgs& A, const Meg
   const int kv = (warp - part * wpp) * 32 + lane;
   const bool active = part < n_parts && kv < n_kvec;
   const bool ln = g.ln_s2 != nullptr;
-  int* s_tr = reinterpret_cast<int*>(s_stat + 912);  // [912, 1056): event trace
-  trace_ev(A, ctid, s_tr, 1);
   float* s_bias = s_stat + 16;         // [<=384] bias (LN: folded bias) of this CTA's columns
   float* s_s2 = s_stat + 400;          // [<=384] LN fold vector of this CTA's columns
   float* s_xown = s_stat + 784;        // [8][16] residual-stream columns owned by this CTA (kept across phases)
@@ -375,10 +334,8 @@ __device__ __noinline__ void consume_gemv(Ring& rg, const MegaArgs& A, const Meg
         }
       }
       // ---- weights of this unit from the ring
-      trace_ev(A, ctid, s_tr, 2);
       const int st = unit % MG_NSTAGE;
       mbar_wait(ring_full0 + 8u * st, (unit / MG_NSTAGE) & 1u);
-      trace_ev(A, ctid, s_tr, 3);
       if (active) {
         const uint32_t stage = ring_data0 + st * MG_STAGE_BYTES;  // shared-space address: ld.shared, not generic loads
         // two columns at a time, k-element outermost: 2 * NR independent FMA chains are interleaved so the 4-cycle FMA
@@ -414,7 +371,6 @@ __device__ __noinline__ void consume_gemv(Ring& rg, const MegaArgs& A, const Meg
       ++unit;
     }
     // ---- group done: reduce over the K-slices (lanes by a transposing shuffle network, warps through smem)
-    trace_ev(A, ctid, s_tr, 4);
     float* sr = s_red + (grp_idx & 1) * (NSET * MG_CONS_WARPS * 32);  // double buffered: one barrier per group
     float red[32];
 #pragma unroll
@@ -438,9 +394,7 @@ __device__ __noinline__ void consume_gemv(Ring& rg, const MegaArgs& A, const Meg
       s_lnred[warp * 32 + lane] = warp_transpose_reduce32(red, lane);
     }
     ++grp_idx;
-    trace_ev(A, ctid, s_tr, 5);
     cons_sync();
-    trace_ev(A, ctid, s_tr, 6);
     // the last two consumer warps finish the outputs (with d_model >= 1280 they hold no K-slice, so this overlaps the
     // other warps' next group; the reduction buffer is double buffered and the next cons_sync orders its reuse)
     if (ctid >= MG_CONS - 64) {
@@ -504,7 +458,7 @@ __device__ __noinline__ void consume_gemv(Ring& rg, const MegaArgs& A, const Meg
 // P.V product then runs from shared memory with lanes over the head dimension.  The step position, the ping-pong flag and
 // the warp's cache-slot table are pass constants, read once at kernel start (`pos_dec`, `flipv`, `s_slot_tab`).
 __device__ __noinline__ void consume_self_attn(const MegaArgs& A, const MegaLayer& ly, int ctid, uint8_t* s_scr,
-                                               const unsigned short* s_slot_tab, int pos_dec, int flipv, int* s_tr) {
+                                               const unsigned short* s_slot_tab, int pos_dec, int flipv) {
   const int lane = ctid & 31, warp = ctid >> 5;
   const int d = A.d, H = A.H;
   const int n_tasks = A.R * H;
@@ -514,7 +468,6 @@ __device__ __noinline__ void consume_self_attn(const MegaArgs& A, const MegaLaye
   const unsigned short* my_slots = s_slot_tab + warp * 448;
   const __half* kcache = ly.kcache;
   const __half* vcache = ly.vcache;
-  trace_ev(A, ctid, s_tr, 20);
   for (int base = blockIdx.x * MG_CONS_WARPS; base < n_tasks; base += gridDim.x * MG_CONS_WARPS) {
     const int task = base + warp;
     if (task < n_tasks) {
@@ -554,7 +507,6 @@ __device__ __noinline__ void consume_self_attn(const MegaArgs& A, const MegaLaye
           sc0 = fmaf(qb.z, f3.x, sc0); sc1 = fmaf(qb.w, f3.y, sc1);
         }
         const float sc = valid ? (sc0 + sc1) * 0.125f : -INFINITY;
-        trace_ev(A, ctid, s_tr, 21);
 #pragma unroll
         for (int i = 0; i < 8; ++i) sts128(sv + lane * 128 + ((i ^ (lane & 7)) << 4), vu[i]);
         const float mn = fmaxf(m, warp_max(sc));
@@ -566,7 +518,6 @@ __device__ __noinline__ void consume_self_attn(const MegaArgs& A, const MegaLaye
         m = mn;
         sp[lane] = p;
         __syncwarp();
-        trace_ev(A, ctid, s_tr, 22);
         const int nb = min(32, pos - t0 + 1);
 #pragma unroll 4
         for (int tt = 0; tt < nb; ++tt) {
@@ -578,10 +529,8 @@ __device__ __noinline__ void consume_self_attn(const MegaArgs& A, const MegaLaye
         }
         __syncwarp();
       }
-      trace_ev(A, ctid, s_tr, 23);
       const float inv = 1.0f / l;
       store_ctx2(A, r, h * HEAD_DIM + 2 * lane, o0 * inv, o1 * inv);
-      trace_ev(A, ctid, s_tr, 24);
     }
   }
 }
@@ -590,20 +539,13 @@ __device__ __noinline__ void consume_self_attn(const MegaArgs& A, const MegaLaye
 // 28 groups of 8 lanes walk the split's keys with an online softmax for all beams at once (K/V are read once for every
 // beam); groups are merged by shuffles (4 per warp) and shared memory into one partial (acc[64], m, l) per beam; the
 // last split of a head to arrive (atomic counter) merges the S partials into ctx.
-// kOneArrive: the ring's empty barriers count ONE arrival per stage instead of one per consumer warp
 // second half of a cross-attention task: the warps' partials (s_part: [warp][beam][64 acc, m, l]) are merged into the CTA's
 // partial for its key split, published, and split 0 of the head merges the S partials into the attention output
-template <int NB, bool kOneArrive, bool kMma>
-__device__ __forceinline__ void cross_tail(const MegaArgs& A, const CrossGeom& cg, int ctid, float* s_part, unsigned tag, int* s_tr,
-                                           uint32_t xbar, unsigned* x_count, int uh, int u, int h, int split, int beam,
-                                           uint32_t ring_empty0, int stK, int stV) {
+template <int NB, bool kMma>
+__device__ __forceinline__ void cross_tail(const MegaArgs& A, const CrossGeom& cg, int ctid, float* s_part, unsigned tag,
+                                           uint32_t xbar, unsigned* x_count, int uh, int u, int h, int split, int beam) {
   float* cross_part = A.cross_part;
-  trace_ev(A, ctid, s_tr, 14);
   cons_sync();
-  if (kOneArrive && ctid == 0) {  // every warp has left the K / V stages
-    mbar_arrive(ring_empty0 + 8u * stK);
-    mbar_arrive(ring_empty0 + 8u * stV);
-  }
   for (int idx = ctid; idx < beam * HEAD_DIM; idx += MG_CONS) {
     const int k = idx / HEAD_DIM, e = idx - k * HEAD_DIM;
     float mm = -INFINITY;
@@ -625,7 +567,6 @@ __device__ __forceinline__ void cross_tail(const MegaArgs& A, const CrossGeom& c
   // split-K fix-up without atomics or fences on the critical path: every split publishes an epoch-tagged flag (release
   // store by one thread after the CTA barrier); split 0 of the head polls the S flags (acquire) and merges the partials.
   // All other CTAs go straight on to the grid barrier.
-  trace_ev(A, ctid, s_tr, 15);
   cons_sync();
   if (ctid == 0) st_release_gpu(A.cross_flags + (uh * 16 + split) * 32, tag);
   if (split == 0) {
@@ -634,7 +575,6 @@ __device__ __forceinline__ void cross_tail(const MegaArgs& A, const CrossGeom& c
       while (ld_acquire_gpu(f) != tag) {
       }
     }
-    trace_ev(A, ctid, s_tr, 16);
     cons_sync();
     const float* pbase = cross_part + (static_cast<long long>(uh) * cg.S) * (MAX_BEAM * 68);
     // warp-MMA pass: the S partial blocks of the head are contiguous -- one bulk copy into the (now idle) merge area
@@ -685,13 +625,11 @@ __device__ __forceinline__ void cross_tail(const MegaArgs& A, const CrossGeom& c
       store_ctx2(A, u * beam + k, h * HEAD_DIM + e, ax * inv, ay * inv);
     }
   }
-  trace_ev(A, ctid, s_tr, 17);
   cons_sync();
 }
 
-template <int NB, bool kOneArrive = false, int NS = MG_NSTAGE, bool kMma = false>
-__device__ __forceinline__ void consume_cross_impl(Ring& rg, const MegaArgs& A, int ctid, float* s_part, unsigned tag, int* s_tr,
-                                                uint32_t xbar = 0, unsigned* x_count = nullptr) {
+template <int NB>
+__device__ __noinline__ void consume_cross(Ring& rg, const MegaArgs& A, int ctid, float* s_part, unsigned tag) {
   const int grp = ctid >> 3, gl = ctid & 7;
   constexpr int NGRP = MG_CONS / 8;  // 28
   const int d = A.d, beam = A.beam, H = A.H;
@@ -701,14 +639,13 @@ __device__ __forceinline__ void consume_cross_impl(Ring& rg, const MegaArgs& A, 
   unsigned unit = rg.unit;
   const unsigned gmask = 0xFFu << (ctid & 24);
   const CrossGeom cg = cross_geom(A.n_utt, H);
-  trace_ev(A, ctid, s_tr, 10);
   for (int task = blockIdx.x; task < cg.n_tasks; task += gridDim.x) {
     const int split = task % cg.S, uh = task / cg.S;
     const int u = uh / H, h = uh - u * H;
     const int t0 = split * cg.KS;
     int nk = min(cg.KS, T_ENC - t0);  // keys >= 1500 (padding rows) are never touched
     if (nk < 0) nk = 0;
-    const int stK = unit % NS, stV = (unit + 1) % NS;
+    const int stK = unit % MG_NSTAGE, stV = (unit + 1) % MG_NSTAGE;
     float qv[NB][8];
 #pragma unroll
     for (int k = 0; k < NB; ++k) {
@@ -729,11 +666,9 @@ __device__ __forceinline__ void consume_cross_impl(Ring& rg, const MegaArgs& A, 
 #pragma unroll
       for (int i = 0; i < 8; ++i) acc[k][i] = 0.f;
     }
-    trace_ev(A, ctid, s_tr, 11);
-    mbar_wait(ring_full0 + 8u * stK, (unit / NS) & 1u);
-    mbar_wait(ring_full0 + 8u * stV, ((unit + 1) / NS) & 1u);
+    mbar_wait(ring_full0 + 8u * stK, (unit / MG_NSTAGE) & 1u);
+    mbar_wait(ring_full0 + 8u * stV, ((unit + 1) / MG_NSTAGE) & 1u);
     const uint32_t sK = ring_data0 + stK * MG_STAGE_BYTES, sV = ring_data0 + stV * MG_STAGE_BYTES;
-    trace_ev(A, ctid, s_tr, 12);
 #pragma unroll 1
     for (int tl = grp; tl < nk; tl += 2 * NGRP) {
       // two keys per step with one joint running-max update: shorter dependency chains, 3 exps and 3 FMAs per pair
@@ -788,9 +723,8 @@ __device__ __forceinline__ void consume_cross_impl(Ring& rg, const MegaArgs& A, 
         m[k] = mn;
       }
     }
-    trace_ev(A, ctid, s_tr, 13);
     __syncwarp();
-    if (!kOneArrive && (ctid & 31) == 0) {
+    if ((ctid & 31) == 0) {
       mbar_arrive(ring_empty0 + 8u * stK);
       mbar_arrive(ring_empty0 + 8u * stV);
     }
@@ -823,14 +757,9 @@ __device__ __forceinline__ void consume_cross_impl(Ring& rg, const MegaArgs& A, 
         }
       }
     }
-    cross_tail<NB, kOneArrive, kMma>(A, cg, ctid, s_part, tag, s_tr, xbar, x_count, uh, u, h, split, beam, ring_empty0, stK, stV);
+    cross_tail<NB, false>(A, cg, ctid, s_part, tag, 0, nullptr, uh, u, h, split, beam);
   }
   rg.unit = unit;
-}
-
-template <int NB>
-__device__ __noinline__ void consume_cross(Ring& rg, const MegaArgs& A, int ctid, float* s_part, unsigned tag, int* s_tr) {
-  consume_cross_impl<NB, false, MG_NSTAGE, false>(rg, A, ctid, s_part, tag, s_tr);
 }
 
 template <int NR>
@@ -840,7 +769,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) dec_pass_kernel(const MegaArgs 
   uint8_t* ring_data = mg_smem;
   uint64_t* bars = reinterpret_cast<uint64_t*>(mg_smem + MG_NSTAGE * MG_STAGE_BYTES);
   float* s_red = reinterpret_cast<float*>(mg_smem + MG_NSTAGE * MG_STAGE_BYTES + 1024);
-  float* s_stat = s_red + MG_RED_FLOATS;  // 1056 floats: [0,256) unused, bias, s2, own residual columns, flags
+  float* s_stat = s_red + MG_RED_FLOATS;  // 1056 floats: [0,16) unused, bias, s2, own residual columns, [912,1056) unused
   float* s_part = s_stat + 1056;  // [warps][NB][66] for the cross-attention merge; also self-attention scratch
   unsigned short* s_slot_tab = reinterpret_cast<unsigned short*>(reinterpret_cast<uint8_t*>(s_part) + MG_SCRATCH);
   MegaLayer* s_ly = reinterpret_cast<MegaLayer*>(reinterpret_cast<uint8_t*>(s_slot_tab) + MG_SLOT_BYTES);  // [2] at 512 B
@@ -880,11 +809,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) dec_pass_kernel(const MegaArgs 
   }
   // ============================== consumers
   const int ctid = tid;
-  unsigned epoch = *A.epoch_base;  // flags hold the epoch of the previous launch
-  const unsigned epoch0 = epoch;
-  int* s_tr0 = reinterpret_cast<int*>(s_stat + 912);  // [912, 1056): event trace
-  if (ctid == 0) s_tr0[0] = -1;
-  if (A.trace != nullptr && blockIdx.x == 0 && ctid == 0) A.trace[0] = globaltimer_ns();
+  unsigned epoch = *A.epoch_base;  // the epoch the previous launch ended at
   // layer descriptors travel to shared memory one layer ahead (cp.async), so no phase starts with a global round trip
   auto prefetch_layer = [&](int l) {
     if (ctid < static_cast<int>(sizeof(MegaLayer) / 16))
@@ -916,37 +841,33 @@ __global__ void __launch_bounds__(MG_THREADS, 1) dec_pass_kernel(const MegaArgs 
       A.x[static_cast<long long>(r) * A.d + lo + c] = v;
     }
   }
-  grid_barrier(A, epoch, ctid, epoch0);
+  grid_barrier(A, epoch, ctid);
   for (int l = 0; l < L; ++l) {
     const MegaLayer& ly = *reinterpret_cast<const MegaLayer*>(reinterpret_cast<const uint8_t*>(s_ly) + (l & 1) * MG_LY_STRIDE);
     if (l + 1 < L) prefetch_layer(l + 1);  // the other buffer was last read in layer l - 1
-    trace_open(A, ctid, s_tr0, l);
     consume_gemv<NR>(rg, A, ly.qkv, &ly, ctid, s_red, s_stat);
-    grid_barrier(A, epoch, ctid, epoch0);
-    consume_self_attn(A, ly, ctid, reinterpret_cast<uint8_t*>(s_part), s_slot_tab, pos_dec, flipv, s_tr0);
-    grid_barrier(A, epoch, ctid, epoch0);
+    grid_barrier(A, epoch, ctid);
+    consume_self_attn(A, ly, ctid, reinterpret_cast<uint8_t*>(s_part), s_slot_tab, pos_dec, flipv);
+    grid_barrier(A, epoch, ctid);
     consume_gemv<NR>(rg, A, ly.o, &ly, ctid, s_red, s_stat);
-    grid_barrier(A, epoch, ctid, epoch0);
+    grid_barrier(A, epoch, ctid);
     consume_gemv<NR>(rg, A, ly.cq, &ly, ctid, s_red, s_stat);
-    grid_barrier(A, epoch, ctid, epoch0);
-    consume_cross<NR>(rg, A, ctid, s_part, epoch + 1, s_tr0);  // beam <= rows <= NR; tag = a value unique to this phase
-    grid_barrier(A, epoch, ctid, epoch0);
+    grid_barrier(A, epoch, ctid);
+    consume_cross<NR>(rg, A, ctid, s_part, epoch + 1);  // beam <= rows <= NR; tag = a value unique to this phase
+    grid_barrier(A, epoch, ctid);
     consume_gemv<NR>(rg, A, ly.co, &ly, ctid, s_red, s_stat);
-    grid_barrier(A, epoch, ctid, epoch0);
+    grid_barrier(A, epoch, ctid);
     consume_gemv<NR>(rg, A, ly.fc1, &ly, ctid, s_red, s_stat);
-    grid_barrier(A, epoch, ctid, epoch0);
+    grid_barrier(A, epoch, ctid);
     consume_gemv<NR>(rg, A, ly.fc2, &ly, ctid, s_red, s_stat);
     cp_async_wait_all();  // next layer's descriptor has landed; the barrier's CTA sync publishes it
-    grid_barrier(A, epoch, ctid, epoch0);
+    grid_barrier(A, epoch, ctid);
   }
   if (A.with_logits) consume_gemv<NR>(rg, A, A.vocab, nullptr, ctid, s_red, s_stat);
-  // publish the final epoch for the next launch (every CTA leaves the same value behind)
-  grid_barrier(A, epoch, ctid, epoch0);
-  trace_dump(A, ctid, s_tr0);
-  if (blockIdx.x == 0 && ctid == 0) {
-    *A.epoch_base = epoch;
-    A.epoch_base[8] = epoch * gridDim.x;  // keeps the counter of the atomic barrier mode in step whatever mode ran
-  }
+  // publish the final epoch for the next launch (every CTA leaves the same value behind; the barrier counter already
+  // stands at epoch * gridDim.x)
+  grid_barrier(A, epoch, ctid);
+  if (blockIdx.x == 0 && ctid == 0) *A.epoch_base = epoch;
 }
 
 
@@ -966,7 +887,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) dec_pass_kernel(const MegaArgs 
 // Activations are rounded to fp16 when they become the B operand (the encoder and the batched pass do the same).
 // =====================================================================================================================
 // shared-memory plan of the warp-MMA kernel: ring | B operand (aliased by the attention scratch) | partial tiles | barriers,
-// statistics, trace cursor, owned residual columns | cache-slot tables | layer descriptors | phase geometry
+// statistics, owned residual columns | cache-slot tables | layer descriptors | phase geometry
 constexpr int FUSED_B_OFF = 36864;  // fused cross phase: its B operand image inside s_b, above the merge area and the statistic shares
 template <int NR>
 struct MmaSmem {
@@ -978,7 +899,8 @@ struct MmaSmem {
   static constexpr int OFF_PART = OFF_B + B_ALLOC;
   static constexpr int PART_BYTES = MG_CONS_WARPS * 8 * 68 * 4;
   static constexpr int OFF_BARS = OFF_PART + PART_BYTES;
-  static constexpr int OFF_STAT = OFF_BARS + 256;            // 1056 floats, same map as the SIMT kernel's s_stat
+  // 1056 floats: [0, 16) row statistics, [16, 784) unused, [784, 912) owned residual columns, [912, 1056) unused
+  static constexpr int OFF_STAT = OFF_BARS + 256;
   static constexpr int OFF_SLOT = OFF_STAT + 4224;
   static constexpr int OFF_LY = OFF_SLOT + MG_SLOT_BYTES;
   static constexpr int OFF_GEOM = OFF_LY + MG_LY_BYTES;
@@ -1022,7 +944,7 @@ __device__ __forceinline__ MmaGeom mma_geom(int N, int K) {
 }
 
 template <int NS>
-__device__ __forceinline__ void produce_gemv_mma(Ring& rg, const MegaGemv& g, const MmaGeom* s_geom, int dbg) {
+__device__ __forceinline__ void produce_gemv_mma(Ring& rg, const MegaGemv& g, const MmaGeom* s_geom) {
   const MmaGeom mg = s_geom[g.shape];
   const int n_groups = mg.n_full + (mg.tail ? 1 : 0);
   const int kblocks = g.K / 64;
@@ -1037,8 +959,7 @@ __device__ __forceinline__ void produce_gemv_mma(Ring& rg, const MegaGemv& g, co
       const int kb0 = u * kbu, nkb = min(kbu, kblocks - kb0);
       const int st = rg.unit % NS;
       mbar_wait(rg.empty(st), ((rg.unit / NS) & 1u) ^ 1u);
-      uint32_t bytes = static_cast<uint32_t>(nkb * rows * 128);
-      if (dbg & 2) bytes = (bytes >> 2) & ~15u;  // diagnostics: a quarter of the weight traffic (results are garbage)
+      const uint32_t bytes = static_cast<uint32_t>(nkb * rows * 128);
       mbar_arrive_expect_tx(rg.full(st), bytes);
       bulk_load_1d_hint(rg.data0 + st * MG_STAGE_BYTES, base + static_cast<long long>(kb0) * rows * 64, bytes, rg.full(st), pol);
       ++rg.unit;
@@ -1127,12 +1048,11 @@ __device__ __forceinline__ void mma_unit(float (&acc)[4][4], uint32_t a_kb, uint
 // [head][row][64] exchange layout of the QKV epilogue.
 constexpr int SA_WARPS = 2;
 __device__ __forceinline__ void consume_self_attn_mma(const MegaArgs& A, const MegaLayer& ly, int ctid, uint8_t* s_scr,
-                                                   const unsigned short* s_slot_tab, int pos_dec, int flipv, int* s_tr) {
+                                                   const unsigned short* s_slot_tab, int pos_dec, int flipv) {
   const int lane = ctid & 31, warp = ctid >> 5;
   const int d = A.d, H = A.H, G = static_cast<int>(gridDim.x);
   const int n_tasks = A.R * H;
   const bool pf = A.pf_len > 0;
-  trace_ev(A, ctid, s_tr, 20);
   if (warp >= SA_WARPS) return;
   const uint32_t sK = smem_u32(s_scr) + warp * 8192, sV = sK + 4096;
   const unsigned short* my_slots = s_slot_tab + warp * 448;
@@ -1180,7 +1100,6 @@ __device__ __forceinline__ void consume_self_attn_mma(const MegaArgs& A, const M
       }
       cp_async_wait_all();
       __syncwarp();
-      trace_ev(A, ctid, s_tr, 21);
       // ---- scores: 4 tiles of 8 keys x 4 k-steps of 16 dims
       float sc[4][4];
 #pragma unroll
@@ -1242,55 +1161,24 @@ __device__ __forceinline__ void consume_self_attn_mma(const MegaArgs& A, const M
         }
       }
       __syncwarp();  // the next block's gather overwrites the rows
-      trace_ev(A, ctid, s_tr, 22);
     }
     if (gq == 0) {
       const float inv = 1.0f / l_run;
 #pragma unroll
       for (int j = 0; j < 8; ++j) store_ctx2(A, r, h * HEAD_DIM + 8 * j + 2 * tq, o[j][0] * inv, o[j][1] * inv);
     }
-    trace_ev(A, ctid, s_tr, 24);
   }
 }
 
-// grid barrier of the warp-MMA pass (shared counter: one release-add per CTA, thread 0 spins).  The thread that sees the
-// barrier open issues the NEXT phase's activation reload at once (bulk copies onto `xbar`): the copy is the first link of
-// every phase's dependency chain, so it should not wait for the CTA-wide sync, the call and the descriptor loads.
+// Activation reload of the warp-MMA pass: the thread that sees a grid barrier open issues the NEXT phase's reload at once
+// (bulk copies onto `xbar`): the copy is the first link of every phase's dependency chain, so it should not wait for the
+// CTA-wide sync, the call and the descriptor loads.
 struct Reload {
   const void* src = nullptr;   // fp16 exchange image -> s_b + dst_off
   uint32_t bytes = 0, dst_off = 0;
   const void* src2 = nullptr;  // per-CTA statistic shares -> s_b + stat_off
   uint32_t bytes2 = 0;
 };
-__device__ __forceinline__ void grid_barrier_mma(const MegaArgs& A, unsigned& epoch, int ctid, unsigned epoch0, Reload rl, uint32_t s_b_addr,
-                                              uint32_t stat_off, uint32_t xbar, int* s_tr) {
-  trace_ev(A, ctid, s_tr, 30);
-  if (A.trace != nullptr && ctid == 0) {
-    const unsigned long long t = globaltimer_ns();
-    if (blockIdx.x == 0) A.trace[2 * (epoch - epoch0) + 1] = t;
-    if (epoch - epoch0 < 264u) A.trace[2048 + blockIdx.x * 264 + (epoch - epoch0)] = t;  // arrival of every CTA at every barrier
-  }
-  cons_sync();
-  trace_ev(A, ctid, s_tr, 31);
-  ++epoch;
-  if (ctid == 0) {
-    unsigned* counter = A.epoch_base + 8;
-    asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
-    trace_ev(A, ctid, s_tr, 32);
-    const unsigned target = epoch * gridDim.x;
-    while (static_cast<int>(ld_acquire_gpu(counter) - target) < 0) {
-    }
-    trace_ev(A, ctid, s_tr, 33);
-    if (rl.bytes != 0) {
-      asm volatile("fence.proxy.async.global;" ::: "memory");  // other CTAs' generic-proxy stores (ordered by the barrier) -> async-proxy read
-      mbar_arrive_expect_tx(xbar, rl.bytes + rl.bytes2);
-      bulk_load_1d(s_b_addr + rl.dst_off, rl.src, rl.bytes, xbar);
-      if (rl.bytes2 != 0) bulk_load_1d(s_b_addr + stat_off, rl.src2, rl.bytes2, xbar);
-    }
-  }
-  cons_sync();
-  if (A.trace != nullptr && blockIdx.x == 0 && ctid == 0) A.trace[2 * (epoch - epoch0)] = globaltimer_ns();
-}
 // reload of a GEMV phase: its input image, plus the statistic shares when it carries a LayerNorm
 __device__ __forceinline__ Reload gemv_reload(const MegaArgs& A, const MegaGemv& g, const MmaGeom* s_geom) {
   Reload rl;
@@ -1308,7 +1196,7 @@ __device__ __forceinline__ Reload gemv_reload(const MegaArgs& A, const MegaGemv&
 
 template <int NR>
 __device__ __forceinline__ void consume_gemv_mma(Ring& rg, const MegaArgs& A, const MegaGemv& g_mem, const MegaLayer* ly, int ctid,
-                                             uint8_t* s_b, float* s_lnstat, float* s_mpart, float* s_xown, int* s_tr,
+                                             uint8_t* s_b, float* s_lnstat, float* s_mpart, float* s_xown,
                                              const MmaGeom* s_geom, uint32_t xbar, unsigned& x_count) {
   using SM = MmaSmem<NR>;
   constexpr int NS = SM::NS;
@@ -1322,7 +1210,6 @@ __device__ __forceinline__ void consume_gemv_mma(Ring& rg, const MegaArgs& A, co
   const int G = static_cast<int>(gridDim.x);
   // ---- activations: the fp16 exchange image IS the B operand -- one bulk copy; LayerNorm inputs bring the per-CTA shares
   //      of the row statistics along; both were issued by the thread that saw the preceding grid barrier open
-  trace_ev(A, ctid, s_tr, 1);
   // ---- everything that does not need the activations happens while they travel: epilogue operands of this thread's
   //      outputs (bias, LayerNorm fold term, next LayerNorm's gain) and the lane's fragment addresses
   constexpr int NSLOT = (NR * MM_GROUP_ROWS + MG_CONS - 1) / MG_CONS;
@@ -1354,7 +1241,6 @@ __device__ __forceinline__ void consume_gemv_mma(Ring& rg, const MegaArgs& A, co
   unsigned st = unit % NS, par = (unit / NS) & 1u;
   mbar_wait(xbar, x_count & 1u);
   ++x_count;
-  trace_ev(A, ctid, s_tr, 2);
   for (int gi = 0; gi < n_groups; ++gi) {
     const bool full = gi < mg.n_full;
     const int rows = full ? MM_GROUP_ROWS : mg.tail;
@@ -1372,7 +1258,6 @@ __device__ __forceinline__ void consume_gemv_mma(Ring& rg, const MegaArgs& A, co
       const int nkb = min(kbu, kblocks - kb0);
       // every warp waits for the unit (also the ones without a k-block in it: their arrival below must not run ahead of the ring)
       mbar_wait(rg.full(st), par);
-      if (u == 0 && gi == 0) trace_ev(A, ctid, s_tr, 3);
       const int kbi = kb_next - kb0;
       const int n_it = kbi < nkb ? (nkb - kbi + MG_CONS_WARPS - 1) / MG_CONS_WARPS : 0;
       const uint32_t a_kb = a_lane + st * MG_STAGE_BYTES + kbi * rows * 128;
@@ -1393,7 +1278,6 @@ __device__ __forceinline__ void consume_gemv_mma(Ring& rg, const MegaArgs& A, co
         par ^= 1u;
       }
     }
-    trace_ev(A, ctid, s_tr, 4);
     // ---- row statistics (first group only): quantity q = (row, sum | sum of squares) is added up over the G per-CTA
     //      shares by 16 lanes, in a fixed order
     if (gi == 0 && ln) {
@@ -1419,7 +1303,6 @@ __device__ __forceinline__ void consume_gemv_mma(Ring& rg, const MegaArgs& A, co
         p[MM_PART_LD + 8] = acc[m][3];
       }
     cons_sync();
-    trace_ev(A, ctid, s_tr, 5);
 #pragma unroll
     for (int j = 0; j < NSLOT; ++j) {
       const int idx = ctid + j * MG_CONS;
@@ -1472,7 +1355,6 @@ __device__ __forceinline__ void consume_gemv_mma(Ring& rg, const MegaArgs& A, co
     }
     if (gi + 1 < n_groups) cons_sync();  // the partial tiles are rewritten by the next group
   }
-  trace_ev(A, ctid, s_tr, 6);
   rg.unit = unit;
 }
 
@@ -1517,7 +1399,7 @@ __device__ __forceinline__ void produce_cross_fused(Ring& rg, const MegaArgs& A,
 
 template <int NB, int NS>
 __device__ __forceinline__ void consume_cross_fused(Ring& rg, const MegaArgs& A, const MegaLayer& ly, int ctid, uint8_t* s_b, float* s_mpart,
-                                                    float* s_lnstat, int* s_tr, const MmaGeom* s_geom, uint32_t xbar, unsigned& x_count,
+                                                    float* s_lnstat, const MmaGeom* s_geom, uint32_t xbar, unsigned& x_count,
                                                     unsigned tag, int stat_off) {
   float* s_part = reinterpret_cast<float*>(s_b);  // attention scratch: merge area, queries at +4096 floats
   float* s_q = s_part + 4096;
@@ -1528,7 +1410,6 @@ __device__ __forceinline__ void consume_cross_fused(Ring& rg, const MegaArgs& A,
   const int kblocks = d / 64, units = s_geom[4].units_full, kbu = s_geom[4].kbu_full;
   const uint32_t ring_data0 = rg.data0, ring_full0 = rg.full0, ring_empty0 = rg.empty0;
   unsigned unit = rg.unit;
-  trace_ev(A, ctid, s_tr, 10);
   // the LayerNorm-scaled residual rows + statistic shares (issued by the thread that saw the barrier open)
   mbar_wait(xbar, x_count & 1u);
   ++x_count;
@@ -1610,7 +1491,6 @@ __device__ __forceinline__ void consume_cross_fused(Ring& rg, const MegaArgs& A,
       }
     }
     cons_sync();
-    trace_ev(A, ctid, s_tr, 11);
     // ---- warp-MMA walk (FlashAttention-2 register layout): S = Q K^T with the utterance's <= 8 beams as the MMA's M rows
     //      (rows 8..15 are zero), 16 keys per block, 7 warps over the blocks; P stays in registers as the A operand of
     //      O += P V (V through ldmatrix.trans).  Every warp ends with (m, l, O[64]) per beam, merged in cross_tail.
@@ -1633,7 +1513,6 @@ __device__ __forceinline__ void consume_cross_fused(Ring& rg, const MegaArgs& A,
       for (int i = 0; i < 4; ++i) o[j][i] = 0.f;
     mbar_wait(ring_full0 + 8u * stK, (unit / NS) & 1u);
     mbar_wait(ring_full0 + 8u * stV, ((unit + 1) / NS) & 1u);
-    trace_ev(A, ctid, s_tr, 12);
     // (the cross K/V rows arrive chunk-swizzled by the key index -- gemm_tc.cu EPI_CROSSKV kv_swizzle -- so ldmatrix is
     //  conflict-free: lane's row inside a 16-key half, 16-byte chunk (2 kq + lane / 16) ^ (key & 7))
     const uint32_t lane_row = static_cast<uint32_t>(((lane & 7) + ((lane >> 3) & 1) * 8) * 128);
@@ -1699,7 +1578,6 @@ __device__ __forceinline__ void consume_cross_fused(Ring& rg, const MegaArgs& A,
         }
       }
     }
-    trace_ev(A, ctid, s_tr, 13);
     __syncwarp();
     if (lane == 0) {
       mbar_arrive(ring_empty0 + 8u * stK);
@@ -1715,7 +1593,7 @@ __device__ __forceinline__ void consume_cross_fused(Ring& rg, const MegaArgs& A,
         dst[65] = l_run;
       }
     }
-    cross_tail<NB, false, true>(A, cg, ctid, s_part, tag, s_tr, xbar, &x_count, uh, u, h, split, beam, ring_empty0, stK, stV);
+    cross_tail<NB, true>(A, cg, ctid, s_part, tag, xbar, &x_count, uh, u, h, split, beam);
   }
   rg.unit = unit;
 }
@@ -1736,7 +1614,6 @@ __global__ void __launch_bounds__(MG_THREADS, 1) dec_pass_mma_kernel(const MegaA
   MegaLayer* s_ly = reinterpret_cast<MegaLayer*>(mg_smem + SM::OFF_LY);
   MmaGeom* s_geom = reinterpret_cast<MmaGeom*>(mg_smem + SM::OFF_GEOM);
   float* s_xown = s_stat + 784;
-  int* s_tr = reinterpret_cast<int*>(s_stat + 16);  // [16, 784): event trace (1 + 2 x 380 words)
   Ring rg;
   rg.data = mg_smem;
   rg.data0 = smem_u32(mg_smem);
@@ -1770,13 +1647,13 @@ __global__ void __launch_bounds__(MG_THREADS, 1) dec_pass_mma_kernel(const MegaA
       //  local memory, and every acquire of the barrier invalidates the L1 -- each access after it was an L2 round trip)
       for (int l = 0; l <= L; ++l) {
         if (l == L) {
-          if (A.with_logits) produce_gemv_mma<NS>(rg, A.vocab, s_geom, A.dbg);
+          if (A.with_logits) produce_gemv_mma<NS>(rg, A.vocab, s_geom);
           break;
         }
         const MegaLayer& ly = A.layers[l];
         for (int j = 0; j < 6; ++j) {  // qkv, o, [cross-q of the task's head + cross K/V], cross-o, fc1, fc2
           if (j == 2) produce_cross_fused<NS>(rg, A, ly, s_geom);
-          else produce_gemv_mma<NS>(rg, (&ly.qkv)[j], s_geom, A.dbg);  // (index 2, the cross-query GEMV, is the fused phase's)
+          else produce_gemv_mma<NS>(rg, (&ly.qkv)[j], s_geom);  // (index 2, the cross-query GEMV, is the fused phase's)
         }
       }
     }
@@ -1785,9 +1662,6 @@ __global__ void __launch_bounds__(MG_THREADS, 1) dec_pass_mma_kernel(const MegaA
   // ============================== consumers
   const int ctid = tid;
   unsigned epoch = *A.epoch_base;
-  const unsigned epoch0 = epoch;
-  if (ctid == 0) s_tr[0] = -1;
-  if (A.trace != nullptr && blockIdx.x == 0 && ctid == 0) A.trace[0] = globaltimer_ns();
   auto prefetch_layer = [&](int l) {
     if (ctid < static_cast<int>(sizeof(MegaLayer) / 16))
       cp_async16(smem_u32(reinterpret_cast<uint8_t*>(s_ly) + (l & 1) * MG_LY_STRIDE) + ctid * 16,
@@ -1832,18 +1706,17 @@ __global__ void __launch_bounds__(MG_THREADS, 1) dec_pass_mma_kernel(const MegaA
     if (vocab_layer && !A.with_logits) break;
     const MegaLayer& ly = *reinterpret_cast<const MegaLayer*>(reinterpret_cast<const uint8_t*>(s_ly) + ((l < 0 ? 0 : l) & 1) * MG_LY_STRIDE);
     if (l >= 0 && l + 1 < L) prefetch_layer(l + 1);
-    if (l >= 0) trace_open(A, ctid, s_tr, l);
     const int n_ph = (l < 0 || vocab_layer) ? 1 : 7;
     for (int ph = 0; ph < n_ph; ++ph) {
       if (l < 0) {
         // (the embedding phase ran above; this iteration only lends its barrier)
       } else if (!vocab_layer && ph == 1) {
-        consume_self_attn_mma(A, ly, ctid, reinterpret_cast<uint8_t*>(s_part), s_slot_tab, pos_dec, flipv, s_tr);
+        consume_self_attn_mma(A, ly, ctid, reinterpret_cast<uint8_t*>(s_part), s_slot_tab, pos_dec, flipv);
       } else if (!vocab_layer && ph == 3) {
-        consume_cross_fused<NR, NS>(rg, A, ly, ctid, s_b, s_mpart, s_lnstat, s_tr, s_geom, xbar, x_count, epoch + 1, SM::STAT_OFF);
+        consume_cross_fused<NR, NS>(rg, A, ly, ctid, s_b, s_mpart, s_lnstat, s_geom, xbar, x_count, epoch + 1, SM::STAT_OFF);
       } else {
         const MegaGemv& g = vocab_layer ? A.vocab : (&ly.qkv)[ph == 0 ? 0 : (ph == 2 ? 1 : ph - 1)];
-        consume_gemv_mma<NR>(rg, A, g, &ly, ctid, s_b, s_lnstat, s_mpart, s_xown, s_tr, s_geom, xbar, x_count);
+        consume_gemv_mma<NR>(rg, A, g, &ly, ctid, s_b, s_lnstat, s_mpart, s_xown, s_geom, xbar, x_count);
       }
       Reload rl = rl_next;
       if (l >= 0) {
@@ -1864,14 +1737,17 @@ __global__ void __launch_bounds__(MG_THREADS, 1) dec_pass_mma_kernel(const MegaA
           }
         }
       }
-      grid_barrier_mma(A, epoch, ctid, epoch0, rl, sba, SM::STAT_OFF, xbar, s_tr);
+      grid_barrier(A, epoch, ctid, [=] {  // (by value: a reference to `rl` costs the kernel up to 5 registers)
+        if (rl.bytes != 0) {
+          asm volatile("fence.proxy.async.global;" ::: "memory");  // other CTAs' generic-proxy stores (ordered by the barrier) -> async-proxy read
+          mbar_arrive_expect_tx(xbar, rl.bytes + rl.bytes2);
+          bulk_load_1d(sba + rl.dst_off, rl.src, rl.bytes, xbar);
+          if (rl.bytes2 != 0) bulk_load_1d(sba + SM::STAT_OFF, rl.src2, rl.bytes2, xbar);
+        }
+      });
     }
   }
-  trace_dump(A, ctid, s_tr);
-  if (blockIdx.x == 0 && ctid == 0) {
-    *A.epoch_base = epoch;
-    A.epoch_base[8] = epoch * gridDim.x;
-  }
+  if (blockIdx.x == 0 && ctid == 0) *A.epoch_base = epoch;  // (the barrier counter already stands at epoch * gridDim.x)
 }
 
 __global__ void chunk_major_kernel(const __half* __restrict__ src, __half* __restrict__ dst, int N, int K, int n_chunks) {
@@ -1957,13 +1833,13 @@ void mega_chunk_major(const __half* src, __half* dst, int N, int K, cudaStream_t
   WISB_CUDA(cudaGetLastError());
 }
 
-size_t mega_flags_words() { return 160 * 32 + 32; }
+size_t mega_flags_words() { return 9; }
 
 void dec_pass_run(const MegaArgs& a, int num_sms, cudaStream_t stream) {
   WISB_REQUIRE(a.R >= 1 && a.R <= 8, "decoder pass: 1..8 rows");
   WISB_REQUIRE(a.d % 64 == 0 && a.d <= MG_KC_MAX, "decoder pass: d_model <= 1536");
   WISB_REQUIRE((a.d + num_sms - 1) / num_sms <= 16, "decoder pass: too few SMs for the per-CTA residual slice");
-  WISB_REQUIRE(num_sms <= 160, "decoder pass: more SMs than barrier flags");
+  WISB_REQUIRE(num_sms <= 160, "decoder pass: more than 160 SMs (the warp-MMA pass's row-statistic shares are sized for 160 CTAs)");
   static std::atomic<unsigned long long> once{0};  // per device: function attributes belong to the device's context
   once_per_device(once, [] {
     WISB_CUDA(cudaFuncSetAttribute(dec_pass_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, MG_SMEM));

@@ -142,7 +142,7 @@ struct wisb_handle {
   int search_rows = 0;  // rows the search / state buffers above are sized for
   int search_gen = 0, bd_search_gen = -1;  // reallocation count of those buffers / the one the batched-pass plans were built for
   // batched decoder pass (more than DEC_MAX_ROWS rows): workspaces for bd_rows (multiple of 128) rows, bd_tcap positions
-  int batch_rows = 320, batch_pdl = 1, decoder_batch = 1, mega_barrier = 1, cross_tc = 1, debug_chunk = 1;  // options: row capacity of one shared pass; programmatic dependent launch
+  int batch_rows = 320, batch_pdl = 1, decoder_batch = 1, cross_tc = 1, debug_chunk = 1;  // options: row capacity of one shared pass; programmatic dependent launch
   int bd_rows = 0, bd_tcap = 0, bd_launches_step = 0;
   DevBuf<float> bx, bq, bpart, blogits;
   DevBuf<__half> bxn, bctx, bh, bkc, bvc;
@@ -151,7 +151,7 @@ struct wisb_handle {
   DevBuf<MegaLayer> mega_layers;
   DevBuf<__half> mega_img;  // warp-MMA pass: decoder weights as per-CTA shared-memory images (mega_mma_image)
   int enc_pdl = 1;  // encoder: programmatic dependent launch along the whole kernel chain (227 launches per window)
-  int mega_tc = 1, mega_dbg = 0;  // mega_dbg (timing experiments only): bit 0 every layer streams layer 0's weights and cross K/V (L2 resident), bit 1 a quarter of every weight unit
+  int mega_mma = 1;  // 1: the warp-MMA persistent pass, 0: the SIMT persistent pass (option "mega_mma")
   DevBuf<unsigned> mega_flags;
   // optional reuse of the encoder output + cross K/V between consecutive calls on identical host features
   // (detect_language -> generate -> translate on one window, main.py:633-644, 514-547): option "encoder_cache"
@@ -170,8 +170,6 @@ struct wisb_handle {
   int al_A = 0;
   DevBuf<int> al_items, al_head, al_ntext, al_nframes, al_text, al_path, al_len;
   DevBuf<float> al_cap, al_mat, al_probs;
-  DevBuf<unsigned long long> mega_trace;
-  int mega_trace_on = 0, mega_trace_cta = 0, mega_trace_layer = 0;
   cudaEvent_t ev_flag[2] = {nullptr, nullptr};  // decode loop: `all_done` copies of the last two steps
   PinBuf<MegaLayer> mega_layers_host;
   PinBuf<int> pin_i;
@@ -496,7 +494,7 @@ void finish_create(wisb_handle* h) {
     }
     mega_mma_image(h->H("dec.tok_emb"), h->mega_img.p + per_layer * d.n_dec_layers, d.n_vocab, d.d_model, h->num_sms, h->stream);
   } else {
-    h->mega_tc = 0;
+    h->mega_mma = 0;
   }
   WISB_CUDA(cudaStreamSynchronize(h->stream));
 }
@@ -610,7 +608,7 @@ bool use_persistent_pass(const wisb_handle* h, int rows) {
 // cross-K/V layout the decoder pass reads: chunk-swizzled (1) for the persistent warp-MMA pass (ldmatrix without bank
 // conflicts), linear (0) for the SIMT persistent pass, the batched pass and the alignment capture
 int ckv_layout(const wisb_handle* h, bool persistent_pass) {
-  return persistent_pass && h->mega_tc ? 1 : 0;
+  return persistent_pass && h->mega_mma ? 1 : 0;
 }
 
 // Encoder stem on the plans ensure_encoder(h, B) bound: conv1 of windows [mel_first, mel_first + B) of h->mel into h1
@@ -849,9 +847,9 @@ void upload_mega_layers(wisb_handle* h, const DecodeCfg& c) {
     set(m.cq, w.cqw, fb + 7 * d, w.ln2g, fb + 6 * d, h->dx.p, h->dq.p, d, d, d, GV_STORE);
     set(m.co, w.cow, w.cob, nullptr, nullptr, h->dctx.p, h->dx.p, d, d, d, GV_RESID);
     set(m.fc1, w.fc1w, fb + 12 * d, w.ln3g, fb + 8 * d, h->dx.p, h->dh.p, 4 * d, 4 * d, d, GV_GELU);
-    const __half* fc2w = (h->fc2_chunked.p && !h->mega_tc) ? h->fc2_chunked.p + static_cast<size_t>(4) * d * d * i : w.fc2w;
+    const __half* fc2w = (h->fc2_chunked.p && !h->mega_mma) ? h->fc2_chunked.p + static_cast<size_t>(4) * d * d * i : w.fc2w;
     set(m.fc2, fc2w, w.fc2b, nullptr, nullptr, h->dh.p, h->dx.p, d, d, 4 * d, GV_RESID);
-    if (h->mega_tc) {
+    if (h->mega_mma) {
       m.o.x16 = h->dctx16.p;
       m.co.x16 = h->dctx16.p;
       m.fc1.out16 = h->dh16.p;
@@ -866,7 +864,7 @@ void upload_mega_layers(wisb_handle* h, const DecodeCfg& c) {
       m.co.next_g = w.ln3g;
       m.fc2.next_g = i + 1 < dm.n_dec_layers ? h->dec_w[i + 1].ln1g : h->F("dec.ln.g");
       const size_t dd = d;
-      const __half* img = h->mega_img.p + 14 * dd * dd * ((h->mega_dbg & 1) ? 0 : i);
+      const __half* img = h->mega_img.p + 14 * dd * dd * i;
       m.qkv.w = img;
       m.o.w = img + 3 * dd * dd;
       m.cq.w = img + 4 * dd * dd;
@@ -874,7 +872,7 @@ void upload_mega_layers(wisb_handle* h, const DecodeCfg& c) {
       m.fc1.w = img + 6 * dd * dd;
       m.fc2.w = img + 10 * dd * dd;
     }
-    bind_cross_kv(h, m, (h->mega_dbg & 1) ? 0 : i, c.u0, c.B_total);
+    bind_cross_kv(h, m, i, c.u0, c.B_total);
     m.kcache = h->kcache.p + i * layer_cache;
     m.vcache = h->vcache.p + i * layer_cache;
   }
@@ -902,10 +900,9 @@ void enqueue_decoder_forward(wisb_handle* h, const DecodeCfg& c, bool with_logit
   a.vocab.N = dm.n_vocab;
   a.vocab.K = dm.d_model;
   a.vocab.epi = GV_STORE;
-  if (h->mega_tc) {
+  if (h->mega_mma) {
     a.vocab.w = h->mega_img.p + static_cast<size_t>(14) * dm.d_model * dm.d_model * dm.n_dec_layers;
     a.tc = 1;
-    a.dbg = h->mega_dbg;
     a.ctx16 = h->dctx16.p;
     a.xn16 = h->dxn16.p;
     a.q16 = h->dq16.p;
@@ -940,16 +937,7 @@ void enqueue_decoder_forward(wisb_handle* h, const DecodeCfg& c, bool with_logit
   a.st = h->st.p;
   a.cross_part = h->cross_part.p;
   a.cross_flags = h->cross_flags.p;
-  a.flags = h->mega_flags.p;
-  a.epoch_base = h->mega_flags.p + 160 * 32;
-  a.barrier_mode = h->mega_barrier;
-  if (h->mega_trace_on) {
-    h->mega_trace.ensure(2048 + 160 * 264, true);
-    a.trace = h->mega_trace.p;
-    a.trace_cta = h->mega_trace_cta;
-    a.trace_layer = h->mega_trace_layer;
-    a.trace_cap = h->mega_tc ? 380 : 70;
-  }
+  a.epoch_base = h->mega_flags.p;
   dec_pass_run(a, h->num_sms, h->stream);
 }
 
@@ -1604,21 +1592,16 @@ int wisb_set_option(wisb_handle* h, const char* key, int value) {
       h->encoder_cache = value ? 1 : 0;
       h->enc_valid = false;
     }
-    else if (k == "mega_trace") h->mega_trace_on = value;
-    else if (k == "mega_dbg") h->mega_dbg = value;
     else if (k == "enc_pdl") h->enc_pdl = value ? 1 : 0;
-    else if (k == "mega_trace_cta") h->mega_trace_cta = value;
-    else if (k == "mega_trace_layer") h->mega_trace_layer = value;
     else if (k == "batch_rows") {
       WISB_REQUIRE(value >= 8 && value <= 1024, "batch_rows must be in [8, 1024]");
       h->batch_rows = value;
     }
     else if (k == "batch_pdl") h->batch_pdl = value ? 1 : 0;
-    else if (k == "mega_barrier") h->mega_barrier = value ? 1 : 0;
     else if (k == "debug_chunk") h->debug_chunk = value;
-    else if (k == "mega_tc" || k == "mega_mma") {  // 1: GEMV phases of the persistent pass on the warp-level tensor path, 0: the SIMT pass
+    else if (k == "mega_mma") {  // 1: GEMV phases of the persistent pass on the warp-level tensor path, 0: the SIMT pass
       WISB_REQUIRE(!value || h->mega_img.p != nullptr, "mega_mma needs d_model <= 1280 and a multiple of 64");
-      h->mega_tc = value ? 1 : 0;
+      h->mega_mma = value ? 1 : 0;
     }
     else if (k == "cross_tc") {  // 1: wgmma cross-attention in the batched pass, 0: the SIMT cluster kernel (cross-check)
       h->cross_tc = value ? 1 : 0;
@@ -2395,14 +2378,6 @@ int wisb_debug_dec_embed_ln(wisb_handle* h, int R, int cap, int d, int n_vocab, 
   });
 }
 
-int wisb_debug_read_trace(wisb_handle* h, unsigned long long* out, int n) {
-  return guarded(h, [&] {
-    WISB_REQUIRE(out != nullptr && n > 0 && n <= 2048 + 160 * 264, "trace: at most 2048 + 160 * 264 words");
-    h->mega_trace.ensure(2048 + 160 * 264, true);
-    WISB_CUDA(cudaMemcpy(out, h->mega_trace.p, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost));
-  });
-}
-
 int wisb_debug_encode(wisb_handle* h, const float* mel, int B, float* enc_out, int n_layers) {
   return guarded(h, [&] {
     WISB_REQUIRE(h->blob != nullptr && enc_out != nullptr && B >= 1, "bad arguments");
@@ -2570,8 +2545,8 @@ int wisb_debug_dec_pass(wisb_handle* h, const int32_t* prm, int n_prm, const int
     h->plan_ckv.epi.kv_swizzle = 0;
     gemm_run(h->plan_ckv, s);
     WISB_CUDA(cudaMemcpyAsync(ckv_out, h->ckv.p, ckv_elems * sizeof(__half), cudaMemcpyDeviceToHost, s));
-    const int saved_tc = h->mega_tc;
-    h->mega_tc = impl;
+    const int saved_mma = h->mega_mma;
+    h->mega_mma = impl;
     const int sw = ckv_layout(h, true);
     if (sw != 0) {
       h->plan_ckv.epi.kv_swizzle = sw;
@@ -2604,10 +2579,10 @@ int wisb_debug_dec_pass(wisb_handle* h, const int32_t* prm, int n_prm, const int
       upload_mega_layers(h, c);
       enqueue_decoder_forward(h, c, with_logits != 0, pf_len > 0);
     } catch (...) {
-      h->mega_tc = saved_tc;
+      h->mega_mma = saved_mma;
       throw;
     }
-    h->mega_tc = saved_tc;
+    h->mega_mma = saved_mma;
     WISB_CUDA(cudaMemcpyAsync(kcache, h->kcache.p, cache * sizeof(__half), cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaMemcpyAsync(vcache, h->vcache.p, cache * sizeof(__half), cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaMemcpyAsync(x, h->dx.p, xs * sizeof(float), cudaMemcpyDeviceToHost, s));
