@@ -119,6 +119,30 @@ int wisb_align(wisb_handle* h, const float* mel, int B, const int32_t* start_seq
                const int32_t* text_len, int text_stride, const int32_t* num_frames, int median_filter_width,
                int32_t* out_path, int path_stride, int32_t* out_path_len, float* out_token_probs);
 
+/* (7) encoder output as a value of its own, CTranslate2's Whisper.encode: faster-whisper encodes each window once and
+ * passes the result to detect_language, to generate (once per temperature retry) and to align.
+ * wisb_buffer_alloc: `nbytes` of device memory on `device`, owned by no handle (the library links the CUDA runtime
+ * statically, so a caller has no other way to allocate device memory it can hand back here).  wisb_buffer_free works from
+ * any current device and after every handle is destroyed; NULL is a no-op, any other pointer it did not hand out is
+ * refused (code 1). */
+int wisb_buffer_alloc(int device, size_t nbytes, void** out);
+int wisb_buffer_free(void* p);
+/* the first nbytes (<= its size) of a live wisb_buffer_alloc buffer -> host memory; blocks until the copy is done */
+int wisb_buffer_to_host(const void* p, void* host, size_t nbytes);
+/* features [B,n_mels,3000] float32 host (or NULL: the features kept by wisb_logmel) -> the encoder output after the final
+ * LayerNorm, fp16 [B, 1500, d_model], into `out`: a host pointer, or (out_on_device != 0) device memory on the handle's
+ * device.  Encodes in groups of at most option batch_rows / 5 windows (generate's group at beam 5), so it sizes no
+ * workspace beyond what generate would.  Invalidates the cached encoder output.  Stage timings: [1 h2d, 2 encoder,
+ * 5 total, 7 kernel launches] and, with option "profile", 8-12 as for generate. */
+int wisb_encode(wisb_handle* h, const float* mel, int B, void* out, int out_on_device);
+/* An encoder output [B, 1500, d_model] (dtype 0 fp16, 1 fp32: converted on the device, rounded to nearest even), host
+ * memory or (on_device != 0) device memory on the handle's device, copied into a handle-owned buffer.  It becomes the
+ * source of the next wisb_generate* / wisb_detect_language / wisb_align calls that pass mel == NULL: whichever of
+ * wisb_logmel(keep_on_device) and this call came last decides that source, and such a call with another B fails with
+ * code 1.  Those calls skip the encoder and run only the cross-K/V GEMM on these rows; they leave nothing for option
+ * "encoder_cache" to reuse.  A host copy's time is reported in timing slot 1 (h2d). */
+int wisb_load_encoder_output(wisb_handle* h, const void* enc, int B, int dtype, int on_device);
+
 /* stage timings (ms, CUDA events on the launching stream) of the last wisb_logmel / wisb_generate:
  * [0 logmel, 1 h2d, 2 encoder, 3 cross_kv, 4 decode, 5 total_generate, 6 decode_steps, 7 kernel_launches,
  *  8 sum of GEMM kernels, 9 attention kernels, 10 LayerNorm kernels, 11 conv1, 12 number of GEMM launches, 13-15 0]

@@ -44,6 +44,11 @@ _SIGS = {
                                      C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int,
                                      C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_detect_language": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "wisb_buffer_alloc": (C.c_int, [C.c_int, C.c_size_t, C.POINTER(C.c_void_p)]),
+    "wisb_buffer_free": (C.c_int, [C.c_void_p]),
+    "wisb_buffer_to_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "wisb_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
+    "wisb_load_encoder_output": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]),
     "wisb_align": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                              C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_debug_align_capture": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
@@ -254,6 +259,45 @@ class Handle:
         probs = np.zeros((B, nl), np.float32)
         check(lib().wisb_detect_language(self._h, ptr(mel), B, ptr(ids), ptr(probs)))
         return ids, probs
+
+    def encode(self, mel, out=None, on_device=False):
+        """wisb_encode: features float32 [B, n_mels, 3000] (None: the features logmel kept, B = out's first dimension)
+        -> encoder output float16 [B, 1500, d_model].  out: a C-contiguous float16 host array of that shape (None: a new
+        one), or with on_device=True a device address (int) on this handle's GPU holding that many bytes."""
+        if mel is not None:
+            self._check_features(mel)
+        d = self.dims()["d_model"]
+        if on_device:
+            if mel is None:
+                raise ValueError("a device `out` needs the features (mel), which give the batch size")
+            check(lib().wisb_encode(self._h, ptr(mel), mel.shape[0], C.c_void_p(int(out)), 1))
+            return out
+        if out is None:
+            if mel is None:
+                raise ValueError("encode(None) needs `out`, whose first dimension is the batch size")
+            out = np.empty((mel.shape[0], 1500, d), np.float16)
+        if not isinstance(out, np.ndarray) or out.dtype != np.float16 or out.ndim != 3 or out.shape[1:] != (1500, d) \
+                or not out.flags["C_CONTIGUOUS"] or (mel is not None and out.shape[0] != mel.shape[0]):
+            raise ValueError(f"out must be a C-contiguous float16 array [B, 1500, {d}]")
+        check(lib().wisb_encode(self._h, ptr(mel), out.shape[0], ptr(out), 0))
+        return out
+
+    def load_encoder_output(self, enc, on_device=False, B=None, dtype=np.float16):
+        """wisb_load_encoder_output: enc float16 or float32 [B, 1500, d_model], a host array, or with on_device=True a
+        device address (int) on this handle's GPU (then B and dtype say what it holds).  Calls with mel=None, B=B then
+        decode it."""
+        d = self.dims()["d_model"]
+        if on_device:
+            dt = np.dtype(dtype)
+            p = C.c_void_p(int(enc))
+        else:
+            enc = np.asarray(enc)
+            if enc.ndim != 3 or enc.shape[1:] != (1500, d) or not enc.flags["C_CONTIGUOUS"]:
+                raise ValueError(f"the encoder output must be a C-contiguous array [B, 1500, {d}]")
+            dt, B, p = enc.dtype, enc.shape[0], ptr(enc)
+        if dt not in (np.float16, np.float32):
+            raise ValueError("the encoder output must be float16 or float32")
+        check(lib().wisb_load_encoder_output(self._h, p, int(B), 0 if dt == np.float16 else 1, 1 if on_device else 0))
 
     def align(self, mel, start_sequence, text_tokens, num_frames, median_filter_width=7, B=None):
         """wisb_align -> (paths: list of int32 [len, 2] arrays of (text index, frame), token probs: list of float lists).
@@ -641,6 +685,25 @@ class Handle:
         out = np.zeros((tokens.shape[0], self.dims()["n_vocab"]), np.float32)
         check(lib().wisb_debug_forced_logits(self._h, ptr(mel), ptr(tokens), tokens.shape[0], ptr(out)))
         return out
+
+
+def buffer_alloc(device: int, nbytes: int) -> int:
+    """wisb_buffer_alloc: `nbytes` of device memory on GPU `device`, owned by no handle -> its address"""
+    p = C.c_void_p()
+    check(lib().wisb_buffer_alloc(int(device), int(nbytes), C.byref(p)))
+    return p.value
+
+
+def buffer_free(addr: int):
+    check(lib().wisb_buffer_free(C.c_void_p(addr)))
+
+
+def buffer_to_host(addr: int, out: np.ndarray):
+    """the first out.nbytes bytes of buffer `addr` -> out (a C-contiguous host array)"""
+    if not out.flags["C_CONTIGUOUS"]:
+        raise ValueError("out must be C-contiguous")
+    check(lib().wisb_buffer_to_host(C.c_void_p(addr), ptr(out), out.nbytes))
+    return out
 
 
 def flac_decode(data: bytes):

@@ -3,6 +3,7 @@
 // Replaces (reference side) the encoder half of ctranslate2.models.Whisper.generate
 // (main.py:687-692 of the reference server; SURVEY.md section 2b rows K2, K4, K6).  Architecture per
 // [HF] modeling_whisper.py:567-568,619-625 (conv stem), :361-415 (encoder layer).
+#include <algorithm>
 #include <mutex>
 
 #include "kernels.h"
@@ -397,6 +398,18 @@ void enc_attn_run(const AttnPlan& p, cudaStream_t stream) {
 void enc_attn_ref_run(const __half* qkv, __half* ctx, int B, int d, int H, cudaStream_t stream) {
   dim3 grid(T_ENC_PAD / 128, H, B);
   enc_attn_ref_kernel<<<grid, 128, 0, stream>>>(qkv, ctx, d);
+  WISB_CUDA(cudaGetLastError());
+}
+
+// float32 encoder output handed to wisb_load_encoder_output -> fp16, each element rounded to nearest even
+__global__ void __launch_bounds__(256) f32_to_f16_kernel(const float* __restrict__ x, __half* __restrict__ y, size_t n) {
+  for (size_t i = blockIdx.x * 256ull + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * 256)
+    y[i] = __float2half_rn(x[i]);
+}
+
+void f32_to_f16_run(const float* x, __half* y, size_t n, cudaStream_t stream) {
+  const int grid = static_cast<int>(std::min<size_t>((n + 255) / 256, 8192));
+  f32_to_f16_kernel<<<grid, 256, 0, stream>>>(x, y, n);
   WISB_CUDA(cudaGetLastError());
 }
 

@@ -118,6 +118,10 @@ struct wisb_handle {
   DevBuf<int> pcm_n;
   DevBuf<float> mel;  // [B,n_mels,3000]
   int mel_B = 0;      // utterances currently held in `mel`
+  // encoder output of enc_in_B windows from wisb_load_encoder_output, fp16 [enc_in_B, 1500, d].  While enc_in_B > 0 it,
+  // not the features wisb_logmel kept, is what a call with mel == NULL decodes.
+  DevBuf<__half> enc_in;
+  int enc_in_B = 0;
   // encoder workspaces (capacity enc_cap utterances)
   int enc_cap = 0;
   DevBuf<__half> h1, xn, qkv, vt, ctx, hbuf, enc_out, ckv;
@@ -711,16 +715,46 @@ bool upload_mel(wisb_handle* h, const float* mel, int B) {
   return false;
 }
 
+// True when a call with these arguments decodes the encoder output wisb_load_encoder_output loaded: mel == NULL after
+// that call rather than after wisb_logmel(keep_on_device).  The call must then have the loaded batch size.
+bool loaded_source(const wisb_handle* h, const float* mel, int B) {
+  if (mel != nullptr || h->enc_in_B == 0) return false;
+  WISB_REQUIRE(h->enc_in_B == B, "mel == NULL but wisb_load_encoder_output loaded an encoder output of another batch size");
+  return true;
+}
+
+// `p` must be device memory on the handle's device (wisb_encode's out, wisb_load_encoder_output's enc)
+void require_on_device(const wisb_handle* h, const void* p, const char* what) {
+  cudaPointerAttributes a{};
+  WISB_CUDA(cudaPointerGetAttributes(&a, p));
+  WISB_REQUIRE(a.type == cudaMemoryTypeDevice && a.device == h->device,
+               std::string(what) + " is not device memory on the handle's device");
+}
+
 // Encoder stage of a call on the B windows placed by upload_mel: leaves the encoder output and the cross K/V of windows
 // [g0, g0 + n) in HBM, the cross K/V in layout `ckv_sw` (ckv_layout).  What is already there is reused only when
 // upload_mel reported a hit (`cached`) and this group is the whole call (the cache holds a batch of B windows); cached
-// cross K/V in the other layout is rewritten by the cross-K/V GEMM alone.  Records the stage events ev[2] (start), ev[3]
-// (encoder done) and ev[4] (cross K/V done).
-void encode_stage(wisb_handle* h, bool cached, int B, int g0, int n, int ckv_sw) {
+// cross K/V in the other layout is rewritten by the cross-K/V GEMM alone.  With `loaded` (loaded_source) the group's rows
+// of the loaded encoder output take the encoder's place.  Records the stage events ev[2] (start), ev[3] (encoder done)
+// and ev[4] (cross K/V done).
+void encode_stage(wisb_handle* h, bool cached, bool loaded, int B, int g0, int n, int ckv_sw) {
   cudaStream_t s = h->stream;
   const bool reuse = cached && n == B;
   WISB_CUDA(cudaEventRecord(h->ev[2], s));
-  if (!reuse) run_encoder(h, n, -1, g0);
+  if (loaded) {
+    // rows [g0, g0 + n) into enc_out's padded layout; padding rows 1500..1535 are zero (the cross-attention masks keys
+    // >= 1500, so they never reach a result).  These rows belong to no features: the encoder cache must not claim them.
+    ensure_encoder(h, n);
+    h->enc_valid = false;
+    h->mel_cache_B = 0;
+    const size_t row = static_cast<size_t>(h->dims.d_model) * sizeof(__half);
+    WISB_CUDA(cudaMemcpy2DAsync(h->enc_out.p, T_ENC_PAD * row, h->enc_in.p + static_cast<size_t>(g0) * T_ENC * h->dims.d_model,
+                                T_ENC * row, T_ENC * row, n, cudaMemcpyDeviceToDevice, s));
+    WISB_CUDA(cudaMemset2DAsync(reinterpret_cast<char*>(h->enc_out.p) + T_ENC * row, T_ENC_PAD * row, 0,
+                                (T_ENC_PAD - T_ENC) * row, n, s));
+  } else if (!reuse) {
+    run_encoder(h, n, -1, g0);
+  }
   WISB_CUDA(cudaEventRecord(h->ev[3], s));
   if (!reuse || h->ckv_is_sw != ckv_sw) {
     ensure_encoder(h, n);
@@ -1420,6 +1454,29 @@ void align_group(wisb_handle* h, int g0, int n, const int32_t* start_seq, int S,
     if (nt[u] == 0) out_path_len[g0 + u] = 0;
 }
 
+// entry points without a handle (wisb_buffer_*): the error handling of guarded
+template <typename Fn>
+int guarded_nohandle(Fn&& fn) {
+  try {
+    fn();
+    return 0;
+  } catch (const Error& e) {
+    g_last_error = e.what();
+    return e.code;
+  } catch (const std::exception& e) {
+    g_last_error = e.what();
+    return 2;
+  }
+}
+
+// device and size of every live wisb_buffer_alloc allocation (never destroyed: a buffer may be freed during process
+// teardown)
+std::mutex g_buffer_mu;
+std::map<const void*, std::pair<int, size_t>>& buffer_devices() {
+  static auto* m = new std::map<const void*, std::pair<int, size_t>>;
+  return *m;
+}
+
 template <typename Fn>
 int guarded(wisb_handle* h, Fn&& fn) {
   try {
@@ -1654,6 +1711,7 @@ int wisb_logmel(wisb_handle* h, const void* pcm, int pcm_dtype, int pcm_on_devic
     WISB_CUDA(cudaStreamSynchronize(s));
     WISB_CUDA(cudaEventElapsedTime(&h->timing[0], h->ev[0], h->ev[1]));
     h->mel_B = keep_on_device ? B : 0;
+    if (keep_on_device) h->enc_in_B = 0;  // kept features are now the source of calls with mel == NULL
     h->enc_valid = false;  // the device feature buffer was rewritten
     h->mel_cache_B = 0;
   });
@@ -1708,7 +1766,8 @@ int wisb_generate_proc(wisb_handle* h, const float* mel, int B, const int32_t* p
     h->launches = 0;
     for (int i = 1; i <= 5; ++i) h->timing[i] = 0.f;
     WISB_CUDA(cudaEventRecord(h->ev[0], s));
-    const bool cached = upload_mel(h, mel, B);
+    const bool loaded = loaded_source(h, mel, B);
+    const bool cached = !loaded && upload_mel(h, mel, B);
     set_extra_suppress(h, extra_suppress, n_extra);
     time_h2d(h);
     DecodeCfg c;
@@ -1730,7 +1789,7 @@ int wisb_generate_proc(wisb_handle* h, const float* mel, int B, const int32_t* p
     int steps = 0;
     for (int g0 = 0; g0 < B; g0 += group) {
       const int n = B - g0 < group ? B - g0 : group;
-      encode_stage(h, cached, B, g0, n, ckv_layout(h, persistent));
+      encode_stage(h, cached, loaded, B, g0, n, ckv_layout(h, persistent));
       c.u0 = 0;
       c.n_utt = n;
       c.B_total = n;
@@ -1787,8 +1846,9 @@ int wisb_detect_language(wisb_handle* h, const float* mel, int B, int32_t* lang_
     WISB_REQUIRE(B >= 1 && B <= 4096, "B out of range");
     WISB_REQUIRE(lang_ids_out != nullptr && probs_out != nullptr, "output pointer is NULL");
     cudaStream_t s = h->stream;
-    const bool cached = upload_mel(h, mel, B);
-    encode_stage(h, cached, B, 0, B, ckv_layout(h, true));  // language detection always runs the persistent pass
+    const bool loaded = loaded_source(h, mel, B);
+    const bool cached = !loaded && upload_mel(h, mel, B);
+    encode_stage(h, cached, loaded, B, 0, B, ckv_layout(h, true));  // language detection always runs the persistent pass
     const int nl = dm.n_langs;
     h->lang_ids.ensure(nl);
     std::vector<int> ids(nl);
@@ -1822,6 +1882,117 @@ int wisb_detect_language(wisb_handle* h, const float* mel, int B, int32_t* lang_
         }
       }
     }
+  });
+}
+
+int wisb_buffer_alloc(int device, size_t nbytes, void** out) {
+  return guarded_nohandle([&] {
+    WISB_REQUIRE(out != nullptr, "out is NULL");
+    *out = nullptr;
+    WISB_REQUIRE(nbytes > 0, "nbytes must be > 0");
+    WISB_CUDA(cudaSetDevice(device));
+    void* p = nullptr;
+    WISB_CUDA(cudaMalloc(&p, nbytes));
+    std::lock_guard<std::mutex> lock(g_buffer_mu);
+    buffer_devices()[p] = {device, nbytes};
+    *out = p;
+  });
+}
+
+int wisb_buffer_free(void* p) {
+  return guarded_nohandle([&] {
+    if (p == nullptr) return;
+    int device;
+    {
+      std::lock_guard<std::mutex> lock(g_buffer_mu);
+      auto it = buffer_devices().find(p);
+      WISB_REQUIRE(it != buffer_devices().end(), "wisb_buffer_free: not a live wisb_buffer_alloc allocation");
+      device = it->second.first;
+      buffer_devices().erase(it);
+    }
+    WISB_CUDA(cudaSetDevice(device));
+    WISB_CUDA(cudaFree(p));
+  });
+}
+
+int wisb_buffer_to_host(const void* p, void* host, size_t nbytes) {
+  return guarded_nohandle([&] {
+    WISB_REQUIRE(host != nullptr || nbytes == 0, "host is NULL");
+    int device;
+    {
+      std::lock_guard<std::mutex> lock(g_buffer_mu);
+      auto it = buffer_devices().find(p);
+      WISB_REQUIRE(it != buffer_devices().end(), "wisb_buffer_to_host: not a live wisb_buffer_alloc allocation");
+      WISB_REQUIRE(nbytes <= it->second.second, "wisb_buffer_to_host: nbytes exceeds the buffer");
+      device = it->second.first;
+    }
+    WISB_CUDA(cudaSetDevice(device));
+    if (nbytes) WISB_CUDA(cudaMemcpy(host, p, nbytes, cudaMemcpyDeviceToHost));
+  });
+}
+
+int wisb_encode(wisb_handle* h, const float* mel, int B, void* out, int out_on_device) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(h->blob != nullptr, "handle has no model (created by wisb_create_frontend)");
+    WISB_REQUIRE(B >= 1 && B <= 4096, "B out of range");
+    WISB_REQUIRE(out != nullptr, "out is NULL");
+    if (out_on_device) require_on_device(h, out, "out");
+    cudaStream_t s = h->stream;
+    const size_t row = static_cast<size_t>(h->dims.d_model) * sizeof(__half);
+    h->launches = 0;
+    for (int i = 1; i <= 5; ++i) h->timing[i] = 0.f;
+    WISB_CUDA(cudaEventRecord(h->ev[0], s));
+    upload_mel(h, mel, B);
+    h->mel_cache_B = 0;  // enc_out is about to hold rows the encoder cache knows nothing of
+    time_h2d(h);
+    // generate's group at beam 5, so that encoding sizes no workspace beyond what generate would
+    const int group = std::max(1, h->batch_rows / 5);
+    for (int g0 = 0; g0 < B; g0 += group) {
+      const int n = std::min(group, B - g0);
+      WISB_CUDA(cudaEventRecord(h->ev[2], s));
+      run_encoder(h, n, -1, g0);
+      WISB_CUDA(cudaEventRecord(h->ev[3], s));
+      // the valid rows only: 1500 of each window's 1536
+      WISB_CUDA(cudaMemcpy2DAsync(static_cast<char*>(out) + static_cast<size_t>(g0) * T_ENC * row, T_ENC * row,
+                                  h->enc_out.p, T_ENC_PAD * row, T_ENC * row, n, cudaMemcpyDefault, s));
+      time_group(h, {2});
+    }
+    WISB_CUDA(cudaEventRecord(h->ev[4], s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+    WISB_CUDA(cudaEventElapsedTime(&h->timing[5], h->ev[0], h->ev[4]));
+    h->timing[7] = static_cast<float>(h->launches);
+    h->prof_collect();
+  });
+}
+
+int wisb_load_encoder_output(wisb_handle* h, const void* enc, int B, int dtype, int on_device) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(h->blob != nullptr, "handle has no model (created by wisb_create_frontend)");
+    WISB_REQUIRE(B >= 1 && B <= 4096, "B out of range");
+    WISB_REQUIRE(enc != nullptr, "enc is NULL");
+    WISB_REQUIRE(dtype == 0 || dtype == 1, "dtype must be 0 (float16) or 1 (float32)");
+    if (on_device) require_on_device(h, enc, "enc");
+    cudaStream_t s = h->stream;
+    const size_t n = static_cast<size_t>(B) * T_ENC * h->dims.d_model;
+    h->enc_in_B = 0;  // a failure below leaves no half-loaded source behind
+    h->enc_in.ensure(n);
+    for (int i = 1; i <= 5; ++i) h->timing[i] = 0.f;
+    DevBuf<float> staged;  // float32 host input, converted on the device
+    WISB_CUDA(cudaEventRecord(h->ev[0], s));
+    if (dtype == 0) {
+      WISB_CUDA(cudaMemcpyAsync(h->enc_in.p, enc, n * sizeof(__half), on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
+    } else if (on_device) {
+      f32_to_f16_run(static_cast<const float*>(enc), h->enc_in.p, n, s);
+    } else {
+      staged.ensure(n);
+      WISB_CUDA(cudaMemcpyAsync(staged.p, enc, n * sizeof(float), cudaMemcpyHostToDevice, s));
+    }
+    WISB_CUDA(cudaEventRecord(h->ev[1], s));
+    if (staged.p) f32_to_f16_run(staged.p, h->enc_in.p, n, s);
+    WISB_CUDA(cudaStreamSynchronize(s));
+    if (!on_device) WISB_CUDA(cudaEventElapsedTime(&h->timing[1], h->ev[0], h->ev[1]));
+    h->enc_in_B = B;
+    h->mel_B = 0;  // the loaded output, not kept features, is now the source of calls with mel == NULL
   });
 }
 
@@ -2121,14 +2292,15 @@ static void align_impl(wisb_handle* h, const float* mel, int B, const int32_t* s
     cudaStream_t s = h->stream;
     h->launches = 0;
     WISB_CUDA(cudaEventRecord(h->ev[0], s));
-    const bool cached = upload_mel(h, mel, B);
+    const bool loaded = loaded_source(h, mel, B);
+    const bool cached = !loaded && upload_mel(h, mel, B);
     time_h2d(h);
     const size_t per_utt = static_cast<size_t>(h->al_A) * (n_max + 1) * f_max * sizeof(float);
     int group = std::min(h->batch_rows / MAX_BEAM, static_cast<int>(std::min<size_t>(ALIGN_WS_BYTES / per_utt, 4096)));
     if (group < 1) group = 1;
     for (int g0 = 0; g0 < B; g0 += group) {
       const int n = std::min(group, B - g0);
-      encode_stage(h, cached, B, g0, n, ckv_layout(h, false));  // the capture and the batched pass read linear cross K/V
+      encode_stage(h, cached, loaded, B, g0, n, ckv_layout(h, false));  // the capture and the batched pass read linear cross K/V
       align_group(h, g0, n, start_seq, start_len, text, text_len, text_stride, num_frames, median_filter_width, n_max, f_max,
                   out_path, path_stride, out_path_len, out_token_probs, cap_out);
       time_group(h, {2, 2, 3, 4, 14});  // encoder + cross K/V, passes, filter, DTW
@@ -2481,7 +2653,7 @@ int wisb_debug_forced_logits(wisb_handle* h, const float* mel, const int32_t* to
     WISB_REQUIRE(h->blob != nullptr && tokens != nullptr && logits_out != nullptr && n_tokens >= 1 && n_tokens <= dm.n_text_ctx, "bad arguments");
     cudaStream_t s = h->stream;
     const bool batched = h->decoder_batch == 2;
-    encode_stage(h, upload_mel(h, mel, 1), 1, 0, 1, ckv_layout(h, !batched));
+    encode_stage(h, upload_mel(h, mel, 1), false, 1, 0, 1, ckv_layout(h, !batched));
     DecodeCfg c;
     c.u0 = 0; c.n_utt = 1; c.B_total = 1; c.beam = 1; c.prompt_len = n_tokens; c.max_new = 1; c.max_hyp = 1; c.lp = 1.f;
     if (batched) {  // the batched pass, one row: position p of the token list per pass

@@ -86,5 +86,7 @@ void enc_attn_plan(AttnPlan& p, const __half* qkv, const __half* vt, __half* ctx
 void enc_attn_run(const AttnPlan& p, cudaStream_t stream);
 // SIMT cross-check of the same attention (diagnostics only)
 void enc_attn_ref_run(const __half* qkv, __half* ctx, int B, int d, int H, cudaStream_t stream);
+// n floats -> n fp16 values, rounded to nearest even (encoder outputs loaded as float32)
+void f32_to_f16_run(const float* x, __half* y, size_t n, cudaStream_t stream);
 
 }  // namespace wisb

@@ -6,6 +6,8 @@
     results = model.generate(feats, [prompt] * n, beam_size=5, return_scores=False)
     results[i].sequences_ids[0]                                # list[int]
     model.detect_language(feats)[0][0]                         # ("<|en|>", prob)
+    enc = model.encode(feats)                                  # float16 [n, 1500, d_model], on the GPU (faster-whisper)
+    model.generate(enc, [prompt] * n)                          # generate / detect_language / align take it for features
 
 Same names, argument meaning and error behaviour (ValueError for bad shapes/arguments, RuntimeError for device
 failures).  What differs by design: ``device`` must be "cuda" (no CPU fallback), ``compute_type`` is accepted and
@@ -29,23 +31,61 @@ from .languages import LANGUAGE_CODES
 
 
 class StorageView:
-    """ctranslate2.StorageView stand-in: a borrowed view of a host float32 array (main.py:638,685)."""
+    """ctranslate2.StorageView stand-in.  Host form: a borrowed view of a host float32 array (features, main.py:638,685)
+    or of a float16 / float32 encoder output.  Device form (Whisper.encode with to_cpu=False): a float16 encoder output in
+    one device buffer of its own on GPU ``device_index``, freed with the view, whether or not the model still exists."""
 
     def __init__(self, array: np.ndarray):
         self.array = array
+        self._buf = None         # device form: address of its wisb_buffer_alloc buffer (float16, C order)
+        self._device_index = 0
+        self._shape = None
 
     @classmethod
     def from_array(cls, array):
         a = np.asarray(array)
-        if a.dtype != np.float32:
-            raise ValueError(f"StorageView.from_array: unsupported dtype {a.dtype} (float32 expected)")
+        if a.dtype not in (np.float32, np.float16):
+            raise ValueError(f"StorageView.from_array: unsupported dtype {a.dtype} (float32 or float16 expected)")
         if not a.flags["C_CONTIGUOUS"]:
             raise ValueError("StorageView.from_array: the array must be C-contiguous")
         return cls(a)
 
+    @classmethod
+    def _empty_on_device(cls, device_index: int, shape):
+        """an uninitialised float16 device view of `shape` on GPU `device_index`"""
+        sv = cls(None)
+        sv._buf = _lib.buffer_alloc(device_index, 2 * int(np.prod(shape)))
+        sv._device_index = int(device_index)
+        sv._shape = [int(v) for v in shape]
+        return sv
+
     @property
     def shape(self):
-        return list(self.array.shape)
+        return list(self._shape) if self._buf is not None else list(self.array.shape)
+
+    @property
+    def device(self) -> str:
+        return "cuda" if self._buf is not None else "cpu"
+
+    @property
+    def device_index(self) -> int:
+        return self._device_index
+
+    def to_device(self, device: str):
+        """to_device("cpu"): a host StorageView of the same data and dtype (the view itself when it is one already)"""
+        if device != "cpu":
+            raise ValueError("StorageView.to_device: only 'cpu' is supported")
+        if self._buf is None:
+            return self
+        return StorageView(_lib.buffer_to_host(self._buf, np.empty(self._shape, np.float16)))
+
+    def __del__(self):
+        if self._buf is not None:
+            buf, self._buf = self._buf, None
+            try:
+                _lib.buffer_free(buf)
+            except Exception:
+                pass
 
 
 @dataclass
@@ -77,6 +117,15 @@ def _features_array(features, n_mels: int) -> np.ndarray:
     if a.dtype != np.float32 or a.ndim != 3 or tuple(a.shape[1:]) != (n_mels, 3000):
         raise ValueError(f"features must be float32 [n, {n_mels}, 3000] for this model, got {a.dtype} {tuple(a.shape)}")
     return np.ascontiguousarray(a)
+
+
+@dataclass
+class _Input:
+    """what a generate / detect_language / align call decodes: features, a host encoder output, or a device one"""
+    n: int
+    mel: np.ndarray = None   # float32 [n, n_mels, 3000]
+    enc: np.ndarray = None   # float16 / float32 [n, 1500, d_model] in host memory
+    dev: StorageView = None  # device form of a float16 [n, 1500, d_model] encoder output
 
 
 class Whisper:
@@ -123,6 +172,8 @@ class Whisper:
         self._pool = ThreadPoolExecutor(max_workers=len(self._handles)) if len(self._handles) > 1 else None
         self._rr = 0
         self._lock = threading.Lock()
+        # loading an encoder output and the call that decodes it must not interleave with another such pair
+        self._replica_locks = [threading.Lock() for _ in self._handles]
 
     # ----------------------------------------------------------------------------------------------------------
     @property
@@ -160,6 +211,71 @@ class Whisper:
             return [fn() for fn in jobs]
         return [f.result() for f in [self._pool.submit(fn) for fn in jobs]]
 
+    def _input(self, features) -> _Input:
+        """CTranslate2's rule: an input [n, 1500, d_model] is an encoder output from encode(), anything else must be the
+        model's features [n, n_mels, 3000]"""
+        if isinstance(features, StorageView) and features.device == "cuda":
+            shape = features.shape
+        else:
+            a = features.array if isinstance(features, StorageView) else np.asarray(features)
+            shape = list(a.shape)
+        if len(shape) != 3 or shape[1] != 1500:
+            mel = _features_array(features, self.n_mels)
+            return _Input(mel.shape[0], mel=mel)
+        d = self._dims["d_model"]
+        if isinstance(features, StorageView) and features.device == "cuda":
+            if shape[2] != d:
+                raise ValueError(f"an encoder output must be [n, 1500, {d}] for this model, got {tuple(shape)}")
+            if features.device_index not in self.device_index:
+                raise ValueError(f"the encoder output is on GPU {features.device_index}, where this model has no replica")
+            return _Input(shape[0], dev=features)
+        if a.dtype not in (np.float16, np.float32) or shape[2] != d:
+            raise ValueError(f"an encoder output must be float16 or float32 [n, 1500, {d}] for this model, got {a.dtype} "
+                             f"{tuple(shape)}")
+        return _Input(shape[0], enc=np.ascontiguousarray(a))
+
+    def _dispatch(self, src: _Input, fn):
+        """fn(handle, mel, s, e) for each part [s, e) of the windows, on the replicas _split picks (features and host
+        encoder outputs) or on the replica on the GPU of a device encoder output.  For an encoder output, mel is None and
+        the part is loaded into the handle just before (the call then decodes it, passing B = e - s)."""
+        if src.dev is not None:
+            parts = [(self.device_index.index(src.dev.device_index), 0, src.n)]
+        else:
+            parts = self._split(src.n, src.mel)
+
+        def job(i, s, e):
+            h = self._handles[i]
+            if src.mel is not None:
+                return lambda: fn(h, src.mel[s:e], s, e)
+
+            def run():
+                with self._replica_locks[i]:
+                    if src.dev is not None:
+                        h.load_encoder_output(src.dev._buf, on_device=True, B=src.n, dtype=np.float16)
+                    else:
+                        h.load_encoder_output(src.enc[s:e])
+                    return fn(h, None, s, e)
+            return run
+
+        return self._run([job(*pt) for pt in parts])
+
+    def encode(self, features, to_cpu: bool = False) -> StorageView:
+        """ctranslate2.models.Whisper.encode: features -> the encoder output, float16 [n, 1500, d_model], for
+        detect_language, generate and align.  On the GPU of the replica that encoded it (one replica, round robin, runs
+        the whole call), or with to_cpu=True in host memory (the replicas then split the windows as in generate)."""
+        mel = _features_array(features, self.n_mels)
+        n, d = mel.shape[0], self._dims["d_model"]
+        if to_cpu:
+            out = np.empty((n, 1500, d), np.float16)
+            self._run([(lambda i=i, s=s, e=e: self._handles[i].encode(mel[s:e], out[s:e])) for i, s, e in self._split(n)])
+            return StorageView(out)
+        with self._lock:
+            i = self._rr % len(self._handles)
+            self._rr += 1
+        sv = StorageView._empty_on_device(self.device_index[i], (n, 1500, d))
+        self._handles[i].encode(mel, sv._buf, on_device=True)
+        return sv
+
     def generate(self, features, prompts, *, asynchronous: bool = False, beam_size: int = 5, patience: float = 1,
                  num_hypotheses: int = 1, length_penalty: float = 1, repetition_penalty: float = 1,
                  no_repeat_ngram_size: int = 0, max_length: int = 448, return_scores: bool = False,
@@ -167,8 +283,8 @@ class Whisper:
                  suppress_blank: bool = True, suppress_tokens=(-1,), sampling_topk: int = 1,
                  sampling_temperature: float = 1):
         """ctranslate2.models.Whisper.generate for the options WIS relies on (SURVEY.md section 8b defaults)."""
-        mel = _features_array(features, self.n_mels)
-        n = mel.shape[0]
+        src = self._input(features)
+        n = src.n
         if len(prompts) != n:
             raise ValueError(f"expected {n} prompts (one per feature window), got {len(prompts)}")
         lens = {len(p) for p in prompts}
@@ -199,7 +315,6 @@ class Whisper:
             raise ValueError("max_initial_timestamp_index must be a non-negative int")
         extra = [int(t) for t in suppress_tokens if t >= 0]
         p = np.asarray(prompts, np.int32)
-        parts = self._split(n, mel)
         # extension over CTranslate2: `max_length` may be one int per window (requests with different limits coalesced
         # into one call by batcher.TranscribeBatcher); a plain int is the CTranslate2 meaning
         ml = None if np.isscalar(max_length) else np.asarray(max_length, np.int32)
@@ -210,12 +325,12 @@ class Whisper:
         if repetition_penalty != 1 or no_repeat_ngram_size != 0:
             proc = dict(repetition_penalty=float(repetition_penalty), no_repeat_ngram_size=int(no_repeat_ngram_size))
 
-        def job(i, s, e):
-            return lambda: self._handles[i].generate(mel[s:e], p[s:e], beam_size, patience, length_penalty,
-                                                     max_length if ml is None else ml[s:e], extra, timestamps=timestamps,
-                                                     max_initial_timestamp_index=int(max_initial_timestamp_index), **proc)
+        def run(h, mel, s, e):
+            return h.generate(mel, p[s:e], beam_size, patience, length_penalty, max_length if ml is None else ml[s:e],
+                              extra, B=e - s, timestamps=timestamps,
+                              max_initial_timestamp_index=int(max_initial_timestamp_index), **proc)
 
-        outs = self._run([job(*pt) for pt in parts])
+        outs = self._dispatch(src, run)
         results = []
         for ids, scores in outs:
             for seq, sc in zip(ids, scores):
@@ -223,15 +338,10 @@ class Whisper:
         return results
 
     def detect_language(self, features):
-        mel = _features_array(features, self.n_mels)
-        parts = self._split(mel.shape[0], mel)
-
-        def job(i, s, e):
-            return lambda: self._handles[i].detect_language(mel[s:e])
-
+        src = self._input(features)
         out = []
         first = self._dims["lang_first"]
-        for ids, probs in self._run([job(*pt) for pt in parts]):
+        for ids, probs in self._dispatch(src, lambda h, mel, s, e: h.detect_language(mel, B=e - s)):
             for row_ids, row_p in zip(ids, probs):
                 out.append([(f"<|{LANGUAGE_CODES[int(t) - first]}|>" if int(t) - first < len(LANGUAGE_CODES) else f"<|{int(t)}|>",
                              float(pr)) for t, pr in zip(row_ids, row_p)])
@@ -242,8 +352,8 @@ class Whisper:
         alignment heads' cross-attention, and each text token's probability.  The decoder is teacher-forced with
         start_sequence + [<|notimestamps|>] + text_tokens[b]; num_frames is an int or one int per window (feature frames,
         the path covers num_frames // 2 encoder frames).  Word grouping needs a tokenizer and stays with the caller."""
-        mel = _features_array(features, self.n_mels)
-        n = mel.shape[0]
+        src = self._input(features)
+        n = src.n
         if len(text_tokens) != n:
             raise ValueError(f"expected {n} text token lists (one per feature window), got {len(text_tokens)}")
         if any(isinstance(t, str) for seq in text_tokens for t in seq) or any(isinstance(t, str) for t in start_sequence):
@@ -259,11 +369,9 @@ class Whisper:
         text = [list(t) for t in text_tokens]
         start = list(start_sequence)
 
-        def job(i, s, e):
-            return lambda: self._handles[i].align(mel[s:e], start, text[s:e], nf[s:e], median_filter_width)
-
         results = []
-        for paths, probs in self._run([job(*pt) for pt in self._split(n, mel)]):
+        for paths, probs in self._dispatch(src, lambda h, mel, s, e: h.align(mel, start, text[s:e], nf[s:e],
+                                                                              median_filter_width, B=e - s)):
             for p, pr in zip(paths, probs):
                 results.append(WhisperAlignmentResult([(int(a), int(b)) for a, b in p], [float(v) for v in pr]))
         return results
