@@ -4,10 +4,11 @@
 //   hann(400) periodic, STFT n_fft=400 hop=160 center/reflect, |.|^2 of the first 3000 frames, NMx201 Slaney mel
 //   filterbank (NM = 80, or 128 for the large-v3 family), log10(clamp 1e-10), max(x, utterance_max - 8), (x + 4) / 4.
 // Differences in HOW (not what): zero-padding / trimming to 480000 samples and the optional s16 -> f32 conversion are
-// fused into the frame gather (the padded PCM is never materialised); the 400-point real DFT is evaluated directly in
-// fp32 FMA using the even/odd symmetry of the windowed frame (201 x 200 MACs per frame instead of an FFT -- single-pass
-// TF32 tensor cores miss the 1e-4 parity bar, see BASELINE.md section 2); frames that lie wholly in the zero padding
-// skip the DFT.  HBM traffic per window: <= 1.92 MB PCM in, 0.96 MB out at 80 bins / 1.54 MB at 128 (+ the same again
+// fused into the frame gather (the padded PCM is never materialised); the 400-point real DFT is evaluated directly
+// using the even/odd symmetry of the windowed frame (201 x 200 MACs per frame instead of an FFT -- single-pass TF32
+// tensor cores miss the 1e-4 parity bar, see BASELINE.md section 2), from fp32 samples and fp32 twiddle tables into
+// fp64 accumulators (an fp32 chain is up to 4e-4 off float64 in the quiet bins beside a loud tone); frames that lie
+// wholly in the zero padding skip the DFT.  HBM traffic per window: <= 1.92 MB PCM in, 0.96 MB out at 80 bins / 1.54 MB at 128 (+ the same again
 // re-read/written by the clamp pass).
 #include <math.h>
 
@@ -103,15 +104,17 @@ logmel_power_kernel(const void* __restrict__ pcm, const long long* __restrict__ 
     if (tid < KQ * 4) {
       const int kq = tid % KQ;
       const int fg = tid / KQ;  // 8 frames each
-      float re[4][8], im[4][8];
+      // float64 accumulators: each product of two floats is exact in float64, so the only roundings left are the
+      // fold's and the tables' (one each per term) -- a float32 chain loses the small bins next to a loud tone
+      double re[4][8], im[4][8];
 #pragma unroll
       for (int j = 0; j < 4; ++j)
 #pragma unroll
-        for (int f = 0; f < 8; ++f) re[j][f] = im[j][f] = 0.f;
+        for (int f = 0; f < 8; ++f) re[j][f] = im[j][f] = 0.0;
       const float* xb = xs + fg * 8 * HOP;
 #pragma unroll 2
       for (int n = 0; n <= N_FFT / 2; ++n) {
-        float c[4], s[4];
+        double c[4], s[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           c[j] = __ldg(tw + n * BINS_PAD + kq + KQ * j);
@@ -121,18 +124,19 @@ logmel_power_kernel(const void* __restrict__ pcm, const long long* __restrict__ 
         for (int f = 0; f < 8; ++f) {
           const float a = xb[f * HOP + n];
           const float bq = (n == 0 || n == N_FFT / 2) ? 0.f : xb[f * HOP + N_FFT - n];
-          const float ev = a + bq, od = a - bq;
+          const double ev = a + bq, od = a - bq;
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
-            re[j][f] = fmaf(ev, c[j], re[j][f]);
-            im[j][f] = fmaf(od, s[j], im[j][f]);
+            re[j][f] = fma(ev, c[j], re[j][f]);
+            im[j][f] = fma(od, s[j], im[j][f]);
           }
         }
       }
 #pragma unroll
       for (int j = 0; j < 4; ++j)
 #pragma unroll
-        for (int f = 0; f < 8; ++f) pw[fg * 8 + f][kq + KQ * j] = re[j][f] * re[j][f] + im[j][f] * im[j][f];
+        for (int f = 0; f < 8; ++f)
+          pw[fg * 8 + f][kq + KQ * j] = static_cast<float>(re[j][f] * re[j][f] + im[j][f] * im[j][f]);
     }
     __syncthreads();
     for (int i = tid; i < NM * FT; i += LM_THREADS) {
