@@ -98,6 +98,21 @@ int wisb_generate_proc(wisb_handle* h, const float* mel, int B, const int32_t* p
                        float repetition_penalty, int no_repeat_ngram_size, int32_t* out_ids, int out_stride,
                        int32_t* out_len, float* out_score);
 
+/* Same call with the search options per window, each an array [B] or NULL (then the scalar applies to every window):
+ * beam_per_utt in [1, 8], patience_per_utt finite and > 0, length_penalty_per_utt finite (else code 1).  Window b
+ * searches with its own beam, finishes once max(1, round half up of beam x patience in fp32) hypotheses exist and ranks
+ * them with its own length penalty, exactly as it would alone; prompts already come per window.  Like the per-window
+ * max_length, this is what CTranslate2's per-call options become when a batcher coalesces several calls into one: every
+ * window keeps a block of rows of the largest beam B of its group (at most batch_rows / B windows per group), searches
+ * its first b rows and leaves the others dead.  A group whose windows agree on beam, max_hyp and length penalty runs
+ * the scalar search.  wisb_generate_proc is this call with three NULLs. */
+int wisb_generate_mixed(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
+                        float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
+                        const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
+                        float repetition_penalty, int no_repeat_ngram_size, const int32_t* beam_per_utt,
+                        const float* patience_per_utt, const float* length_penalty_per_utt, int32_t* out_ids,
+                        int out_stride, int32_t* out_len, float* out_score);
+
 /* (5) per utterance: language token ids sorted by probability (descending) and the probabilities.
  * lang_ids_out int32 [B, n_langs], probs_out float32 [B, n_langs]. */
 int wisb_detect_language(wisb_handle* h, const float* mel, int B, int32_t* lang_ids_out, float* probs_out);
@@ -188,6 +203,15 @@ int wisb_debug_gemm(wisb_handle* h, const int32_t* prm, int n_prm, const uint16_
 int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, float length_penalty, const float* logits,
                            const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
                            float* state_f, int32_t* cand_idx, float* cand_score, float* row_lse);
+/* The same step with per-utterance search options (wisb_generate_mixed): prm[1] is the row block B of every utterance,
+ * utterance u searches rows [0, beam_u[u]) (beam_u[u] in [1, B]) with 2 beam_u[u] candidates, finishes at max_hyp_u[u]
+ * (>= 1) hypotheses and normalises with length_penalty_u[u] (finite); prm[9] (>= 1) is unused.  Its other rows are
+ * dead: cum -inf, token eot, never a candidate (cand_idx entries 2 beam_u[u] .. 15 are -1) or a hypothesis.  With
+ * init, search initialisation makes them dead. */
+int wisb_debug_search_step_mixed(wisb_handle* h, const int32_t* prm, int n_prm, const float* logits, const uint8_t* mask,
+                                 const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i, float* state_f,
+                                 int32_t* cand_idx, float* cand_score, float* row_lse, const int32_t* beam_u,
+                                 const int32_t* max_hyp_u, const float* length_penalty_u);
 /* encoder self-attention on caller data: qkv [B*1536, 3d] fp16 -> ctx [B*1536, d] fp16, d = 64 H; impl 0 = wgmma with
  * MN-major V, 1 = wgmma with the transposed Vt layout (built from the same qkv), 2 = SIMT check */
 int wisb_debug_enc_attn(wisb_handle* h, const uint16_t* qkv16, int B, int d, int H, int impl, uint16_t* ctx16_out);

@@ -43,6 +43,9 @@ _SIGS = {
     "wisb_generate_proc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
                                      C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int,
                                      C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "wisb_generate_mixed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
+                                      C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_detect_language": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_buffer_alloc": (C.c_int, [C.c_int, C.c_size_t, C.POINTER(C.c_void_p)]),
     "wisb_buffer_free": (C.c_int, [C.c_void_p]),
@@ -62,6 +65,9 @@ _SIGS = {
                                   C.c_void_p]),
     "wisb_debug_search_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wisb_debug_search_step_mixed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_enc_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "wisb_debug_dec_cross_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_dec_self_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -115,6 +121,18 @@ def ptr(a):
     if a is None:
         return None
     return a.ctypes.data_as(C.c_void_p)
+
+
+def per_window(value, n: int, dtype, name: str):
+    """A generate option given as a scalar (-> None) or as one value per window (-> a C-contiguous [n] array of dtype):
+    integers for an int32 option, integers or floats for a float32 one; no silent truncation of a float to an int."""
+    if np.isscalar(value):
+        return None
+    a = np.asarray(value)
+    kinds = "iu" if np.dtype(dtype).kind in "iu" else "iuf"
+    if a.shape != (n,) or a.dtype.kind not in kinds:
+        raise ValueError(f"{name} must be a scalar or one {'int' if kinds == 'iu' else 'number'} per window ({n})")
+    return np.ascontiguousarray(a, dtype)
 
 
 class Handle:
@@ -212,7 +230,9 @@ class Handle:
                  B=None, timestamps=False, max_initial_timestamp_index=50, repetition_penalty=1.0, no_repeat_ngram_size=0):
         """-> (token ids per utterance, length-normalised scores).  timestamps=True applies Whisper's timestamp rules
         (wisb_generate_ts); the prompt must then contain neither <|notimestamps|> nor timestamp tokens.
-        repetition_penalty != 1 or no_repeat_ngram_size > 0 switches on the history processors (wisb_generate_proc)."""
+        repetition_penalty != 1 or no_repeat_ngram_size > 0 switches on the history processors (wisb_generate_proc).
+        beam_size, patience and length_penalty, like max_length, may each be one value per window
+        (wisb_generate_mixed)."""
         prompts = np.ascontiguousarray(prompts, np.int32)
         if prompts.ndim != 2:
             raise ValueError("prompts must be [B, prompt_len]")
@@ -232,7 +252,20 @@ class Handle:
         lens = np.zeros(B, np.int32)
         scores = np.zeros(B, np.float32)
         extra = np.ascontiguousarray(list(extra_suppress), np.int32)
-        if repetition_penalty != 1 or no_repeat_ngram_size != 0:
+        beams = per_window(beam_size, B, np.int32, "beam_size")
+        pats = per_window(patience, B, np.float32, "patience")
+        lps = per_window(length_penalty, B, np.float32, "length_penalty")
+        if beams is not None or pats is not None or lps is not None:
+            # (the scalars stand in for the options given per window; the engine ignores them there)
+            check(lib().wisb_generate_mixed(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1],
+                                            1 if beams is not None else int(beam_size),
+                                            1.0 if pats is not None else float(patience),
+                                            1.0 if lps is not None else float(length_penalty), int(max_length),
+                                            ptr(per_utt), ptr(extra) if extra.size else None, extra.size,
+                                            1 if timestamps else 0, int(max_initial_timestamp_index),
+                                            float(repetition_penalty), int(no_repeat_ngram_size), ptr(beams), ptr(pats),
+                                            ptr(lps), ptr(ids), stride, ptr(lens), ptr(scores)))
+        elif repetition_penalty != 1 or no_repeat_ngram_size != 0:
             check(lib().wisb_generate_proc(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], int(beam_size),
                                            float(patience), float(length_penalty), int(max_length), ptr(per_utt),
                                            ptr(extra) if extra.size else None, extra.size, 1 if timestamps else 0,
@@ -453,12 +486,14 @@ class Handle:
     def debug_search_step_state(self, logits, mask, state, *, beam: int, max_hyp: int, eot: int, V: int = 0, no_timestamps: int = 0,
                           timestamps: bool = False, max_initial_timestamp_index: int = 50, length_penalty: float = 1.0,
                           max_new_u=None, prompt=None, shared_prefix: int = 0, repetition_penalty=None,
-                          no_repeat_ngram_size=None):
+                          no_repeat_ngram_size=None, beam_u=None, max_hyp_u=None, length_penalty_u=None):
         """One production search step on caller state.  logits float32 [n_utt*beam, ldl] (only columns < V are read; V
         = ldl by default); mask uint8 [V] (bit 0 every step, bit 1 at the first generated step); state as made by
         search_state (its shapes give max_new and t_max); prompt int [n_utt, prompt_len]: run the search initialisation
         (with shared_prefix) first; repetition_penalty / no_repeat_ngram_size: the history processors (either one
-        given: the 15-parameter form, the other one off; neither: the 13-parameter form).
+        given: the 15-parameter form, the other one off; neither: the 13-parameter form); beam_u / max_hyp_u /
+        length_penalty_u (all three, [n_utt] each): wisb_debug_search_step_mixed, `beam` the row block of every
+        utterance, max_hyp and length_penalty unused.
         -> (new state, cand_idx int32 [n_utt, 2*beam] = beam*V + token or -1, cand_score
         float32 [n_utt, 2*beam], row_lse float32 [n_utt*beam])."""
         logits = np.ascontiguousarray(logits, np.float32)
@@ -489,8 +524,15 @@ class Handle:
         ci = np.zeros((n_utt, 16), np.int32)
         cs = np.zeros((n_utt, 16), np.float32)
         lse = np.zeros(R, np.float32)
-        check(lib().wisb_debug_search_step(self._h, ptr(prm), prm.size, float(length_penalty), ptr(logits), ptr(mask),
-                                           ptr(caps), ptr(pr), ptr(si), ptr(sf), ptr(ci), ptr(cs), ptr(lse)))
+        if beam_u is None and max_hyp_u is None and length_penalty_u is None:
+            check(lib().wisb_debug_search_step(self._h, ptr(prm), prm.size, float(length_penalty), ptr(logits), ptr(mask),
+                                               ptr(caps), ptr(pr), ptr(si), ptr(sf), ptr(ci), ptr(cs), ptr(lse)))
+        else:
+            bu, hu = (None if v is None else np.ascontiguousarray(v, np.int32).reshape(n_utt) for v in (beam_u, max_hyp_u))
+            lu = None if length_penalty_u is None else np.ascontiguousarray(length_penalty_u, np.float32).reshape(n_utt)
+            check(lib().wisb_debug_search_step_mixed(self._h, ptr(prm), prm.size, ptr(logits), ptr(mask), ptr(caps), ptr(pr),
+                                                     ptr(si), ptr(sf), ptr(ci), ptr(cs), ptr(lse), ptr(bu), ptr(hu),
+                                                     ptr(lu)))
         out, oi, of = {}, 0, 0
         for k, v in want.items():
             if k in self._STATE_F:

@@ -15,8 +15,19 @@ This module is the piece a WIS maintainer puts between the endpoints and the eng
     results = batcher.submit(features, prompt, beam_size=5).result()      # from plain threads
 
 Requests are compatible when they share the prompt and every generation option except ``max_length`` (same decoder
-configuration; the length limits travel per window); a batch is closed when ``max_batch`` windows are collected or
-``max_wait_ms`` after its oldest request arrived, whichever is first.  Latency note: every request of a batch is
+configuration; the length limits travel per window).  With an engine that takes the search options per window
+(``models.Whisper.per_window_options``) the rule is wider: prompts need only the same length and the same timestamp mode
+(whether ``<|notimestamps|>`` is in them), and ``beam_size``, ``patience`` and ``length_penalty`` travel per window too,
+so short commands at beam 1, dictation at beam 3 and requests in other languages or for translation share one call.
+Every other option (``max_initial_timestamp_index``, ``suppress_tokens``, the history processors) must still match.
+Those three options are checked at ``submit`` (``ValueError`` there), and a call that the engine refuses as invalid
+(``ValueError``) is retried request by request, so one client's bad request never fails the requests it was merged with.
+Every window of such a call keeps as many decoder rows as the call's largest beam, so a batch keeps its padded rows at
+most its real ones (windows x largest beam <= 2 x the sum of the beams), leaving the newest requests whose beams are
+farthest from the oldest request's for the next batch: on an H100 (700 W power limit), 63 greedy windows and one at
+beam 8 in one call (512 rows for 71 real ones) took 1.45x the time of two calls, while WIS's mix of beam 1 and beam 3
+windows (168 rows for 88) took 0.94x (DESIGN.md section 6).  A batch is closed when ``max_batch`` windows are collected
+or ``max_wait_ms`` after its oldest request arrived, whichever is first.  Latency note: every request of a batch is
 answered when the whole batch has been decoded (the slowest window decides), so ``max_batch`` trades throughput against
 the latency of short requests; ``max_batch`` above the engine's row capacity / beam only adds queueing.
 The engine call runs on the batcher's own thread, so the event loop is never blocked (the C ABI releases the GIL).
@@ -34,16 +45,41 @@ import numpy as np
 from .models import StorageView
 
 
-class _Request:
-    __slots__ = ("features", "n", "key", "prompt", "opts", "max_length", "future", "t_arrival")
+# search options an engine with per_window_options takes per window, with the defaults of CTranslate2's generate (which
+# stand in for a request that does not set one when it shares a call with one that does)
+PER_WINDOW_DEFAULTS = {"beam_size": 5, "patience": 1.0, "length_penalty": 1.0}
 
-    def __init__(self, features, prompt, opts):
+
+def _check_search_option(name, v):
+    """A per-window search option as models.Whisper.generate accepts it: beam_size an int in [1, 8], patience a finite
+    number > 0, length_penalty a finite number; anything else raises ValueError."""
+    if name == "beam_size":
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or not 1 <= v <= 8:
+            raise ValueError(f"beam_size must be an int in [1, 8], got {v!r}")
+        return int(v)
+    number = isinstance(v, (int, float, np.integer, np.floating)) and not isinstance(v, (bool, np.bool_))
+    if not number or not np.isfinite(v) or (name == "patience" and v <= 0):
+        raise ValueError(f"{name} must be a finite number{' > 0' if name == 'patience' else ''}, got {v!r}")
+    return float(v)
+
+
+class _Request:
+    __slots__ = ("features", "n", "key", "prompt", "opts", "search", "max_length", "future", "t_arrival")
+
+    def __init__(self, features, prompt, opts, no_timestamps=None):
+        """no_timestamps: the engine's <|notimestamps|> id when it takes prompts and search options per window, else
+        None (then the prompt and every option but max_length are part of the key)"""
         self.features = features
         self.n = int(features.shape[0])
         self.prompt = list(prompt)
         self.opts = dict(opts)
         self.max_length = int(self.opts.pop("max_length", 448))  # per request; merged per window by the worker
-        self.key = (tuple(self.prompt), tuple(sorted((k, _freeze(v)) for k, v in self.opts.items())))
+        self.search = {}
+        prompt_key = tuple(self.prompt)
+        if no_timestamps is not None:
+            self.search = {k: _check_search_option(k, self.opts.pop(k)) for k in PER_WINDOW_DEFAULTS if k in self.opts}
+            prompt_key = (len(self.prompt), no_timestamps in self.prompt)
+        self.key = (prompt_key, tuple(sorted((k, _freeze(v)) for k, v in self.opts.items())))
         self.future = Future()
         self.t_arrival = time.monotonic()
 
@@ -60,6 +96,9 @@ class TranscribeBatcher:
         # features are checked at submit against the model's bin count (CTranslate2's Whisper.n_mels); an engine
         # without that property takes the 80-bin features of every Whisper model before large-v3
         self._n_mels = int(getattr(model, "n_mels", 80))
+        # an engine that takes the prompt and the search options per window lets requests that differ in them share a
+        # call; any other (CTranslate2's Whisper among them) gets calls with one prompt and one set of options
+        self._no_ts = int(model.dims["no_timestamps"]) if getattr(model, "per_window_options", False) else None
         self.max_batch = int(max_batch)
         self.max_wait = float(max_wait_ms) / 1e3
         self.max_queue_windows = int(max_queue_windows)
@@ -84,7 +123,7 @@ class TranscribeBatcher:
             if any(list(p) != list(prompt[0]) for p in prompt) or len(prompt) != arr.shape[0]:
                 raise ValueError("one request carries one prompt for all of its windows (as main.py:689 builds it)")
             prompt = prompt[0]
-        req = _Request(np.ascontiguousarray(arr), prompt, generate_options)
+        req = _Request(np.ascontiguousarray(arr), prompt, generate_options, self._no_ts)
         with self._cv:
             if self._closed:
                 raise RuntimeError("batcher is closed")
@@ -142,10 +181,31 @@ class TranscribeBatcher:
                 r = q.popleft()
                 batch.append(r)
                 total += r.n
+            rest = []
+            while not self._padding_ok(batch):
+                # the newest of the requests whose beam is farthest from the oldest one's waits for the next batch
+                b0 = self._beam(batch[0])
+                far = max(range(1, len(batch)), key=lambda i: (abs(self._beam(batch[i]) - b0), i))
+                rest.append(batch.pop(far))
+                total -= rest[-1].n
+            q.extendleft(sorted(rest, key=lambda r: r.t_arrival, reverse=True))
             if not q:
                 del self._queues[key]
             self._queued_windows -= total
             return batch
+
+    @staticmethod
+    def _beam(r) -> int:
+        return int(r.search.get("beam_size", PER_WINDOW_DEFAULTS["beam_size"]))
+
+    def _padding_ok(self, reqs) -> bool:
+        """padded rows <= real rows when these requests share a call (always true without per-window options)"""
+        if self._no_ts is None:
+            return True
+        beams = [self._beam(r) for r in reqs]
+        windows = sum(r.n for r in reqs)
+        real = sum(r.n * b for r, b in zip(reqs, beams))
+        return windows * max(beams) <= 2 * real
 
     def _loop(self):
         while True:
@@ -156,22 +216,43 @@ class TranscribeBatcher:
             live = [r for r in batch if r.future.set_running_or_notify_cancel()]
             if not live:
                 continue
-            n = sum(r.n for r in live)
             try:
-                feats = live[0].features if len(live) == 1 else np.concatenate([r.features for r in live], axis=0)
-                limits = [r.max_length for r in live for _ in range(r.n)]
-                ml = limits[0] if len(set(limits)) == 1 else np.asarray(limits, np.int32)
-                out = self._model.generate(StorageView.from_array(feats), [live[0].prompt] * n, max_length=ml, **live[0].opts)
-                if len(out) != n:
-                    raise RuntimeError(f"engine returned {len(out)} results for {n} windows")
+                self._answer(live)
+            except ValueError as e:
+                if len(live) == 1:
+                    live[0].future.set_exception(e)
+                    continue
+                # the engine refused an argument of one of the requests (a prompt token, a length limit, ...): each
+                # request alone, so that only the one it belongs to fails
+                for r in live:
+                    try:
+                        self._answer([r])
+                    except BaseException as e1:  # noqa: BLE001 -- the waiter must learn about it
+                        r.future.set_exception(e1)
             except BaseException as e:  # noqa: BLE001 -- every waiter must learn about it
                 for r in live:
                     r.future.set_exception(e)
-                continue
-            self.stats["engine_calls"] += 1
-            self.stats["windows"] += n
-            self.stats["max_windows_per_call"] = max(self.stats["max_windows_per_call"], n)
-            pos = 0
-            for r in live:
-                r.future.set_result(out[pos : pos + r.n])
-                pos += r.n
+
+    def _answer(self, live):
+        """ONE engine call for the windows of these requests; sets their results (raises, setting none, on failure)."""
+        n = sum(r.n for r in live)
+        feats = live[0].features if len(live) == 1 else np.concatenate([r.features for r in live], axis=0)
+        limits = [r.max_length for r in live for _ in range(r.n)]
+        ml = limits[0] if len(set(limits)) == 1 else np.asarray(limits, np.int32)
+        opts = dict(live[0].opts)
+        for k, default in PER_WINDOW_DEFAULTS.items():  # (equal values stay a scalar: the CTranslate2 meaning)
+            if any(k in r.search for r in live):
+                vals = [r.search.get(k, default) for r in live for _ in range(r.n)]
+                same = all(v == vals[0] for v in vals)
+                opts[k] = vals[0] if same else np.asarray(vals, np.int32 if k == "beam_size" else np.float32)
+        prompts = [r.prompt for r in live for _ in range(r.n)]
+        out = self._model.generate(StorageView.from_array(feats), prompts, max_length=ml, **opts)
+        if len(out) != n:
+            raise RuntimeError(f"engine returned {len(out)} results for {n} windows")
+        self.stats["engine_calls"] += 1
+        self.stats["windows"] += n
+        self.stats["max_windows_per_call"] = max(self.stats["max_windows_per_call"], n)
+        pos = 0
+        for r in live:
+            r.future.set_result(out[pos : pos + r.n])
+            pos += r.n

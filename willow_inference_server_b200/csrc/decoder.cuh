@@ -63,6 +63,12 @@ struct SearchArgs {
   // history processors on every row's generated tokens (search.cu): 1 / 0 = off
   float rep_penalty = 1.f;        // repetition_penalty, finite and > 0
   int no_repeat_ngram = 0;        // no_repeat_ngram_size, >= 0
+  // per-utterance search options (all three or none): utterance u searches rows [0, beam_u[u]) of its block of `beam`
+  // rows with 2 * beam_u[u] candidates, max_hyp_u[u] hypotheses and length penalty lp_u[u]; its rows >= beam_u[u] are
+  // dead (eot, cum -inf).  `beam` is then the largest of them, `n_cand` 2 * beam; max_hyp / length_penalty are unused.
+  const int* beam_u = nullptr;    // [n_utt] in [1, beam]
+  const int* max_hyp_u = nullptr; // [n_utt] >= 1
+  const float* lp_u = nullptr;    // [n_utt]
 };
 void search_step_run(const SearchArgs& a, cudaStream_t stream);
 // prompt prefill: no search, just feed the next prompt token and advance the position

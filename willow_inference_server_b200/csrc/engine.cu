@@ -85,6 +85,7 @@ struct GraphKey {
   float lp;
   float rep_penalty;    // history processors (baked in too)
   int no_repeat_ngram;
+  int mixed;            // per-utterance beam / max_hyp / length penalty in device arrays (beam = the largest; max_hyp, lp 0)
   bool operator<(const GraphKey& o) const {
     return memcmp(this, &o, sizeof(GraphKey)) < 0;
   }
@@ -143,6 +144,8 @@ struct wisb_handle {
   DevBuf<int> cand_idx, tokens, seq0, seq1, ind0, ind1, flip, done, n_hyp, best_len, best_tokens, prompt_dev, lang_ids;
   DevBuf<DecState> st;
   DevBuf<int> row_pos, row_slot, max_new_u;
+  DevBuf<int> beam_u, max_hyp_u;  // per-utterance search options of a call that mixes them (SearchArgs::beam_u)
+  DevBuf<float> lp_u;
   int search_rows = 0;  // rows the search / state buffers above are sized for
   int search_gen = 0, bd_search_gen = -1;  // reallocation count of those buffers / the one the batched-pass plans were built for
   // batched decoder pass (more than DEC_MAX_ROWS rows): workspaces for bd_rows (multiple of 128) rows, bd_tcap positions
@@ -348,8 +351,9 @@ void ensure_search(wisb_handle* h, int rows) {
   h->best_tokens.ensure(R * T_MAX, true);
   h->prompt_dev.ensure(R * T_MAX);
   h->row_pos.ensure(R, true); h->row_slot.ensure(R, true); h->max_new_u.ensure(R, true);
+  h->beam_u.ensure(R, true); h->max_hyp_u.ensure(R, true); h->lp_u.ensure(R, true);
   h->lang_probs.ensure(R * 128);
-  h->pin_i.ensure(4 + R * (T_MAX + 2));
+  h->pin_i.ensure(4 + R * (T_MAX + 5));  // (upload_prompts: prompts and four per-utterance words)
   h->pin_f.ensure(R * 130);
   h->search_rows = rows;
   ++h->search_gen;  // whoever baked these pointers into plans must rebuild them
@@ -800,6 +804,12 @@ struct DecodeCfg {
   int ts_max_init = 0;      // max_initial_timestamp_index
   float rep_penalty = 1.f;  // repetition_penalty (1 = off)
   int no_repeat_ngram = 0;  // no_repeat_ngram_size (0 = off)
+  // per-utterance search options (host arrays indexed like max_new_host, from u0): beam is then the largest of beam_host
+  // over the slice, and max_hyp / lp are unused
+  int mixed = 0;
+  const int* beam_host = nullptr;
+  const int* max_hyp_host = nullptr;
+  const float* lp_host = nullptr;
 };
 
 SearchArgs make_search_args(wisb_handle* h, const DecodeCfg& c) {
@@ -842,6 +852,11 @@ SearchArgs make_search_args(wisb_handle* h, const DecodeCfg& c) {
   a.max_new_u = c.per_utt_max_new ? h->max_new_u.p : nullptr;
   a.rep_penalty = c.rep_penalty;
   a.no_repeat_ngram = c.no_repeat_ngram;
+  if (c.mixed) {
+    a.beam_u = h->beam_u.p;
+    a.max_hyp_u = h->max_hyp_u.p;
+    a.lp_u = h->lp_u.p;
+  }
   if (c.ts) {
     a.ts = 1;
     a.no_ts = dm.no_timestamps;
@@ -1002,8 +1017,9 @@ void set_extra_suppress(wisb_handle* h, const int32_t* extra, int n_extra) {
   h->mask_extra = want;
 }
 
-// prompts [n_utt][prompt_len] of utterances [u0, u0 + n_utt) -> h->prompt_dev and, when c.per_utt_max_new, their caps on
-// new tokens (max_new_host[u0 + u]) -> h->max_new_u.  Both are staged through the pinned buffer, whose first 4 words hold
+// prompts [n_utt][prompt_len] of utterances [u0, u0 + n_utt) -> h->prompt_dev, when c.per_utt_max_new their caps on
+// new tokens (max_new_host[u0 + u]) -> h->max_new_u, and when c.mixed their search options -> h->beam_u / max_hyp_u /
+// lp_u.  All are staged through the pinned buffer, whose first 4 words hold
 // the step loop's flags: the host may rewrite it only after the stream sync that ends the previous group, because these
 // asynchronous copies read from it.
 void upload_prompts(wisb_handle* h, const int32_t* prompts, const int* max_new_host, const DecodeCfg& c) {
@@ -1014,6 +1030,15 @@ void upload_prompts(wisb_handle* h, const int32_t* prompts, const int* max_new_h
   if (c.per_utt_max_new) {
     memcpy(pin + n, max_new_host + c.u0, sizeof(int) * c.n_utt);
     WISB_CUDA(cudaMemcpyAsync(h->max_new_u.p, pin + n, sizeof(int) * c.n_utt, cudaMemcpyHostToDevice, h->stream));
+  }
+  if (c.mixed) {
+    int* pm = pin + n + c.n_utt;
+    memcpy(pm, c.beam_host + c.u0, sizeof(int) * c.n_utt);
+    memcpy(pm + c.n_utt, c.max_hyp_host + c.u0, sizeof(int) * c.n_utt);
+    memcpy(pm + 2 * c.n_utt, c.lp_host + c.u0, sizeof(float) * c.n_utt);
+    WISB_CUDA(cudaMemcpyAsync(h->beam_u.p, pm, sizeof(int) * c.n_utt, cudaMemcpyHostToDevice, h->stream));
+    WISB_CUDA(cudaMemcpyAsync(h->max_hyp_u.p, pm + c.n_utt, sizeof(int) * c.n_utt, cudaMemcpyHostToDevice, h->stream));
+    WISB_CUDA(cudaMemcpyAsync(h->lp_u.p, pm + 2 * c.n_utt, sizeof(float) * c.n_utt, cudaMemcpyHostToDevice, h->stream));
   }
 }
 
@@ -1326,7 +1351,8 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
       GraphKey key;
       memset(&key, 0, sizeof(key));
       key.n_utt = c.n_utt; key.beam = c.beam; key.prompt_len = c.prompt_len; key.max_new = c.max_new;
-      key.max_hyp = c.max_hyp; key.lp = c.lp; key.u0 = c.u0; key.b_total = c.B_total;
+      key.max_hyp = c.mixed ? 0 : c.max_hyp; key.lp = c.mixed ? 0.f : c.lp; key.u0 = c.u0; key.b_total = c.B_total;
+      key.mixed = c.mixed;
       key.per_utt_max_new = c.per_utt_max_new;
       key.ts = c.ts; key.ts_max_init = c.ts ? c.ts_max_init : 0;
       key.rep_penalty = c.rep_penalty; key.no_repeat_ngram = c.no_repeat_ngram;
@@ -1717,20 +1743,49 @@ int wisb_logmel(wisb_handle* h, const void* pcm, int pcm_dtype, int pcm_on_devic
   });
 }
 
-int wisb_generate_proc(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
-                       float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                       const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
-                       float repetition_penalty, int no_repeat_ngram_size, int32_t* out_ids, int out_stride,
-                       int32_t* out_len, float* out_score) {
+int wisb_generate_mixed(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
+                        float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
+                        const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
+                        float repetition_penalty, int no_repeat_ngram_size, const int32_t* beam_per_utt,
+                        const float* patience_per_utt, const float* length_penalty_per_utt, int32_t* out_ids,
+                        int out_stride, int32_t* out_len, float* out_score) {
   return guarded(h, [&] {
     const Dims& dm = h->dims;
     WISB_REQUIRE(h->blob != nullptr, "handle has no model (created by wisb_create_frontend)");
     WISB_REQUIRE(B >= 1 && B <= 4096, "B out of range");
     WISB_REQUIRE(prompts != nullptr && out_ids != nullptr && out_len != nullptr, "prompts / out_ids / out_len is NULL");
-    WISB_REQUIRE(beam_size >= 1 && beam_size <= MAX_BEAM, "beam_size must be in [1, 8]");
+    if (beam_per_utt == nullptr) WISB_REQUIRE(beam_size >= 1 && beam_size <= MAX_BEAM, "beam_size must be in [1, 8]");
     WISB_REQUIRE(prompt_len >= 1 && prompt_len <= dm.n_text_ctx, "prompt length out of range");
     WISB_REQUIRE(max_length >= 1 && max_length <= dm.n_text_ctx, "max_length must be in [1, n_text_ctx]");
-    WISB_REQUIRE(patience > 0.f, "patience must be positive");
+    if (patience_per_utt == nullptr) WISB_REQUIRE(patience > 0.f, "patience must be positive");
+    // hypotheses that finish a window: round half up of beam x patience in fp32, at least 1.  A search records at most
+    // beam hypotheses per step over at most 448 steps, so every count above 8 x 448 means "never by count"; clamping
+    // at twice that keeps a huge patience from overflowing the int conversion
+    auto max_hyp_of = [](int beam, float p) {
+      return std::max(1, static_cast<int>(std::min(beam * p + 0.5f, static_cast<float>(2 * MAX_BEAM * T_MAX))));
+    };
+    // per-window search options: beam, max_hyp and length penalty of every window, and the largest beam (the row block
+    // of every window)
+    const bool per_window = beam_per_utt != nullptr || patience_per_utt != nullptr || length_penalty_per_utt != nullptr;
+    std::vector<int> beam_w, hyp_w;
+    std::vector<float> lp_w;
+    int beam_max = beam_size;
+    if (per_window) {
+      beam_w.resize(B);
+      hyp_w.resize(B);
+      lp_w.resize(B);
+      beam_max = 1;
+      for (int b = 0; b < B; ++b) {
+        beam_w[b] = beam_per_utt ? beam_per_utt[b] : beam_size;
+        WISB_REQUIRE(beam_w[b] >= 1 && beam_w[b] <= MAX_BEAM, "per-window beam_size must be in [1, 8]");
+        const float p = patience_per_utt ? patience_per_utt[b] : patience;
+        if (patience_per_utt) WISB_REQUIRE(std::isfinite(p) && p > 0.f, "per-window patience must be finite and > 0");
+        lp_w[b] = length_penalty_per_utt ? length_penalty_per_utt[b] : length_penalty;
+        if (length_penalty_per_utt) WISB_REQUIRE(std::isfinite(lp_w[b]), "per-window length_penalty must be finite");
+        hyp_w[b] = max_hyp_of(beam_w[b], p);
+        beam_max = std::max(beam_max, beam_w[b]);
+      }
+    }
     WISB_REQUIRE(n_extra >= 0 && (n_extra == 0 || extra_suppress != nullptr), "bad extra_suppress");
     for (long long i = 0; i < static_cast<long long>(B) * prompt_len; ++i)
       WISB_REQUIRE(prompts[i] >= 0 && prompts[i] < dm.n_vocab, "prompt token outside the vocabulary");
@@ -1771,11 +1826,7 @@ int wisb_generate_proc(wisb_handle* h, const float* mel, int B, const int32_t* p
     set_extra_suppress(h, extra_suppress, n_extra);
     time_h2d(h);
     DecodeCfg c;
-    c.beam = beam_size;
     c.prompt_len = prompt_len;
-    c.max_hyp = static_cast<int>(beam_size * patience + 0.5f);
-    if (c.max_hyp < 1) c.max_hyp = 1;
-    c.lp = length_penalty;
     c.ts = timestamps;
     c.ts_max_init = max_initial_timestamp_index;
     c.rep_penalty = repetition_penalty;
@@ -1783,8 +1834,8 @@ int wisb_generate_proc(wisb_handle* h, const float* mel, int B, const int32_t* p
     // Utterances are encoded and decoded in groups that share every decoder pass: the group's rows (utterances x beams)
     // are the M dimension of the batched pass, so the decoder weights stream once per generated token for the whole
     // group.  The group size only bounds the workspaces (cross K/V: 252 MB per large-v2 utterance).
-    const bool persistent = use_persistent_pass(h, B * beam_size);
-    int group = persistent ? B : h->batch_rows / beam_size;
+    const bool persistent = use_persistent_pass(h, B * beam_max);
+    int group = persistent ? B : h->batch_rows / beam_max;
     if (group < 1) group = 1;
     int steps = 0;
     for (int g0 = 0; g0 < B; g0 += group) {
@@ -1793,6 +1844,24 @@ int wisb_generate_proc(wisb_handle* h, const float* mel, int B, const int32_t* p
       c.u0 = 0;
       c.n_utt = n;
       c.B_total = n;
+      // a group whose windows agree on every search option runs the scalar search, else the per-utterance one with
+      // the group's largest beam as the row block
+      c.beam = beam_size;
+      c.max_hyp = max_hyp_of(beam_size, patience);
+      c.lp = length_penalty;
+      c.mixed = 0;
+      if (per_window) {
+        c.beam = beam_w[g0];
+        c.max_hyp = hyp_w[g0];
+        c.lp = lp_w[g0];
+        for (int u = g0 + 1; u < g0 + n; ++u) {
+          if (beam_w[u] != beam_w[g0] || hyp_w[u] != hyp_w[g0] || lp_w[u] != lp_w[g0]) c.mixed = 1;
+          c.beam = std::max(c.beam, beam_w[u]);
+        }
+        c.beam_host = beam_w.data() + g0;
+        c.max_hyp_host = hyp_w.data() + g0;
+        c.lp_host = lp_w.data() + g0;
+      }
       c.max_new = max_new;
       c.per_utt_max_new = 0;
       if (!per_utt.empty()) {
@@ -1813,6 +1882,17 @@ int wisb_generate_proc(wisb_handle* h, const float* mel, int B, const int32_t* p
     h->timing[7] = static_cast<float>(h->launches);
     h->prof_collect();
   });
+}
+
+int wisb_generate_proc(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
+                       float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
+                       const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
+                       float repetition_penalty, int no_repeat_ngram_size, int32_t* out_ids, int out_stride,
+                       int32_t* out_len, float* out_score) {
+  return wisb_generate_mixed(h, mel, B, prompts, prompt_len, beam_size, patience, length_penalty, max_length,
+                             max_length_per_utt, extra_suppress, n_extra, timestamps, max_initial_timestamp_index,
+                             repetition_penalty, no_repeat_ngram_size, nullptr, nullptr, nullptr, out_ids, out_stride,
+                             out_len, out_score);
 }
 
 int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
@@ -2115,9 +2195,11 @@ int wisb_debug_gemm(wisb_handle* h, const int32_t* prm, int n_prm, const uint16_
   });
 }
 
-int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, float length_penalty, const float* logits,
-                           const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
-                           float* state_f, int32_t* cand_idx, float* cand_score, float* row_lse) {
+// wisb_debug_search_step's body; beam_u / max_hyp_u / lp_u (all three or none): wisb_debug_search_step_mixed
+static int debug_search_step_impl(wisb_handle* h, const int32_t* prm, int n_prm, float length_penalty, const float* logits,
+                                  const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
+                                  float* state_f, int32_t* cand_idx, float* cand_score, float* row_lse,
+                                  const int32_t* beam_u, const int32_t* max_hyp_u, const float* lp_u) {
   return guarded(h, [&] {
     WISB_REQUIRE(prm != nullptr && (n_prm == 13 || n_prm == 15) && logits && mask && state_i && state_f && cand_idx && cand_score && row_lse,
                  "debug_search_step: bad arguments");
@@ -2166,11 +2248,19 @@ int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, float 
     if (max_new_u)
       for (int u = 0; u < n_utt; ++u)
         WISB_REQUIRE(max_new_u[u] >= 0 && max_new_u[u] <= max_new, "debug_search_step: per-utterance cap outside [0, max_new]");
+    const bool mixed = beam_u != nullptr;
+    if (mixed) {
+      WISB_REQUIRE(max_hyp_u != nullptr && lp_u != nullptr, "debug_search_step: beam_u / max_hyp_u / lp_u come as a set");
+      for (int u = 0; u < n_utt; ++u)
+        WISB_REQUIRE(beam_u[u] >= 1 && beam_u[u] <= beam && max_hyp_u[u] >= 1 && std::isfinite(lp_u[u]),
+                     "debug_search_step: per-utterance beam outside [1, beam], max_hyp < 1 or length penalty not finite");
+    }
     cudaStream_t s = h->stream;
     DevBuf<float> d_logits, d_lse, d_pmax, d_psum, d_f, d_cs;
     DevBuf<unsigned long long> d_part;
     DevBuf<uint8_t> d_mask;
-    DevBuf<int> d_i, d_ci, d_cap, d_prompt, d_slot;
+    DevBuf<int> d_i, d_ci, d_cap, d_prompt, d_slot, d_beam, d_hyp;
+    DevBuf<float> d_lp;
     d_logits.ensure(static_cast<size_t>(R) * ldl);
     d_mask.ensure(V);
     d_pmax.ensure(static_cast<size_t>(R) * (TOPK_CHUNKS + 1));
@@ -2189,6 +2279,14 @@ int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, float 
     if (max_new_u) {
       d_cap.ensure(n_utt);
       WISB_CUDA(cudaMemcpyAsync(d_cap.p, max_new_u, sizeof(int) * n_utt, cudaMemcpyHostToDevice, s));
+    }
+    if (mixed) {
+      d_beam.ensure(n_utt);
+      d_hyp.ensure(n_utt);
+      d_lp.ensure(n_utt);
+      WISB_CUDA(cudaMemcpyAsync(d_beam.p, beam_u, sizeof(int) * n_utt, cudaMemcpyHostToDevice, s));
+      WISB_CUDA(cudaMemcpyAsync(d_hyp.p, max_hyp_u, sizeof(int) * n_utt, cudaMemcpyHostToDevice, s));
+      WISB_CUDA(cudaMemcpyAsync(d_lp.p, lp_u, sizeof(float) * n_utt, cudaMemcpyHostToDevice, s));
     }
     if (init) {
       d_prompt.ensure(static_cast<size_t>(n_utt) * prompt_len);
@@ -2238,6 +2336,11 @@ int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, float 
     a.max_new_u = max_new_u ? d_cap.p : nullptr;
     a.rep_penalty = rep_penalty;
     a.no_repeat_ngram = no_repeat_ngram;
+    if (mixed) {
+      a.beam_u = d_beam.p;
+      a.max_hyp_u = d_hyp.p;
+      a.lp_u = d_lp.p;
+    }
     static_assert(sizeof(DecState) == 5 * sizeof(int), "DecState is five ints");
     if (init) search_init_run(a, d_prompt.p, s, init - 1);
     search_step_run(a, s);  // the production step: processors, top-k partials, merge, bookkeeping and step advance
@@ -2248,6 +2351,25 @@ int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, float 
     WISB_CUDA(cudaMemcpyAsync(row_lse, d_lse.p, sizeof(float) * R, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaStreamSynchronize(s));
   });
+}
+
+int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, float length_penalty, const float* logits,
+                           const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
+                           float* state_f, int32_t* cand_idx, float* cand_score, float* row_lse) {
+  return debug_search_step_impl(h, prm, n_prm, length_penalty, logits, mask, max_new_u, prompt, state_i, state_f, cand_idx,
+                                cand_score, row_lse, nullptr, nullptr, nullptr);
+}
+
+int wisb_debug_search_step_mixed(wisb_handle* h, const int32_t* prm, int n_prm, const float* logits, const uint8_t* mask,
+                                 const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i, float* state_f,
+                                 int32_t* cand_idx, float* cand_score, float* row_lse, const int32_t* beam_u,
+                                 const int32_t* max_hyp_u, const float* length_penalty_u) {
+  if (beam_u == nullptr || max_hyp_u == nullptr || length_penalty_u == nullptr) {
+    g_last_error = "debug_search_step_mixed: beam_u / max_hyp_u / length_penalty_u is NULL";
+    return 1;
+  }
+  return debug_search_step_impl(h, prm, n_prm, 1.f, logits, mask, max_new_u, prompt, state_i, state_f, cand_idx,
+                                cand_score, row_lse, beam_u, max_hyp_u, length_penalty_u);
 }
 
 // wisb_align's body; cap_out (wisb_debug_align_capture) receives the raw capture buffer [B][A][n_max + 1][F_max]

@@ -31,6 +31,13 @@
 //     is bit-exact; an id the masks turn off is -inf whatever the processors did.
 // They run in the topk_partial_kernel<NCH, true> instantiation, picked only when one is on: each (chunk, row) block
 // stages hist in shared memory and flags its chunk's ids before it reads the logits.
+// Per-utterance beam, patience and length penalty (SearchArgs::beam_u; a call that mixes windows with different search
+// options): every utterance keeps a block of `beam` rows (the call's largest beam B) and searches only its first b_u
+// rows, with 2 b_u candidates, its own max_hyp and length penalty; rows b_u .. B - 1 are dead from search_init on (eot,
+// cum -inf) and never become a candidate or a hypothesis.  topk_partial_kernel is shared: it still emits 2 B partials
+// per chunk, of which the merge takes the first 2 b_u (a chunk's partials are sorted, so this is the chunk's top 2 b_u).
+// Only the search_tail_kernel<NCH, true> / search_init_kernel<true> instantiations read the per-utterance arrays; a call
+// whose windows agree runs the <false> ones.
 #include "decoder.cuh"
 
 namespace wisb {
@@ -254,7 +261,7 @@ __global__ void __launch_bounds__(TK_THREADS) topk_partial_kernel(const SearchAr
 template <int NCH>
 constexpr int tm_per() { return (MAX_BEAM * NCH * MAX_CAND + TK_THREADS - 1) / TK_THREADS; }  // 16 / 17
 
-template <int NCH>
+template <int NCH, bool MIXED>
 __device__ __forceinline__ void topk_merge_body(const SearchArgs& a, unsigned long long* s_red, unsigned long long* s_out,
                                                 float* s_lse, int* s_ts_only) {
   constexpr bool TS = NCH > TOPK_CHUNKS;
@@ -262,8 +269,12 @@ __device__ __forceinline__ void topk_merge_body(const SearchArgs& a, unsigned lo
   const int u = blockIdx.x;
   const int gen = a.st->gen_step;
   const bool first = gen == 0;
-  const float norm = (a.length_penalty != 0.f) ? powf(static_cast<float>(gen + 1), a.length_penalty) : 1.f;
-  if (threadIdx.x < a.beam) {  // row log-sum-exp from the chunk partials
+  // rows of the utterance's block that it searches, candidates it keeps, its length penalty (MIXED: its own)
+  const int beam = MIXED ? a.beam_u[u] : a.beam;
+  const int n_cand = MIXED ? 2 * beam : a.n_cand;
+  const float lp = MIXED ? a.lp_u[u] : a.length_penalty;
+  const float norm = (lp != 0.f) ? powf(static_cast<float>(gen + 1), lp) : 1.f;
+  if (threadIdx.x < beam) {  // row log-sum-exp from the chunk partials
     const int r = u * a.beam + threadIdx.x;
     float mx = -INFINITY;
     for (int c = 0; c < NCH; ++c) mx = fmaxf(mx, a.part_max[r * NCH + c]);
@@ -287,15 +298,15 @@ __device__ __forceinline__ void topk_merge_body(const SearchArgs& a, unsigned lo
     a.row_lse[r] = lse;
   }
   __syncthreads();
-  const int total = a.beam * NCH * a.n_cand;
+  const int total = beam * NCH * n_cand;
   unsigned long long keys[TM_PER];
 #pragma unroll
   for (int i = 0; i < TM_PER; ++i) {
     const int j = threadIdx.x + i * TK_THREADS;
     keys[i] = 0ull;
     if (j < total) {
-      const int c = j % a.n_cand;
-      const int rc = j / a.n_cand;       // (beam row, chunk)
+      const int c = j % n_cand;          // (MIXED: the chunk's first n_cand of its a.n_cand sorted partials)
+      const int rc = j / n_cand;         // (beam row, chunk)
       const int k = rc / NCH;            // beam index
       const unsigned long long pk = a.part[(static_cast<long long>(u * a.beam) * NCH + rc) * MAX_CAND + c];
       // at the first step every beam holds the same prefix: only beam 0 counts
@@ -308,11 +319,11 @@ __device__ __forceinline__ void topk_merge_body(const SearchArgs& a, unsigned lo
       }
     }
   }
-  block_select<TM_PER>(keys, a.n_cand, s_out, s_red);
+  block_select<TM_PER>(keys, n_cand, s_out, s_red);
   __syncthreads();
-  if (threadIdx.x < a.n_cand) {
+  if (threadIdx.x < a.n_cand) {  // (MIXED: entries n_cand .. a.n_cand - 1 are none)
     const unsigned long long key = s_out[threadIdx.x];
-    const bool valid = key != 0ull;
+    const bool valid = key != 0ull && (!MIXED || static_cast<int>(threadIdx.x) < n_cand);
     a.cand_score[u * MAX_CAND + threadIdx.x] = valid ? ord2f(static_cast<unsigned>(key >> 32)) : -INFINITY;
     a.cand_idx[u * MAX_CAND + threadIdx.x] = valid ? static_cast<int>(~static_cast<unsigned>(key & 0xffffffffull)) : -1;
   }
@@ -320,9 +331,11 @@ __device__ __forceinline__ void topk_merge_body(const SearchArgs& a, unsigned lo
 
 // ---------------------------------------------------------------------------------------------------------------------
 // one warp: the CTranslate2 bookkeeping for one utterance
+template <bool MIXED>
 __device__ __forceinline__ void search_bookkeeping_body(const SearchArgs& a, int* s_pick, int& s_best_k, int& s_finished) {
   const int u = blockIdx.x, lane = threadIdx.x;
-  const int beam = a.beam, V = a.n_vocab, nc = a.n_cand;
+  const int rows = a.beam;  // row block of an utterance
+  const int beam = MIXED ? a.beam_u[u] : a.beam, V = a.n_vocab, nc = MIXED ? 2 * beam : a.n_cand;
   const int gen = a.st->gen_step, pos = a.st->pos;
   const int cur = *a.flip, nxt_buf = cur ^ 1;
   const int* seq_cur = a.seq[cur];
@@ -332,8 +345,8 @@ __device__ __forceinline__ void search_bookkeeping_body(const SearchArgs& a, int
 
   if (a.done[u]) {
     // frozen utterance: carry the state over unchanged so the ping-pong buffers stay coherent
-    for (int k = 0; k < beam; ++k) {
-      const int r = u * beam + k;
+    for (int k = 0; k < rows; ++k) {
+      const int r = u * rows + k;
       for (int t = lane; t < a.max_new; t += 32) seq_nxt[r * a.max_new + t] = seq_cur[r * a.max_new + t];
       for (int t = lane; t < a.t_max; t += 32) ind_nxt[r * a.t_max + t] = (t == pos) ? r : ind_cur[r * a.t_max + t];
     }
@@ -344,7 +357,8 @@ __device__ __forceinline__ void search_bookkeeping_body(const SearchArgs& a, int
   const int cap = a.max_new_u != nullptr ? a.max_new_u[u] : a.max_new;
   const bool is_last = gen + 1 >= cap;
   const bool capped = gen >= cap;  // a cap of 0 new tokens: the utterance finishes without a hypothesis
-  const float norm = (a.length_penalty != 0.f) ? powf(static_cast<float>(gen + 1), a.length_penalty) : 1.f;
+  const float lp = MIXED ? a.lp_u[u] : a.length_penalty;
+  const float norm = (lp != 0.f) ? powf(static_cast<float>(gen + 1), lp) : 1.f;
   if (lane == 0) {
     int n_hyp = a.n_hyp[u];
     float best = a.best_score[u];
@@ -373,7 +387,7 @@ __device__ __forceinline__ void search_bookkeeping_body(const SearchArgs& a, int
     a.n_hyp[u] = n_hyp;
     a.best_score[u] = best;
     s_best_k = best_k;
-    const int fin = (is_last || n_hyp >= a.max_hyp) ? 1 : 0;
+    const int fin = (is_last || n_hyp >= (MIXED ? a.max_hyp_u[u] : a.max_hyp)) ? 1 : 0;
     s_finished = fin;
     if (fin) {
       a.done[u] = 1;
@@ -385,7 +399,7 @@ __device__ __forceinline__ void search_bookkeeping_body(const SearchArgs& a, int
     const int k = s_best_k;
     const int idx = ci[k];
     const int parent = idx / V, tok = idx % V;
-    const int pr = u * beam + parent;
+    const int pr = u * rows + parent;
     for (int t = lane; t < gen; t += 32) a.best_tokens[u * a.max_new + t] = seq_cur[pr * a.max_new + t];
     if (lane == 0) {
       int len = gen;
@@ -396,13 +410,14 @@ __device__ __forceinline__ void search_bookkeeping_body(const SearchArgs& a, int
       a.best_len[u] = len;
     }
   }
-  // next alive beams (also written when finished: harmless, keeps buffers defined)
-  for (int k = 0; k < beam; ++k) {
-    const int r = u * beam + k;
-    const int idx = ci[s_pick[k]];
+  // next alive beams (also written when finished: harmless, keeps buffers defined); a row the utterance does not search
+  // carries itself over as a dead row
+  for (int k = 0; k < rows; ++k) {
+    const int r = u * rows + k;
+    const int idx = (!MIXED || k < beam) ? ci[s_pick[k]] : -1;
     const int parent = idx < 0 ? k : idx / V;
     const int tok = idx < 0 ? a.eot : idx % V;
-    const int pr = u * beam + parent;
+    const int pr = u * rows + parent;
     for (int t = lane; t < gen; t += 32) seq_nxt[r * a.max_new + t] = seq_cur[pr * a.max_new + t];
     for (int t = lane; t < pos; t += 32) ind_nxt[r * a.t_max + t] = ind_cur[pr * a.t_max + t];
     if (lane == 0) {
@@ -417,7 +432,7 @@ __device__ __forceinline__ void search_bookkeeping_body(const SearchArgs& a, int
 // grid (n_utt) x TK_THREADS: candidate merge, then (warp 0) the bookkeeping of the utterance, then -- by the last CTA to get
 // there -- the step advance (position, generation step, ping-pong flip, per-row positions).  One launch instead of three:
 // the tail of a decoding step is launch-latency bound.
-template <int NCH>
+template <int NCH, bool MIXED>
 __global__ void __launch_bounds__(TK_THREADS) search_tail_kernel(const SearchArgs a) {
   __shared__ unsigned long long s_red[32];
   __shared__ unsigned long long s_out[MAX_CAND];
@@ -428,9 +443,9 @@ __global__ void __launch_bounds__(TK_THREADS) search_tail_kernel(const SearchArg
   __shared__ int s_finished;
   __shared__ int s_last;
   if (a.st->all_done) return;  // a step enqueued ahead of the host's poll: nothing left to do
-  topk_merge_body<NCH>(a, s_red, s_out, s_lse, s_ts_only);
+  topk_merge_body<NCH, MIXED>(a, s_red, s_out, s_lse, s_ts_only);
   __syncthreads();  // the candidate list (global) is complete for this CTA's readers
-  if (threadIdx.x < 32) search_bookkeeping_body(a, s_pick, s_best_k, s_finished);
+  if (threadIdx.x < 32) search_bookkeeping_body<MIXED>(a, s_pick, s_best_k, s_finished);
   __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence();
@@ -472,7 +487,8 @@ __global__ void prefill_advance_kernel(int* tokens, const int* prompt, int promp
 
 // shared_prefix: the prompt prefix (all but the last prompt token) is forwarded once per utterance into the cache slot of
 // its first beam by a single prefill pass; decoding then starts at the last prompt token and every beam's indirection
-// points at that slot.
+// points at that slot.  MIXED: rows an utterance does not search start dead (eot, cum -inf).
+template <bool MIXED>
 __global__ void search_init_kernel(const SearchArgs a, const int* prompt, int shared_prefix) {
   const int R = a.n_utt * a.beam;
   const int tid = blockIdx.x * blockDim.x + threadIdx.x, n = gridDim.x * blockDim.x;
@@ -485,8 +501,9 @@ __global__ void search_init_kernel(const SearchArgs a, const int* prompt, int sh
     *a.flip = 0;
   }
   for (int i = tid; i < R; i += n) {
-    a.tokens[i] = prompt[(i / a.beam) * a.prompt_len + (shared_prefix ? a.prompt_len - 1 : 0)];
-    a.cum[i] = 0.f;
+    const bool dead = MIXED && i % a.beam >= a.beam_u[i / a.beam];
+    a.tokens[i] = dead ? a.eot : prompt[(i / a.beam) * a.prompt_len + (shared_prefix ? a.prompt_len - 1 : 0)];
+    a.cum[i] = dead ? -INFINITY : 0.f;
     if (a.row_pos != nullptr) {
       a.row_pos[i] = shared_prefix ? a.prompt_len - 1 : 0;
       a.row_slot[i] = i;
@@ -537,18 +554,26 @@ void search_step_run(const SearchArgs& a, cudaStream_t stream) {
   const bool hist = a.rep_penalty != 1.f || a.no_repeat_ngram > 0;
   WISB_REQUIRE(!hist || (a.max_new <= HIST_MAX && a.rep_penalty > 0.f && a.no_repeat_ngram >= 0),
                "search: bad history processor arguments");
+  const bool mixed = a.beam_u != nullptr;
+  WISB_REQUIRE(!mixed || (a.max_hyp_u != nullptr && a.lp_u != nullptr), "search: per-utterance options come as a set");
   if (a.ts) {
     if (hist)
       topk_partial_kernel<TOPK_CHUNKS + 1, true><<<dim3(TOPK_CHUNKS + 1, R), TK_THREADS, 0, stream>>>(a);
     else
       topk_partial_kernel<TOPK_CHUNKS + 1, false><<<dim3(TOPK_CHUNKS + 1, R), TK_THREADS, 0, stream>>>(a);
-    search_tail_kernel<TOPK_CHUNKS + 1><<<a.n_utt, TK_THREADS, 0, stream>>>(a);
+    if (mixed)
+      search_tail_kernel<TOPK_CHUNKS + 1, true><<<a.n_utt, TK_THREADS, 0, stream>>>(a);
+    else
+      search_tail_kernel<TOPK_CHUNKS + 1, false><<<a.n_utt, TK_THREADS, 0, stream>>>(a);
   } else {
     if (hist)
       topk_partial_kernel<TOPK_CHUNKS, true><<<dim3(TOPK_CHUNKS, R), TK_THREADS, 0, stream>>>(a);
     else
       topk_partial_kernel<TOPK_CHUNKS, false><<<dim3(TOPK_CHUNKS, R), TK_THREADS, 0, stream>>>(a);
-    search_tail_kernel<TOPK_CHUNKS><<<a.n_utt, TK_THREADS, 0, stream>>>(a);
+    if (mixed)
+      search_tail_kernel<TOPK_CHUNKS, true><<<a.n_utt, TK_THREADS, 0, stream>>>(a);
+    else
+      search_tail_kernel<TOPK_CHUNKS, false><<<a.n_utt, TK_THREADS, 0, stream>>>(a);
   }
   WISB_CUDA(cudaGetLastError());
 }
@@ -566,7 +591,10 @@ void prefill_advance_run(int* tokens, const int* prompt, int prompt_len, int R, 
 }
 
 void search_init_run(const SearchArgs& a, const int* prompt, cudaStream_t stream, int shared_prefix) {
-  search_init_kernel<<<8, 256, 0, stream>>>(a, prompt, shared_prefix);
+  if (a.beam_u != nullptr)
+    search_init_kernel<true><<<8, 256, 0, stream>>>(a, prompt, shared_prefix);
+  else
+    search_init_kernel<false><<<8, 256, 0, stream>>>(a, prompt, shared_prefix);
   WISB_CUDA(cudaGetLastError());
 }
 

@@ -129,6 +129,10 @@ class _Input:
 
 
 class Whisper:
+    # generate takes one prompt per window and beam_size / patience / length_penalty / max_length as one value per window:
+    # batcher.TranscribeBatcher puts requests that differ in those into one call
+    per_window_options = True
+
     def __init__(self, model_path, device: str = "cuda", *, device_index=0, compute_type: str = "default",
                  inter_threads: int = 1, intra_threads: int = 0, max_queued_batches: int = 0, files=None,
                  reuse_encoder=None, _handles=None, **_ignored):
@@ -320,13 +324,33 @@ class Whisper:
         ml = None if np.isscalar(max_length) else np.asarray(max_length, np.int32)
         if ml is not None and ml.shape != (n,):
             raise ValueError("max_length must be an int or one int per feature window")
+        # the same extension for the search options: each window searches with its own beam, patience and length
+        # penalty, as it would in a call of its own (prompts already come per window)
+        search = {"beam_size": beam_size, "patience": patience, "length_penalty": length_penalty}
+        for name, v in search.items():
+            if np.isscalar(v):
+                continue
+            a = np.asarray(v)
+            kinds = "iu" if name == "beam_size" else "iuf"
+            if a.shape != (n,) or a.dtype.kind not in kinds:
+                raise ValueError(f"{name} must be a scalar or one {'int' if name == 'beam_size' else 'number'} per "
+                                 "feature window")
+            if name == "beam_size" and ((a < 1) | (a > 8)).any():
+                raise ValueError("beam_size must be in [1, 8]")
+            if name == "patience" and not (np.isfinite(a) & (a > 0)).all():
+                raise ValueError("patience must be finite and > 0")
+            if name == "length_penalty" and not np.isfinite(a).all():
+                raise ValueError("length_penalty must be finite")
+            search[name] = a
+        window = lambda v, s, e: v if np.isscalar(v) else v[s:e]  # noqa: E731
 
         proc = {}
         if repetition_penalty != 1 or no_repeat_ngram_size != 0:
             proc = dict(repetition_penalty=float(repetition_penalty), no_repeat_ngram_size=int(no_repeat_ngram_size))
 
         def run(h, mel, s, e):
-            return h.generate(mel, p[s:e], beam_size, patience, length_penalty, max_length if ml is None else ml[s:e],
+            return h.generate(mel, p[s:e], window(search["beam_size"], s, e), window(search["patience"], s, e),
+                              window(search["length_penalty"], s, e), max_length if ml is None else ml[s:e],
                               extra, B=e - s, timestamps=timestamps,
                               max_initial_timestamp_index=int(max_initial_timestamp_index), **proc)
 
