@@ -113,6 +113,22 @@ int wisb_generate_mixed(wisb_handle* h, const float* mel, int B, const int32_t* 
                         const float* patience_per_utt, const float* length_penalty_per_utt, int32_t* out_ids,
                         int out_stride, int32_t* out_len, float* out_score);
 
+/* Sampling (CTranslate2's generate with beam_size 1 and sampling_topk != 1): every window draws num_hypotheses (in
+ * [1, 8]) independent hypotheses from softmax(l_S / sampling_temperature) (finite, > 0) over the processed logits l,
+ * S = every token (sampling_topk 0) or the sampling_topk (in [2, 16]) largest, with Gumbel-max noise from Philox4x32-10
+ * keyed by seeds[b] (uint64 [B]).  The result depends only on the window's features, prompt, options and seed, not on
+ * its batch position.  Scores are the untempered cumulative log-probs over (generated tokens)^length_penalty.  Outputs
+ * hold num_hypotheses entries per window, window b's at [b * num_hypotheses, (b + 1) * num_hypotheses), sorted by score
+ * (descending, ties to the lower hypothesis index): out_ids int32 [B * n, out_stride], out_len int32 [B * n], out_score
+ * float32 [B * n] (required).  A hypothesis that found no token to sample is empty with score -inf; a cap of 0 new tokens
+ * gives n empty ones with score 0.  The other arguments are those of wisb_generate_proc.  Code 1 for a bad argument. */
+int wisb_generate_sample(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len,
+                         int num_hypotheses, int sampling_topk, float sampling_temperature, const uint64_t* seeds,
+                         float length_penalty, int max_length, const int32_t* max_length_per_utt,
+                         const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
+                         float repetition_penalty, int no_repeat_ngram_size, int32_t* out_ids, int out_stride,
+                         int32_t* out_len, float* out_score);
+
 /* (5) per utterance: language token ids sorted by probability (descending) and the probabilities.
  * lang_ids_out int32 [B, n_langs], probs_out float32 [B, n_langs]. */
 int wisb_detect_language(wisb_handle* h, const float* mel, int B, int32_t* lang_ids_out, float* probs_out);
@@ -212,6 +228,15 @@ int wisb_debug_search_step_mixed(wisb_handle* h, const int32_t* prm, int n_prm, 
                                  const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i, float* state_f,
                                  int32_t* cand_idx, float* cand_score, float* row_lse, const int32_t* beam_u,
                                  const int32_t* max_hyp_u, const float* length_penalty_u);
+/* One production sampling step (wisb_generate_sample): prm as for wisb_debug_search_step with prm[1] = the hypotheses
+ * n per utterance (prm[9] >= 1 unused), seeds uint64 [n_utt].  state_i / state_f as there, except best_len [R],
+ * best_tokens [R][max_new] and best_score [R]: one hypothesis per row.  Outputs: sampled int32 [R] (the token row r
+ * drew, -1 = none: the row was dead, frozen or had nothing to sample), key float32 [R] (its Gumbel key), row_lse
+ * float32 [R]. */
+int wisb_debug_search_step_sample(wisb_handle* h, const int32_t* prm, int n_prm, float length_penalty, int sampling_topk,
+                                  float sampling_temperature, const uint64_t* seeds, const float* logits,
+                                  const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
+                                  float* state_f, int32_t* sampled, float* key, float* row_lse);
 /* encoder self-attention on caller data: qkv [B*1536, 3d] fp16 -> ctx [B*1536, d] fp16, d = 64 H; impl 0 = wgmma with
  * MN-major V, 1 = wgmma with the transposed Vt layout (built from the same qkv), 2 = SIMT check */
 int wisb_debug_enc_attn(wisb_handle* h, const uint16_t* qkv16, int B, int d, int H, int impl, uint16_t* ctx16_out);

@@ -9,8 +9,8 @@ Everything numeric runs in libwisb200.so (hand-written sm_90a CUDA, include/wisb
 host-side mirror of the reference's Python surface.  Importing it does not need a GPU; calling it does.
 """
 from . import audio, models, weights  # noqa: F401
-from .models import StorageView, Whisper, WhisperGenerationResult, get_supported_compute_types  # noqa: F401
+from .models import StorageView, Whisper, WhisperGenerationResult, get_supported_compute_types, set_random_seed  # noqa: F401
 
 __all__ = ["audio", "models", "weights", "StorageView", "Whisper", "WhisperGenerationResult",
-           "get_supported_compute_types"]
+           "get_supported_compute_types", "set_random_seed"]
 __version__ = "0.1.0"

@@ -46,6 +46,9 @@ _SIGS = {
     "wisb_generate_mixed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
                                       C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "wisb_generate_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float,
+                                       C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                       C.c_float, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_detect_language": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_buffer_alloc": (C.c_int, [C.c_int, C.c_size_t, C.POINTER(C.c_void_p)]),
     "wisb_buffer_free": (C.c_int, [C.c_void_p]),
@@ -68,6 +71,9 @@ _SIGS = {
     "wisb_debug_search_step_mixed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wisb_debug_search_step_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_float,
+                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_enc_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "wisb_debug_dec_cross_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_dec_self_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -283,6 +289,44 @@ class Handle:
                                          ptr(scores)))
         return [ids[b, : lens[b]].tolist() for b in range(B)], scores.tolist()
 
+    def generate_sample(self, mel, prompts, num_hypotheses, sampling_topk, sampling_temperature, seeds,
+                        length_penalty=1.0, max_length=448, extra_suppress=(), B=None, timestamps=False,
+                        max_initial_timestamp_index=50, repetition_penalty=1.0, no_repeat_ngram_size=0):
+        """wisb_generate_sample: num_hypotheses sampled hypotheses per window, window b seeded by seeds[b] (uint64) ->
+        (per window the n token lists, per window the n scores), each window's sorted by score, descending."""
+        prompts = np.ascontiguousarray(prompts, np.int32)
+        if prompts.ndim != 2:
+            raise ValueError("prompts must be [B, prompt_len]")
+        if mel is not None:
+            self._check_features(mel)
+            B = mel.shape[0]
+        if B is None or prompts.shape[0] != B:
+            raise ValueError("one prompt per feature window is required")
+        seeds = np.asarray(seeds)
+        if seeds.shape != (B,) or seeds.dtype != np.uint64:
+            raise ValueError("seeds must be a uint64 array with one seed per window")
+        seeds = np.ascontiguousarray(seeds)
+        per_utt = None
+        if not np.isscalar(max_length):
+            per_utt = np.ascontiguousarray(max_length, np.int32)
+            if per_utt.shape != (B,):
+                raise ValueError("max_length must be an int or one int per utterance")
+            max_length = int(per_utt.max())
+        n = int(num_hypotheses)
+        stride = max(1, int(max_length) // 2)
+        ids = np.zeros((B * n, stride), np.int32)
+        lens = np.zeros(B * n, np.int32)
+        scores = np.zeros(B * n, np.float32)
+        extra = np.ascontiguousarray(list(extra_suppress), np.int32)
+        check(lib().wisb_generate_sample(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], n, int(sampling_topk),
+                                         float(sampling_temperature), ptr(seeds), float(length_penalty), int(max_length),
+                                         ptr(per_utt), ptr(extra) if extra.size else None, extra.size,
+                                         1 if timestamps else 0, int(max_initial_timestamp_index),
+                                         float(repetition_penalty), int(no_repeat_ngram_size), ptr(ids), stride,
+                                         ptr(lens), ptr(scores)))
+        seqs = [ids[i, : lens[i]].tolist() for i in range(B * n)]
+        return [seqs[b * n: (b + 1) * n] for b in range(B)], [scores[b * n: (b + 1) * n].tolist() for b in range(B)]
+
     def detect_language(self, mel, B=None):
         if mel is not None:
             self._check_features(mel)
@@ -440,15 +484,17 @@ class Handle:
         return out
 
     @staticmethod
-    def search_state(n_utt: int, beam: int, max_new: int, t_max: int) -> dict:
-        """A zeroed search state for debug_search_step_state (best_score -inf): name -> array, in the entry's order."""
+    def search_state(n_utt: int, beam: int, max_new: int, t_max: int, sample: bool = False) -> dict:
+        """A zeroed search state for debug_search_step_state (best_score -inf): name -> array, in the entry's order.
+        sample: the layout of debug_search_step_sample (beam = the hypotheses; best_* per row)."""
         R = n_utt * beam
+        H = R if sample else n_utt
         return {"st": np.zeros(5, np.int32), "flip": np.zeros(1, np.int32),   # DecState: pos, gen_step, n_done, all_done, ticket
                 "seq": np.zeros((2, R, max_new), np.int32), "indir": np.zeros((2, R, t_max), np.int32),
                 "tokens": np.zeros(R, np.int32), "row_pos": np.zeros(R, np.int32), "done": np.zeros(n_utt, np.int32),
-                "n_hyp": np.zeros(n_utt, np.int32), "best_len": np.zeros(n_utt, np.int32),
-                "best_tokens": np.zeros((n_utt, max_new), np.int32),
-                "cum": np.zeros(R, np.float32), "best_score": np.full(n_utt, -np.inf, np.float32)}
+                "n_hyp": np.zeros(n_utt, np.int32), "best_len": np.zeros(H, np.int32),
+                "best_tokens": np.zeros((H, max_new), np.int32),
+                "cum": np.zeros(R, np.float32), "best_score": np.full(H, -np.inf, np.float32)}
 
     _STATE_F = ("cum", "best_score")
 
@@ -540,6 +586,54 @@ class Handle:
             else:
                 out[k], oi = si[oi : oi + v.size].reshape(v.shape).copy(), oi + v.size
         return out, ci[:, : 2 * beam], cs[:, : 2 * beam], lse
+
+    def debug_search_step_sample(self, logits, mask, state, seeds, *, n: int, sampling_topk: int,
+                                 sampling_temperature: float, eot: int, V: int = 0, no_timestamps: int = 0,
+                                 timestamps: bool = False, max_initial_timestamp_index: int = 50,
+                                 length_penalty: float = 1.0, max_new_u=None, prompt=None, shared_prefix: int = 0,
+                                 repetition_penalty=None, no_repeat_ngram_size=None):
+        """One production sampling step on caller state (wisb_debug_search_step_sample).  As debug_search_step_state
+        with n hypotheses per utterance, the state made by search_state(..., sample=True) and seeds uint64 [n_utt].
+        -> (new state, sampled int32 [R] (-1 = none), key float32 [R], row_lse float32 [R])."""
+        logits = np.ascontiguousarray(logits, np.float32)
+        R, ldl = logits.shape
+        V = V or ldl
+        if R % n:
+            raise ValueError("logits rows must be n_utt * n")
+        n_utt = R // n
+        mask = np.ascontiguousarray(mask, np.uint8)
+        if mask.shape != (V,):
+            raise ValueError("mask must have V entries")
+        seeds = np.ascontiguousarray(np.asarray(seeds, np.uint64).reshape(n_utt))
+        _, _, max_new = state["seq"].shape
+        t_max = state["indir"].shape[2]
+        want = self.search_state(n_utt, n, max_new, t_max, sample=True)
+        for k, v in want.items():
+            if np.shape(state[k]) != v.shape:
+                raise ValueError(f"state[{k!r}] must have shape {v.shape}")
+        si = np.concatenate([np.asarray(state[k], np.int32).ravel() for k in want if k not in self._STATE_F])
+        sf = np.concatenate([np.asarray(state[k], np.float32).ravel() for k in self._STATE_F])
+        caps = None if max_new_u is None else np.ascontiguousarray(max_new_u, np.int32).reshape(n_utt)
+        pr = None if prompt is None else np.ascontiguousarray(prompt, np.int32).reshape(n_utt, -1)
+        init = 0 if pr is None else 1 + int(shared_prefix)
+        prm = np.asarray([n_utt, n, V, ldl, eot, no_timestamps, 1 if timestamps else 0, max_initial_timestamp_index,
+                          max_new, 1, t_max, init, 0 if pr is None else pr.shape[1]], np.int32)
+        if repetition_penalty is not None or no_repeat_ngram_size is not None:
+            rp = np.float32(1.0 if repetition_penalty is None else repetition_penalty)
+            prm = np.concatenate([prm, [rp.view(np.int32), int(no_repeat_ngram_size or 0)]]).astype(np.int32)
+        sampled = np.zeros(R, np.int32)
+        key = np.zeros(R, np.float32)
+        lse = np.zeros(R, np.float32)
+        check(lib().wisb_debug_search_step_sample(self._h, ptr(prm), prm.size, float(length_penalty), int(sampling_topk),
+                                                  float(sampling_temperature), ptr(seeds), ptr(logits), ptr(mask),
+                                                  ptr(caps), ptr(pr), ptr(si), ptr(sf), ptr(sampled), ptr(key), ptr(lse)))
+        out, oi, of = {}, 0, 0
+        for k, v in want.items():
+            if k in self._STATE_F:
+                out[k], of = sf[of: of + v.size].reshape(v.shape).copy(), of + v.size
+            else:
+                out[k], oi = si[oi: oi + v.size].reshape(v.shape).copy(), oi + v.size
+        return out, sampled, key, lse
 
     def debug_enc_attn(self, qkv16: np.ndarray, n_heads: int, impl: int = 0) -> np.ndarray:
         """Encoder self-attention on qkv fp16 [B, 1536, 3d] -> ctx fp16 [B, 1536, d]; impl 0 = wgmma (MN-major V),

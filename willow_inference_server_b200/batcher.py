@@ -20,6 +20,10 @@ configuration; the length limits travel per window).  With an engine that takes 
 (whether ``<|notimestamps|>`` is in them), and ``beam_size``, ``patience`` and ``length_penalty`` travel per window too,
 so short commands at beam 1, dictation at beam 3 and requests in other languages or for translation share one call.
 Every other option (``max_initial_timestamp_index``, ``suppress_tokens``, the history processors) must still match.
+Sampling requests (``beam_size=1``, ``sampling_topk != 1``) share a call only with sampling requests of the same
+``num_hypotheses``, ``sampling_topk``, ``sampling_temperature`` and search options, never with beam requests.  Each
+gets its seed at ``submit`` (its own ``random_seed``, or a draw from the stream ``set_random_seed`` resets) and the
+call takes one seed per window, so a merged request returns exactly what it returns alone with that seed.
 Those three options are checked at ``submit`` (``ValueError`` there), and a call that the engine refuses as invalid
 (``ValueError``) is retried request by request, so one client's bad request never fails the requests it was merged with.
 Every window of such a call keeps as many decoder rows as the call's largest beam, so a batch keeps its padded rows at
@@ -42,7 +46,7 @@ from concurrent.futures import Future
 
 import numpy as np
 
-from .models import StorageView
+from .models import StorageView, check_sampling_options, draw_seed, window_seeds
 
 
 # search options an engine with per_window_options takes per window, with the defaults of CTranslate2's generate (which
@@ -64,7 +68,7 @@ def _check_search_option(name, v):
 
 
 class _Request:
-    __slots__ = ("features", "n", "key", "prompt", "opts", "search", "max_length", "future", "t_arrival")
+    __slots__ = ("features", "n", "key", "prompt", "opts", "search", "max_length", "seed", "future", "t_arrival")
 
     def __init__(self, features, prompt, opts, no_timestamps=None):
         """no_timestamps: the engine's <|notimestamps|> id when it takes prompts and search options per window, else
@@ -76,8 +80,21 @@ class _Request:
         self.max_length = int(self.opts.pop("max_length", 448))  # per request; merged per window by the worker
         self.search = {}
         prompt_key = tuple(self.prompt)
+        # sampling: the request's seed, fixed now (its windows get seed + w); its search options stay in the key
+        self.seed = None
+        random_seed = self.opts.pop("random_seed", None)
+        sampling = any(k in self.opts for k in ("num_hypotheses", "sampling_topk")) and check_sampling_options(
+            self.opts.get("num_hypotheses", 1), self.opts.get("sampling_topk", 1), self.opts.get("sampling_temperature", 1),
+            self.opts.get("beam_size", PER_WINDOW_DEFAULTS["beam_size"]), self.opts.get("patience", 1.0),
+            self.opts.get("length_penalty", 1.0))
+        if sampling:
+            if random_seed is not None and (isinstance(random_seed, (bool, np.bool_)) or
+                                            not isinstance(random_seed, (int, np.integer))):
+                raise ValueError(f"random_seed of a request must be None or an int, got {random_seed!r}")
+            self.seed = draw_seed() if random_seed is None else int(random_seed) % (1 << 64)
         if no_timestamps is not None:
-            self.search = {k: _check_search_option(k, self.opts.pop(k)) for k in PER_WINDOW_DEFAULTS if k in self.opts}
+            if not sampling:
+                self.search = {k: _check_search_option(k, self.opts.pop(k)) for k in PER_WINDOW_DEFAULTS if k in self.opts}
             prompt_key = (len(self.prompt), no_timestamps in self.prompt)
         self.key = (prompt_key, tuple(sorted((k, _freeze(v)) for k, v in self.opts.items())))
         self.future = Future()
@@ -246,6 +263,8 @@ class TranscribeBatcher:
                 same = all(v == vals[0] for v in vals)
                 opts[k] = vals[0] if same else np.asarray(vals, np.int32 if k == "beam_size" else np.float32)
         prompts = [r.prompt for r in live for _ in range(r.n)]
+        if live[0].seed is not None:  # (a sampling batch: every request has its seed)
+            opts["random_seed"] = np.concatenate([window_seeds(r.seed, r.n) for r in live])
         out = self._model.generate(StorageView.from_array(feats), prompts, max_length=ml, **opts)
         if len(out) != n:
             raise RuntimeError(f"engine returned {len(out)} results for {n} windows")

@@ -17,7 +17,7 @@ struct DecState {
   int gen_step;   // 0-based index of the token being generated (valid once pos >= prompt_len - 1)
   int n_done;     // utterances finished
   int all_done;   // n_done == n_utt
-  int ticket;     // CTAs of search_tail_kernel that finished this step's bookkeeping (the last one advances the step)
+  int ticket;     // CTAs of the search tail that finished this step's bookkeeping (the last one advances the step)
 };
 
 enum GemvEpi : int {
@@ -69,6 +69,14 @@ struct SearchArgs {
   const int* beam_u = nullptr;    // [n_utt] in [1, beam]
   const int* max_hyp_u = nullptr; // [n_utt] >= 1
   const float* lp_u = nullptr;    // [n_utt]
+  // sampling (beam_size 1 with sampling_topk != 1; search.cu): every utterance keeps `beam` = num_hypotheses independent
+  // rows, each sampling from softmax(l_S / temperature) with the Gumbel-max trick on a Philox stream keyed by the
+  // utterance's seed.  best_len / best_score / best_tokens then hold one hypothesis per ROW ([R], [R], [R][max_new]);
+  // max_hyp, n_cand and the per-utterance arrays are unused.
+  int sample = 0;
+  int topk = 0;                   // 0: every token with a finite processed logit; else in [2, MAX_CAND]
+  float temperature = 1.f;        // finite, > 0
+  const unsigned long long* seed_u = nullptr;  // [n_utt]
 };
 void search_step_run(const SearchArgs& a, cudaStream_t stream);
 // prompt prefill: no search, just feed the next prompt token and advance the position

@@ -86,6 +86,8 @@ struct GraphKey {
   float rep_penalty;    // history processors (baked in too)
   int no_repeat_ngram;
   int mixed;            // per-utterance beam / max_hyp / length penalty in device arrays (beam = the largest; max_hyp, lp 0)
+  int sample, topk;     // sampling (the seeds live in a device array: one graph serves every seed)
+  float temperature;
   bool operator<(const GraphKey& o) const {
     return memcmp(this, &o, sizeof(GraphKey)) < 0;
   }
@@ -146,6 +148,7 @@ struct wisb_handle {
   DevBuf<int> row_pos, row_slot, max_new_u;
   DevBuf<int> beam_u, max_hyp_u;  // per-utterance search options of a call that mixes them (SearchArgs::beam_u)
   DevBuf<float> lp_u;
+  DevBuf<unsigned long long> seed_u;  // per-utterance seeds of a sampling call (SearchArgs::seed_u)
   int search_rows = 0;  // rows the search / state buffers above are sized for
   int search_gen = 0, bd_search_gen = -1;  // reallocation count of those buffers / the one the batched-pass plans were built for
   // batched decoder pass (more than DEC_MAX_ROWS rows): workspaces for bd_rows (multiple of 128) rows, bd_tcap positions
@@ -352,6 +355,7 @@ void ensure_search(wisb_handle* h, int rows) {
   h->prompt_dev.ensure(R * T_MAX);
   h->row_pos.ensure(R, true); h->row_slot.ensure(R, true); h->max_new_u.ensure(R, true);
   h->beam_u.ensure(R, true); h->max_hyp_u.ensure(R, true); h->lp_u.ensure(R, true);
+  h->seed_u.ensure(R, true);
   h->lang_probs.ensure(R * 128);
   h->pin_i.ensure(4 + R * (T_MAX + 5));  // (upload_prompts: prompts and four per-utterance words)
   h->pin_f.ensure(R * 130);
@@ -810,6 +814,10 @@ struct DecodeCfg {
   const int* beam_host = nullptr;
   const int* max_hyp_host = nullptr;
   const float* lp_host = nullptr;
+  // sampling: beam is the number of hypotheses per utterance, seeds (host, indexed like max_new_host) -> h->seed_u
+  int sample = 0, topk = 0;
+  float temperature = 1.f;
+  const uint64_t* seed_host = nullptr;
 };
 
 SearchArgs make_search_args(wisb_handle* h, const DecodeCfg& c) {
@@ -856,6 +864,12 @@ SearchArgs make_search_args(wisb_handle* h, const DecodeCfg& c) {
     a.beam_u = h->beam_u.p;
     a.max_hyp_u = h->max_hyp_u.p;
     a.lp_u = h->lp_u.p;
+  }
+  if (c.sample) {
+    a.sample = 1;
+    a.topk = c.topk;
+    a.temperature = c.temperature;
+    a.seed_u = h->seed_u.p;
   }
   if (c.ts) {
     a.ts = 1;
@@ -1018,8 +1032,8 @@ void set_extra_suppress(wisb_handle* h, const int32_t* extra, int n_extra) {
 }
 
 // prompts [n_utt][prompt_len] of utterances [u0, u0 + n_utt) -> h->prompt_dev, when c.per_utt_max_new their caps on
-// new tokens (max_new_host[u0 + u]) -> h->max_new_u, and when c.mixed their search options -> h->beam_u / max_hyp_u /
-// lp_u.  All are staged through the pinned buffer, whose first 4 words hold
+// new tokens (max_new_host[u0 + u]) -> h->max_new_u, when c.mixed their search options -> h->beam_u / max_hyp_u /
+// lp_u, and when c.sample their seeds -> h->seed_u.  All are staged through the pinned buffer, whose first 4 words hold
 // the step loop's flags: the host may rewrite it only after the stream sync that ends the previous group, because these
 // asynchronous copies read from it.
 void upload_prompts(wisb_handle* h, const int32_t* prompts, const int* max_new_host, const DecodeCfg& c) {
@@ -1040,6 +1054,11 @@ void upload_prompts(wisb_handle* h, const int32_t* prompts, const int* max_new_h
     WISB_CUDA(cudaMemcpyAsync(h->max_hyp_u.p, pm + c.n_utt, sizeof(int) * c.n_utt, cudaMemcpyHostToDevice, h->stream));
     WISB_CUDA(cudaMemcpyAsync(h->lp_u.p, pm + 2 * c.n_utt, sizeof(float) * c.n_utt, cudaMemcpyHostToDevice, h->stream));
   }
+  if (c.sample) {  // (never together with c.mixed: the same staging words)
+    int* ps = pin + n + c.n_utt;
+    memcpy(ps, c.seed_host + c.u0, sizeof(uint64_t) * c.n_utt);
+    WISB_CUDA(cudaMemcpyAsync(h->seed_u.p, ps, sizeof(uint64_t) * c.n_utt, cudaMemcpyHostToDevice, h->stream));
+  }
 }
 
 // best hypothesis of every utterance of the pass (search state) -> the caller's host arrays at utterance u0.  An
@@ -1047,6 +1066,34 @@ void upload_prompts(wisb_handle* h, const int32_t* prompts, const int* max_new_h
 void read_results(wisb_handle* h, const DecodeCfg& c, const int* max_new_host, int32_t* out_ids, int out_stride,
                   int32_t* out_len, float* out_score) {
   cudaStream_t s = h->stream;
+  if (c.sample) {
+    // sampling: the hypothesis of every row; utterance u's n = c.beam go to entries (u0 + u) * n + [0, n), sorted by
+    // score, descending, ties to the lower hypothesis index
+    const int n = c.beam, R = c.n_utt * n;
+    int* lens = h->pin_i.p + 4;
+    int* toks = lens + R;
+    const int mn = c.max_new > 0 ? c.max_new : 1;
+    WISB_CUDA(cudaMemcpyAsync(lens, h->best_len.p, sizeof(int) * R, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(toks, h->best_tokens.p, sizeof(int) * R * mn, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(h->pin_f.p, h->best_score.p, sizeof(float) * R, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+    std::vector<int> order(n);
+    for (int u = 0; u < c.n_utt; ++u) {
+      const int cap = c.per_utt_max_new ? max_new_host[c.u0 + u] : c.max_new;
+      const float* sc = h->pin_f.p + u * n;
+      for (int k = 0; k < n; ++k) order[k] = k;
+      if (cap > 0) std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return sc[x] > sc[y]; });
+      for (int i = 0; i < n; ++i) {
+        const int k = order[i], r = u * n + k;
+        const size_t o = static_cast<size_t>(c.u0 + u) * n + i;
+        const int len = cap > 0 ? lens[r] : 0;
+        out_len[o] = len;
+        for (int t = 0; t < len && t < out_stride; ++t) out_ids[o * out_stride + t] = toks[static_cast<size_t>(r) * mn + t];
+        if (out_score) out_score[o] = cap > 0 ? sc[k] : 0.f;
+      }
+    }
+    return;
+  }
   int* lens = h->pin_i.p + 4;
   int* toks = lens + c.n_utt;
   const int mn = c.max_new > 0 ? c.max_new : 1;
@@ -1356,6 +1403,7 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
       key.per_utt_max_new = c.per_utt_max_new;
       key.ts = c.ts; key.ts_max_init = c.ts ? c.ts_max_init : 0;
       key.rep_penalty = c.rep_penalty; key.no_repeat_ngram = c.no_repeat_ngram;
+      key.sample = c.sample; key.topk = c.sample ? c.topk : 0; key.temperature = c.sample ? c.temperature : 0.f;
       auto it = h->graphs.find(key);
       if (it == h->graphs.end()) {
         if (h->graphs.size() > 64) drop_graphs(h);
@@ -1743,12 +1791,25 @@ int wisb_logmel(wisb_handle* h, const void* pcm, int pcm_dtype, int pcm_on_devic
   });
 }
 
-int wisb_generate_mixed(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
-                        float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                        const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
-                        float repetition_penalty, int no_repeat_ngram_size, const int32_t* beam_per_utt,
-                        const float* patience_per_utt, const float* length_penalty_per_utt, int32_t* out_ids,
-                        int out_stride, int32_t* out_len, float* out_score) {
+}  // extern "C"
+
+namespace {
+
+// sampling options of a wisb_generate_sample call (its windows all sample; beam_size 1, no per-window options)
+struct SampleCall {
+  int n = 1, topk = 0;
+  float temperature = 1.f;
+  const uint64_t* seeds = nullptr;  // [B]
+};
+
+// the body of wisb_generate_mixed (sc == nullptr) and wisb_generate_sample; with sc the output arrays hold sc->n entries
+// per window
+int generate_impl(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
+                  float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
+                  const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
+                  float repetition_penalty, int no_repeat_ngram_size, const int32_t* beam_per_utt,
+                  const float* patience_per_utt, const float* length_penalty_per_utt, const SampleCall* sc,
+                  int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score) {
   return guarded(h, [&] {
     const Dims& dm = h->dims;
     WISB_REQUIRE(h->blob != nullptr, "handle has no model (created by wisb_create_frontend)");
@@ -1767,9 +1828,18 @@ int wisb_generate_mixed(wisb_handle* h, const float* mel, int B, const int32_t* 
     // per-window search options: beam, max_hyp and length penalty of every window, and the largest beam (the row block
     // of every window)
     const bool per_window = beam_per_utt != nullptr || patience_per_utt != nullptr || length_penalty_per_utt != nullptr;
+    if (sc) {
+      WISB_REQUIRE(!per_window && beam_size == 1, "sampling: beam_size must be 1, with no per-window search options");
+      WISB_REQUIRE(sc->n >= 1 && sc->n <= MAX_BEAM, "num_hypotheses must be in [1, 8]");
+      WISB_REQUIRE(sc->topk == 0 || (sc->topk >= 2 && sc->topk <= MAX_CAND), "sampling_topk must be 0 or in [2, 16]");
+      WISB_REQUIRE(std::isfinite(sc->temperature) && sc->temperature > 0.f, "sampling_temperature must be finite and > 0");
+      WISB_REQUIRE(sc->seeds != nullptr && out_score != nullptr, "seeds / out_score is NULL");
+      WISB_REQUIRE(std::isfinite(length_penalty), "length_penalty must be finite");
+    }
     std::vector<int> beam_w, hyp_w;
     std::vector<float> lp_w;
-    int beam_max = beam_size;
+    // rows of every window: its beam, or its hypotheses when sampling
+    int beam_max = sc ? sc->n : beam_size;
     if (per_window) {
       beam_w.resize(B);
       hyp_w.resize(B);
@@ -1850,6 +1920,13 @@ int wisb_generate_mixed(wisb_handle* h, const float* mel, int B, const int32_t* 
       c.max_hyp = max_hyp_of(beam_size, patience);
       c.lp = length_penalty;
       c.mixed = 0;
+      if (sc) {
+        c.beam = sc->n;
+        c.sample = 1;
+        c.topk = sc->topk;
+        c.temperature = sc->temperature;
+        c.seed_host = sc->seeds + g0;
+      }
       if (per_window) {
         c.beam = beam_w[g0];
         c.max_hyp = hyp_w[g0];
@@ -1871,10 +1948,11 @@ int wisb_generate_mixed(wisb_handle* h, const float* mel, int B, const int32_t* 
       }
       const int32_t* gp = prompts + static_cast<size_t>(g0) * prompt_len;
       const int* gmx = per_utt.empty() ? nullptr : per_utt.data() + g0;
-      int32_t* gi = out_ids + static_cast<size_t>(g0) * out_stride;
-      float* gs = out_score ? out_score + g0 : nullptr;
-      steps += persistent ? decode_pass(h, c, gp, gmx, gi, out_stride, out_len + g0, gs)
-                          : decode_batch(h, c, gp, gmx, gi, out_stride, out_len + g0, gs);
+      const size_t per = sc ? sc->n : 1;  // output entries per window
+      int32_t* gi = out_ids + g0 * per * out_stride;
+      float* gs = out_score ? out_score + g0 * per : nullptr;
+      steps += persistent ? decode_pass(h, c, gp, gmx, gi, out_stride, out_len + g0 * per, gs)
+                          : decode_batch(h, c, gp, gmx, gi, out_stride, out_len + g0 * per, gs);
       WISB_CUDA(cudaEventRecord(h->ev[5], s));
       time_group(h, {2, 3, 4});  // encoder, cross K/V, decode
     }
@@ -1882,6 +1960,38 @@ int wisb_generate_mixed(wisb_handle* h, const float* mel, int B, const int32_t* 
     h->timing[7] = static_cast<float>(h->launches);
     h->prof_collect();
   });
+}
+
+}  // namespace
+
+extern "C" {
+
+int wisb_generate_mixed(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
+                        float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
+                        const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
+                        float repetition_penalty, int no_repeat_ngram_size, const int32_t* beam_per_utt,
+                        const float* patience_per_utt, const float* length_penalty_per_utt, int32_t* out_ids,
+                        int out_stride, int32_t* out_len, float* out_score) {
+  return generate_impl(h, mel, B, prompts, prompt_len, beam_size, patience, length_penalty, max_length,
+                       max_length_per_utt, extra_suppress, n_extra, timestamps, max_initial_timestamp_index,
+                       repetition_penalty, no_repeat_ngram_size, beam_per_utt, patience_per_utt, length_penalty_per_utt,
+                       nullptr, out_ids, out_stride, out_len, out_score);
+}
+
+int wisb_generate_sample(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len,
+                         int num_hypotheses, int sampling_topk, float sampling_temperature, const uint64_t* seeds,
+                         float length_penalty, int max_length, const int32_t* max_length_per_utt,
+                         const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
+                         float repetition_penalty, int no_repeat_ngram_size, int32_t* out_ids, int out_stride,
+                         int32_t* out_len, float* out_score) {
+  SampleCall sc;
+  sc.n = num_hypotheses;
+  sc.topk = sampling_topk;
+  sc.temperature = sampling_temperature;
+  sc.seeds = seeds;
+  return generate_impl(h, mel, B, prompts, prompt_len, 1, 1.f, length_penalty, max_length, max_length_per_utt,
+                       extra_suppress, n_extra, timestamps, max_initial_timestamp_index, repetition_penalty,
+                       no_repeat_ngram_size, nullptr, nullptr, nullptr, &sc, out_ids, out_stride, out_len, out_score);
 }
 
 int wisb_generate_proc(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
@@ -2195,11 +2305,13 @@ int wisb_debug_gemm(wisb_handle* h, const int32_t* prm, int n_prm, const uint16_
   });
 }
 
-// wisb_debug_search_step's body; beam_u / max_hyp_u / lp_u (all three or none): wisb_debug_search_step_mixed
+// wisb_debug_search_step's body; beam_u / max_hyp_u / lp_u (all three or none): wisb_debug_search_step_mixed; sc:
+// wisb_debug_search_step_sample (`beam` = the hypotheses per utterance, per-row best_len / best_tokens / best_score)
 static int debug_search_step_impl(wisb_handle* h, const int32_t* prm, int n_prm, float length_penalty, const float* logits,
                                   const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
                                   float* state_f, int32_t* cand_idx, float* cand_score, float* row_lse,
-                                  const int32_t* beam_u, const int32_t* max_hyp_u, const float* lp_u) {
+                                  const int32_t* beam_u, const int32_t* max_hyp_u, const float* lp_u,
+                                  const SampleCall* sc = nullptr) {
   return guarded(h, [&] {
     WISB_REQUIRE(prm != nullptr && (n_prm == 13 || n_prm == 15) && logits && mask && state_i && state_f && cand_idx && cand_score && row_lse,
                  "debug_search_step: bad arguments");
@@ -2216,11 +2328,17 @@ static int debug_search_step_impl(wisb_handle* h, const int32_t* prm, int n_prm,
     WISB_REQUIRE(std::isfinite(rep_penalty) && rep_penalty > 0.f && no_repeat_ngram >= 0 && no_repeat_ngram <= T_MAX,
                  "debug_search_step: bad history processor arguments");
     const int R = n_utt * beam;
+    if (sc)
+      WISB_REQUIRE(sc->seeds != nullptr && (sc->topk == 0 || (sc->topk >= 2 && sc->topk <= MAX_CAND)) &&
+                       std::isfinite(sc->temperature) && sc->temperature > 0.f && std::isfinite(length_penalty),
+                   "debug_search_step_sample: bad sampling arguments");
     // state_i: DecState (5) | flip | seq [2][R][max_new] | indir [2][R][t_max] | tokens [R] | row_pos [R] | done [n_utt] |
-    // n_hyp [n_utt] | best_len [n_utt] | best_tokens [n_utt][max_new];  state_f: cum [R] | best_score [n_utt]
+    // n_hyp [n_utt] | best_len [H] | best_tokens [H][max_new];  state_f: cum [R] | best_score [H]  (H = n_utt, or R when
+    // sampling)
+    const int H = sc ? R : n_utt;
     const size_t o_seq = 6, o_ind = o_seq + 2ull * R * max_new, o_tok = o_ind + 2ull * R * t_max, o_rpos = o_tok + R;
-    const size_t o_done = o_rpos + R, o_nhyp = o_done + n_utt, o_blen = o_nhyp + n_utt, o_btok = o_blen + n_utt;
-    const size_t n_i = o_btok + static_cast<size_t>(n_utt) * max_new, n_f = static_cast<size_t>(R) + n_utt;
+    const size_t o_done = o_rpos + R, o_nhyp = o_done + n_utt, o_blen = o_nhyp + n_utt, o_btok = o_blen + H;
+    const size_t n_i = o_btok + static_cast<size_t>(H) * max_new, n_f = static_cast<size_t>(R) + H;
     if (init) {
       WISB_REQUIRE(prompt != nullptr && prompt_len >= 1 && prompt_len <= t_max, "debug_search_step: bad prompt");
       for (long long i = 0; i < static_cast<long long>(n_utt) * prompt_len; ++i)
@@ -2261,6 +2379,7 @@ static int debug_search_step_impl(wisb_handle* h, const int32_t* prm, int n_prm,
     DevBuf<uint8_t> d_mask;
     DevBuf<int> d_i, d_ci, d_cap, d_prompt, d_slot, d_beam, d_hyp;
     DevBuf<float> d_lp;
+    DevBuf<unsigned long long> d_seed;
     d_logits.ensure(static_cast<size_t>(R) * ldl);
     d_mask.ensure(V);
     d_pmax.ensure(static_cast<size_t>(R) * (TOPK_CHUNKS + 1));
@@ -2287,6 +2406,10 @@ static int debug_search_step_impl(wisb_handle* h, const int32_t* prm, int n_prm,
       WISB_CUDA(cudaMemcpyAsync(d_beam.p, beam_u, sizeof(int) * n_utt, cudaMemcpyHostToDevice, s));
       WISB_CUDA(cudaMemcpyAsync(d_hyp.p, max_hyp_u, sizeof(int) * n_utt, cudaMemcpyHostToDevice, s));
       WISB_CUDA(cudaMemcpyAsync(d_lp.p, lp_u, sizeof(float) * n_utt, cudaMemcpyHostToDevice, s));
+    }
+    if (sc) {
+      d_seed.ensure(n_utt);
+      WISB_CUDA(cudaMemcpyAsync(d_seed.p, sc->seeds, sizeof(uint64_t) * n_utt, cudaMemcpyHostToDevice, s));
     }
     if (init) {
       d_prompt.ensure(static_cast<size_t>(n_utt) * prompt_len);
@@ -2341,6 +2464,12 @@ static int debug_search_step_impl(wisb_handle* h, const int32_t* prm, int n_prm,
       a.max_hyp_u = d_hyp.p;
       a.lp_u = d_lp.p;
     }
+    if (sc) {
+      a.sample = 1;
+      a.topk = sc->topk;
+      a.temperature = sc->temperature;
+      a.seed_u = d_seed.p;
+    }
     static_assert(sizeof(DecState) == 5 * sizeof(int), "DecState is five ints");
     if (init) search_init_run(a, d_prompt.p, s, init - 1);
     search_step_run(a, s);  // the production step: processors, top-k partials, merge, bookkeeping and step advance
@@ -2370,6 +2499,37 @@ int wisb_debug_search_step_mixed(wisb_handle* h, const int32_t* prm, int n_prm, 
   }
   return debug_search_step_impl(h, prm, n_prm, 1.f, logits, mask, max_new_u, prompt, state_i, state_f, cand_idx,
                                 cand_score, row_lse, beam_u, max_hyp_u, length_penalty_u);
+}
+
+int wisb_debug_search_step_sample(wisb_handle* h, const int32_t* prm, int n_prm, float length_penalty, int sampling_topk,
+                                  float sampling_temperature, const uint64_t* seeds, const float* logits,
+                                  const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
+                                  float* state_f, int32_t* sampled, float* key, float* row_lse) {
+  if (prm == nullptr || n_prm < 2 || sampled == nullptr || key == nullptr) {
+    g_last_error = "debug_search_step_sample: bad arguments";
+    return 1;
+  }
+  const int n_utt = prm[0], n = prm[1];
+  if (n_utt < 1 || n < 1 || n > MAX_BEAM || n_utt * n > 1024) {
+    g_last_error = "debug_search_step_sample: bad scalar parameters";
+    return 1;
+  }
+  SampleCall sc;
+  sc.n = n;
+  sc.topk = sampling_topk;
+  sc.temperature = sampling_temperature;
+  sc.seeds = seeds;
+  // the tail leaves row k of utterance u's sampled id and key in candidate slot k of u
+  std::vector<int32_t> ci(static_cast<size_t>(n_utt) * MAX_CAND);
+  std::vector<float> cs(static_cast<size_t>(n_utt) * MAX_CAND);
+  const int rc = debug_search_step_impl(h, prm, n_prm, length_penalty, logits, mask, max_new_u, prompt, state_i, state_f,
+                                        ci.data(), cs.data(), row_lse, nullptr, nullptr, nullptr, &sc);
+  if (rc == 0)
+    for (int r = 0; r < n_utt * n; ++r) {
+      sampled[r] = ci[static_cast<size_t>(r / n) * MAX_CAND + r % n];
+      key[r] = cs[static_cast<size_t>(r / n) * MAX_CAND + r % n];
+    }
+  return rc;
 }
 
 // wisb_align's body; cap_out (wisb_debug_align_capture) receives the raw capture buffer [B][A][n_max + 1][F_max]

@@ -38,6 +38,29 @@
 // per chunk, of which the merge takes the first 2 b_u (a chunk's partials are sorted, so this is the chunk's top 2 b_u).
 // Only the search_tail_kernel<NCH, true> / search_init_kernel<true> instantiations read the per-utterance arrays; a call
 // whose windows agree runs the <false> ones.
+//
+// Sampling (SearchArgs::sample: beam_size 1 and sampling_topk != 1; CTranslate2's RandomSampler with num_hypotheses n,
+// made deterministic by a per-window seed).  Each window keeps a block of n = `beam` rows, one per hypothesis; rows are
+// independent and never reorder (indir[r][pos] = r, a row's history is its own) and every row is live at gen 0.  One
+// step of row r of window u, hypothesis k = r mod n, generated-token index gen:
+//   1. the processors above run unchanged (penalty, n-gram ban, masks, timestamp rules including rule 5), giving the
+//      processed logits l_v and the row's lse over them;
+//   2. candidates S: topk == 0 every v with a finite l_v; topk == K in [2, 16] the K largest finite l_v (ties: lowest
+//      id); rule 5 (ts_only) keeps only the timestamps, as for beam rows;
+//   3. noise: x = word 0 of Philox4x32-10 with counter (v, gen, k, 0) and key (lo32(seed_u), hi32(seed_u));
+//      u = ((x >> 9) + 0.5) * 2^-23 (exact in fp32, in (0, 1)); g_v = -logf(-logf(u)) in fp32;
+//   4. sample: the v in S with the largest key_v = fp32(l_v / T) + g_v (IEEE division), ties to the lowest id.  This is
+//      Gumbel-max: v ~ softmax(l_S / T), transformers' TemperatureLogitsWarper followed by TopKLogitsWarper;
+//   5. cum += l_v - lse, the untempered log-prob (CTranslate2's RandomSampler gathers from the untempered scores;
+//      UNPINNED like the rest of its search).
+// A row finishes when it samples eot or at its window's last step; its hypothesis is its tokens without eot, scored
+// cum / (gen + 1)^length_penalty in fp32 (beam 1's normalisation), and it is dead from then on (eot, cum -inf).  A row
+// left with an empty S is dead with no hypothesis (empty, score -inf).  A window is done once all its rows are.
+// topk == 0 runs topk_partial_kernel<NCH, HIST, true>: each (chunk, row) block draws the noise of its finite tokens and
+// emits the chunk's best packed (key, id) in part slot 0 and that id's processed logit in slot 1, beside the usual lse
+// partials.  topk > 0 runs the plain partial kernel with K candidates per chunk; sample_tail_kernel merges them to the
+// row's top K and draws the noise of those.  sample_tail_kernel (one warp per row) then does the bookkeeping above and
+// the step advance; search_init_kernel<false, true> also resets the per-row hypotheses.
 #include "decoder.cuh"
 
 namespace wisb {
@@ -54,6 +77,41 @@ __device__ __forceinline__ float ord2f(unsigned u) {
 // larger key == better candidate: higher score first, then lower index
 __device__ __forceinline__ unsigned long long pack_key(float score, unsigned idx) {
   return (static_cast<unsigned long long>(f2ord(score)) << 32) | static_cast<unsigned long long>(~idx);
+}
+
+// word 0 of Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11) of counter (c0..c3) and
+// key (k0, k1)
+__device__ __forceinline__ unsigned philox4x32_10_w0(unsigned c0, unsigned c1, unsigned c2, unsigned c3, unsigned k0,
+                                                    unsigned k1) {
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    const unsigned hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
+    const unsigned hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
+    c0 = hi1 ^ c1 ^ k0;
+    c1 = lo1;
+    c2 = hi0 ^ c3 ^ k1;
+    c3 = lo0;
+    k0 += 0x9E3779B9u;
+    k1 += 0xBB67AE85u;
+  }
+  return c0;
+}
+
+// the Gumbel noise of token v for hypothesis k at generated-token index gen of a window with this seed
+__device__ __forceinline__ float gumbel_noise(unsigned long long seed, int k, int gen, int v) {
+  const unsigned x = philox4x32_10_w0(static_cast<unsigned>(v), static_cast<unsigned>(gen), static_cast<unsigned>(k), 0u,
+                                      static_cast<unsigned>(seed), static_cast<unsigned>(seed >> 32));
+  const float u = (static_cast<float>(x >> 9) + 0.5f) * 0x1p-23f;  // exact: 24 significant bits at most
+  return -logf(-logf(u));
+}
+
+__device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long x) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long y = __shfl_xor_sync(0xffffffffu, x, o);
+    x = y > x ? y : x;
+  }
+  return x;
 }
 
 __device__ __forceinline__ float masked_logit(const SearchArgs& a, const float* row, int v, bool first_step) {
@@ -174,11 +232,12 @@ __device__ __forceinline__ float hist_logit(const SearchArgs& a, float x, unsign
   return ban ? -INFINITY : x;
 }
 
-template <int NCH, bool HIST>
+template <int NCH, bool HIST, bool SAMPLE = false>
 __global__ void __launch_bounds__(TK_THREADS) topk_partial_kernel(const SearchArgs a) {
   // Within one row the ranking by processed logit equals the ranking by score, so the per-chunk stage needs no
   // log-sum-exp: it emits the chunk's top-n_cand logits plus (max, sum exp) partials; the merge stage turns them into
-  // the row's lse and into scores, with no separate two-pass lse kernel.
+  // the row's lse and into scores, with no separate two-pass lse kernel.  SAMPLE (sampling over the whole vocabulary):
+  // the chunk's best Gumbel key instead of its top logits.
   constexpr bool TS = NCH > TOPK_CHUNKS;
   __shared__ unsigned long long s_red[32];
   __shared__ float s_f[32];
@@ -253,6 +312,50 @@ __global__ void __launch_bounds__(TK_THREADS) topk_partial_kernel(const SearchAr
     for (int w = 0; w < TK_THREADS / 32; ++w) t += s_f[w];
     a.part_max[r * NCH + chunk] = mx;
     a.part_sum[r * NCH + chunk] = t;
+  }
+  if constexpr (SAMPLE) {
+    // the chunk's largest key fp32(l / T) + g (ties: lowest id) -> part slot 0, packed; its processed logit -> slot 1
+    __shared__ float s_l[32];
+    const int u = r / a.beam, k = r - u * a.beam, gen = a.st->gen_step;
+    const unsigned long long seed = a.seed_u[u];
+    unsigned long long best = 0ull;
+    float best_l = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < TK_PER; ++i) {
+      if (lg[i] == -INFINITY) continue;
+      const int v = v0 + tid + i * TK_THREADS;
+      const float key = __fdiv_rn(lg[i], a.temperature) + gumbel_noise(seed, k, gen, v);
+      const unsigned long long pk = pack_key(key, static_cast<unsigned>(v));
+      if (pk > best) {
+        best = pk;
+        best_l = lg[i];
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long ob = __shfl_xor_sync(0xffffffffu, best, o);
+      const float ol = __shfl_xor_sync(0xffffffffu, best_l, o);
+      if (ob > best) {
+        best = ob;
+        best_l = ol;
+      }
+    }
+    if (lane == 0) {
+      s_red[warp] = best;
+      s_l[warp] = best_l;
+    }
+    __syncthreads();
+    if (tid == 0) {  // (holds warp 0's best already)
+      for (int w = 1; w < TK_THREADS / 32; ++w)
+        if (s_red[w] > best) {
+          best = s_red[w];
+          best_l = s_l[w];
+        }
+      unsigned long long* out = a.part + (static_cast<long long>(r) * NCH + chunk) * MAX_CAND;
+      out[0] = best;
+      out[1] = __float_as_uint(best_l);
+    }
+    return;
   }
   block_select<TK_PER>(keys, a.n_cand, a.part + (static_cast<long long>(r) * NCH + chunk) * MAX_CAND, s_red);
 }
@@ -429,24 +532,9 @@ __device__ __forceinline__ void search_bookkeeping_body(const SearchArgs& a, int
   }
 }
 
-// grid (n_utt) x TK_THREADS: candidate merge, then (warp 0) the bookkeeping of the utterance, then -- by the last CTA to get
-// there -- the step advance (position, generation step, ping-pong flip, per-row positions).  One launch instead of three:
-// the tail of a decoding step is launch-latency bound.
-template <int NCH, bool MIXED>
-__global__ void __launch_bounds__(TK_THREADS) search_tail_kernel(const SearchArgs a) {
-  __shared__ unsigned long long s_red[32];
-  __shared__ unsigned long long s_out[MAX_CAND];
-  __shared__ float s_lse[MAX_BEAM];
-  __shared__ int s_ts_only[MAX_BEAM];
-  __shared__ int s_pick[MAX_BEAM];
-  __shared__ int s_best_k;
-  __shared__ int s_finished;
-  __shared__ int s_last;
-  if (a.st->all_done) return;  // a step enqueued ahead of the host's poll: nothing left to do
-  topk_merge_body<NCH, MIXED>(a, s_red, s_out, s_lse, s_ts_only);
-  __syncthreads();  // the candidate list (global) is complete for this CTA's readers
-  if (threadIdx.x < 32) search_bookkeeping_body<MIXED>(a, s_pick, s_best_k, s_finished);
-  __syncthreads();
+// End of a search tail launch (every thread, after a barrier that follows the CTA's bookkeeping): the last CTA to take a
+// ticket advances the step (position, generation step, ping-pong flip, per-row positions) and sets all_done.
+__device__ __forceinline__ void step_advance(const SearchArgs& a, int& s_last) {
   if (threadIdx.x == 0) {
     __threadfence();
     const int t = atomicAdd(&a.st->ticket, 1);
@@ -468,6 +556,167 @@ __global__ void __launch_bounds__(TK_THREADS) search_tail_kernel(const SearchArg
   }
 }
 
+// grid (n_utt) x TK_THREADS: candidate merge, then (warp 0) the bookkeeping of the utterance, then -- by the last CTA to get
+// there -- the step advance (position, generation step, ping-pong flip, per-row positions).  One launch instead of three:
+// the tail of a decoding step is launch-latency bound.
+template <int NCH, bool MIXED>
+__global__ void __launch_bounds__(TK_THREADS) search_tail_kernel(const SearchArgs a) {
+  __shared__ unsigned long long s_red[32];
+  __shared__ unsigned long long s_out[MAX_CAND];
+  __shared__ float s_lse[MAX_BEAM];
+  __shared__ int s_ts_only[MAX_BEAM];
+  __shared__ int s_pick[MAX_BEAM];
+  __shared__ int s_best_k;
+  __shared__ int s_finished;
+  __shared__ int s_last;
+  if (a.st->all_done) return;  // a step enqueued ahead of the host's poll: nothing left to do
+  topk_merge_body<NCH, MIXED>(a, s_red, s_out, s_lse, s_ts_only);
+  __syncthreads();  // the candidate list (global) is complete for this CTA's readers
+  if (threadIdx.x < 32) search_bookkeeping_body<MIXED>(a, s_pick, s_best_k, s_finished);
+  __syncthreads();
+  step_advance(a, s_last);
+}
+
+// grid (n_utt) x TK_THREADS, sampling: warp k does hypothesis row k of the utterance (selection from the chunk partials,
+// then its bookkeeping), thread 0 decides whether the utterance is done, then the step advance of search_tail_kernel.
+template <int NCH>
+__global__ void __launch_bounds__(TK_THREADS) sample_tail_kernel(const SearchArgs a) {
+  constexpr bool TS = NCH > TOPK_CHUNKS;
+  constexpr int PER = (NCH * MAX_CAND + 31) / 32;  // a row's chunk partials per lane (topk > 0): 16 / 17
+  __shared__ int s_live[MAX_BEAM];
+  __shared__ int s_last;
+  if (a.st->all_done) return;  // a step enqueued ahead of the host's poll: nothing left to do
+  const int u = blockIdx.x, k = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n = a.beam, r = u * n + k;
+  const int gen = a.st->gen_step, pos = a.st->pos;
+  const int cur = *a.flip;
+  const bool frozen = a.done[u] != 0;  // (written below only after a barrier)
+  const int cap = a.max_new_u != nullptr ? a.max_new_u[u] : a.max_new;
+  const bool is_last = gen + 1 >= cap;
+  const bool capped = gen >= cap;  // a cap of 0 new tokens: the utterance finishes without a hypothesis
+  if (k < n) {
+    const int* seq_cur = a.seq[cur] + static_cast<long long>(r) * a.max_new;
+    int* seq_nxt = a.seq[cur ^ 1] + static_cast<long long>(r) * a.max_new;
+    const int* ind_cur = a.indir[cur] + static_cast<long long>(r) * a.t_max;
+    int* ind_nxt = a.indir[cur ^ 1] + static_cast<long long>(r) * a.t_max;
+    // rows never reorder: the history and the cache indirection carry over, this step's K/V are the row's own
+    for (int t = lane; t < gen; t += 32) seq_nxt[t] = seq_cur[t];
+    for (int t = lane; t < pos; t += 32) ind_nxt[t] = ind_cur[t];
+    // row log-sum-exp from the chunk partials (every lane), rule 5 as in topk_merge_body
+    float mx = -INFINITY;
+    for (int c = 0; c < NCH; ++c) mx = fmaxf(mx, a.part_max[r * NCH + c]);
+    float t = 0.f;
+    for (int c = 0; c < NCH; ++c) {
+      const float pm = a.part_max[r * NCH + c];
+      if (pm != -INFINITY) t += a.part_sum[r * NCH + c] * __expf(pm - mx);
+    }
+    float lse = mx + logf(t);
+    bool ts_only = false;
+    if (TS) {
+      float text_max = -INFINITY;
+      for (int c = 0; c < TOPK_CHUNKS; ++c) text_max = fmaxf(text_max, a.part_max[r * NCH + c]);
+      const float pm = a.part_max[r * NCH + TOPK_CHUNKS];
+      const float ts_lse = pm == -INFINITY ? -INFINITY : pm + logf(a.part_sum[r * NCH + TOPK_CHUNKS]);
+      ts_only = ts_lse > text_max;
+      if (ts_only) lse = ts_lse;
+    }
+    const float cum = a.cum[r];
+    const bool live = !frozen && !capped && cum != -INFINITY;
+    unsigned long long best = 0ull;  // packed (key, ~id) of the sampled token, 0 = none
+    float best_l = -INFINITY;        // its processed logit
+    if (live) {
+      const unsigned long long* part = a.part + static_cast<long long>(r) * NCH * MAX_CAND;
+      if (a.topk == 0) {
+        unsigned long long pk = 0ull;  // the lane's best chunk key (chunks lane and lane + 32)
+        int pc = 0;
+        for (int c = lane; c < NCH; c += 32) {
+          const unsigned long long q = (TS && ts_only && c < TOPK_CHUNKS) ? 0ull : part[c * MAX_CAND];
+          if (q > pk) {
+            pk = q;
+            pc = c;
+          }
+        }
+        best = warp_max_u64(pk);
+        const unsigned owner = __ballot_sync(0xffffffffu, pk == best && best != 0ull);
+        const int c_best = __shfl_sync(0xffffffffu, pc, owner ? __ffs(owner) - 1 : 0);
+        if (best != 0ull) best_l = __uint_as_float(static_cast<unsigned>(part[c_best * MAX_CAND + 1]));
+      } else {
+        // the row's top-K processed logits from the chunks' sorted top K (lane i keeps the i-th), then their keys
+        const int K = a.topk;
+        unsigned long long e[PER];
+#pragma unroll
+        for (int i = 0; i < PER; ++i) {
+          const int j = lane + 32 * i, c = j / K;
+          e[i] = 0ull;
+          if (j < NCH * K && !(TS && ts_only && c < TOPK_CHUNKS)) e[i] = part[c * MAX_CAND + (j - c * K)];
+        }
+        unsigned long long mine = 0ull;
+        for (int s = 0; s < K; ++s) {
+          unsigned long long m = 0ull;
+#pragma unroll
+          for (int i = 0; i < PER; ++i) m = e[i] > m ? e[i] : m;
+          m = warp_max_u64(m);
+          if (m == 0ull) break;  // (warp-uniform) fewer than K finite logits
+#pragma unroll
+          for (int i = 0; i < PER; ++i)
+            if (e[i] == m) e[i] = 0ull;  // keys are unique (the id is part of the key)
+          if (lane == s) mine = m;
+        }
+        unsigned long long pk = 0ull;
+        float lm = -INFINITY;
+        if (mine != 0ull) {
+          lm = ord2f(static_cast<unsigned>(mine >> 32));
+          const unsigned v = ~static_cast<unsigned>(mine & 0xffffffffull);
+          const float key = __fdiv_rn(lm, a.temperature) + gumbel_noise(a.seed_u[u], k, gen, static_cast<int>(v));
+          pk = pack_key(key, v);
+        }
+        best = warp_max_u64(pk);
+        const unsigned owner = __ballot_sync(0xffffffffu, pk == best && best != 0ull);
+        best_l = __shfl_sync(0xffffffffu, lm, owner ? __ffs(owner) - 1 : 0);
+      }
+    }
+    const bool has = best != 0ull;
+    const int tok = has ? static_cast<int>(~static_cast<unsigned>(best & 0xffffffffull)) : a.eot;
+    const float cum_new = has ? (best_l - lse) + cum : -INFINITY;
+    const bool finish = has && (tok == a.eot || is_last);
+    if (finish)  // the hypothesis: the row's tokens, plus the last one unless eot
+      for (int t2 = lane; t2 < gen; t2 += 32) a.best_tokens[static_cast<long long>(r) * a.max_new + t2] = seq_cur[t2];
+    if (lane == 0) {
+      a.row_lse[r] = lse;
+      if (gen < a.max_new) seq_nxt[gen] = tok;
+      ind_nxt[pos] = r;
+      if (finish) {
+        int len = gen;
+        if (tok != a.eot) {
+          a.best_tokens[static_cast<long long>(r) * a.max_new + gen] = tok;
+          len = gen + 1;
+        }
+        const float lp = a.length_penalty;
+        const float norm = (lp != 0.f) ? powf(static_cast<float>(gen + 1), lp) : 1.f;
+        a.best_len[r] = len;
+        a.best_score[r] = cum_new / norm;
+      }
+      const bool cont = has && !finish;
+      a.tokens[r] = cont ? tok : a.eot;
+      a.cum[r] = cont ? cum_new : -INFINITY;
+      a.cand_idx[u * MAX_CAND + k] = has ? tok : -1;
+      a.cand_score[u * MAX_CAND + k] = has ? ord2f(static_cast<unsigned>(best >> 32)) : -INFINITY;
+      s_live[k] = cont ? 1 : 0;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && !frozen) {
+    int any = 0;
+    for (int j = 0; j < n; ++j) any |= s_live[j];
+    if (!any) {  // (at the last step, or capped, no row continues)
+      a.done[u] = 1;
+      atomicAdd(&a.st->n_done, 1);
+    }
+  }
+  __syncthreads();
+  step_advance(a, s_last);
+}
+
 __global__ void prefill_rows_kernel(int* tokens, int* row_pos, int* row_slot, const int* prompt, int prompt_len, int rows,
                                     int p0, int chunk, int beam) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -487,8 +736,9 @@ __global__ void prefill_advance_kernel(int* tokens, const int* prompt, int promp
 
 // shared_prefix: the prompt prefix (all but the last prompt token) is forwarded once per utterance into the cache slot of
 // its first beam by a single prefill pass; decoding then starts at the last prompt token and every beam's indirection
-// points at that slot.  MIXED: rows an utterance does not search start dead (eot, cum -inf).
-template <bool MIXED>
+// points at that slot.  MIXED: rows an utterance does not search start dead (eot, cum -inf).  SAMPLE: every row is live
+// and has no hypothesis yet (the per-row best_len / best_score).
+template <bool MIXED, bool SAMPLE = false>
 __global__ void search_init_kernel(const SearchArgs a, const int* prompt, int shared_prefix) {
   const int R = a.n_utt * a.beam;
   const int tid = blockIdx.x * blockDim.x + threadIdx.x, n = gridDim.x * blockDim.x;
@@ -515,6 +765,11 @@ __global__ void search_init_kernel(const SearchArgs a, const int* prompt, int sh
     a.best_score[i] = -INFINITY;
     a.best_len[i] = 0;
   }
+  if constexpr (SAMPLE)
+    for (int i = tid; i < R; i += n) {
+      a.best_score[i] = -INFINITY;
+      a.best_len[i] = 0;
+    }
   for (int i = tid; i < R * a.t_max; i += n) {
     const int r = i / a.t_max;
     const int slot = shared_prefix ? (r / a.beam) * a.beam : r;  // else identity: every row holds its own prefix copy
@@ -556,6 +811,33 @@ void search_step_run(const SearchArgs& a, cudaStream_t stream) {
                "search: bad history processor arguments");
   const bool mixed = a.beam_u != nullptr;
   WISB_REQUIRE(!mixed || (a.max_hyp_u != nullptr && a.lp_u != nullptr), "search: per-utterance options come as a set");
+  if (a.sample) {
+    WISB_REQUIRE(!mixed && a.seed_u != nullptr && (a.topk == 0 || (a.topk >= 2 && a.topk <= MAX_CAND)) &&
+                     std::isfinite(a.temperature) && a.temperature > 0.f,
+                 "search: bad sampling arguments");
+    SearchArgs b = a;
+    b.n_cand = a.topk;  // topk > 0: the plain partial kernel emits each chunk's top K logits
+    const dim3 grid(a.ts ? TOPK_CHUNKS + 1 : TOPK_CHUNKS, R);
+    if (a.ts) {
+      if (a.topk == 0)
+        hist ? topk_partial_kernel<TOPK_CHUNKS + 1, true, true><<<grid, TK_THREADS, 0, stream>>>(b)
+             : topk_partial_kernel<TOPK_CHUNKS + 1, false, true><<<grid, TK_THREADS, 0, stream>>>(b);
+      else
+        hist ? topk_partial_kernel<TOPK_CHUNKS + 1, true><<<grid, TK_THREADS, 0, stream>>>(b)
+             : topk_partial_kernel<TOPK_CHUNKS + 1, false><<<grid, TK_THREADS, 0, stream>>>(b);
+      sample_tail_kernel<TOPK_CHUNKS + 1><<<a.n_utt, TK_THREADS, 0, stream>>>(b);
+    } else {
+      if (a.topk == 0)
+        hist ? topk_partial_kernel<TOPK_CHUNKS, true, true><<<grid, TK_THREADS, 0, stream>>>(b)
+             : topk_partial_kernel<TOPK_CHUNKS, false, true><<<grid, TK_THREADS, 0, stream>>>(b);
+      else
+        hist ? topk_partial_kernel<TOPK_CHUNKS, true><<<grid, TK_THREADS, 0, stream>>>(b)
+             : topk_partial_kernel<TOPK_CHUNKS, false><<<grid, TK_THREADS, 0, stream>>>(b);
+      sample_tail_kernel<TOPK_CHUNKS><<<a.n_utt, TK_THREADS, 0, stream>>>(b);
+    }
+    WISB_CUDA(cudaGetLastError());
+    return;
+  }
   if (a.ts) {
     if (hist)
       topk_partial_kernel<TOPK_CHUNKS + 1, true><<<dim3(TOPK_CHUNKS + 1, R), TK_THREADS, 0, stream>>>(a);
@@ -591,7 +873,9 @@ void prefill_advance_run(int* tokens, const int* prompt, int prompt_len, int R, 
 }
 
 void search_init_run(const SearchArgs& a, const int* prompt, cudaStream_t stream, int shared_prefix) {
-  if (a.beam_u != nullptr)
+  if (a.sample)
+    search_init_kernel<false, true><<<8, 256, 0, stream>>>(a, prompt, shared_prefix);
+  else if (a.beam_u != nullptr)
     search_init_kernel<true><<<8, 256, 0, stream>>>(a, prompt, shared_prefix);
   else
     search_init_kernel<false><<<8, 256, 0, stream>>>(a, prompt, shared_prefix);

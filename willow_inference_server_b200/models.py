@@ -105,6 +105,73 @@ class WhisperAlignmentResult:
     text_token_probs: list  # list[float]
 
 
+# The stream the seeds of sampling calls without `random_seed` are drawn from (one 64-bit seed per call).
+_seed_lock = threading.Lock()
+_seed_stream = np.random.default_rng()
+
+
+def set_random_seed(seed: int):
+    """ctranslate2.set_random_seed: restart the stream that seeds sampling calls made without ``random_seed``, so
+    that a sequence of such calls repeats."""
+    global _seed_stream
+    if isinstance(seed, (bool, np.bool_)) or not isinstance(seed, (int, np.integer)):
+        raise ValueError(f"the random seed must be an int, got {seed!r}")
+    with _seed_lock:
+        _seed_stream = np.random.default_rng(int(seed) % (1 << 64))
+
+
+def draw_seed() -> int:
+    """the next 64-bit call seed of the stream set_random_seed resets"""
+    with _seed_lock:
+        return int(_seed_stream.integers(0, 1 << 64, dtype=np.uint64, endpoint=False))
+
+
+def _is_int(v) -> bool:
+    return isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_))
+
+
+def check_sampling_options(num_hypotheses, sampling_topk, sampling_temperature, beam_size, patience,
+                           length_penalty) -> bool:
+    """CTranslate2's switch: beam_size 1 with sampling_topk != 1 samples.  Returns whether these options sample, after
+    checking them (ValueError): sampling_topk 0 (the whole vocabulary) or in [2, 16], sampling_temperature finite and
+    > 0, num_hypotheses in [1, 8], scalar beam_size (1), patience and length_penalty.  num_hypotheses > 1 without
+    sampling is refused; with sampling_topk 1 the temperature is ignored (greedy or beam search)."""
+    if not _is_int(sampling_topk):
+        raise ValueError(f"sampling_topk must be an int, got {sampling_topk!r}")
+    if not _is_int(num_hypotheses) or not 1 <= num_hypotheses <= 8:
+        raise ValueError(f"num_hypotheses must be an int in [1, 8], got {num_hypotheses!r}")
+    if sampling_topk == 1:
+        if num_hypotheses != 1:
+            raise ValueError("num_hypotheses > 1 needs sampling (beam_size=1 and sampling_topk != 1)")
+        return False
+    if not all(np.isscalar(v) for v in (beam_size, patience, length_penalty)):
+        raise ValueError("a sampling call takes beam_size, patience and length_penalty as scalars")
+    if beam_size != 1:
+        raise ValueError("sampling (sampling_topk != 1) needs beam_size=1")
+    if not (sampling_topk == 0 or 2 <= sampling_topk <= 16):
+        raise ValueError(f"sampling_topk must be 0 (the whole vocabulary), 1 or in [2, 16], got {sampling_topk}")
+    number = lambda v: isinstance(v, (int, float, np.integer, np.floating)) and not isinstance(v, (bool, np.bool_))  # noqa: E731
+    if not number(sampling_temperature) or not np.isfinite(sampling_temperature) or sampling_temperature <= 0:
+        raise ValueError(f"sampling_temperature must be a finite number > 0, got {sampling_temperature!r}")
+    if not number(length_penalty) or not np.isfinite(length_penalty):
+        raise ValueError(f"length_penalty must be a finite number, got {length_penalty!r}")
+    return True
+
+
+def window_seeds(random_seed, n: int) -> np.ndarray:
+    """The seed of each of the n windows of a sampling call: random_seed None (one call seed s drawn from the stream
+    set_random_seed resets), an int s, or one int per window.  For a call seed s window w gets s + w mod 2^64, so a
+    window's result depends on its seed alone, not on how calls are batched."""
+    if random_seed is None:
+        random_seed = draw_seed()
+    if _is_int(random_seed):
+        return np.arange(n, dtype=np.uint64) + np.uint64(int(random_seed) % (1 << 64))  # (wraps mod 2^64)
+    vals = list(random_seed) if isinstance(random_seed, (list, tuple, np.ndarray)) else None
+    if vals is None or len(vals) != n or not all(_is_int(v) for v in vals):
+        raise ValueError("random_seed must be None, an int or one int per feature window")
+    return np.asarray([int(v) % (1 << 64) for v in vals], np.uint64)
+
+
 def get_supported_compute_types(device: str, device_index: int = 0):
     """main.py:454 only logs this.  One compute path exists: fp16 weights/activations, fp32 accumulation."""
     if device != "cuda":
@@ -285,8 +352,11 @@ class Whisper:
                  no_repeat_ngram_size: int = 0, max_length: int = 448, return_scores: bool = False,
                  return_no_speech_prob: bool = False, max_initial_timestamp_index: int = 50,
                  suppress_blank: bool = True, suppress_tokens=(-1,), sampling_topk: int = 1,
-                 sampling_temperature: float = 1):
-        """ctranslate2.models.Whisper.generate for the options WIS relies on (SURVEY.md section 8b defaults)."""
+                 sampling_temperature: float = 1, random_seed=None):
+        """ctranslate2.models.Whisper.generate for the options WIS relies on (SURVEY.md section 8b defaults).  With
+        beam_size=1 and sampling_topk != 1 it samples num_hypotheses hypotheses per window (``check_sampling_options``),
+        returned best first; random_seed (an extension: None, an int or one int per window, ``window_seeds``) makes
+        that reproducible."""
         src = self._input(features)
         n = src.n
         if len(prompts) != n:
@@ -296,8 +366,8 @@ class Whisper:
             raise ValueError("all prompts must be non-empty and of the same length")
         if isinstance(prompts[0][0], str):
             raise ValueError("prompts must be token ids (WIS builds them with convert_tokens_to_ids, main.py:656-663)")
-        if num_hypotheses != 1 or sampling_topk != 1:
-            raise ValueError("only num_hypotheses=1 and sampling_topk=1 (the CTranslate2 defaults WIS uses) are implemented")
+        sampling = check_sampling_options(num_hypotheses, sampling_topk, sampling_temperature, beam_size, patience,
+                                          length_penalty)
         # history processors on each hypothesis's generated tokens (csrc/search.cu)
         if isinstance(repetition_penalty, (bool, np.bool_)) or not isinstance(repetition_penalty, (int, float, np.number)) \
                 or not np.isfinite(repetition_penalty) or repetition_penalty <= 0:
@@ -347,6 +417,23 @@ class Whisper:
         proc = {}
         if repetition_penalty != 1 or no_repeat_ngram_size != 0:
             proc = dict(repetition_penalty=float(repetition_penalty), no_repeat_ngram_size=int(no_repeat_ngram_size))
+
+        if sampling:
+            seeds = window_seeds(random_seed, n)
+
+            def run_sample(h, mel, s, e):
+                seqs, scores = h.generate_sample(mel, p[s:e], int(num_hypotheses), int(sampling_topk),
+                                                 float(sampling_temperature), seeds[s:e], float(length_penalty),
+                                                 max_length if ml is None else ml[s:e], extra, B=e - s,
+                                                 timestamps=timestamps,
+                                                 max_initial_timestamp_index=int(max_initial_timestamp_index), **proc)
+                return seqs, scores
+
+            results = []
+            for seqs, scores in self._dispatch(src, run_sample):
+                for hyp, sc in zip(seqs, scores):
+                    results.append(WhisperGenerationResult(hyp, list(sc) if return_scores else []))
+            return results
 
         def run(h, mel, s, e):
             return h.generate(mel, p[s:e], window(search["beam_size"], s, e), window(search["patience"], s, e),
