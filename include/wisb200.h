@@ -9,7 +9,8 @@
  * the duration of the call; the handle owns device weights, workspaces, KV caches, streams and CUDA graphs.
  * All functions return 0 on success, 1 for invalid arguments (-> ValueError in the Python shim), 2 for CUDA/runtime
  * failures (-> RuntimeError); wisb_last_error() returns a thread-local message.  There is NO CPU fallback: without a
- * CUDA device every entry point except wisb_last_error / wisb_abi_version fails with code 2.
+ * CUDA device every entry point except wisb_last_error / wisb_abi_version / wisb_generate_options_init fails with
+ * code 2.
  * Calls on one handle are serialised internally; different handles may be used from different threads.
  */
 #ifndef WISB200_H_
@@ -24,7 +25,7 @@ extern "C" {
 
 typedef struct wisb_handle wisb_handle;
 
-#define WISB_ABI_VERSION 1
+#define WISB_ABI_VERSION 2
 #define WISB_PCM_F32 0 /* float32 in [-1, 1]  (what librosa.load hands do_whisper, main.py:579) */
 #define WISB_PCM_S16 1 /* int16 little endian (what /api/willow receives, main.py:1277-1299); scaled by 1/32768 on device */
 #define WISB_N_DIMS 20
@@ -56,78 +57,71 @@ int wisb_get_dims(wisb_handle* h, int32_t* dims /* [WISB_N_DIMS] */);
 int wisb_logmel(wisb_handle* h, const void* pcm, int pcm_dtype, int pcm_on_device, const int64_t* offsets,
                 const int32_t* n_samples, int B, float* mel_out, int keep_on_device);
 
+/* (4) the options of Whisper.generate (main.py:687-692), CTranslate2's defaults from wisb_generate_options_init.
+ * struct_size is sizeof(wisb_generate_options) as the caller was compiled (wisb_generate refuses any other value).
+ * Every per-window array is [B] or NULL, NULL meaning "the scalar applies to every window". */
+typedef struct wisb_generate_options {
+  uint32_t struct_size;
+  /* beam search (sampling_topk == 1): beam_size in [1, 8], 1 = greedy.  A window finishes once max(1, round half up of
+   * beam_size x patience in fp32) hypotheses exist (patience finite, > 0) and ranks them by cumulative log-prob over
+   * (generated tokens)^length_penalty (finite). */
+  int32_t beam_size;            /* 5 */
+  float patience;               /* 1 */
+  float length_penalty;         /* 1 */
+  /* at most min(max_length / 2, max_length - prompt_len) new tokens; max_length in [1, n_text_ctx] */
+  int32_t max_length;           /* 448 */
+  /* Whisper's timestamp rules, 0 or 1: what CTranslate2 does for a prompt WITHOUT <|notimestamps|> (the 3-token sot,
+   * language, task prompt).  The returned ids then contain timestamp tokens (ids > no_timestamps), which come in pairs
+   * except directly before <|endoftext|> and never decrease; the first generated token is a timestamp <= no_timestamps
+   * + 1 + max_initial_timestamp_index (50: 1.00 s).  With timestamps the prompt must contain neither <|notimestamps|>
+   * nor timestamp tokens.  max_initial_timestamp_index >= 0 in both modes. */
+  int32_t timestamps;                   /* 0 */
+  int32_t max_initial_timestamp_index;  /* 50 */
+  /* the history processors: repetition_penalty (finite, > 0; 1 = off) divides a positive logit and multiplies a
+   * negative one of every distinct token the hypothesis has generated so far; no_repeat_ngram_size (in [0, n_text_ctx];
+   * 0 = off) bans every token that would complete an n-gram the hypothesis already holds.  History = the hypothesis's
+   * generated tokens (timestamp tokens included, prompt tokens not).  They apply before the suppress masks and the
+   * timestamp rules. */
+  float repetition_penalty;      /* 1 */
+  int32_t no_repeat_ngram_size;  /* 0 */
+  /* sampling_topk != 1 samples (CTranslate2's rule; beam_size must then be 1, patience is not read and no per-window
+   * search option may be given): every window draws num_hypotheses (in [1, 8]; 1 unless sampling) independent
+   * hypotheses from softmax(l_S / sampling_temperature) (finite, > 0) over the processed logits l, S = every token
+   * (sampling_topk 0) or the sampling_topk (in [2, 16]) largest, with Gumbel-max noise from Philox4x32-10 keyed by
+   * seeds[b].  The result depends only on the window's features, prompt, options and seed, not on its batch position.
+   * Scores are the untempered cumulative log-probs over (generated tokens)^length_penalty. */
+  int32_t num_hypotheses;        /* 1 */
+  int32_t sampling_topk;         /* 1 */
+  float sampling_temperature;    /* 1 */
+  /* ids suppressed in addition to the model's suppress_ids (CT2 `suppress_tokens=[-1, ...]`) */
+  int32_t n_extra;
+  const int32_t* extra_suppress;
+  /* The per-window options are what CTranslate2's per-call options become when a batcher coalesces several calls into
+   * ONE shared decoder pass.  max_length_per_window in [1, n_text_ctx].  beam_per_window in [1, 8],
+   * patience_per_window finite and > 0, length_penalty_per_window finite: window b searches with its own beam, patience
+   * and length penalty exactly as it would alone.  Every window keeps a block of rows of the largest beam B of its group
+   * (at most batch_rows / B windows per group), searches its first b rows and leaves the others dead; a group whose
+   * windows agree on beam, max_hyp and length penalty runs the scalar search. */
+  const int32_t* max_length_per_window;
+  const int32_t* beam_per_window;
+  const float* patience_per_window;
+  const float* length_penalty_per_window;
+  const uint64_t* seeds;  /* uint64 [B], required when sampling */
+} wisb_generate_options;
+
+/* CTranslate2's defaults (the values above, every pointer NULL) and struct_size; needs no CUDA device and no handle.
+ * Code 1 if opt is NULL. */
+int wisb_generate_options_init(wisb_generate_options* opt);
+
 /* (3)+(4) features [B,n_mels,3000] float32 host (or NULL: use the features kept by wisb_logmel) -> token ids.
- * prompts: int32 [B, prompt_len] (WIS passes the same 4-token prompt for every window, main.py:689).  This entry always
- * decodes without timestamp rules; wisb_generate_ts switches them on.
- * beam_size 1 = greedy.  patience / length_penalty / max_length: CTranslate2 defaults 1, 1, 448.
- * extra_suppress: ids suppressed in addition to the model's suppress_ids (CT2 `suppress_tokens=[-1, ...]`), may be NULL.
- * out_ids: int32 [B, out_stride] (out_stride >= min(max_length/2, max_length-prompt_len)); out_len: int32 [B];
- * out_score (may be NULL): float32 [B] length-normalised log-probability of the returned hypothesis. */
-int wisb_generate(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
-                  float patience, float length_penalty, int max_length, const int32_t* extra_suppress, int n_extra,
-                  int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score);
-
-/* Same call with a per-utterance `max_length` (int32 [B], may be NULL = `max_length` for all): lets a cross-request
- * batcher put requests with different length limits into ONE shared decoder pass (CTranslate2's generate takes a single
- * max_length per call, main.py:687-692; the per-utterance form is what its semantics become when
- * several such calls are coalesced).  out_stride >= the largest per-utterance limit of new tokens. */
-int wisb_generate_ex(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
-                     float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                     const int32_t* extra_suppress, int n_extra, int32_t* out_ids, int out_stride, int32_t* out_len,
-                     float* out_score);
-
-/* Same call with Whisper's timestamp rules switched on (timestamps = 1) or off (0: exactly wisb_generate_ex).
- * Timestamp mode is what CTranslate2 does for a prompt WITHOUT <|notimestamps|> (the 3-token sot, language, task
- * prompt): the returned ids then contain timestamp tokens (ids > no_timestamps), which come in pairs except directly
- * before <|endoftext|> and never decrease; the first generated token is a timestamp <= no_timestamps + 1 +
- * max_initial_timestamp_index (CTranslate2 default 50, i.e. 1.00 s).  In timestamp mode the prompt must contain neither
- * <|notimestamps|> nor timestamp tokens.  max_initial_timestamp_index >= 0 in both modes. */
-int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
-                     float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                     const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
-                     int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score);
-
-/* Same call with the history processors of CTranslate2's Whisper.generate: repetition_penalty (finite, > 0; 1 = off)
- * divides a positive logit and multiplies a negative one of every distinct token the hypothesis has generated so far;
- * no_repeat_ngram_size (in [0, n_text_ctx]; 0 = off) bans every token that would complete an n-gram the hypothesis
- * already holds.  History = the hypothesis's generated tokens (timestamp tokens included, prompt tokens not).  They
- * apply before the suppress masks and the timestamp rules.  wisb_generate_ts is this call with (1, 0). */
-int wisb_generate_proc(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
-                       float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                       const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
-                       float repetition_penalty, int no_repeat_ngram_size, int32_t* out_ids, int out_stride,
-                       int32_t* out_len, float* out_score);
-
-/* Same call with the search options per window, each an array [B] or NULL (then the scalar applies to every window):
- * beam_per_utt in [1, 8], patience_per_utt finite and > 0, length_penalty_per_utt finite (else code 1).  Window b
- * searches with its own beam, finishes once max(1, round half up of beam x patience in fp32) hypotheses exist and ranks
- * them with its own length penalty, exactly as it would alone; prompts already come per window.  Like the per-window
- * max_length, this is what CTranslate2's per-call options become when a batcher coalesces several calls into one: every
- * window keeps a block of rows of the largest beam B of its group (at most batch_rows / B windows per group), searches
- * its first b rows and leaves the others dead.  A group whose windows agree on beam, max_hyp and length penalty runs
- * the scalar search.  wisb_generate_proc is this call with three NULLs. */
-int wisb_generate_mixed(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
-                        float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                        const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
-                        float repetition_penalty, int no_repeat_ngram_size, const int32_t* beam_per_utt,
-                        const float* patience_per_utt, const float* length_penalty_per_utt, int32_t* out_ids,
-                        int out_stride, int32_t* out_len, float* out_score);
-
-/* Sampling (CTranslate2's generate with beam_size 1 and sampling_topk != 1): every window draws num_hypotheses (in
- * [1, 8]) independent hypotheses from softmax(l_S / sampling_temperature) (finite, > 0) over the processed logits l,
- * S = every token (sampling_topk 0) or the sampling_topk (in [2, 16]) largest, with Gumbel-max noise from Philox4x32-10
- * keyed by seeds[b] (uint64 [B]).  The result depends only on the window's features, prompt, options and seed, not on
- * its batch position.  Scores are the untempered cumulative log-probs over (generated tokens)^length_penalty.  Outputs
- * hold num_hypotheses entries per window, window b's at [b * num_hypotheses, (b + 1) * num_hypotheses), sorted by score
- * (descending, ties to the lower hypothesis index): out_ids int32 [B * n, out_stride], out_len int32 [B * n], out_score
- * float32 [B * n] (required).  A hypothesis that found no token to sample is empty with score -inf; a cap of 0 new tokens
- * gives n empty ones with score 0.  The other arguments are those of wisb_generate_proc.  Code 1 for a bad argument. */
-int wisb_generate_sample(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len,
-                         int num_hypotheses, int sampling_topk, float sampling_temperature, const uint64_t* seeds,
-                         float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                         const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
-                         float repetition_penalty, int no_repeat_ngram_size, int32_t* out_ids, int out_stride,
-                         int32_t* out_len, float* out_score);
+ * prompts: int32 [B, prompt_len] (WIS passes the same 4-token prompt for every window, main.py:689).
+ * Outputs hold n = num_hypotheses entries per window when sampling, else one: window b's at [b * n, (b + 1) * n),
+ * sorted by score (descending, ties to the lower hypothesis index).  out_ids int32 [B * n, out_stride] (out_stride >=
+ * the largest number of new tokens of any window), out_len int32 [B * n], out_score float32 [B * n] (may be NULL unless
+ * sampling) the length-normalised log-probability of each hypothesis.  A sampled hypothesis that found no token to
+ * sample is empty with score -inf; a cap of 0 new tokens gives n empty ones with score 0.  Code 1 for a bad argument. */
+int wisb_generate(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len,
+                  const wisb_generate_options* opt, int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score);
 
 /* (5) per utterance: language token ids sorted by probability (descending) and the probabilities.
  * lang_ids_out int32 [B, n_langs], probs_out float32 [B, n_langs]. */
@@ -168,7 +162,7 @@ int wisb_buffer_to_host(const void* p, void* host, size_t nbytes);
 int wisb_encode(wisb_handle* h, const float* mel, int B, void* out, int out_on_device);
 /* An encoder output [B, 1500, d_model] (dtype 0 fp16, 1 fp32: converted on the device, rounded to nearest even), host
  * memory or (on_device != 0) device memory on the handle's device, copied into a handle-owned buffer.  It becomes the
- * source of the next wisb_generate* / wisb_detect_language / wisb_align calls that pass mel == NULL: whichever of
+ * source of the next wisb_generate / wisb_detect_language / wisb_align calls that pass mel == NULL: whichever of
  * wisb_logmel(keep_on_device) and this call came last decides that source, and such a call with another B fails with
  * code 1.  Those calls skip the encoder and run only the cross-K/V GEMM on these rows; they leave nothing for option
  * "encoder_cache" to reuse.  A host copy's time is reported in timing slot 1 (h2d). */
@@ -202,41 +196,33 @@ int wisb_set_option(wisb_handle* h, const char* key, int value);
 int wisb_debug_gemm(wisb_handle* h, const int32_t* prm, int n_prm, const uint16_t* a, const uint16_t* w, const float* bias,
                     const float* pos, const int32_t* row_slot, const int32_t* row_pos, void* out, size_t out_bytes, void* aux,
                     size_t aux_bytes, void* aux2, size_t aux2_bytes, int32_t* plan_out);
-/* ONE production token-search step (wisb_generate's processors, top-k, beam bookkeeping and step advance) on caller
- * search state, which it returns.  prm[13] int32: n_utt, beam, V, ldl (>= V), eot, no_timestamps, timestamps (0/1),
- * max_initial_timestamp_index, max_new (1..448), max_hyp (>= 1), t_max (1..448), init (0: the state as given; 1 / 2:
- * search initialisation from `prompt` first, with shared_prefix 0 / 1), prompt_len; n_prm == 15 adds the history
- * processors of wisb_generate_proc: prm[13] = repetition_penalty's float32 bit pattern, prm[14] = no_repeat_ngram_size
- * (n_prm == 13: both off).  n_utt * beam <= 1024.
+/* ONE production token-search step (wisb_generate's processors, top-k or sampling, bookkeeping and step advance) on
+ * caller search state, which it returns.  prm[15] int32: n_utt, beam, V, ldl (>= V), eot, no_timestamps, timestamps
+ * (0/1), max_initial_timestamp_index, max_new (1..448), max_hyp (>= 1), t_max (1..448), init (0: the state as given;
+ * 1 / 2: search initialisation from `prompt` first, with shared_prefix 0 / 1), prompt_len, no_repeat_ngram_size,
+ * sampling_topk (1 = search).  fprm[3] float32: length_penalty, repetition_penalty, sampling_temperature.  The options
+ * mean what they mean in wisb_generate_options.  n_utt * beam <= 1024.
  * logits float32 [n_utt*beam, ldl] (columns >= V are never read); mask uint8 [V] (bit 0: suppressed every step, bit 1:
  * at the first generated step); max_new_u int32 [n_utt] per-utterance caps in [0, max_new] or NULL; prompt int32
  * [n_utt, prompt_len] (init only).  state_i int32 in / out: DecState {pos, gen_step, n_done, all_done, ticket (0)},
  * flip, seq [2][R][max_new], indir [2][R][t_max], tokens [R], row_pos [R], done [n_utt], n_hyp [n_utt], best_len
- * [n_utt], best_tokens [n_utt][max_new]; state_f float32 in / out: cum [R], best_score [n_utt]  (R = n_utt * beam).
- * Outputs: cand_idx int32 [n_utt, 16] (beam * V + token, -1 = none) and cand_score float32 [n_utt, 16], the first
- * 2*beam entries used; row_lse float32 [n_utt*beam].  Sizes, the current history tokens and indirection entries are
- * checked before anything is launched. */
-int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, float length_penalty, const float* logits,
-                           const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
-                           float* state_f, int32_t* cand_idx, float* cand_score, float* row_lse);
-/* The same step with per-utterance search options (wisb_generate_mixed): prm[1] is the row block B of every utterance,
- * utterance u searches rows [0, beam_u[u]) (beam_u[u] in [1, B]) with 2 beam_u[u] candidates, finishes at max_hyp_u[u]
- * (>= 1) hypotheses and normalises with length_penalty_u[u] (finite); prm[9] (>= 1) is unused.  Its other rows are
- * dead: cum -inf, token eot, never a candidate (cand_idx entries 2 beam_u[u] .. 15 are -1) or a hypothesis.  With
- * init, search initialisation makes them dead. */
-int wisb_debug_search_step_mixed(wisb_handle* h, const int32_t* prm, int n_prm, const float* logits, const uint8_t* mask,
-                                 const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i, float* state_f,
-                                 int32_t* cand_idx, float* cand_score, float* row_lse, const int32_t* beam_u,
-                                 const int32_t* max_hyp_u, const float* length_penalty_u);
-/* One production sampling step (wisb_generate_sample): prm as for wisb_debug_search_step with prm[1] = the hypotheses
- * n per utterance (prm[9] >= 1 unused), seeds uint64 [n_utt].  state_i / state_f as there, except best_len [R],
- * best_tokens [R][max_new] and best_score [R]: one hypothesis per row.  Outputs: sampled int32 [R] (the token row r
- * drew, -1 = none: the row was dead, frozen or had nothing to sample), key float32 [R] (its Gumbel key), row_lse
- * float32 [R]. */
-int wisb_debug_search_step_sample(wisb_handle* h, const int32_t* prm, int n_prm, float length_penalty, int sampling_topk,
-                                  float sampling_temperature, const uint64_t* seeds, const float* logits,
-                                  const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
-                                  float* state_f, int32_t* sampled, float* key, float* row_lse);
+ * [H], best_tokens [H][max_new]; state_f float32 in / out: cum [R], best_score [H]  (R = n_utt * beam; H = n_utt, or R
+ * when sampling: one hypothesis per row).
+ * Per-utterance search options (beam_u, max_hyp_u, length_penalty_u: all three, or none) make prm[1] the row block B of
+ * every utterance: utterance u searches rows [0, beam_u[u]) (beam_u[u] in [1, B]) with 2 beam_u[u] candidates,
+ * finishes at max_hyp_u[u] (>= 1) hypotheses and normalises with length_penalty_u[u] (finite); prm[9] (>= 1) and
+ * fprm[0] are unused.  Its other rows are dead: cum -inf, token eot, never a candidate (cand_idx entries 2 beam_u[u] ..
+ * 15 are -1) or a hypothesis.  With init, search initialisation makes them dead.  Sampling takes none of them; prm[1]
+ * is then the hypotheses n per utterance, prm[9] (>= 1) is unused and seeds is uint64 [n_utt].
+ * Outputs: cand_idx int32 [n_utt, 16] and cand_score float32 [n_utt, 16]: searching, the first 2*beam entries are the
+ * candidates (beam * V + token, -1 = none) and their scores; sampling, entry k < n is the token row k drew (-1 = none:
+ * the row was dead, frozen or had nothing to sample) and its Gumbel key.  row_lse float32 [n_utt*beam].  Sizes, the
+ * current history tokens and indirection entries are checked before anything is launched. */
+int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, const float* fprm, int n_fprm,
+                           const float* logits, const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt,
+                           const int32_t* beam_u, const int32_t* max_hyp_u, const float* length_penalty_u,
+                           const uint64_t* seeds, int32_t* state_i, float* state_f, int32_t* cand_idx, float* cand_score,
+                           float* row_lse);
 /* encoder self-attention on caller data: qkv [B*1536, 3d] fp16 -> ctx [B*1536, d] fp16, d = 64 H; impl 0 = wgmma with
  * MN-major V, 1 = wgmma with the transposed Vt layout (built from the same qkv), 2 = SIMT check */
 int wisb_debug_enc_attn(wisb_handle* h, const uint16_t* qkv16, int B, int d, int H, int impl, uint16_t* ctx16_out);

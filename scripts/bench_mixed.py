@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Windows with different beam sizes and prompts: one engine call per class of options, against one mixed call
-(wisb_generate_mixed, every window its own beam / prompt / length limit in one shared decoder pass per token), against
+(wisb_generate with per-window options, every window its own beam / prompt / length limit in one shared decoder pass
+per token), against
 the batcher fed by concurrent submits of the same windows.  Synthetic large-v2 weights (peaked, as bench.py), features
 computed once; <|endoftext|> is suppressed and every window has its own max_length, so each window generates a fixed
 number of tokens (3.5 per second of audio) in every arm and the arms do the same search work.

@@ -121,7 +121,8 @@ def test_asyncio_face_and_queue_limit():
 
 
 def test_requests_with_different_max_length_share_one_call():
-    # the engine takes one length limit per window (wisb_generate_ex), so max_length is not part of the compatibility key
+    # the engine takes one length limit per window (wisb_generate_options.max_length_per_window), so max_length is not
+    # part of the compatibility key
     eng = FakeEngine(delay=0.05)
     with TranscribeBatcher(eng, max_batch=16, max_wait_ms=30) as b:
         f1 = b.submit(_window(1, 2), PROMPT, beam_size=5, max_length=30)

@@ -68,7 +68,7 @@ def test_batch16_equals_single_and_oracle(pair, beam):
 
 
 def test_per_utterance_max_length_in_one_pass(pair):
-    # requests with different length limits coalesced into ONE shared pass (wisb_generate_ex) decode exactly what
+    # requests with different length limits coalesced into ONE shared pass (max_length_per_window) decode exactly what
     # separate calls with those limits decode -- checked against the oracle on every robust case
     dims, oracle, h = pair
     mel = mel_inputs(6)

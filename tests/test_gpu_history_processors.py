@@ -10,6 +10,7 @@
   its robust cases on every decoder pass, in one timestamp case and in a multi-utterance call; with n set no returned
   sequence holds an n-gram twice; either processor changes most transcripts.
 """
+import ctypes
 import functools
 import zlib
 
@@ -445,26 +446,61 @@ def test_multi_utterance_call_matches_solo_runs():
 
 
 @pytest.mark.gpu
-def test_processors_off_is_generate_ts_bit_for_bit():
+def test_options_from_init_and_from_python_bit_for_bit():
     dims, oracle, h = loop_pair()
     mel = mel_inputs(6)
     lib = _lib.lib()
     for nb, beam in ((1, 5), (2, 1), (6, 5)):                         # persistent pass and batched pass
         P = np.ascontiguousarray(np.repeat(np.array([PROMPT], np.int32), nb, 0))
         out = []
-        for proc in (False, True):
+        for explicit in (False, True):
             ids = np.zeros((nb, 224), np.int32)
             lens = np.zeros(nb, np.int32)
             scores = np.zeros(nb, np.float32)
             m = np.ascontiguousarray(mel[:nb])
-            args = (h._h, _lib.ptr(m), nb, _lib.ptr(P), P.shape[1], beam, 1.0, 1.0, 448, None, None, 0, 0, 50)
-            if proc:
-                _lib.check(lib.wisb_generate_proc(*args, 1.0, 0, _lib.ptr(ids), 224, _lib.ptr(lens), _lib.ptr(scores)))
-            else:
-                _lib.check(lib.wisb_generate_ts(*args, _lib.ptr(ids), 224, _lib.ptr(lens), _lib.ptr(scores)))
+            if explicit:  # every field written from Python, processors off: what the ctypes mirror hands the engine
+                opt = _lib.GenerateOptions(
+                    struct_size=ctypes.sizeof(_lib.GenerateOptions), beam_size=beam, patience=1.0, length_penalty=1.0,
+                    max_length=448, timestamps=0, max_initial_timestamp_index=50, repetition_penalty=1.0,
+                    no_repeat_ngram_size=0, num_hypotheses=1, sampling_topk=1, sampling_temperature=1.0, n_extra=0,
+                    extra_suppress=None, max_length_per_window=None, beam_per_window=None, patience_per_window=None,
+                    length_penalty_per_window=None, seeds=None)
+            else:         # wisb_generate_options_init's defaults
+                opt = _lib.GenerateOptions()
+                _lib.check(lib.wisb_generate_options_init(ctypes.byref(opt)))
+                opt.beam_size, opt.max_length = beam, 448
+            _lib.check(lib.wisb_generate(h._h, _lib.ptr(m), nb, _lib.ptr(P), P.shape[1], ctypes.byref(opt), _lib.ptr(ids),
+                                         224, _lib.ptr(lens), _lib.ptr(scores)))
             out.append((ids.copy(), lens.copy(), scores.copy(), h.timing()["launches"]))
         for a, b in zip(*out):
             assert np.array_equal(a, b)
+
+
+@pytest.mark.gpu
+def test_options_struct_is_checked():
+    dims, oracle, h = loop_pair()
+    m = np.ascontiguousarray(mel_inputs(2)[:1])
+    P = np.array([PROMPT], np.int32)
+    ids, lens, scores = np.zeros((1, 224), np.int32), np.zeros(1, np.int32), np.zeros(1, np.float32)
+    lib = _lib.lib()
+
+    def run(**fields):
+        opt = _lib.GenerateOptions()
+        _lib.check(lib.wisb_generate_options_init(ctypes.byref(opt)))
+        for k, v in fields.items():
+            setattr(opt, k, v)
+        rc = lib.wisb_generate(h._h, _lib.ptr(m), 1, _lib.ptr(P), P.shape[1], ctypes.byref(opt), _lib.ptr(ids), 224,
+                               _lib.ptr(lens), _lib.ptr(scores))
+        return rc, lib.wisb_last_error().decode()
+
+    assert run(beam_size=1)[0] == 0
+    for fields, msg in ((dict(struct_size=ctypes.sizeof(_lib.GenerateOptions) - 8), "struct_size"),
+                        (dict(num_hypotheses=2), "num_hypotheses"),
+                        (dict(sampling_topk=0, num_hypotheses=2), "beam_size must be 1")):
+        rc, err = run(**fields)
+        assert rc == 1 and msg in err, (fields, err)
+    assert lib.wisb_generate(h._h, _lib.ptr(m), 1, _lib.ptr(P), P.shape[1], None, _lib.ptr(ids), 224, _lib.ptr(lens),
+                             _lib.ptr(scores)) == 1
 
 
 @pytest.mark.gpu

@@ -1,5 +1,6 @@
 """GPU: one generate call whose windows differ in beam size, patience, length penalty and prompt (other language or task
-token, same length) -- ``wisb_generate_mixed``, what ``batcher.TranscribeBatcher`` sends when it coalesces such requests.
+token, same length) -- ``wisb_generate`` with per-window options, what ``batcher.TranscribeBatcher`` sends when it
+coalesces such requests.
 
 On the peaked, timestamp-scripted synthetic model at a tiny width, every window of a mixed call must return what its solo
 call returns and what the oracle (``tests.proc_oracle.ProcOracle``: the CTranslate2 search, the timestamp rules and the

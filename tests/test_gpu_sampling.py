@@ -1,6 +1,6 @@
-"""GPU: sampling with num_hypotheses (``wisb_generate_sample``), one step at a time and end to end.
+"""GPU: sampling with num_hypotheses (``wisb_generate`` with ``sampling_topk != 1``), one step at a time and end to end.
 
-One step (``wisb_debug_search_step_sample``) on caller state is compared with the oracle's draw on the same processed
+One step (``wisb_debug_search_step`` sampling) on caller state is compared with the oracle's draw on the same processed
 logits (``tests.sampling_oracle.check_draws``): the sampled id wherever the float64 key gap beats the fp32 bound (at
 least 99 % of the rows), keys, cum within 4 ulps, and the whole integer state exactly.  Many seeds on identical logits
 check the device generator's frequencies against softmax(l_S / T) on their own.  End to end, on the peaked synthetic

@@ -550,7 +550,7 @@ def test_comparator_rejects_injected_defects(defect):
 
 
 def test_oracle_step_rules():
-    # the rules the oracle step pins (engine side: search.cu, wisb_generate_ts)
+    # the rules the oracle step pins (engine side: search.cu, wisb_generate with timestamps)
     assert [max_hypotheses(5, 0.5), max_hypotheses(2, 1.25), max_hypotheses(5, 2.0), max_hypotheses(1, 0.1)] == [3, 3, 10, 1]
     V, eot = 100, 99
     st = BeamState([[1], [2]], [-1.0, -2.0])

@@ -1,5 +1,6 @@
 """The device token search one step at a time with a beam, patience and length penalty of each utterance's own
-(``wisb_debug_search_step_mixed``, the search of ``wisb_generate_mixed``).
+(``wisb_debug_search_step`` with beam_u / max_hyp_u / length_penalty_u, the search of ``wisb_generate`` with per-window
+options).
 
 Every utterance keeps a block of B rows (B = the largest beam of the call) and searches its first b_u of them.  The step
 must equal, utterance by utterance, the oracle's ``beam_step`` at that utterance's own beam, max_hyp and length penalty

@@ -4,7 +4,7 @@
   processors + timestamp rules + log-softmax + top-2*beam exactly (ids), scores within 1e-5.
 * End to end on the timestamp-scripted test model (``weights.synth_state_dict(ts_script=...)``), 3-token prompt, against
   ``tests.ts_oracle.TimestampOracle`` on its robust cases: every decoder path, every utterance equal to its solo run.
-* ``wisb_generate_ts(..., timestamps=0)`` is ``wisb_generate_ex`` bit for bit, launch count included.
+* With timestamps off, ``max_initial_timestamp_index`` changes nothing: bit for bit, launch count included.
 """
 import functools
 import threading
@@ -255,9 +255,9 @@ def test_timestamps_off_is_generate_ex_bit_for_bit():
     mel = mel_inputs(6)
     for n, beam in ((1, 5), (2, 1), (6, 5)):                  # persistent pass and batched pass
         P = np.repeat(np.array([PROMPT], np.int32), n, 0)
-        a_ids, a_sc = h.generate(mel[:n], P, beam)                                   # wisb_generate_ex
+        a_ids, a_sc = h.generate(mel[:n], P, beam)                                   # the default index, 50
         a_t = h.timing()
-        b_ids, b_sc = h.generate(mel[:n], P, beam, max_initial_timestamp_index=7)    # wisb_generate_ts, timestamps=0
+        b_ids, b_sc = h.generate(mel[:n], P, beam, max_initial_timestamp_index=7)    # timestamps still off
         b_t = h.timing()
         assert a_ids == b_ids and np.array_equal(np.float32(a_sc), np.float32(b_sc))
         assert a_t["launches"] == b_t["launches"] and a_t["decode_steps"] == b_t["decode_steps"]

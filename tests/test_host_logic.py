@@ -44,7 +44,7 @@ def test_pad_or_trim():
     assert audio.pad_or_trim(np.zeros(5, np.float32)).shape == (480000,)
 
 
-def test_c_abi_exports_every_declared_symbol():
+def test_c_abi_v2_exports_every_declared_symbol():
     hdr = open(os.path.join(ROOT, "include", "wisb200.h")).read()
     declared = sorted(set(re.findall(r"\b(wisb_[a-z_0-9]+)\s*\(", hdr)))
     assert declared, "no declarations found"
@@ -53,7 +53,7 @@ def test_c_abi_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/wisb200.h but not exported"
     assert sorted(_lib.EXPORTS) == declared  # the ctypes table binds exactly the header
-    assert _lib.lib().wisb_abi_version() == 1
+    assert _lib.lib().wisb_abi_version() == 2
     # ... with the same number of parameters per entry point as the C prototypes
     flat = re.sub(r"/\*.*?\*/", " ", hdr, flags=re.S)
     for name, params in re.findall(r"\b(wisb_[a-z_0-9]+)\s*\(([^)]*)\)\s*;", flat):

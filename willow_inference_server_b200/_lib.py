@@ -22,6 +22,18 @@ EPI_F16, EPI_F16_GELU, EPI_RESID_F32, EPI_CONV2, EPI_CROSSKV, EPI_F32, EPI_QKV_V
 
 _lib = None
 
+
+class GenerateOptions(C.Structure):
+    """ctypes mirror of wisb_generate_options (include/wisb200.h); the pointer fields take ptr(array) or None"""
+    _fields_ = [("struct_size", C.c_uint32), ("beam_size", C.c_int32), ("patience", C.c_float),
+                ("length_penalty", C.c_float), ("max_length", C.c_int32), ("timestamps", C.c_int32),
+                ("max_initial_timestamp_index", C.c_int32), ("repetition_penalty", C.c_float),
+                ("no_repeat_ngram_size", C.c_int32), ("num_hypotheses", C.c_int32), ("sampling_topk", C.c_int32),
+                ("sampling_temperature", C.c_float), ("n_extra", C.c_int32), ("extra_suppress", C.c_void_p),
+                ("max_length_per_window", C.c_void_p), ("beam_per_window", C.c_void_p),
+                ("patience_per_window", C.c_void_p), ("length_penalty_per_window", C.c_void_p), ("seeds", C.c_void_p)]
+
+
 _SIGS = {
     "wisb_abi_version": (C.c_int, []),
     "wisb_last_error": (C.c_char_p, []),
@@ -33,22 +45,9 @@ _SIGS = {
     "wisb_destroy": (C.c_int, [C.c_void_p]),
     "wisb_get_dims": (C.c_int, [C.c_void_p, C.c_void_p]),
     "wisb_logmel": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
-    "wisb_generate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
-                                C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
-    "wisb_generate_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
-                                   C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
-    "wisb_generate_ts": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
-                                   C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
-                                   C.c_void_p, C.c_void_p]),
-    "wisb_generate_proc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
-                                     C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int,
-                                     C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
-    "wisb_generate_mixed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
-                                      C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int,
-                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
-    "wisb_generate_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float,
-                                       C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
-                                       C.c_float, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "wisb_generate_options_init": (C.c_int, [C.POINTER(GenerateOptions)]),
+    "wisb_generate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(GenerateOptions),
+                                C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_detect_language": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_buffer_alloc": (C.c_int, [C.c_int, C.c_size_t, C.POINTER(C.c_void_p)]),
     "wisb_buffer_free": (C.c_int, [C.c_void_p]),
@@ -66,14 +65,9 @@ _SIGS = {
     "wisb_debug_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
                                   C.c_void_p]),
-    "wisb_debug_search_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
-                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "wisb_debug_search_step_mixed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
-                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                               C.c_void_p, C.c_void_p, C.c_void_p]),
-    "wisb_debug_search_step_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_float,
-                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wisb_debug_search_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_enc_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "wisb_debug_dec_cross_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_dec_self_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -108,7 +102,7 @@ def lib():
             fn = getattr(l, name)  # AttributeError here = the .so does not match include/wisb200.h
             fn.restype = res
             fn.argtypes = args
-        if l.wisb_abi_version() != 1:
+        if l.wisb_abi_version() != 2:
             raise ImportError("libwisb200.so ABI version mismatch")
         _lib = l
     return _lib
@@ -234,11 +228,40 @@ class Handle:
 
     def generate(self, mel, prompts, beam_size=5, patience=1.0, length_penalty=1.0, max_length=448, extra_suppress=(),
                  B=None, timestamps=False, max_initial_timestamp_index=50, repetition_penalty=1.0, no_repeat_ngram_size=0):
-        """-> (token ids per utterance, length-normalised scores).  timestamps=True applies Whisper's timestamp rules
-        (wisb_generate_ts); the prompt must then contain neither <|notimestamps|> nor timestamp tokens.
-        repetition_penalty != 1 or no_repeat_ngram_size > 0 switches on the history processors (wisb_generate_proc).
-        beam_size, patience and length_penalty, like max_length, may each be one value per window
-        (wisb_generate_mixed)."""
+        """-> (token ids per utterance, length-normalised scores).  The options are those of wisb_generate_options:
+        timestamps=True applies Whisper's timestamp rules (the prompt must then contain neither <|notimestamps|> nor
+        timestamp tokens); repetition_penalty != 1 or no_repeat_ngram_size > 0 switches on the history processors.
+        beam_size, patience and length_penalty, like max_length, may each be one value per window."""
+        ids, lens, scores = self._generate(
+            mel, prompts, B, max_length, extra_suppress, 1, beam_size=beam_size, patience=patience,
+            length_penalty=length_penalty, timestamps=1 if timestamps else 0,
+            max_initial_timestamp_index=int(max_initial_timestamp_index), repetition_penalty=float(repetition_penalty),
+            no_repeat_ngram_size=int(no_repeat_ngram_size))
+        return [ids[b, : lens[b]].tolist() for b in range(len(lens))], scores.tolist()
+
+    def generate_sample(self, mel, prompts, num_hypotheses, sampling_topk, sampling_temperature, seeds,
+                        length_penalty=1.0, max_length=448, extra_suppress=(), B=None, timestamps=False,
+                        max_initial_timestamp_index=50, repetition_penalty=1.0, no_repeat_ngram_size=0):
+        """num_hypotheses sampled hypotheses per window (sampling_topk != 1), window b seeded by seeds[b] (uint64) ->
+        (per window the n token lists, per window the n scores), each window's sorted by score, descending."""
+        n = int(num_hypotheses)
+        ids, lens, scores = self._generate(
+            mel, prompts, B, max_length, extra_suppress, n, beam_size=1, patience=1.0, length_penalty=length_penalty,
+            num_hypotheses=n, sampling_topk=int(sampling_topk), sampling_temperature=float(sampling_temperature),
+            seeds=seeds, timestamps=1 if timestamps else 0, max_initial_timestamp_index=int(max_initial_timestamp_index),
+            repetition_penalty=float(repetition_penalty), no_repeat_ngram_size=int(no_repeat_ngram_size))
+        seqs = [ids[i, : lens[i]].tolist() for i in range(len(lens))]
+        return [seqs[b * n: (b + 1) * n] for b in range(len(lens) // n)], \
+            [scores[b * n: (b + 1) * n].tolist() for b in range(len(lens) // n)]
+
+    _PER_WINDOW = (("beam_size", "beam_per_window", np.int32), ("patience", "patience_per_window", np.float32),
+                   ("length_penalty", "length_penalty_per_window", np.float32))
+
+    def _generate(self, mel, prompts, B, max_length, extra_suppress, n, **options):
+        """The one wisb_generate call behind generate and generate_sample: checks the prompts, features, max_length (an
+        int or one per window), seeds and per-window search options, sets `options` (arrays by address) over
+        wisb_generate_options_init's defaults -> (ids int32 [B * n, stride], lens int32 [B * n], scores float32
+        [B * n]), n entries per window."""
         prompts = np.ascontiguousarray(prompts, np.int32)
         if prompts.ndim != 2:
             raise ValueError("prompts must be [B, prompt_len]")
@@ -247,85 +270,35 @@ class Handle:
             B = mel.shape[0]
         if B is None or prompts.shape[0] != B:
             raise ValueError("one prompt per feature window is required")
+        if "seeds" in options:
+            seeds = np.asarray(options["seeds"])
+            if seeds.shape != (B,) or seeds.dtype != np.uint64:
+                raise ValueError("seeds must be a uint64 array with one seed per window")
+            options["seeds"] = np.ascontiguousarray(seeds)
         per_utt = None
         if not np.isscalar(max_length):  # one limit per utterance (requests coalesced by the batcher)
             per_utt = np.ascontiguousarray(max_length, np.int32)
             if per_utt.shape != (B,):
                 raise ValueError("max_length must be an int or one int per utterance")
             max_length = int(per_utt.max())
-        stride = max(1, int(max_length) // 2)
-        ids = np.zeros((B, stride), np.int32)
-        lens = np.zeros(B, np.int32)
-        scores = np.zeros(B, np.float32)
-        extra = np.ascontiguousarray(list(extra_suppress), np.int32)
-        beams = per_window(beam_size, B, np.int32, "beam_size")
-        pats = per_window(patience, B, np.float32, "patience")
-        lps = per_window(length_penalty, B, np.float32, "length_penalty")
-        if beams is not None or pats is not None or lps is not None:
-            # (the scalars stand in for the options given per window; the engine ignores them there)
-            check(lib().wisb_generate_mixed(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1],
-                                            1 if beams is not None else int(beam_size),
-                                            1.0 if pats is not None else float(patience),
-                                            1.0 if lps is not None else float(length_penalty), int(max_length),
-                                            ptr(per_utt), ptr(extra) if extra.size else None, extra.size,
-                                            1 if timestamps else 0, int(max_initial_timestamp_index),
-                                            float(repetition_penalty), int(no_repeat_ngram_size), ptr(beams), ptr(pats),
-                                            ptr(lps), ptr(ids), stride, ptr(lens), ptr(scores)))
-        elif repetition_penalty != 1 or no_repeat_ngram_size != 0:
-            check(lib().wisb_generate_proc(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], int(beam_size),
-                                           float(patience), float(length_penalty), int(max_length), ptr(per_utt),
-                                           ptr(extra) if extra.size else None, extra.size, 1 if timestamps else 0,
-                                           int(max_initial_timestamp_index), float(repetition_penalty),
-                                           int(no_repeat_ngram_size), ptr(ids), stride, ptr(lens), ptr(scores)))
-        elif timestamps or max_initial_timestamp_index != 50:
-            check(lib().wisb_generate_ts(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], int(beam_size),
-                                         float(patience), float(length_penalty), int(max_length), ptr(per_utt),
-                                         ptr(extra) if extra.size else None, extra.size, 1 if timestamps else 0,
-                                         int(max_initial_timestamp_index), ptr(ids), stride, ptr(lens), ptr(scores)))
-        else:
-            check(lib().wisb_generate_ex(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], int(beam_size),
-                                         float(patience), float(length_penalty), int(max_length), ptr(per_utt),
-                                         ptr(extra) if extra.size else None, extra.size, ptr(ids), stride, ptr(lens),
-                                         ptr(scores)))
-        return [ids[b, : lens[b]].tolist() for b in range(B)], scores.tolist()
-
-    def generate_sample(self, mel, prompts, num_hypotheses, sampling_topk, sampling_temperature, seeds,
-                        length_penalty=1.0, max_length=448, extra_suppress=(), B=None, timestamps=False,
-                        max_initial_timestamp_index=50, repetition_penalty=1.0, no_repeat_ngram_size=0):
-        """wisb_generate_sample: num_hypotheses sampled hypotheses per window, window b seeded by seeds[b] (uint64) ->
-        (per window the n token lists, per window the n scores), each window's sorted by score, descending."""
-        prompts = np.ascontiguousarray(prompts, np.int32)
-        if prompts.ndim != 2:
-            raise ValueError("prompts must be [B, prompt_len]")
-        if mel is not None:
-            self._check_features(mel)
-            B = mel.shape[0]
-        if B is None or prompts.shape[0] != B:
-            raise ValueError("one prompt per feature window is required")
-        seeds = np.asarray(seeds)
-        if seeds.shape != (B,) or seeds.dtype != np.uint64:
-            raise ValueError("seeds must be a uint64 array with one seed per window")
-        seeds = np.ascontiguousarray(seeds)
-        per_utt = None
-        if not np.isscalar(max_length):
-            per_utt = np.ascontiguousarray(max_length, np.int32)
-            if per_utt.shape != (B,):
-                raise ValueError("max_length must be an int or one int per utterance")
-            max_length = int(per_utt.max())
-        n = int(num_hypotheses)
+        for name, field, dt in self._PER_WINDOW:
+            options[field] = per_window(options[name], B, dt, name)
+            # (a scalar given per window stands in as 1; the engine reads the array)
+            options[name] = 1 if options[field] is not None else dt(options[name]).item()
         stride = max(1, int(max_length) // 2)
         ids = np.zeros((B * n, stride), np.int32)
         lens = np.zeros(B * n, np.int32)
         scores = np.zeros(B * n, np.float32)
         extra = np.ascontiguousarray(list(extra_suppress), np.int32)
-        check(lib().wisb_generate_sample(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], n, int(sampling_topk),
-                                         float(sampling_temperature), ptr(seeds), float(length_penalty), int(max_length),
-                                         ptr(per_utt), ptr(extra) if extra.size else None, extra.size,
-                                         1 if timestamps else 0, int(max_initial_timestamp_index),
-                                         float(repetition_penalty), int(no_repeat_ngram_size), ptr(ids), stride,
-                                         ptr(lens), ptr(scores)))
-        seqs = [ids[i, : lens[i]].tolist() for i in range(B * n)]
-        return [seqs[b * n: (b + 1) * n] for b in range(B)], [scores[b * n: (b + 1) * n].tolist() for b in range(B)]
+        opt = GenerateOptions()
+        check(lib().wisb_generate_options_init(C.byref(opt)))
+        options.update(max_length=int(max_length), max_length_per_window=per_utt, n_extra=extra.size,
+                       extra_suppress=extra if extra.size else None)
+        for k, v in options.items():  # (the arrays stay referenced by `options` until the call returns)
+            setattr(opt, k, ptr(v) if v is None or isinstance(v, np.ndarray) else v)
+        check(lib().wisb_generate(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], C.byref(opt), ptr(ids), stride,
+                                  ptr(lens), ptr(scores)))
+        return ids, lens, scores
 
     def detect_language(self, mel, B=None):
         if mel is not None:
@@ -536,55 +509,16 @@ class Handle:
         """One production search step on caller state.  logits float32 [n_utt*beam, ldl] (only columns < V are read; V
         = ldl by default); mask uint8 [V] (bit 0 every step, bit 1 at the first generated step); state as made by
         search_state (its shapes give max_new and t_max); prompt int [n_utt, prompt_len]: run the search initialisation
-        (with shared_prefix) first; repetition_penalty / no_repeat_ngram_size: the history processors (either one
-        given: the 15-parameter form, the other one off; neither: the 13-parameter form); beam_u / max_hyp_u /
-        length_penalty_u (all three, [n_utt] each): wisb_debug_search_step_mixed, `beam` the row block of every
-        utterance, max_hyp and length_penalty unused.
+        (with shared_prefix) first; repetition_penalty / no_repeat_ngram_size: the history processors (None: off);
+        beam_u / max_hyp_u / length_penalty_u (all three, [n_utt] each): per-utterance search options, `beam` the row
+        block of every utterance, max_hyp and length_penalty unused.
         -> (new state, cand_idx int32 [n_utt, 2*beam] = beam*V + token or -1, cand_score
         float32 [n_utt, 2*beam], row_lse float32 [n_utt*beam])."""
-        logits = np.ascontiguousarray(logits, np.float32)
-        R, ldl = logits.shape
-        V = V or ldl
-        if R % beam:
-            raise ValueError("logits rows must be n_utt * beam")
-        n_utt = R // beam
-        mask = np.ascontiguousarray(mask, np.uint8)
-        if mask.shape != (V,):
-            raise ValueError("mask must have V entries")
-        _, _, max_new = state["seq"].shape
-        t_max = state["indir"].shape[2]
-        want = self.search_state(n_utt, beam, max_new, t_max)
-        for k, v in want.items():
-            if np.shape(state[k]) != v.shape:
-                raise ValueError(f"state[{k!r}] must have shape {v.shape}")
-        si = np.concatenate([np.asarray(state[k], np.int32).ravel() for k in want if k not in self._STATE_F])
-        sf = np.concatenate([np.asarray(state[k], np.float32).ravel() for k in self._STATE_F])
-        caps = None if max_new_u is None else np.ascontiguousarray(max_new_u, np.int32).reshape(n_utt)
-        pr = None if prompt is None else np.ascontiguousarray(prompt, np.int32).reshape(n_utt, -1)
-        init = 0 if pr is None else 1 + int(shared_prefix)
-        prm = np.asarray([n_utt, beam, V, ldl, eot, no_timestamps, 1 if timestamps else 0, max_initial_timestamp_index,
-                          max_new, max_hyp, t_max, init, 0 if pr is None else pr.shape[1]], np.int32)
-        if repetition_penalty is not None or no_repeat_ngram_size is not None:
-            rp = np.float32(1.0 if repetition_penalty is None else repetition_penalty)
-            prm = np.concatenate([prm, [rp.view(np.int32), int(no_repeat_ngram_size or 0)]]).astype(np.int32)
-        ci = np.zeros((n_utt, 16), np.int32)
-        cs = np.zeros((n_utt, 16), np.float32)
-        lse = np.zeros(R, np.float32)
-        if beam_u is None and max_hyp_u is None and length_penalty_u is None:
-            check(lib().wisb_debug_search_step(self._h, ptr(prm), prm.size, float(length_penalty), ptr(logits), ptr(mask),
-                                               ptr(caps), ptr(pr), ptr(si), ptr(sf), ptr(ci), ptr(cs), ptr(lse)))
-        else:
-            bu, hu = (None if v is None else np.ascontiguousarray(v, np.int32).reshape(n_utt) for v in (beam_u, max_hyp_u))
-            lu = None if length_penalty_u is None else np.ascontiguousarray(length_penalty_u, np.float32).reshape(n_utt)
-            check(lib().wisb_debug_search_step_mixed(self._h, ptr(prm), prm.size, ptr(logits), ptr(mask), ptr(caps), ptr(pr),
-                                                     ptr(si), ptr(sf), ptr(ci), ptr(cs), ptr(lse), ptr(bu), ptr(hu),
-                                                     ptr(lu)))
-        out, oi, of = {}, 0, 0
-        for k, v in want.items():
-            if k in self._STATE_F:
-                out[k], of = sf[of : of + v.size].reshape(v.shape).copy(), of + v.size
-            else:
-                out[k], oi = si[oi : oi + v.size].reshape(v.shape).copy(), oi + v.size
+        out, ci, cs, lse = self._search_step(
+            logits, mask, state, beam, max_hyp, 1, 1.0, None, (beam_u, max_hyp_u, length_penalty_u), eot=eot, V=V,
+            no_timestamps=no_timestamps, timestamps=timestamps, max_initial_timestamp_index=max_initial_timestamp_index,
+            length_penalty=length_penalty, max_new_u=max_new_u, prompt=prompt, shared_prefix=shared_prefix,
+            repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size)
         return out, ci[:, : 2 * beam], cs[:, : 2 * beam], lse
 
     def debug_search_step_sample(self, logits, mask, state, seeds, *, n: int, sampling_topk: int,
@@ -592,22 +526,39 @@ class Handle:
                                  timestamps: bool = False, max_initial_timestamp_index: int = 50,
                                  length_penalty: float = 1.0, max_new_u=None, prompt=None, shared_prefix: int = 0,
                                  repetition_penalty=None, no_repeat_ngram_size=None):
-        """One production sampling step on caller state (wisb_debug_search_step_sample).  As debug_search_step_state
-        with n hypotheses per utterance, the state made by search_state(..., sample=True) and seeds uint64 [n_utt].
+        """One production sampling step on caller state.  As debug_search_step_state with n hypotheses per utterance,
+        the state made by search_state(..., sample=True) and seeds uint64 [n_utt].
         -> (new state, sampled int32 [R] (-1 = none), key float32 [R], row_lse float32 [R])."""
+        seeds = np.ascontiguousarray(np.asarray(seeds, np.uint64).ravel())
+        out, ci, cs, lse = self._search_step(
+            logits, mask, state, n, 1, int(sampling_topk), float(sampling_temperature), seeds, (None, None, None),
+            eot=eot, V=V, no_timestamps=no_timestamps, timestamps=timestamps,
+            max_initial_timestamp_index=max_initial_timestamp_index, length_penalty=length_penalty, max_new_u=max_new_u,
+            prompt=prompt, shared_prefix=shared_prefix, repetition_penalty=repetition_penalty,
+            no_repeat_ngram_size=no_repeat_ngram_size)
+        # row k of utterance u drew the token in candidate slot k of u, with its Gumbel key as the score
+        return out, ci[:, :n].reshape(-1), cs[:, :n].reshape(-1), lse
+
+    def _search_step(self, logits, mask, state, rows: int, max_hyp: int, topk: int, temperature: float, seeds, per_utt,
+                     *, eot, V, no_timestamps, timestamps, max_initial_timestamp_index, length_penalty, max_new_u,
+                     prompt, shared_prefix, repetition_penalty, no_repeat_ngram_size):
+        """wisb_debug_search_step with `rows` rows per utterance (sampling when topk != 1) and per_utt = (beam_u,
+        max_hyp_u, length_penalty_u) -> (new state, cand_idx int32 [n_utt, 16], cand_score float32 [n_utt, 16],
+        row_lse float32 [R])."""
         logits = np.ascontiguousarray(logits, np.float32)
         R, ldl = logits.shape
         V = V or ldl
-        if R % n:
-            raise ValueError("logits rows must be n_utt * n")
-        n_utt = R // n
+        if R % rows:
+            raise ValueError(f"logits rows must be n_utt * {rows}")
+        n_utt = R // rows
         mask = np.ascontiguousarray(mask, np.uint8)
         if mask.shape != (V,):
             raise ValueError("mask must have V entries")
-        seeds = np.ascontiguousarray(np.asarray(seeds, np.uint64).reshape(n_utt))
+        if seeds is not None and seeds.shape != (n_utt,):
+            raise ValueError("seeds must have n_utt entries")
         _, _, max_new = state["seq"].shape
         t_max = state["indir"].shape[2]
-        want = self.search_state(n_utt, n, max_new, t_max, sample=True)
+        want = self.search_state(n_utt, rows, max_new, t_max, sample=topk != 1)
         for k, v in want.items():
             if np.shape(state[k]) != v.shape:
                 raise ValueError(f"state[{k!r}] must have shape {v.shape}")
@@ -616,24 +567,26 @@ class Handle:
         caps = None if max_new_u is None else np.ascontiguousarray(max_new_u, np.int32).reshape(n_utt)
         pr = None if prompt is None else np.ascontiguousarray(prompt, np.int32).reshape(n_utt, -1)
         init = 0 if pr is None else 1 + int(shared_prefix)
-        prm = np.asarray([n_utt, n, V, ldl, eot, no_timestamps, 1 if timestamps else 0, max_initial_timestamp_index,
-                          max_new, 1, t_max, init, 0 if pr is None else pr.shape[1]], np.int32)
-        if repetition_penalty is not None or no_repeat_ngram_size is not None:
-            rp = np.float32(1.0 if repetition_penalty is None else repetition_penalty)
-            prm = np.concatenate([prm, [rp.view(np.int32), int(no_repeat_ngram_size or 0)]]).astype(np.int32)
-        sampled = np.zeros(R, np.int32)
-        key = np.zeros(R, np.float32)
+        prm = np.asarray([n_utt, rows, V, ldl, eot, no_timestamps, 1 if timestamps else 0, max_initial_timestamp_index,
+                          max_new, max_hyp, t_max, init, 0 if pr is None else pr.shape[1], int(no_repeat_ngram_size or 0),
+                          topk], np.int32)
+        rp = 1.0 if repetition_penalty is None else repetition_penalty
+        fprm = np.asarray([length_penalty, rp, temperature], np.float32)
+        bu, hu, lu = (None if v is None else np.ascontiguousarray(v, dt).reshape(n_utt)
+                      for v, dt in zip(per_utt, (np.int32, np.int32, np.float32)))
+        ci = np.zeros((n_utt, 16), np.int32)
+        cs = np.zeros((n_utt, 16), np.float32)
         lse = np.zeros(R, np.float32)
-        check(lib().wisb_debug_search_step_sample(self._h, ptr(prm), prm.size, float(length_penalty), int(sampling_topk),
-                                                  float(sampling_temperature), ptr(seeds), ptr(logits), ptr(mask),
-                                                  ptr(caps), ptr(pr), ptr(si), ptr(sf), ptr(sampled), ptr(key), ptr(lse)))
+        check(lib().wisb_debug_search_step(self._h, ptr(prm), prm.size, ptr(fprm), fprm.size, ptr(logits), ptr(mask),
+                                           ptr(caps), ptr(pr), ptr(bu), ptr(hu), ptr(lu), ptr(seeds), ptr(si), ptr(sf),
+                                           ptr(ci), ptr(cs), ptr(lse)))
         out, oi, of = {}, 0, 0
         for k, v in want.items():
             if k in self._STATE_F:
-                out[k], of = sf[of: of + v.size].reshape(v.shape).copy(), of + v.size
+                out[k], of = sf[of : of + v.size].reshape(v.shape).copy(), of + v.size
             else:
-                out[k], oi = si[oi: oi + v.size].reshape(v.shape).copy(), oi + v.size
-        return out, sampled, key, lse
+                out[k], oi = si[oi : oi + v.size].reshape(v.shape).copy(), oi + v.size
+        return out, ci, cs, lse
 
     def debug_enc_attn(self, qkv16: np.ndarray, n_heads: int, impl: int = 0) -> np.ndarray:
         """Encoder self-attention on qkv fp16 [B, 1536, 3d] -> ctx fp16 [B, 1536, d]; impl 0 = wgmma (MN-major V),

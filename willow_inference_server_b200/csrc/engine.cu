@@ -1791,34 +1791,40 @@ int wisb_logmel(wisb_handle* h, const void* pcm, int pcm_dtype, int pcm_on_devic
   });
 }
 
-}  // extern "C"
+int wisb_generate_options_init(wisb_generate_options* opt) {
+  return guarded_nohandle([&] {
+    WISB_REQUIRE(opt != nullptr, "options pointer is NULL");
+    *opt = wisb_generate_options{};
+    opt->struct_size = sizeof(wisb_generate_options);
+    opt->beam_size = 5;
+    opt->patience = 1.f;
+    opt->length_penalty = 1.f;
+    opt->max_length = 448;
+    opt->max_initial_timestamp_index = 50;
+    opt->repetition_penalty = 1.f;
+    opt->num_hypotheses = 1;
+    opt->sampling_topk = 1;
+    opt->sampling_temperature = 1.f;
+  });
+}
 
-namespace {
-
-// sampling options of a wisb_generate_sample call (its windows all sample; beam_size 1, no per-window options)
-struct SampleCall {
-  int n = 1, topk = 0;
-  float temperature = 1.f;
-  const uint64_t* seeds = nullptr;  // [B]
-};
-
-// the body of wisb_generate_mixed (sc == nullptr) and wisb_generate_sample; with sc the output arrays hold sc->n entries
-// per window
-int generate_impl(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
-                  float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                  const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
-                  float repetition_penalty, int no_repeat_ngram_size, const int32_t* beam_per_utt,
-                  const float* patience_per_utt, const float* length_penalty_per_utt, const SampleCall* sc,
-                  int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score) {
+int wisb_generate(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len,
+                  const wisb_generate_options* opt, int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score) {
   return guarded(h, [&] {
     const Dims& dm = h->dims;
+    WISB_REQUIRE(opt != nullptr && opt->struct_size == sizeof(wisb_generate_options),
+                 "options are NULL or their struct_size is not sizeof(wisb_generate_options)");
+    const wisb_generate_options& o = *opt;
     WISB_REQUIRE(h->blob != nullptr, "handle has no model (created by wisb_create_frontend)");
     WISB_REQUIRE(B >= 1 && B <= 4096, "B out of range");
     WISB_REQUIRE(prompts != nullptr && out_ids != nullptr && out_len != nullptr, "prompts / out_ids / out_len is NULL");
-    if (beam_per_utt == nullptr) WISB_REQUIRE(beam_size >= 1 && beam_size <= MAX_BEAM, "beam_size must be in [1, 8]");
+    const bool sample = o.sampling_topk != 1;  // CTranslate2's rule
+    const int beam_size = o.beam_size;
+    const float patience = sample ? 1.f : o.patience;  // (sampling finishes a window after one hypothesis per row)
+    if (o.beam_per_window == nullptr) WISB_REQUIRE(beam_size >= 1 && beam_size <= MAX_BEAM, "beam_size must be in [1, 8]");
     WISB_REQUIRE(prompt_len >= 1 && prompt_len <= dm.n_text_ctx, "prompt length out of range");
-    WISB_REQUIRE(max_length >= 1 && max_length <= dm.n_text_ctx, "max_length must be in [1, n_text_ctx]");
-    if (patience_per_utt == nullptr) WISB_REQUIRE(patience > 0.f, "patience must be positive");
+    WISB_REQUIRE(o.max_length >= 1 && o.max_length <= dm.n_text_ctx, "max_length must be in [1, n_text_ctx]");
+    if (o.patience_per_window == nullptr) WISB_REQUIRE(patience > 0.f, "patience must be positive");
     // hypotheses that finish a window: round half up of beam x patience in fp32, at least 1.  A search records at most
     // beam hypotheses per step over at most 448 steps, so every count above 8 x 448 means "never by count"; clamping
     // at twice that keeps a huge patience from overflowing the int conversion
@@ -1827,44 +1833,50 @@ int generate_impl(wisb_handle* h, const float* mel, int B, const int32_t* prompt
     };
     // per-window search options: beam, max_hyp and length penalty of every window, and the largest beam (the row block
     // of every window)
-    const bool per_window = beam_per_utt != nullptr || patience_per_utt != nullptr || length_penalty_per_utt != nullptr;
-    if (sc) {
+    const bool per_window =
+        o.beam_per_window != nullptr || o.patience_per_window != nullptr || o.length_penalty_per_window != nullptr;
+    if (sample) {
       WISB_REQUIRE(!per_window && beam_size == 1, "sampling: beam_size must be 1, with no per-window search options");
-      WISB_REQUIRE(sc->n >= 1 && sc->n <= MAX_BEAM, "num_hypotheses must be in [1, 8]");
-      WISB_REQUIRE(sc->topk == 0 || (sc->topk >= 2 && sc->topk <= MAX_CAND), "sampling_topk must be 0 or in [2, 16]");
-      WISB_REQUIRE(std::isfinite(sc->temperature) && sc->temperature > 0.f, "sampling_temperature must be finite and > 0");
-      WISB_REQUIRE(sc->seeds != nullptr && out_score != nullptr, "seeds / out_score is NULL");
-      WISB_REQUIRE(std::isfinite(length_penalty), "length_penalty must be finite");
+      WISB_REQUIRE(o.num_hypotheses >= 1 && o.num_hypotheses <= MAX_BEAM, "num_hypotheses must be in [1, 8]");
+      WISB_REQUIRE(o.sampling_topk == 0 || (o.sampling_topk >= 2 && o.sampling_topk <= MAX_CAND),
+                   "sampling_topk must be 0 or in [2, 16]");
+      WISB_REQUIRE(std::isfinite(o.sampling_temperature) && o.sampling_temperature > 0.f,
+                   "sampling_temperature must be finite and > 0");
+      WISB_REQUIRE(o.seeds != nullptr && out_score != nullptr, "seeds / out_score is NULL");
+      WISB_REQUIRE(std::isfinite(o.length_penalty), "length_penalty must be finite");
+    } else {
+      WISB_REQUIRE(o.num_hypotheses == 1, "num_hypotheses must be 1 unless sampling (sampling_topk != 1)");
     }
     std::vector<int> beam_w, hyp_w;
     std::vector<float> lp_w;
     // rows of every window: its beam, or its hypotheses when sampling
-    int beam_max = sc ? sc->n : beam_size;
+    int beam_max = sample ? o.num_hypotheses : beam_size;
     if (per_window) {
       beam_w.resize(B);
       hyp_w.resize(B);
       lp_w.resize(B);
       beam_max = 1;
       for (int b = 0; b < B; ++b) {
-        beam_w[b] = beam_per_utt ? beam_per_utt[b] : beam_size;
+        beam_w[b] = o.beam_per_window ? o.beam_per_window[b] : beam_size;
         WISB_REQUIRE(beam_w[b] >= 1 && beam_w[b] <= MAX_BEAM, "per-window beam_size must be in [1, 8]");
-        const float p = patience_per_utt ? patience_per_utt[b] : patience;
-        if (patience_per_utt) WISB_REQUIRE(std::isfinite(p) && p > 0.f, "per-window patience must be finite and > 0");
-        lp_w[b] = length_penalty_per_utt ? length_penalty_per_utt[b] : length_penalty;
-        if (length_penalty_per_utt) WISB_REQUIRE(std::isfinite(lp_w[b]), "per-window length_penalty must be finite");
+        const float p = o.patience_per_window ? o.patience_per_window[b] : patience;
+        if (o.patience_per_window) WISB_REQUIRE(std::isfinite(p) && p > 0.f, "per-window patience must be finite and > 0");
+        lp_w[b] = o.length_penalty_per_window ? o.length_penalty_per_window[b] : o.length_penalty;
+        if (o.length_penalty_per_window) WISB_REQUIRE(std::isfinite(lp_w[b]), "per-window length_penalty must be finite");
         hyp_w[b] = max_hyp_of(beam_w[b], p);
         beam_max = std::max(beam_max, beam_w[b]);
       }
     }
-    WISB_REQUIRE(n_extra >= 0 && (n_extra == 0 || extra_suppress != nullptr), "bad extra_suppress");
+    WISB_REQUIRE(o.n_extra >= 0 && (o.n_extra == 0 || o.extra_suppress != nullptr), "bad extra_suppress");
     for (long long i = 0; i < static_cast<long long>(B) * prompt_len; ++i)
       WISB_REQUIRE(prompts[i] >= 0 && prompts[i] < dm.n_vocab, "prompt token outside the vocabulary");
-    WISB_REQUIRE(timestamps == 0 || timestamps == 1, "timestamps must be 0 or 1");
-    WISB_REQUIRE(max_initial_timestamp_index >= 0, "max_initial_timestamp_index must be >= 0");
-    WISB_REQUIRE(std::isfinite(repetition_penalty) && repetition_penalty > 0.f, "repetition_penalty must be finite and > 0");
-    WISB_REQUIRE(no_repeat_ngram_size >= 0 && no_repeat_ngram_size <= dm.n_text_ctx,
+    WISB_REQUIRE(o.timestamps == 0 || o.timestamps == 1, "timestamps must be 0 or 1");
+    WISB_REQUIRE(o.max_initial_timestamp_index >= 0, "max_initial_timestamp_index must be >= 0");
+    WISB_REQUIRE(std::isfinite(o.repetition_penalty) && o.repetition_penalty > 0.f,
+                 "repetition_penalty must be finite and > 0");
+    WISB_REQUIRE(o.no_repeat_ngram_size >= 0 && o.no_repeat_ngram_size <= dm.n_text_ctx,
                  "no_repeat_ngram_size must be in [0, n_text_ctx]");
-    if (timestamps) {
+    if (o.timestamps) {
       WISB_REQUIRE(dm.no_timestamps > dm.eot && dm.no_timestamps + 1 < dm.n_vocab, "this vocabulary has no timestamp tokens");
       for (long long i = 0; i < static_cast<long long>(B) * prompt_len; ++i) {
         WISB_REQUIRE(prompts[i] != dm.no_timestamps, "timestamp decoding: the prompt must not contain <|notimestamps|>");
@@ -1875,14 +1887,15 @@ int generate_impl(wisb_handle* h, const float* mel, int B, const int32_t* prompt
       int v = ml / 2 < ml - prompt_len ? ml / 2 : ml - prompt_len;
       return v < 0 ? 0 : v;
     };
-    int max_new = new_tokens(max_length);
+    int max_new = new_tokens(o.max_length);
     std::vector<int> per_utt;
-    if (max_length_per_utt != nullptr) {
+    if (o.max_length_per_window != nullptr) {
       per_utt.resize(B);
       max_new = 0;
       for (int b = 0; b < B; ++b) {
-        WISB_REQUIRE(max_length_per_utt[b] >= 1 && max_length_per_utt[b] <= dm.n_text_ctx, "per-utterance max_length out of range");
-        per_utt[b] = new_tokens(max_length_per_utt[b]);
+        WISB_REQUIRE(o.max_length_per_window[b] >= 1 && o.max_length_per_window[b] <= dm.n_text_ctx,
+                     "per-utterance max_length out of range");
+        per_utt[b] = new_tokens(o.max_length_per_window[b]);
         if (per_utt[b] > max_new) max_new = per_utt[b];
       }
     }
@@ -1893,14 +1906,14 @@ int generate_impl(wisb_handle* h, const float* mel, int B, const int32_t* prompt
     WISB_CUDA(cudaEventRecord(h->ev[0], s));
     const bool loaded = loaded_source(h, mel, B);
     const bool cached = !loaded && upload_mel(h, mel, B);
-    set_extra_suppress(h, extra_suppress, n_extra);
+    set_extra_suppress(h, o.extra_suppress, o.n_extra);
     time_h2d(h);
     DecodeCfg c;
     c.prompt_len = prompt_len;
-    c.ts = timestamps;
-    c.ts_max_init = max_initial_timestamp_index;
-    c.rep_penalty = repetition_penalty;
-    c.no_repeat_ngram = no_repeat_ngram_size;
+    c.ts = o.timestamps;
+    c.ts_max_init = o.max_initial_timestamp_index;
+    c.rep_penalty = o.repetition_penalty;
+    c.no_repeat_ngram = o.no_repeat_ngram_size;
     // Utterances are encoded and decoded in groups that share every decoder pass: the group's rows (utterances x beams)
     // are the M dimension of the batched pass, so the decoder weights stream once per generated token for the whole
     // group.  The group size only bounds the workspaces (cross K/V: 252 MB per large-v2 utterance).
@@ -1918,14 +1931,14 @@ int generate_impl(wisb_handle* h, const float* mel, int B, const int32_t* prompt
       // the group's largest beam as the row block
       c.beam = beam_size;
       c.max_hyp = max_hyp_of(beam_size, patience);
-      c.lp = length_penalty;
+      c.lp = o.length_penalty;
       c.mixed = 0;
-      if (sc) {
-        c.beam = sc->n;
+      if (sample) {
+        c.beam = o.num_hypotheses;
         c.sample = 1;
-        c.topk = sc->topk;
-        c.temperature = sc->temperature;
-        c.seed_host = sc->seeds + g0;
+        c.topk = o.sampling_topk;
+        c.temperature = o.sampling_temperature;
+        c.seed_host = o.seeds + g0;
       }
       if (per_window) {
         c.beam = beam_w[g0];
@@ -1948,7 +1961,7 @@ int generate_impl(wisb_handle* h, const float* mel, int B, const int32_t* prompt
       }
       const int32_t* gp = prompts + static_cast<size_t>(g0) * prompt_len;
       const int* gmx = per_utt.empty() ? nullptr : per_utt.data() + g0;
-      const size_t per = sc ? sc->n : 1;  // output entries per window
+      const size_t per = sample ? o.num_hypotheses : 1;  // output entries per window
       int32_t* gi = out_ids + g0 * per * out_stride;
       float* gs = out_score ? out_score + g0 * per : nullptr;
       steps += persistent ? decode_pass(h, c, gp, gmx, gi, out_stride, out_len + g0 * per, gs)
@@ -1960,73 +1973,6 @@ int generate_impl(wisb_handle* h, const float* mel, int B, const int32_t* prompt
     h->timing[7] = static_cast<float>(h->launches);
     h->prof_collect();
   });
-}
-
-}  // namespace
-
-extern "C" {
-
-int wisb_generate_mixed(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
-                        float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                        const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
-                        float repetition_penalty, int no_repeat_ngram_size, const int32_t* beam_per_utt,
-                        const float* patience_per_utt, const float* length_penalty_per_utt, int32_t* out_ids,
-                        int out_stride, int32_t* out_len, float* out_score) {
-  return generate_impl(h, mel, B, prompts, prompt_len, beam_size, patience, length_penalty, max_length,
-                       max_length_per_utt, extra_suppress, n_extra, timestamps, max_initial_timestamp_index,
-                       repetition_penalty, no_repeat_ngram_size, beam_per_utt, patience_per_utt, length_penalty_per_utt,
-                       nullptr, out_ids, out_stride, out_len, out_score);
-}
-
-int wisb_generate_sample(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len,
-                         int num_hypotheses, int sampling_topk, float sampling_temperature, const uint64_t* seeds,
-                         float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                         const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
-                         float repetition_penalty, int no_repeat_ngram_size, int32_t* out_ids, int out_stride,
-                         int32_t* out_len, float* out_score) {
-  SampleCall sc;
-  sc.n = num_hypotheses;
-  sc.topk = sampling_topk;
-  sc.temperature = sampling_temperature;
-  sc.seeds = seeds;
-  return generate_impl(h, mel, B, prompts, prompt_len, 1, 1.f, length_penalty, max_length, max_length_per_utt,
-                       extra_suppress, n_extra, timestamps, max_initial_timestamp_index, repetition_penalty,
-                       no_repeat_ngram_size, nullptr, nullptr, nullptr, &sc, out_ids, out_stride, out_len, out_score);
-}
-
-int wisb_generate_proc(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
-                       float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                       const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
-                       float repetition_penalty, int no_repeat_ngram_size, int32_t* out_ids, int out_stride,
-                       int32_t* out_len, float* out_score) {
-  return wisb_generate_mixed(h, mel, B, prompts, prompt_len, beam_size, patience, length_penalty, max_length,
-                             max_length_per_utt, extra_suppress, n_extra, timestamps, max_initial_timestamp_index,
-                             repetition_penalty, no_repeat_ngram_size, nullptr, nullptr, nullptr, out_ids, out_stride,
-                             out_len, out_score);
-}
-
-int wisb_generate_ts(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
-                     float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                     const int32_t* extra_suppress, int n_extra, int timestamps, int max_initial_timestamp_index,
-                     int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score) {
-  return wisb_generate_proc(h, mel, B, prompts, prompt_len, beam_size, patience, length_penalty, max_length,
-                            max_length_per_utt, extra_suppress, n_extra, timestamps, max_initial_timestamp_index, 1.f, 0,
-                            out_ids, out_stride, out_len, out_score);
-}
-
-int wisb_generate_ex(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
-                     float patience, float length_penalty, int max_length, const int32_t* max_length_per_utt,
-                     const int32_t* extra_suppress, int n_extra, int32_t* out_ids, int out_stride, int32_t* out_len,
-                     float* out_score) {
-  return wisb_generate_ts(h, mel, B, prompts, prompt_len, beam_size, patience, length_penalty, max_length,
-                          max_length_per_utt, extra_suppress, n_extra, 0, 0, out_ids, out_stride, out_len, out_score);
-}
-
-int wisb_generate(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len, int beam_size,
-                  float patience, float length_penalty, int max_length, const int32_t* extra_suppress, int n_extra,
-                  int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score) {
-  return wisb_generate_ex(h, mel, B, prompts, prompt_len, beam_size, patience, length_penalty, max_length, nullptr,
-                          extra_suppress, n_extra, out_ids, out_stride, out_len, out_score);
 }
 
 int wisb_detect_language(wisb_handle* h, const float* mel, int B, int32_t* lang_ids_out, float* probs_out) {
@@ -2305,15 +2251,13 @@ int wisb_debug_gemm(wisb_handle* h, const int32_t* prm, int n_prm, const uint16_
   });
 }
 
-// wisb_debug_search_step's body; beam_u / max_hyp_u / lp_u (all three or none): wisb_debug_search_step_mixed; sc:
-// wisb_debug_search_step_sample (`beam` = the hypotheses per utterance, per-row best_len / best_tokens / best_score)
-static int debug_search_step_impl(wisb_handle* h, const int32_t* prm, int n_prm, float length_penalty, const float* logits,
-                                  const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
-                                  float* state_f, int32_t* cand_idx, float* cand_score, float* row_lse,
-                                  const int32_t* beam_u, const int32_t* max_hyp_u, const float* lp_u,
-                                  const SampleCall* sc = nullptr) {
+int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, const float* fprm, int n_fprm,
+                           const float* logits, const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt,
+                           const int32_t* beam_u, const int32_t* max_hyp_u, const float* lp_u, const uint64_t* seeds,
+                           int32_t* state_i, float* state_f, int32_t* cand_idx, float* cand_score, float* row_lse) {
   return guarded(h, [&] {
-    WISB_REQUIRE(prm != nullptr && (n_prm == 13 || n_prm == 15) && logits && mask && state_i && state_f && cand_idx && cand_score && row_lse,
+    WISB_REQUIRE(prm != nullptr && n_prm == 15 && fprm != nullptr && n_fprm == 3 && logits && mask && state_i && state_f &&
+                     cand_idx && cand_score && row_lse,
                  "debug_search_step: bad arguments");
     const int n_utt = prm[0], beam = prm[1], V = prm[2], ldl = prm[3], eot = prm[4], no_ts = prm[5], ts = prm[6];
     const int max_init = prm[7], max_new = prm[8], max_hyp = prm[9], t_max = prm[10], init = prm[11], prompt_len = prm[12];
@@ -2322,20 +2266,23 @@ static int debug_search_step_impl(wisb_handle* h, const int32_t* prm, int n_prm,
                      max_new <= T_MAX && max_hyp >= 1 && t_max >= 1 && t_max <= T_MAX && init >= 0 && init <= 2,
                  "debug_search_step: bad scalar parameters");
     WISB_REQUIRE(!ts || (no_ts > eot && no_ts + 1 < V && V - no_ts - 1 <= 2048), "debug_search_step: bad timestamp geometry");
-    float rep_penalty = 1.f;  // prm[13]: the float's bit pattern
-    const int no_repeat_ngram = n_prm == 15 ? prm[14] : 0;
-    if (n_prm == 15) memcpy(&rep_penalty, &prm[13], sizeof(float));
+    const int no_repeat_ngram = prm[13], topk = prm[14];
+    const float length_penalty = fprm[0], rep_penalty = fprm[1], temperature = fprm[2];
     WISB_REQUIRE(std::isfinite(rep_penalty) && rep_penalty > 0.f && no_repeat_ngram >= 0 && no_repeat_ngram <= T_MAX,
                  "debug_search_step: bad history processor arguments");
     const int R = n_utt * beam;
-    if (sc)
-      WISB_REQUIRE(sc->seeds != nullptr && (sc->topk == 0 || (sc->topk >= 2 && sc->topk <= MAX_CAND)) &&
-                       std::isfinite(sc->temperature) && sc->temperature > 0.f && std::isfinite(length_penalty),
-                   "debug_search_step_sample: bad sampling arguments");
+    const bool sample = topk != 1;
+    const bool mixed = beam_u != nullptr;
+    WISB_REQUIRE(mixed == (max_hyp_u != nullptr) && mixed == (lp_u != nullptr),
+                 "debug_search_step: beam_u / max_hyp_u / lp_u come as a set");
+    if (sample)
+      WISB_REQUIRE(!mixed && seeds != nullptr && (topk == 0 || (topk >= 2 && topk <= MAX_CAND)) &&
+                       std::isfinite(temperature) && temperature > 0.f && std::isfinite(length_penalty),
+                   "debug_search_step: bad sampling arguments (or per-utterance search options with sampling)");
     // state_i: DecState (5) | flip | seq [2][R][max_new] | indir [2][R][t_max] | tokens [R] | row_pos [R] | done [n_utt] |
     // n_hyp [n_utt] | best_len [H] | best_tokens [H][max_new];  state_f: cum [R] | best_score [H]  (H = n_utt, or R when
     // sampling)
-    const int H = sc ? R : n_utt;
+    const int H = sample ? R : n_utt;
     const size_t o_seq = 6, o_ind = o_seq + 2ull * R * max_new, o_tok = o_ind + 2ull * R * t_max, o_rpos = o_tok + R;
     const size_t o_done = o_rpos + R, o_nhyp = o_done + n_utt, o_blen = o_nhyp + n_utt, o_btok = o_blen + H;
     const size_t n_i = o_btok + static_cast<size_t>(H) * max_new, n_f = static_cast<size_t>(R) + H;
@@ -2366,9 +2313,7 @@ static int debug_search_step_impl(wisb_handle* h, const int32_t* prm, int n_prm,
     if (max_new_u)
       for (int u = 0; u < n_utt; ++u)
         WISB_REQUIRE(max_new_u[u] >= 0 && max_new_u[u] <= max_new, "debug_search_step: per-utterance cap outside [0, max_new]");
-    const bool mixed = beam_u != nullptr;
     if (mixed) {
-      WISB_REQUIRE(max_hyp_u != nullptr && lp_u != nullptr, "debug_search_step: beam_u / max_hyp_u / lp_u come as a set");
       for (int u = 0; u < n_utt; ++u)
         WISB_REQUIRE(beam_u[u] >= 1 && beam_u[u] <= beam && max_hyp_u[u] >= 1 && std::isfinite(lp_u[u]),
                      "debug_search_step: per-utterance beam outside [1, beam], max_hyp < 1 or length penalty not finite");
@@ -2407,9 +2352,9 @@ static int debug_search_step_impl(wisb_handle* h, const int32_t* prm, int n_prm,
       WISB_CUDA(cudaMemcpyAsync(d_hyp.p, max_hyp_u, sizeof(int) * n_utt, cudaMemcpyHostToDevice, s));
       WISB_CUDA(cudaMemcpyAsync(d_lp.p, lp_u, sizeof(float) * n_utt, cudaMemcpyHostToDevice, s));
     }
-    if (sc) {
+    if (sample) {
       d_seed.ensure(n_utt);
-      WISB_CUDA(cudaMemcpyAsync(d_seed.p, sc->seeds, sizeof(uint64_t) * n_utt, cudaMemcpyHostToDevice, s));
+      WISB_CUDA(cudaMemcpyAsync(d_seed.p, seeds, sizeof(uint64_t) * n_utt, cudaMemcpyHostToDevice, s));
     }
     if (init) {
       d_prompt.ensure(static_cast<size_t>(n_utt) * prompt_len);
@@ -2464,10 +2409,10 @@ static int debug_search_step_impl(wisb_handle* h, const int32_t* prm, int n_prm,
       a.max_hyp_u = d_hyp.p;
       a.lp_u = d_lp.p;
     }
-    if (sc) {
+    if (sample) {
       a.sample = 1;
-      a.topk = sc->topk;
-      a.temperature = sc->temperature;
+      a.topk = topk;
+      a.temperature = temperature;
       a.seed_u = d_seed.p;
     }
     static_assert(sizeof(DecState) == 5 * sizeof(int), "DecState is five ints");
@@ -2480,56 +2425,6 @@ static int debug_search_step_impl(wisb_handle* h, const int32_t* prm, int n_prm,
     WISB_CUDA(cudaMemcpyAsync(row_lse, d_lse.p, sizeof(float) * R, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaStreamSynchronize(s));
   });
-}
-
-int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, float length_penalty, const float* logits,
-                           const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
-                           float* state_f, int32_t* cand_idx, float* cand_score, float* row_lse) {
-  return debug_search_step_impl(h, prm, n_prm, length_penalty, logits, mask, max_new_u, prompt, state_i, state_f, cand_idx,
-                                cand_score, row_lse, nullptr, nullptr, nullptr);
-}
-
-int wisb_debug_search_step_mixed(wisb_handle* h, const int32_t* prm, int n_prm, const float* logits, const uint8_t* mask,
-                                 const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i, float* state_f,
-                                 int32_t* cand_idx, float* cand_score, float* row_lse, const int32_t* beam_u,
-                                 const int32_t* max_hyp_u, const float* length_penalty_u) {
-  if (beam_u == nullptr || max_hyp_u == nullptr || length_penalty_u == nullptr) {
-    g_last_error = "debug_search_step_mixed: beam_u / max_hyp_u / length_penalty_u is NULL";
-    return 1;
-  }
-  return debug_search_step_impl(h, prm, n_prm, 1.f, logits, mask, max_new_u, prompt, state_i, state_f, cand_idx,
-                                cand_score, row_lse, beam_u, max_hyp_u, length_penalty_u);
-}
-
-int wisb_debug_search_step_sample(wisb_handle* h, const int32_t* prm, int n_prm, float length_penalty, int sampling_topk,
-                                  float sampling_temperature, const uint64_t* seeds, const float* logits,
-                                  const uint8_t* mask, const int32_t* max_new_u, const int32_t* prompt, int32_t* state_i,
-                                  float* state_f, int32_t* sampled, float* key, float* row_lse) {
-  if (prm == nullptr || n_prm < 2 || sampled == nullptr || key == nullptr) {
-    g_last_error = "debug_search_step_sample: bad arguments";
-    return 1;
-  }
-  const int n_utt = prm[0], n = prm[1];
-  if (n_utt < 1 || n < 1 || n > MAX_BEAM || n_utt * n > 1024) {
-    g_last_error = "debug_search_step_sample: bad scalar parameters";
-    return 1;
-  }
-  SampleCall sc;
-  sc.n = n;
-  sc.topk = sampling_topk;
-  sc.temperature = sampling_temperature;
-  sc.seeds = seeds;
-  // the tail leaves row k of utterance u's sampled id and key in candidate slot k of u
-  std::vector<int32_t> ci(static_cast<size_t>(n_utt) * MAX_CAND);
-  std::vector<float> cs(static_cast<size_t>(n_utt) * MAX_CAND);
-  const int rc = debug_search_step_impl(h, prm, n_prm, length_penalty, logits, mask, max_new_u, prompt, state_i, state_f,
-                                        ci.data(), cs.data(), row_lse, nullptr, nullptr, nullptr, &sc);
-  if (rc == 0)
-    for (int r = 0; r < n_utt * n; ++r) {
-      sampled[r] = ci[static_cast<size_t>(r / n) * MAX_CAND + r % n];
-      key[r] = cs[static_cast<size_t>(r / n) * MAX_CAND + r % n];
-    }
-  return rc;
 }
 
 // wisb_align's body; cap_out (wisb_debug_align_capture) receives the raw capture buffer [B][A][n_max + 1][F_max]
