@@ -73,8 +73,12 @@ typedef struct wisb_generate_options {
   /* Whisper's timestamp rules, 0 or 1: what CTranslate2 does for a prompt WITHOUT <|notimestamps|> (the 3-token sot,
    * language, task prompt).  The returned ids then contain timestamp tokens (ids > no_timestamps), which come in pairs
    * except directly before <|endoftext|> and never decrease; the first generated token is a timestamp <= no_timestamps
-   * + 1 + max_initial_timestamp_index (50: 1.00 s).  With timestamps the prompt must contain neither <|notimestamps|>
-   * nor timestamp tokens.  max_initial_timestamp_index >= 0 in both modes. */
+   * + 1 + max_initial_timestamp_index (50: 1.00 s).  The rules read only the generated tokens, so with timestamps the
+   * prompt may hold any ids, timestamps included, BEFORE its last <|startoftranscript|> (a <|startofprev|> context of
+   * earlier windows' output, as faster-whisper builds with condition_on_previous_text, initial_prompt or hotwords);
+   * from that <|startoftranscript|> on (the whole prompt when it has none) it must contain neither <|notimestamps|> nor
+   * timestamp tokens.  transformers applies its rules from the same begin index; CTranslate2's own check on such prompts
+   * is UNPINNED.  max_initial_timestamp_index >= 0 in both modes. */
   int32_t timestamps;                   /* 0 */
   int32_t max_initial_timestamp_index;  /* 50 */
   /* the history processors: repetition_penalty (finite, > 0; 1 = off) divides a positive logit and multiplies a
@@ -179,7 +183,11 @@ int wisb_get_timing(wisb_handle* h, float* out16);
  * "encoder_cache" (default 0; 1: consecutive wisb_detect_language / wisb_generate / wisb_align calls on byte-identical
  * host features of <= 2 windows reuse the encoder output and cross K/V already in HBM when the call encodes all its
  * windows in one group -- the detect -> transcribe -> translate sequence of main.py:633-644, 514-547 then encodes once
- * instead of three times; cached cross K/V in the other decoder pass's layout is rewritten by the cross-K/V GEMM alone) */
+ * instead of three times; cached cross K/V in the other decoder pass's layout is rewritten by the cross-K/V GEMM alone),
+ * "wide_prefill" (default 1; 0: prompts prefill at most 8 positions per pass, one persistent pass per position when the
+ * one-pass prefill does not fit), "prefill_rows" (default 1024, 8..65536: a prompt of more than 9 tokens is prefilled in
+ * batched passes of min(prompt_len - 1, max(the 8-position chunk, prefill_rows / windows)) positions per window; it
+ * bounds the prefill's activation workspace, about 52 d_model bytes per row) */
 int wisb_set_option(wisb_handle* h, const char* key, int value);
 
 /* ---- diagnostics used by tests/ (run the product kernels on caller data) ---- */
@@ -242,6 +250,14 @@ int wisb_debug_dec_cross_attn(wisb_handle* h, const int32_t* prm, int n_prm, con
  * indir1 int32 [R][t_ind] (slots), done int32 [R / rows_per_utt] or NULL, ctx [R, d] in / out.  Row r attends positions
  * t <= row_pos[r]: slot indir[r][t] for t < row_pos[r], its own slot row_slot[r] at t = row_pos[r] (and at every t with
  * prefill). */
+/* cross-attention of a wide prefill pass (more than 8 query rows per utterance), the kernel the engine's prefill passes
+ * launch.  prm[6] int32: n_utt (1..1024), rows_per_utt (1..448), H (1..32), n_layers, layer, swizzled (0: ckv in the
+ * linear layout of the batched pass, 1: in the persistent warp-MMA pass's layout, where 16-byte chunk c of key t's
+ * 128-byte row lies at chunk c ^ (t & 7)).  d = 64 H.  q float32 [n_utt * rows_per_utt, d] (unscaled), ckv
+ * [n_layers][2 (K, V)][n_utt][H][1536][64] (keys >= 1500 are padding and may hold anything), ctx [n_utt * rows_per_utt,
+ * d] in / out. */
+int wisb_debug_dec_prefill_cross_attn(wisb_handle* h, const int32_t* prm, int n_prm, const float* q, const uint16_t* ckv,
+                                      uint16_t* ctx16);
 int wisb_debug_dec_self_attn(wisb_handle* h, const int32_t* prm, int n_prm, const float* q, const uint16_t* kcache,
                              const uint16_t* vcache, const int32_t* row_pos, const int32_t* row_slot, const int32_t* indir0,
                              const int32_t* indir1, const int32_t* done, uint16_t* ctx16);

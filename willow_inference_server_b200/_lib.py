@@ -70,6 +70,7 @@ _SIGS = {
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_enc_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "wisb_debug_dec_cross_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wisb_debug_dec_prefill_cross_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_dec_self_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_dec_resid_ln": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_size_t,
@@ -229,8 +230,9 @@ class Handle:
     def generate(self, mel, prompts, beam_size=5, patience=1.0, length_penalty=1.0, max_length=448, extra_suppress=(),
                  B=None, timestamps=False, max_initial_timestamp_index=50, repetition_penalty=1.0, no_repeat_ngram_size=0):
         """-> (token ids per utterance, length-normalised scores).  The options are those of wisb_generate_options:
-        timestamps=True applies Whisper's timestamp rules (the prompt must then contain neither <|notimestamps|> nor
-        timestamp tokens); repetition_penalty != 1 or no_repeat_ngram_size > 0 switches on the history processors.
+        timestamps=True applies Whisper's timestamp rules to the generated tokens: the prompt may then hold any ids, timestamps
+        included, before its last <|startoftranscript|> (a <|startofprev|> context), but neither <|notimestamps|> nor
+        timestamp tokens from that token on (in the whole prompt when it has none); repetition_penalty != 1 or no_repeat_ngram_size > 0 switches on the history processors.
         beam_size, patience and length_penalty, like max_length, may each be one value per window."""
         ids, lens, scores = self._generate(
             mel, prompts, B, max_length, extra_suppress, 1, beam_size=beam_size, patience=patience,
@@ -622,6 +624,21 @@ class Handle:
         done = None if done is None else np.ascontiguousarray(np.asarray(done, np.int32).reshape(n_utt))
         prm = np.asarray([n_utt, rows_per_utt, H, L, layer, impl], np.int32)
         check(lib().wisb_debug_dec_cross_attn(self._h, ptr(prm), prm.size, ptr(q), ptr(ckv), ptr(done), ptr(ctx)))
+        return ctx
+
+    def debug_dec_prefill_cross_attn(self, q, ckv, ctx, *, layer: int, rows_per_utt: int, swizzled: bool = False):
+        """Cross-attention of a wide prefill pass: q float32 [n_utt * rows_per_utt, d] (unscaled, rows_per_utt 1..448),
+        ckv float16 [n_layers, 2 (K, V), n_utt, H, 1536, 64], in the persistent warp-MMA pass's chunk-swizzled layout when
+        `swizzled`, ctx float16 [n_utt * rows_per_utt, d] in / out."""
+        if not isinstance(ckv, np.ndarray) or ckv.dtype != np.float16 or ckv.ndim != 6 or ckv.shape[1] != 2 \
+                or ckv.shape[4:] != (1536, 64) or not ckv.flags["C_CONTIGUOUS"]:
+            raise ValueError("ckv must be a C-contiguous float16 array [n_layers, 2, n_utt, H, 1536, 64]")
+        L, _, n_utt, H = ckv.shape[:4]
+        shape = (n_utt * rows_per_utt, 64 * H)
+        q = self._inout(np.ascontiguousarray(q, np.float32), np.float32, shape, "q")
+        self._inout(ctx, np.float16, shape, "ctx")
+        prm = np.asarray([n_utt, rows_per_utt, H, L, layer, 1 if swizzled else 0], np.int32)
+        check(lib().wisb_debug_dec_prefill_cross_attn(self._h, ptr(prm), prm.size, ptr(q), ptr(ckv), ptr(ctx)))
         return ctx
 
     def debug_dec_self_attn(self, q, kcache, vcache, row_pos, row_slot, indir0, indir1, ctx, *, rows_per_utt: int,

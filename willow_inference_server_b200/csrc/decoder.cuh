@@ -102,6 +102,7 @@ struct BatchLayer {
 };
 struct BatchArgs {
   int R = 0, d = 0, H = 0, n_utt = 0, rows_per_utt = 0, t_cap = 0, t_ind = 0, prefill = 0, with_logits = 0, pdl = 0;
+  int wide = 0;                   // wide prefill pass: cross-attention through prefill_cross_attn_launch at any rows_per_utt
   const int* tokens = nullptr;    // [R]
   const int* row_pos = nullptr;   // [R]
   const int* row_slot = nullptr;  // [R]
@@ -142,8 +143,12 @@ constexpr int BD_CROSS_MAX_UTT = 1024;
 void embed_ln_launch(const BatchArgs& a, const float* g, const float* b, cudaStream_t stream);
 // ctx = self-attention of q over ly.kcache / ly.vcache through row_pos, row_slot, indir0 / indir1 (*flip), done, prefill
 void self_attn_launch(const BatchArgs& a, const BatchLayer& ly, cudaStream_t stream);
-// ctx = cross-attention of q over ly.ck / ly.cv; a.cross_tc picks the wgmma kernel (through a.ckv_map) or the SIMT one
+// ctx = cross-attention of q over ly.ck / ly.cv; a.cross_tc picks the wgmma kernel (through a.ckv_map) or the SIMT one.
+// More than 8 rows per utterance (prefill passes) always take prefill_cross_attn_launch.
 void cross_attn_launch(const BatchArgs& a, const BatchLayer& ly, cudaStream_t stream);
+// ctx = cross-attention of a.rows_per_utt (1..448) query rows per utterance, through a.ckv_map: the 128B-swizzled map over
+// linear K/V, or a map without swizzle over the persistent pass's chunk-swizzled K/V (both give the same tile image)
+void prefill_cross_attn_launch(const BatchArgs& a, const BatchLayer& ly, cudaStream_t stream);
 // x += bias + the n_splits partial slabs at a.part (stride a.part_stride), in slab order; xn = LN(x)
 void resid_ln_launch(const BatchArgs& a, int n_splits, const float* bias, const float* g, const float* b, cudaStream_t stream);
 

@@ -578,6 +578,177 @@ bd_cross_attn_tc_kernel(const __grid_constant__ CUtensorMap map_kv, const float*
 }
 
 // =====================================================================================================================
+// cross-attention for wide prefill passes (more than 8 query rows per utterance): one warpgroup CTA per (64-row query
+// tile, head, utterance), the encoder attention's scheme (encoder.cu enc_attn_kernel) on the cross K/V.
+//   Q            : the tile's fp32 rows -> fp16 after the exact 1/8 scale, as bd_cross_attn_tc_kernel rounds them,
+//                  written K-major in the 128-byte-swizzled image; rows past the utterance's last are zero
+//   S = Q K^T    : wgmma.m64n128k16 per 128-key tile, online softmax (running max / sum) on the accumulator fragment
+//   O += P V     : wgmma.m64n64k16 with P as the register A operand, V as loaded (MN-major)
+// Thread 0 feeds a 2-stage K/V ring with TMA.  The map is either the 128B-swizzled map over the linear K/V or a plain map
+// over the persistent pass's chunk-swizzled K/V (16-byte chunk c of key t at c ^ (t & 7)): key tiles start at multiples
+// of 128 keys and the stages are 1024-byte aligned, so both land as the same shared-memory image.  The tiles of one
+// (head, utterance) are adjacent in the grid, so its 384 KB of K/V are read from HBM about once.  Keys >= 1500 are
+// masked, and the last tile's V padding rows are zeroed in shared memory (0 x NaN would poison O).
+// =====================================================================================================================
+constexpr int PX_THREADS = 128;
+constexpr int PX_BM = 64;
+constexpr int PX_NB = T_ENC_PAD / 128;        // 12 key tiles
+constexpr int PX_TILE = 128 * HEAD_DIM * 2;   // 16 KB: 128 keys of K or of V
+constexpr int PX_Q_BYTES = PX_BM * HEAD_DIM * 2;
+constexpr int PX_SMEM = PX_Q_BYTES + 4 * PX_TILE /*K, V x 2 stages*/ + 64 /*barriers*/ + 1024 /*alignment slack*/;
+constexpr int PX_PAD0 = T_ENC - (PX_NB - 1) * 128;  // first padding row of the last tile (92)
+
+__device__ __forceinline__ uint32_t px_pack(float a, float b) {
+  __half2 v = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&v);
+}
+
+__global__ void __launch_bounds__(PX_THREADS, 3)
+bd_prefill_cross_attn_kernel(const __grid_constant__ CUtensorMap map_kv, const float* __restrict__ q, long long row_k0,
+                             long long row_v0, __half* __restrict__ ctx, int rows_per_utt, int d, int H) {
+  extern __shared__ uint8_t px_raw[];
+  const uint32_t raw_addr = smem_u32(px_raw);
+  const uint32_t base = (raw_addr + 1023u) & ~1023u;
+  uint8_t* smem = px_raw + (base - raw_addr);
+  const uint32_t sQ = base;
+  const uint32_t sK = base + PX_Q_BYTES;
+  const uint32_t sV = sK + 2 * PX_TILE;
+  const uint32_t bar0 = sV + 2 * PX_TILE;
+  auto kv_full = [&](int s) { return bar0 + 8u * s; };
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int qt = blockIdx.x, h = blockIdx.y, u = blockIdx.z;
+  const long long item = static_cast<long long>(u) * H + h;
+  const long long rk = row_k0 + item * T_ENC_PAD, rv = row_v0 + item * T_ENC_PAD;
+  const int r0 = qt * PX_BM;
+
+  if (tid == 0) {
+    mbar_init(kv_full(0), 1);
+    mbar_init(kv_full(1), 1);
+    fence_mbar_init();
+    tma_prefetch_desc(&map_kv);
+  }
+  __syncthreads();
+  pdl_launch_dependents();
+  pdl_wait();  // q comes from the cross-query GEMM just before
+
+  auto load_kv = [&](int j) {
+    const int st = j & 1;
+    mbar_arrive_expect_tx(kv_full(st), 2 * PX_TILE);
+    tma_load_2d(sK + st * PX_TILE, &map_kv, kv_full(st), 0, static_cast<int>(rk + j * 128));
+    tma_load_2d(sV + st * PX_TILE, &map_kv, kv_full(st), 0, static_cast<int>(rv + j * 128));
+  };
+  if (tid == 0) {
+    load_kv(0);
+    load_kv(1);
+  }
+  for (int i = tid; i < PX_BM * 8; i += PX_THREADS) {
+    const int r = i >> 3, c = i & 7, row = r0 + r;
+    uint4 v4 = make_uint4(0u, 0u, 0u, 0u);
+    if (row < rows_per_utt) {
+      const float* qr = q + (static_cast<long long>(u) * rows_per_utt + row) * d + h * HEAD_DIM + c * 8;
+      const float4 a0 = *reinterpret_cast<const float4*>(qr), a1 = *reinterpret_cast<const float4*>(qr + 4);
+      v4.x = px_pack(a0.x * 0.125f, a0.y * 0.125f);
+      v4.y = px_pack(a0.z * 0.125f, a0.w * 0.125f);
+      v4.z = px_pack(a1.x * 0.125f, a1.y * 0.125f);
+      v4.w = px_pack(a1.z * 0.125f, a1.w * 0.125f);
+    }
+    *reinterpret_cast<uint4*>(smem + r * 128 + ((c ^ (r & 7)) << 4)) = v4;
+  }
+  fence_proxy_async_smem();
+  __syncthreads();
+
+  // this thread's accumulator rows: 16 warp + lane / 4 and + 8; columns 8 j + 2 (lane % 4) + {0, 1}
+  const int cq = 2 * (lane & 3);
+  const float c = XT_LOG2E;  // (q is already scaled by head_dim^-0.5)
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  float o[HEAD_DIM / 2];
+#pragma unroll
+  for (int i = 0; i < HEAD_DIM / 2; ++i) o[i] = 0.f;
+  const uint64_t dq = make_desc_sw128(sQ, 1024);
+#pragma unroll 1
+  for (int j = 0; j < PX_NB; ++j) {
+    const int st = j & 1;
+    mbar_wait(kv_full(st), (j >> 1) & 1u);
+    if (j == PX_NB - 1) {  // padding rows of V: whole 128-byte rows, so the swizzle does not matter
+      for (int i = tid; i < (128 - PX_PAD0) * 8; i += PX_THREADS)
+        *reinterpret_cast<uint4*>(smem + (sV - base) + st * PX_TILE + PX_PAD0 * 128 + i * 16) = make_uint4(0u, 0u, 0u, 0u);
+      fence_proxy_async_smem();
+      __syncthreads();
+    }
+    float s[64];
+    const uint64_t dk = make_desc_sw128(sK + st * PX_TILE, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_ss<128, 0, 0>(s, dq + 2u * k, dk + 2u * k, k != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_reg_fence(s);
+    const int kv0 = j * 128;
+    if (kv0 + 128 > T_ENC) {
+#pragma unroll
+      for (int i = 0; i < 64; ++i)
+        if (kv0 + (i >> 2) * 8 + cq + (i & 1) >= T_ENC) s[i] = -INFINITY;
+    }
+    float alpha[2], mc[2];
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int nb = 0; nb < 16; ++nb) mx = fmaxf(mx, fmaxf(s[4 * nb + 2 * hr], s[4 * nb + 2 * hr + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[hr], mx);
+      alpha[hr] = exp2f((m_run[hr] - m_new) * c);
+      mc[hr] = m_new * c;
+      m_run[hr] = m_new;
+    }
+    uint32_t pa[8][4];
+    float rs[2] = {0.f, 0.f};
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      float p[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        p[i] = __half2float(__float2half_rn(exp2f(fmaf(s[8 * kk + i], c, -mc[(i >> 1) & 1]))));
+        rs[(i >> 1) & 1] += p[i];  // the sum of what the tensor core will actually multiply
+      }
+      pa[kk][0] = px_pack(p[0], p[1]);
+      pa[kk][1] = px_pack(p[2], p[3]);
+      pa[kk][2] = px_pack(p[4], p[5]);
+      pa[kk][3] = px_pack(p[6], p[7]);
+    }
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) l_run[hr] = l_run[hr] * alpha[hr] + rs[hr];
+#pragma unroll
+    for (int i = 0; i < HEAD_DIM / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) wgmma_rs<HEAD_DIM, 1>(o, pa[kk], make_desc_sw128(sV + st * PX_TILE + kk * 2048, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_reg_fence(o);
+    __syncthreads();  // every thread's MMAs have read stage st: refill it
+    if (tid == 0 && j + 2 < PX_NB) load_kv(j + 2);
+  }
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    l_run[hr] += __shfl_xor_sync(0xffffffffu, l_run[hr], 1);
+    l_run[hr] += __shfl_xor_sync(0xffffffffu, l_run[hr], 2);
+  }
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int row = r0 + warp * 16 + (lane >> 2) + 8 * hr;
+    if (row >= rows_per_utt) continue;
+    const float inv = 1.0f / l_run[hr];
+    __half* out = ctx + (static_cast<long long>(u) * rows_per_utt + row) * d + h * HEAD_DIM + cq;
+#pragma unroll
+    for (int nb = 0; nb < HEAD_DIM / 8; ++nb)
+      *reinterpret_cast<uint32_t*>(out + nb * 8) = px_pack(o[4 * nb + 2 * hr] * inv, o[4 * nb + 2 * hr + 1] * inv);
+  }
+}
+
+// =====================================================================================================================
 // alignment capture (Whisper.align): one CTA per (alignment head of this layer, utterance).  The item's query rows are
 // rounded to fp16 after the exact 1/8 scale, as bd_cross_attn_tc_kernel feeds them to the tensor core, the scores against
 // all 1500 keys stay in shared memory, and one exact fp32 row maximum / row sum gives the probabilities the decoder itself
@@ -733,7 +904,23 @@ void self_attn_launch(const BatchArgs& a, const BatchLayer& ly, cudaStream_t s) 
             a.row_slot, a.indir0, a.indir1, a.flip, a.done, a.ctx, a.d, a.H, a.t_cap, a.t_ind, a.rows_per_utt, a.prefill);
 }
 
+void prefill_cross_attn_launch(const BatchArgs& a, const BatchLayer& ly, cudaStream_t s) {
+  WISB_REQUIRE(a.n_utt >= 1 && a.n_utt <= 65535 && a.rows_per_utt >= 1 && a.rows_per_utt <= BD_SA_TMAX && a.H >= 1 && a.H <= 65535,
+               "prefill cross-attention: 1..65535 utterances and heads, 1..448 rows per utterance");
+  static std::atomic<unsigned long long> once{0};
+  once_per_device(once, [] {
+    WISB_CUDA(cudaFuncSetAttribute(bd_prefill_cross_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PX_SMEM));
+  });
+  const long long row_k0 = (ly.ck - a.ckv_base) / HEAD_DIM, row_v0 = (ly.cv - a.ckv_base) / HEAD_DIM;
+  bd_launch(bd_prefill_cross_attn_kernel, dim3(cdiv(a.rows_per_utt, PX_BM), a.H, a.n_utt), dim3(PX_THREADS), PX_SMEM, s,
+            a.pdl != 0, *a.ckv_map, a.q, row_k0, row_v0, a.ctx, a.rows_per_utt, a.d, a.H);
+}
+
 void cross_attn_launch(const BatchArgs& a, const BatchLayer& ly, cudaStream_t s) {
+  if (a.wide || a.rows_per_utt > MAX_BEAM) {
+    prefill_cross_attn_launch(a, ly, s);
+    return;
+  }
   WISB_REQUIRE(a.n_utt >= 1 && a.n_utt <= BD_CROSS_MAX_UTT,
                "cross-attention: 1.." + std::to_string(BD_CROSS_MAX_UTT) + " utterances in one pass, got " + std::to_string(a.n_utt));
   if (a.cross_tc) {
@@ -781,7 +968,8 @@ void align_capture_run(const AlignCaptureArgs& a, cudaStream_t s) {
 
 int batch_pass_run(const BatchArgs& a, const BatchLayer* layers, int n_layers, cudaStream_t s) {
   WISB_REQUIRE(a.R >= 1 && a.R == a.n_utt * a.rows_per_utt, "batched decoder pass: rows must be utterances x rows per utterance");
-  WISB_REQUIRE(a.rows_per_utt >= 1 && a.rows_per_utt <= MAX_BEAM, "batched decoder pass: 1..8 rows per utterance");
+  WISB_REQUIRE(a.rows_per_utt >= 1 && (a.rows_per_utt <= MAX_BEAM || (a.prefill && a.rows_per_utt <= BD_SA_TMAX)),
+               "batched decoder pass: 1..8 rows per utterance, 1..448 in a prefill pass");
   WISB_REQUIRE(a.d % 128 == 0 && a.d <= 128 * BD_LN_MAX, "batched decoder pass: d_model multiple of 128, <= 1536");
   WISB_REQUIRE(a.t_ind <= BD_SA_TMAX, "batched decoder pass: more than 448 text positions");
   struct Scope {  // brackets one kernel with the optional timing hook

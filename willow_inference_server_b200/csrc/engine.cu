@@ -131,6 +131,7 @@ struct wisb_handle {
   DevBuf<float> x;
   GemmPlan plan_conv2, plan_ckv;
   CUtensorMap ckv_map;
+  CUtensorMap ckv_map_plain;  // the same buffer without swizzle: reads the chunk-swizzled layout (wide prefill passes)
   std::vector<EncLayerPlans> enc_plans;
   AttnPlan attn_plan;
   int plans_B = 0, plans_vmn = -1, plans_pdl = -1;
@@ -158,6 +159,18 @@ struct wisb_handle {
   DevBuf<__half> bxn, bctx, bh, bkc, bvc;
   std::vector<BatchLayer> bd_layers;
   GemmPlan bd_vocab;
+  // wide prefill passes (more than 8 prompt positions per utterance in one pass, options "wide_prefill" / "prefill_rows"):
+  // activation rows, row tables and GEMM plans of their own, so the decode step's workspaces and plans stay as they are.
+  // pf_layers write K/V to pf_kc / pf_vc (layer stride pf_layer_cache, pf_tcap positions per slot); pf_rows is their
+  // row capacity (multiple of 128).
+  int wide_prefill = 1, prefill_rows = 1024;
+  int pf_rows = 0, pf_tcap = 0;
+  size_t pf_layer_cache = 0;
+  const __half* pf_kc = nullptr;
+  DevBuf<float> px, pq, ppart;
+  DevBuf<__half> pxn, pctx, ph;
+  DevBuf<int> ptok, ppos, pslot;
+  std::vector<BatchLayer> pf_layers;
   DevBuf<MegaLayer> mega_layers;
   DevBuf<__half> mega_img;  // warp-MMA pass: decoder weights as per-CTA shared-memory images (mega_mma_image)
   int enc_pdl = 1;  // encoder: programmatic dependent launch along the whole kernel chain (227 launches per window)
@@ -543,6 +556,8 @@ void ensure_encoder(wisb_handle* h, int B) {
     h->ckv.ensure(static_cast<size_t>(dm.n_dec_layers) * 2 * M * d, true);
     // the whole cross-K/V buffer as rows of one head's 64 values (for the wgmma cross-attention of the batched pass)
     make_tmap_f16_2d(&h->ckv_map, h->ckv.p, HEAD_DIM, static_cast<long long>(h->ckv.n / HEAD_DIM), HEAD_DIM, HEAD_DIM, 128);
+    make_tmap_f16_2d_swizzle(&h->ckv_map_plain, h->ckv.p, HEAD_DIM, static_cast<long long>(h->ckv.n / HEAD_DIM), HEAD_DIM,
+                             HEAD_DIM, 128, false);
     h->enc_cap = B;
   }
   // V stays in qkv (MN-major) unless the wgmma attention reads the transposed Vt: the SIMT attention (option
@@ -1153,6 +1168,8 @@ int step_loop(wisb_handle* h, int max_new, bool look_ahead, const std::function<
   return steps;
 }
 
+int wide_prefill_run(wisb_handle* h, const DecodeCfg& c, int chunk, __half* kc, __half* vc, size_t layer_cache, int t_cap);
+
 // decode utterances [u0, u0 + n_utt) of the encoded batch with the persistent pass (<= 8 rows); writes results to the
 // host arrays
 int decode_pass(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, const int* max_new_host, int32_t* out_ids,
@@ -1161,19 +1178,25 @@ int decode_pass(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, cons
   // forward the prompt prefix of all utterances in one pass when it fits the 8-row kernel
   const int pf_rows = c.n_utt * (c.prompt_len - 1);
   const bool one_pass_prefill = c.prompt_len > 1 && pf_rows <= DEC_MAX_ROWS && c.prompt_len - 1 <= MAX_BEAM;
-  persistent_setup(h, c, prompts, max_new_host, one_pass_prefill ? 1 : 0);
+  // longer prompts: batched passes of up to prefill_rows rows instead of one persistent pass per position
+  const bool wide = h->wide_prefill && c.prompt_len - 1 > MAX_BEAM;
+  persistent_setup(h, c, prompts, max_new_host, one_pass_prefill || wide ? 1 : 0);
   if (c.max_new > 0) {
     // the persistent pass is one cooperative launch per step: no graph needed
     if (one_pass_prefill) {
       enqueue_decoder_forward(h, c, false, true);
       ++steps;
+    } else if (wide) {
+      const int chunk = std::min(c.prompt_len - 1, std::max(1, h->prefill_rows / c.n_utt));
+      steps += wide_prefill_run(h, c, chunk, h->kcache.p, h->vcache.p, static_cast<size_t>(DEC_MAX_ROWS) * T_MAX * h->dims.d_model,
+                                T_MAX);
     } else {
       for (int p = 0; p + 1 < c.prompt_len; ++p) {
         enqueue_prefill(h, c);
         ++steps;
       }
     }
-    h->launches += (c.prompt_len - 1) * 2;
+    if (!wide) h->launches += (c.prompt_len - 1) * 2;
     steps += step_loop(h, c.max_new, true, [&] {
       enqueue_step(h, c);
       return 1 + 2;  // the pass + the two kernels of the search step
@@ -1199,6 +1222,59 @@ void plan_dec_gemm(wisb_handle* h, GemmPlan& p, const __half* a, long long lda, 
     e.split_stride = static_cast<long long>(M) * N;
   }
   gemm_plan(p, a, lda, w, M, N, K, e, h->num_sms, bn, 0, splits);
+}
+
+// layer descriptors + GEMM plans of the batched pass for Rp rows (a multiple of 128): A operands xn / ctx / hid, outputs q
+// and the split-K partials `part`; the QKV epilogue writes K/V of row r to slot row_slot[r], position row_pos[r] of
+// kc / vc + layer * layer_cache (t_cap positions per slot)
+void plan_batch_layers(wisb_handle* h, std::vector<BatchLayer>& layers, int Rp, float* q, __half* xn, __half* ctx,
+                       __half* hid, float* part, __half* kc, __half* vc, size_t layer_cache, int t_cap, const int* row_slot,
+                       const int* row_pos) {
+  const Dims& dm = h->dims;
+  const int d = dm.d_model, L = dm.n_dec_layers;
+  layers.assign(L, BatchLayer());
+  for (int i = 0; i < L; ++i) {
+    const DecLayerW& w = h->dec_w[i];
+    BatchLayer& b = layers[i];
+    b.kcache = kc + layer_cache * i;
+    b.vcache = vc + layer_cache * i;
+    b.ln1g = w.ln1g; b.ln1b = w.ln1b;
+    b.ob = w.ob; b.ln2g = w.ln2g; b.ln2b = w.ln2b;
+    b.cob = w.cob; b.ln3g = w.ln3g; b.ln3b = w.ln3b;
+    b.fc2b = w.fc2b;
+    b.next_g = (i + 1 < L) ? h->dec_w[i + 1].ln1g : h->F("dec.ln.g");
+    b.next_b = (i + 1 < L) ? h->dec_w[i + 1].ln1b : h->F("dec.ln.b");
+    GemmEpi e;
+    e.mode = EPI_DEC_QKV;
+    e.bias = w.qkvb;
+    e.out = q;
+    e.ldo = d;
+    e.aux = b.kcache;
+    e.aux2 = b.vcache;
+    e.d_model = d;
+    e.row_slot = row_slot;
+    e.row_pos = row_pos;
+    e.t_cap = t_cap;
+    plan_dec_gemm(h, b.qkv, xn, d, w.qkvw, Rp, 3 * d, d, e, false);
+    GemmEpi ep;  // split-K partials; bias / residual / LayerNorm happen in bd_resid_ln_kernel
+    ep.out = part;
+    ep.ldo = d;
+    plan_dec_gemm(h, b.o, ctx, d, w.ow, Rp, d, d, ep, true);
+    GemmEpi eq;
+    eq.mode = EPI_F32;
+    eq.bias = w.cqb;
+    eq.out = q;
+    eq.ldo = d;
+    plan_dec_gemm(h, b.cq, xn, d, w.cqw, Rp, d, d, eq, false);
+    plan_dec_gemm(h, b.co, ctx, d, w.cow, Rp, d, d, ep, true);
+    GemmEpi e1;
+    e1.mode = EPI_F16_GELU;
+    e1.bias = w.fc1b;
+    e1.out = hid;
+    e1.ldo = 4 * d;
+    plan_dec_gemm(h, b.fc1, xn, d, w.fc1w, Rp, 4 * d, d, e1, false);
+    plan_dec_gemm(h, b.fc2, hid, 4LL * d, w.fc2w, Rp, d, 4 * d, ep, true);
+  }
 }
 
 // workspaces + GEMM plans of the batched pass for `rows` rows and `t_need` text positions per cache slot
@@ -1230,49 +1306,8 @@ void ensure_batch(wisb_handle* h, int rows, int t_need) {
   }
   h->bkc.ensure(layer_cache * L, true);
   h->bvc.ensure(layer_cache * L, true);
-  h->bd_layers.assign(L, BatchLayer());
-  for (int i = 0; i < L; ++i) {
-    const DecLayerW& w = h->dec_w[i];
-    BatchLayer& b = h->bd_layers[i];
-    b.kcache = h->bkc.p + layer_cache * i;
-    b.vcache = h->bvc.p + layer_cache * i;
-    b.ln1g = w.ln1g; b.ln1b = w.ln1b;
-    b.ob = w.ob; b.ln2g = w.ln2g; b.ln2b = w.ln2b;
-    b.cob = w.cob; b.ln3g = w.ln3g; b.ln3b = w.ln3b;
-    b.fc2b = w.fc2b;
-    b.next_g = (i + 1 < L) ? h->dec_w[i + 1].ln1g : h->F("dec.ln.g");
-    b.next_b = (i + 1 < L) ? h->dec_w[i + 1].ln1b : h->F("dec.ln.b");
-    GemmEpi e;
-    e.mode = EPI_DEC_QKV;
-    e.bias = w.qkvb;
-    e.out = h->bq.p;
-    e.ldo = d;
-    e.aux = b.kcache;
-    e.aux2 = b.vcache;
-    e.d_model = d;
-    e.row_slot = h->row_slot.p;
-    e.row_pos = h->row_pos.p;
-    e.t_cap = tc;
-    plan_dec_gemm(h, b.qkv, h->bxn.p, d, w.qkvw, Rp, 3 * d, d, e, false);
-    GemmEpi ep;  // split-K partials; bias / residual / LayerNorm happen in bd_resid_ln_kernel
-    ep.out = h->bpart.p;
-    ep.ldo = d;
-    plan_dec_gemm(h, b.o, h->bctx.p, d, w.ow, Rp, d, d, ep, true);
-    GemmEpi eq;
-    eq.mode = EPI_F32;
-    eq.bias = w.cqb;
-    eq.out = h->bq.p;
-    eq.ldo = d;
-    plan_dec_gemm(h, b.cq, h->bxn.p, d, w.cqw, Rp, d, d, eq, false);
-    plan_dec_gemm(h, b.co, h->bctx.p, d, w.cow, Rp, d, d, ep, true);
-    GemmEpi e1;
-    e1.mode = EPI_F16_GELU;
-    e1.bias = w.fc1b;
-    e1.out = h->bh.p;
-    e1.ldo = 4 * d;
-    plan_dec_gemm(h, b.fc1, h->bxn.p, d, w.fc1w, Rp, 4 * d, d, e1, false);
-    plan_dec_gemm(h, b.fc2, h->bh.p, 4LL * d, w.fc2w, Rp, d, 4 * d, ep, true);
-  }
+  plan_batch_layers(h, h->bd_layers, Rp, h->bq.p, h->bxn.p, h->bctx.p, h->bh.p, h->bpart.p, h->bkc.p, h->bvc.p,
+                    layer_cache, tc, h->row_slot.p, h->row_pos.p);
   {
     GemmEpi ev;
     ev.mode = EPI_F32;
@@ -1374,6 +1409,67 @@ int batch_prefill(wisb_handle* h, const DecodeCfg& c, int tok_stride, int n_pos,
   return passes;
 }
 
+// workspaces + GEMM plans of the wide prefill passes for `rows` rows, K/V into kc / vc (layer stride layer_cache, t_cap
+// positions per slot)
+void ensure_prefill(wisb_handle* h, int rows, __half* kc, __half* vc, size_t layer_cache, int t_cap) {
+  const int d = h->dims.d_model;
+  int Rp = round_up(rows, 128);
+  if (Rp <= h->pf_rows && kc == h->pf_kc && t_cap == h->pf_tcap && layer_cache == h->pf_layer_cache &&
+      !h->pf_layers.empty() && h->pf_layers[0].vcache == vc)
+    return;
+  if (Rp < h->pf_rows) Rp = h->pf_rows;
+  WISB_CUDA(cudaStreamSynchronize(h->stream));
+  const size_t M = static_cast<size_t>(Rp);
+  h->px.ensure(M * d, true);
+  h->pq.ensure(M * d, true);
+  h->pxn.ensure(M * d, true);  // rows beyond the live ones stay finite: GEMM inputs whose outputs are never stored
+  h->pctx.ensure(M * d, true);
+  h->ph.ensure(M * 4 * d, true);
+  h->ppart.ensure(8 * M * d, true);
+  h->ptok.ensure(M, true);
+  h->ppos.ensure(M, true);
+  h->pslot.ensure(M, true);
+  plan_batch_layers(h, h->pf_layers, Rp, h->pq.p, h->pxn.p, h->pctx.p, h->ph.p, h->ppart.p, kc, vc, layer_cache, t_cap,
+                    h->pslot.p, h->ppos.p);
+  h->pf_rows = Rp;
+  h->pf_kc = kc;
+  h->pf_tcap = t_cap;
+  h->pf_layer_cache = layer_cache;
+}
+
+// Wide prefill: prompt positions [0, prompt_len - 1) of every utterance in h->prompt_dev as the rows of batched passes of
+// `chunk` positions per utterance, K/V into cache slot u * c.beam of kc / vc, cross-attention through
+// prefill_cross_attn_launch on h->ckv in the layout the call encoded.  Leaves what the persistent one-pass prefill leaves
+// in the cache (the caller then starts the search with the shared-prefix indirection).  Returns the number of passes.
+int wide_prefill_run(wisb_handle* h, const DecodeCfg& c, int chunk, __half* kc, __half* vc, size_t layer_cache, int t_cap) {
+  const int L = h->dims.n_dec_layers, n_pos = c.prompt_len - 1;
+  ensure_prefill(h, c.n_utt * chunk, kc, vc, layer_cache, t_cap);
+  for (int i = 0; i < L; ++i) bind_cross_kv(h, h->pf_layers[i], i, c.u0, c.B_total);
+  int passes = 0;
+  for (int p0 = 0; p0 < n_pos; p0 += chunk, ++passes) {
+    const int ch = std::min(chunk, n_pos - p0);
+    prefill_rows_run(h->ptok.p, h->ppos.p, h->pslot.p, h->prompt_dev.p, c.prompt_len, c.n_utt, p0, ch, c.beam, h->stream);
+    BatchArgs a = make_batch_args(h, c);
+    a.R = c.n_utt * ch;
+    a.rows_per_utt = ch;
+    a.prefill = 1;
+    a.wide = 1;
+    a.t_cap = t_cap;
+    a.tokens = h->ptok.p;
+    a.row_pos = h->ppos.p;
+    a.row_slot = h->pslot.p;
+    a.x = h->px.p;
+    a.xn = h->pxn.p;
+    a.q = h->pq.p;
+    a.ctx = h->pctx.p;
+    a.part = h->ppart.p;
+    a.part_stride = static_cast<long long>(h->pf_rows) * h->dims.d_model;
+    if (h->ckv_is_sw) a.ckv_map = &h->ckv_map_plain;
+    h->launches += 1 + batch_pass_run(a, h->pf_layers.data(), L, h->stream);
+  }
+  return passes;
+}
+
 // cross K/V of utterance u0 of a batch of B_total encoded windows for every layer of the batched pass
 void bind_batch_cross_kv(wisb_handle* h, int u0, int B_total) {
   for (int i = 0; i < h->dims.n_dec_layers; ++i) bind_cross_kv(h, h->bd_layers[i], i, u0, B_total);
@@ -1391,7 +1487,13 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
     // ---- prompt prefix: every utterance's positions [0, prompt_len - 1) as rows of shared passes (<= 8 positions and
     //      <= the row capacity per pass), K/V into the slot of the utterance's first beam
     const int chunk_max = std::max(1, std::min(h->bd_rows / c.n_utt, MAX_BEAM));
-    steps += batch_prefill(h, c, c.prompt_len, c.prompt_len - 1, chunk_max, c.beam, false);
+    // prompts longer than 9 tokens: wide passes of up to prefill_rows rows (> 8 positions per utterance)
+    const int wide = std::min(c.prompt_len - 1, std::max(chunk_max, h->prefill_rows / c.n_utt));
+    if (h->wide_prefill && c.prompt_len - 1 > MAX_BEAM && wide > chunk_max)
+      steps += wide_prefill_run(h, c, wide, h->bkc.p, h->bvc.p, static_cast<size_t>(h->bd_rows) * h->bd_tcap * h->dims.d_model,
+                                h->bd_tcap);
+    else
+      steps += batch_prefill(h, c, c.prompt_len, c.prompt_len - 1, chunk_max, c.beam, false);
     search_init_run(make_batch_search_args(h, c), h->prompt_dev.p, s, 1);
     cudaGraphExec_t g = nullptr;
     if (h->use_graphs && !h->profile) {  // (the per-kernel timing hook needs eager launches)
@@ -1739,6 +1841,11 @@ int wisb_set_option(wisb_handle* h, const char* key, int value) {
       drop_graphs(h);
     }
     else if (k == "decoder_batch") h->decoder_batch = value;  // 2 = use the batched pass even for <= 8 rows (tests)
+    else if (k == "wide_prefill") h->wide_prefill = value ? 1 : 0;  // 0: prompts prefill at most 8 positions per pass
+    else if (k == "prefill_rows") {
+      WISB_REQUIRE(value >= 8 && value <= 65536, "prefill_rows must be in [8, 65536]");
+      h->prefill_rows = value;
+    }
     else throw Error(1, "unknown option '" + k + "'");
   });
 }
@@ -1878,9 +1985,18 @@ int wisb_generate(wisb_handle* h, const float* mel, int B, const int32_t* prompt
                  "no_repeat_ngram_size must be in [0, n_text_ctx]");
     if (o.timestamps) {
       WISB_REQUIRE(dm.no_timestamps > dm.eot && dm.no_timestamps + 1 < dm.n_vocab, "this vocabulary has no timestamp tokens");
-      for (long long i = 0; i < static_cast<long long>(B) * prompt_len; ++i) {
-        WISB_REQUIRE(prompts[i] != dm.no_timestamps, "timestamp decoding: the prompt must not contain <|notimestamps|>");
-        WISB_REQUIRE(prompts[i] <= dm.no_timestamps, "timestamp decoding: the prompt must not contain timestamp tokens");
+      // the rules read only generated tokens, so a previous-text context (<|startofprev|> ... before the LAST
+      // <|startoftranscript|>) may hold any id, timestamps included; from that sot on (the whole prompt if it has none)
+      // <|notimestamps|> and timestamps are refused
+      for (int b = 0; b < B; ++b) {
+        const int32_t* p = prompts + static_cast<size_t>(b) * prompt_len;
+        int from = 0;
+        for (int i = 0; i < prompt_len; ++i)
+          if (p[i] == dm.sot) from = i;
+        for (int i = from; i < prompt_len; ++i) {
+          WISB_REQUIRE(p[i] != dm.no_timestamps, "timestamp decoding: the prompt must not contain <|notimestamps|>");
+          WISB_REQUIRE(p[i] <= dm.no_timestamps, "timestamp decoding: the prompt must not contain timestamp tokens");
+        }
       }
     }
     auto new_tokens = [&](int ml) {  // CTranslate2: at most max_length / 2 new tokens, max_length in total
@@ -2612,6 +2728,49 @@ int wisb_debug_dec_cross_attn(wisb_handle* h, const int32_t* prm, int n_prm, con
     ly.ck = dckv.p + static_cast<size_t>(2 * layer) * block;
     ly.cv = dckv.p + static_cast<size_t>(2 * layer + 1) * block;
     cross_attn_launch(a, ly, s);
+    WISB_CUDA(cudaMemcpyAsync(ctx16, dctx.p, sizeof(__half) * rows * d, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+int wisb_debug_dec_prefill_cross_attn(wisb_handle* h, const int32_t* prm, int n_prm, const float* q, const uint16_t* ckv,
+                                      uint16_t* ctx16) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(prm != nullptr && n_prm == 6 && q && ckv && ctx16, "debug_dec_prefill_cross_attn: bad arguments");
+    const int n_utt = prm[0], rpu = prm[1], H = prm[2], n_layers = prm[3], layer = prm[4], swizzled = prm[5];
+    WISB_REQUIRE(n_utt >= 1 && n_utt <= BD_CROSS_MAX_UTT,
+                 "debug_dec_prefill_cross_attn: 1.." + std::to_string(BD_CROSS_MAX_UTT) + " utterances in one pass");
+    WISB_REQUIRE(rpu >= 1 && rpu <= T_MAX, "debug_dec_prefill_cross_attn: 1..448 rows per utterance");
+    WISB_REQUIRE(H >= 1 && H <= 32 && n_layers >= 1 && layer >= 0 && layer < n_layers && (swizzled == 0 || swizzled == 1),
+                 "debug_dec_prefill_cross_attn: bad heads / layer / swizzled");
+    cudaStream_t s = h->stream;
+    const int d = H * HEAD_DIM;
+    const size_t rows = static_cast<size_t>(n_utt) * rpu;
+    const size_t block = static_cast<size_t>(n_utt) * H * T_ENC_PAD * HEAD_DIM;  // one layer's K (or V), all utterances
+    const size_t ckv_elems = static_cast<size_t>(n_layers) * 2 * block;
+    WISB_REQUIRE(ckv_elems / HEAD_DIM < (1ull << 31), "debug_dec_prefill_cross_attn: cross K/V too large for one tensor map");
+    DevBuf<float> dq;
+    DevBuf<__half> dckv, dctx;
+    BatchArgs a;
+    a.R = static_cast<int>(rows);
+    a.d = d;
+    a.H = H;
+    a.n_utt = n_utt;
+    a.rows_per_utt = rpu;
+    a.prefill = 1;
+    a.wide = 1;
+    a.q = to_device(dq, q, rows * d, s);
+    a.ctx = to_device(dctx, ctx16, rows * d, s);
+    a.num_sms = h->num_sms;
+    a.ckv_base = to_device(dckv, ckv, ckv_elems, s);
+    CUtensorMap map;  // as the engine's ckv_map (linear layout) or ckv_map_plain (chunk-swizzled layout)
+    make_tmap_f16_2d_swizzle(&map, dckv.p, HEAD_DIM, static_cast<long long>(ckv_elems / HEAD_DIM), HEAD_DIM, HEAD_DIM, 128,
+                             swizzled == 0);
+    a.ckv_map = &map;
+    BatchLayer ly;
+    ly.ck = dckv.p + static_cast<size_t>(2 * layer) * block;
+    ly.cv = dckv.p + static_cast<size_t>(2 * layer + 1) * block;
+    prefill_cross_attn_launch(a, ly, s);
     WISB_CUDA(cudaMemcpyAsync(ctx16, dctx.p, sizeof(__half) * rows * d, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaStreamSynchronize(s));
   });

@@ -399,12 +399,18 @@ EncodeTiledFn get_encode_fn() {
 // 2-D fp16 tensor map: inner dimension `cols` (contiguous), `rows` rows of stride `ld` elements, 128B swizzle
 void make_tmap_f16_2d(CUtensorMap* map, const void* ptr, long long cols, long long rows, long long ld, int box_cols,
                       int box_rows) {
+  make_tmap_f16_2d_swizzle(map, ptr, cols, rows, ld, box_cols, box_rows, true);
+}
+
+void make_tmap_f16_2d_swizzle(CUtensorMap* map, const void* ptr, long long cols, long long rows, long long ld,
+                              int box_cols, int box_rows, bool swizzle_128b) {
   cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
   cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld) * 2};
   cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = get_encode_fn()(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                               CU_TENSOR_MAP_INTERLEAVE_NONE,
+                               swizzle_128b ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) throw Error(2, "cuTensorMapEncodeTiled failed with CUresult " + std::to_string(static_cast<int>(r)));
 }

@@ -56,6 +56,9 @@ void gemm_ref_run(const __half* a, long long lda, const __half* w, float* c, int
 // 2-D fp16 tensor map: inner dimension `cols` (contiguous), `rows` rows of stride `ld` elements, 128B swizzle
 void make_tmap_f16_2d(CUtensorMap* map, const void* ptr, long long cols, long long rows, long long ld, int box_cols,
                       int box_rows);
+// the same with the swizzle chosen: false = none (the box lands in shared memory row-major as it lies in memory)
+void make_tmap_f16_2d_swizzle(CUtensorMap* map, const void* ptr, long long cols, long long rows, long long ld,
+                              int box_cols, int box_rows, bool swizzle_128b);
 
 // ------------------------------------------------------------------ log-mel front end (logmel.cu)
 // pcm: B utterances, f32 or s16, utterance b starts at pcm + offsets[b] (elements) and has n_samples[b] samples

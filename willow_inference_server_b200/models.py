@@ -158,6 +158,21 @@ def check_sampling_options(num_hypotheses, sampling_topk, sampling_temperature, 
     return True
 
 
+def check_timestamp_prompt(prompt, sot: int, no_timestamps: int) -> None:
+    """Raise ValueError unless `prompt` may start a timestamp-mode search (wisb_generate's rule, restated).
+
+    The timestamp rules read only the generated tokens, so everything before the prompt's last <|startoftranscript|>
+    (faster-whisper's <|startofprev|> context of earlier windows' output, timestamps included) may be any id.  From that
+    token on (the whole prompt when it has none) <|notimestamps|> and timestamp ids are refused."""
+    p = [int(t) for t in prompt]
+    start = max((i for i, t in enumerate(p) if t == sot), default=0)
+    for t in p[start:]:
+        if t == no_timestamps:
+            raise ValueError("timestamp decoding: the prompt must not contain <|notimestamps|>")
+        if t > no_timestamps:
+            raise ValueError("timestamp decoding: the prompt must not contain timestamp tokens")
+
+
 def window_seeds(random_seed, n: int) -> np.ndarray:
     """The seed of each of the n windows of a sampling call: random_seed None (one call seed s drawn from the stream
     set_random_seed resets), an int s, or one int per window.  For a call seed s window w gets s + w mod 2^64, so a
@@ -384,6 +399,9 @@ class Whisper:
         if len(with_ts) != 1:
             raise ValueError("the prompts of one call must all contain <|notimestamps|> or all omit it")
         timestamps = with_ts.pop()
+        if timestamps:
+            for q in prompts:
+                check_timestamp_prompt(q, self._dims.get("sot", 50258), no_ts)  # (every Whisper vocabulary: 50258)
         if isinstance(max_initial_timestamp_index, bool) or int(max_initial_timestamp_index) != max_initial_timestamp_index \
                 or max_initial_timestamp_index < 0:
             raise ValueError("max_initial_timestamp_index must be a non-negative int")
