@@ -2,13 +2,13 @@
 positions per pass (0), alternated rep by rep in one process.
 
 Prompts are shaped like faster-whisper's: [<|startofprev|>] + earlier text and timestamps + <|startoftranscript|>
-<|en|> <|transcribe|> (+ <|notimestamps|> with timestamps off), 4 to 227 tokens.  <|endoftext|> is suppressed and
-max_length set so that every arm generates GEN tokens.  Workloads: 1 window at beam 5 (the persistent pass) and 16
+<|en|> <|transcribe|> (+ <|notimestamps|> with timestamps off), 4 to 227 tokens (--lens).  <|endoftext|> is suppressed
+and max_length set so that every arm generates GEN tokens.  Workloads: 1 window at beam 5 (the persistent pass) and 16
 windows at beam 5 (the batched pass).  Per arm: the median call time (device events, encoder included), decode steps,
 and the prefill's share of the call: prefill = decode time of a 1-token call minus one step, a step being the decode
 time difference between the GEN-token and the 1-token call over GEN - 1.
 
-    python scripts/bench_prompt.py [--reps 5] [--out bench_prompt.json]
+    python scripts/bench_prompt.py [--reps 5] [--lens 4,9,32,128,227] [--out bench_prompt.json]
 """
 import argparse
 import json
@@ -42,6 +42,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--out", default="")
+    ap.add_argument("--lens", default="4,9,32,128,227", help="prompt lengths, comma-separated")
     args = ap.parse_args()
     import subprocess
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -57,7 +58,7 @@ def main():
     rows = []
     for n_win in (1, 16):
         for ts in (False, True):
-            for plen in (4, 32, 128, 227):
+            for plen in (int(x) for x in args.lens.split(",")):
                 P = np.repeat(np.array([prompt_of(plen, ts, rng)], np.int32), n_win, 0)
                 ml20, ml1 = max(2 * GEN, plen + GEN), plen + 1
                 res = {0: {"t": [], "d20": [], "d1": []}, 1: {"t": [], "d20": [], "d1": []}}

@@ -77,12 +77,18 @@ struct SearchArgs {
   int topk = 0;                   // 0: every token with a finite processed logit; else in [2, MAX_CAND]
   float temperature = 1.f;        // finite, > 0
   const unsigned long long* seed_u = nullptr;  // [n_utt]
+  // device word written by search_init: prompt positions a prefill pass forwarded into the cache slot of every window's
+  // first row (0, prompt_len - 1, or prompt_len when that pass also produced the first step's logits, in its row
+  // u * prompt_len + prompt_len - 1).  Positions below it are read from that slot by every row.  Null: 0.
+  int* prompt_fed = nullptr;
 };
 void search_step_run(const SearchArgs& a, cudaStream_t stream);
 // prompt prefill: no search, just feed the next prompt token and advance the position
 void prefill_advance_run(int* tokens, const int* prompt /*[n_utt][prompt_len]*/, int prompt_len, int R, int beam,
                          DecState* st, cudaStream_t stream);
-void search_init_run(const SearchArgs& a, const int* prompt, cudaStream_t stream, int shared_prefix = 0);
+// fed: the prompt positions already in each window's prefix slot (SearchArgs::prompt_fed), 0 .. prompt_len; decoding
+// starts at position min(fed, prompt_len - 1)
+void search_init_run(const SearchArgs& a, const int* prompt, cudaStream_t stream, int fed = 0);
 // rows of a batched prefill pass: row i = prompt position p0 + i % chunk of utterance i / chunk, cache slot = the
 // utterance's first beam
 void prefill_rows_run(int* tokens, int* row_pos, int* row_slot, const int* prompt, int prompt_len, int n_utt, int p0,

@@ -147,6 +147,7 @@ struct wisb_handle {
   DevBuf<int> cand_idx, tokens, seq0, seq1, ind0, ind1, flip, done, n_hyp, best_len, best_tokens, prompt_dev, lang_ids;
   DevBuf<DecState> st;
   DevBuf<int> row_pos, row_slot, max_new_u;
+  DevBuf<int> prompt_fed;  // one word: SearchArgs::prompt_fed
   DevBuf<int> beam_u, max_hyp_u;  // per-utterance search options of a call that mixes them (SearchArgs::beam_u)
   DevBuf<float> lp_u;
   DevBuf<unsigned long long> seed_u;  // per-utterance seeds of a sampling call (SearchArgs::seed_u)
@@ -472,6 +473,7 @@ void finish_create(wisb_handle* h) {
   h->vcache.ensure(cache, true);
   h->flip.ensure(1, true);
   h->st.ensure(1, true);
+  h->prompt_fed.ensure(1, true);
   ensure_search(h, DEC_MAX_ROWS);
   h->mega_layers.ensure(d.n_dec_layers);
   h->mega_layers_host.ensure(d.n_dec_layers);
@@ -872,6 +874,7 @@ SearchArgs make_search_args(wisb_handle* h, const DecodeCfg& c) {
   a.st = h->st.p;
   a.row_pos = h->row_pos.p;
   a.row_slot = h->row_slot.p;
+  a.prompt_fed = h->prompt_fed.p;
   a.max_new_u = c.per_utt_max_new ? h->max_new_u.p : nullptr;
   a.rep_penalty = c.rep_penalty;
   a.no_repeat_ngram = c.no_repeat_ngram;
@@ -958,8 +961,9 @@ void upload_mega_layers(wisb_handle* h, const DecodeCfg& c) {
                             cudaMemcpyHostToDevice, h->stream));
 }
 
-// one decoder forward for R <= 8 rows at position st->pos: ONE launch of the persistent pass
-void enqueue_decoder_forward(wisb_handle* h, const DecodeCfg& c, bool with_logits, bool prefill_pass = false) {
+// one decoder forward for R <= 8 rows at position st->pos: ONE launch of the persistent pass.  pf_len > 0: prompt
+// positions [0, pf_len) of every utterance instead (with_logits: logits of every one of those rows)
+void enqueue_decoder_forward(wisb_handle* h, const DecodeCfg& c, bool with_logits, int pf_len = 0) {
   const Dims& dm = h->dims;
   MegaArgs a;
   a.layers = h->mega_layers.p;
@@ -996,8 +1000,8 @@ void enqueue_decoder_forward(wisb_handle* h, const DecodeCfg& c, bool with_logit
   a.beam = c.beam;
   a.t_max = T_MAX;
   a.tokens = h->tokens.p;
-  if (prefill_pass) {  // the whole prompt prefix of every utterance in ONE pass (rows = utterances x prefix positions)
-    a.pf_len = c.prompt_len - 1;
+  if (pf_len > 0) {  // the prompt positions of every utterance in ONE pass (rows = utterances x positions)
+    a.pf_len = pf_len;
     a.pf_tok_stride = c.prompt_len;
     a.pf_slot_stride = c.beam;
     a.R = c.n_utt * a.pf_len;
@@ -1125,20 +1129,20 @@ void read_results(wisb_handle* h, const DecodeCfg& c, const int* max_new_host, i
   }
 }
 
-// setup of the persistent pass for this batch slice: prompts (and caps), search state, layer descriptors
-void persistent_setup(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, const int* max_new_host,
-                      int shared_prefix = 0) {
+// setup of the persistent pass for this batch slice: prompts (and caps), search state (`fed` prompt positions forwarded
+// by one prefill pass, search_init_run), layer descriptors
+void persistent_setup(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, const int* max_new_host, int fed = 0) {
   upload_prompts(h, prompts, max_new_host, c);
-  search_init_run(make_search_args(h, c), h->prompt_dev.p, h->stream, shared_prefix);
+  search_init_run(make_search_args(h, c), h->prompt_dev.p, h->stream, fed);
   upload_mega_layers(h, c);
 }
 
-// Generated-token loop of both decoder passes: enqueue() issues one step and returns its kernel launches; the loop ends at
+// Generated-token loop of both decoder passes: enqueue(gs) issues step gs and returns its kernel launches; the loop ends at
 // the first step whose `all_done` word reads 1.  With look_ahead (the persistent pass) step gs + 1 is enqueued BEFORE the
 // host waits for step gs's word (the kernels of a step that turns out to be superfluous leave at once on the device flag),
 // so neither the launch latency of the cooperative kernel nor the host's wake-up sits between two steps.  The batched
 // pass polls after every step instead: its GEMMs do not exit early.  Returns the steps that did work.
-int step_loop(wisb_handle* h, int max_new, bool look_ahead, const std::function<int()>& enqueue) {
+int step_loop(wisb_handle* h, int max_new, bool look_ahead, const std::function<int(int gs)>& enqueue) {
   cudaStream_t s = h->stream;
   volatile int* flag = h->pin_i.p;
   flag[0] = flag[1] = 0;
@@ -1148,7 +1152,7 @@ int step_loop(wisb_handle* h, int max_new, bool look_ahead, const std::function<
   }
   int steps = 0;
   for (int gs = 0; gs < max_new; ++gs) {
-    h->launches += enqueue();
+    h->launches += enqueue(gs);
     ++steps;
     WISB_CUDA(cudaMemcpyAsync(const_cast<int*>(flag) + (gs & 1), &h->st.p->all_done, sizeof(int), cudaMemcpyDeviceToHost, s));
     if (!look_ahead) {
@@ -1175,32 +1179,41 @@ int wide_prefill_run(wisb_handle* h, const DecodeCfg& c, int chunk, __half* kc, 
 int decode_pass(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, const int* max_new_host, int32_t* out_ids,
                 int out_stride, int32_t* out_len, float* out_score) {
   int steps = 0;
-  // forward the prompt prefix of all utterances in one pass when it fits the 8-row kernel
-  const int pf_rows = c.n_utt * (c.prompt_len - 1);
-  const bool one_pass_prefill = c.prompt_len > 1 && pf_rows <= DEC_MAX_ROWS && c.prompt_len - 1 <= MAX_BEAM;
+  const int P = c.prompt_len;
+  // every prompt position of every utterance fits one pass of the 8-row kernel: that pass also yields the logits of the
+  // first step, which then runs no pass of its own
+  const bool fused = c.n_utt * P <= DEC_MAX_ROWS && P <= MAX_BEAM;
+  // else the prompt prefix (all but the last token) in one pass when it fits
+  const bool one_pass_prefill = !fused && P > 1 && c.n_utt * (P - 1) <= DEC_MAX_ROWS && P - 1 <= MAX_BEAM;
   // longer prompts: batched passes of up to prefill_rows rows instead of one persistent pass per position
-  const bool wide = h->wide_prefill && c.prompt_len - 1 > MAX_BEAM;
-  persistent_setup(h, c, prompts, max_new_host, one_pass_prefill || wide ? 1 : 0);
+  const bool wide = h->wide_prefill && P - 1 > MAX_BEAM;
+  persistent_setup(h, c, prompts, max_new_host, fused ? P : one_pass_prefill || wide ? P - 1 : 0);
   if (c.max_new > 0) {
     // the persistent pass is one cooperative launch per step: no graph needed
-    if (one_pass_prefill) {
-      enqueue_decoder_forward(h, c, false, true);
+    if (fused || one_pass_prefill) {
+      enqueue_decoder_forward(h, c, fused, fused ? P : P - 1);
       ++steps;
+      h->launches += 1;
     } else if (wide) {
-      const int chunk = std::min(c.prompt_len - 1, std::max(1, h->prefill_rows / c.n_utt));
+      const int chunk = std::min(P - 1, std::max(1, h->prefill_rows / c.n_utt));
       steps += wide_prefill_run(h, c, chunk, h->kcache.p, h->vcache.p, static_cast<size_t>(DEC_MAX_ROWS) * T_MAX * h->dims.d_model,
                                 T_MAX);
     } else {
-      for (int p = 0; p + 1 < c.prompt_len; ++p) {
+      for (int p = 0; p + 1 < P; ++p) {
         enqueue_prefill(h, c);
         ++steps;
+        h->launches += 2;
       }
     }
-    if (!wide) h->launches += (c.prompt_len - 1) * 2;
-    steps += step_loop(h, c.max_new, true, [&] {
+    // (fused: step 0 is the search step alone, which is not a pass)
+    steps += step_loop(h, c.max_new, true, [&](int gs) {
+      if (fused && gs == 0) {
+        search_step_run(make_search_args(h, c), h->stream);
+        return 2;
+      }
       enqueue_step(h, c);
       return 1 + 2;  // the pass + the two kernels of the search step
-    });
+    }) - (fused ? 1 : 0);
   }
   read_results(h, c, max_new_host, out_ids, out_stride, out_len, out_score);
   return steps;
@@ -1284,7 +1297,8 @@ void ensure_batch(wisb_handle* h, int rows, int t_need) {
   int Rp = round_up(rows, 128);
   int tc = round_up(t_need, 32);
   if (tc > T_MAX) tc = T_MAX;
-  ensure_search(h, rows);
+  // (row tables for every row a pass can carry: a prefill pass has up to the row capacity, more than the search's rows)
+  ensure_search(h, std::max(Rp, h->bd_rows));
   // (the QKV epilogues hold the row_slot / row_pos pointers of the search state: a reallocation there stales the plans)
   if (Rp <= h->bd_rows && tc <= h->bd_tcap && h->bd_search_gen == h->search_gen) return;
   if (Rp < h->bd_rows) Rp = h->bd_rows;
@@ -1486,15 +1500,20 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
   if (c.max_new > 0) {
     // ---- prompt prefix: every utterance's positions [0, prompt_len - 1) as rows of shared passes (<= 8 positions and
     //      <= the row capacity per pass), K/V into the slot of the utterance's first beam
+    const int P = c.prompt_len;
     const int chunk_max = std::max(1, std::min(h->bd_rows / c.n_utt, MAX_BEAM));
+    // every prompt position in one pass: that pass also yields the logits of the first step, which then runs no pass
+    const bool fused = P <= chunk_max;
     // prompts longer than 9 tokens: wide passes of up to prefill_rows rows (> 8 positions per utterance)
-    const int wide = std::min(c.prompt_len - 1, std::max(chunk_max, h->prefill_rows / c.n_utt));
-    if (h->wide_prefill && c.prompt_len - 1 > MAX_BEAM && wide > chunk_max)
+    const int wide = std::min(P - 1, std::max(chunk_max, h->prefill_rows / c.n_utt));
+    if (fused)
+      steps += batch_prefill(h, c, P, P, chunk_max, c.beam, true);
+    else if (h->wide_prefill && P - 1 > MAX_BEAM && wide > chunk_max)
       steps += wide_prefill_run(h, c, wide, h->bkc.p, h->bvc.p, static_cast<size_t>(h->bd_rows) * h->bd_tcap * h->dims.d_model,
                                 h->bd_tcap);
     else
-      steps += batch_prefill(h, c, c.prompt_len, c.prompt_len - 1, chunk_max, c.beam, false);
-    search_init_run(make_batch_search_args(h, c), h->prompt_dev.p, s, 1);
+      steps += batch_prefill(h, c, P, P - 1, chunk_max, c.beam, false);
+    search_init_run(make_batch_search_args(h, c), h->prompt_dev.p, s, fused ? P : P - 1);
     cudaGraphExec_t g = nullptr;
     if (h->use_graphs && !h->profile) {  // (the per-kernel timing hook needs eager launches)
       GraphKey key;
@@ -1520,10 +1539,15 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
       }
       g = it->second;
     }
-    steps += step_loop(h, c.max_new, false, [&] {
+    // (fused: step 0 is the search step alone, eager, which is not a pass; the graph serves steps >= 1 unchanged)
+    steps += step_loop(h, c.max_new, false, [&](int gs) {
+      if (fused && gs == 0) {
+        search_step_run(make_batch_search_args(h, c), s);
+        return 2;
+      }
       if (g) WISB_CUDA(cudaGraphLaunch(g, s)); else enqueue_batch_step(h, c);
       return h->bd_launches_step;
-    });
+    }) - (fused ? 1 : 0);
   }
   read_results(h, c, max_new_host, out_ids, out_stride, out_len, out_score);
   return steps;
@@ -2532,7 +2556,7 @@ int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, const 
       a.seed_u = d_seed.p;
     }
     static_assert(sizeof(DecState) == 5 * sizeof(int), "DecState is five ints");
-    if (init) search_init_run(a, d_prompt.p, s, init - 1);
+    if (init) search_init_run(a, d_prompt.p, s, init == 2 ? prompt_len - 1 : 0);
     search_step_run(a, s);  // the production step: processors, top-k partials, merge, bookkeeping and step advance
     WISB_CUDA(cudaMemcpyAsync(state_i, d_i.p, sizeof(int) * n_i, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaMemcpyAsync(state_f, d_f.p, sizeof(float) * n_f, cudaMemcpyDeviceToHost, s));
@@ -3085,7 +3109,7 @@ int wisb_debug_dec_pass(wisb_handle* h, const int32_t* prm, int n_prm, const int
     WISB_CUDA(cudaMemcpyAsync(h->logits.p, logits, ls * sizeof(float), cudaMemcpyHostToDevice, s));
     try {
       upload_mega_layers(h, c);
-      enqueue_decoder_forward(h, c, with_logits != 0, pf_len > 0);
+      enqueue_decoder_forward(h, c, with_logits != 0, pf_len);
     } catch (...) {
       h->mega_mma = saved_mma;
       throw;

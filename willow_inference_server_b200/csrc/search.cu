@@ -114,6 +114,12 @@ __device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long x)
   return x;
 }
 
+// cache slot every later step reads the K/V of position pos from, for a row whose step wrote them into slot `own`: a
+// position inside the prompt that a prefill pass forwarded lives only in the slot of the window's first row, prefix
+__device__ __forceinline__ int kv_slot(const SearchArgs& a, int pos, int prefix, int own) {
+  return a.prompt_fed != nullptr && pos < *a.prompt_fed ? prefix : own;
+}
+
 __device__ __forceinline__ float masked_logit(const SearchArgs& a, const float* row, int v, bool first_step) {
   const unsigned char m = a.mask[v];
   if ((m & 1) || (first_step && (m & 2))) return -INFINITY;
@@ -245,7 +251,11 @@ __global__ void __launch_bounds__(TK_THREADS) topk_partial_kernel(const SearchAr
   if (a.st->all_done) return;  // a step enqueued ahead of the host's poll
   const int chunk = blockIdx.x, r = blockIdx.y;
   const bool first = a.st->gen_step == 0;
-  const float* row = a.logits + static_cast<long long>(r) * a.ldl;
+  // the first step after a prefill pass that also produced the logits reads the window's row of its last prompt position
+  const long long lrow = first && a.prompt_fed != nullptr && *a.prompt_fed == a.prompt_len
+                             ? static_cast<long long>(r / a.beam) * a.prompt_len + a.prompt_len - 1
+                             : r;
+  const float* row = a.logits + lrow * a.ldl;
   int v0, v1;
   if (!TS) {
     const int per_chunk = (a.n_vocab + TOPK_CHUNKS - 1) / TOPK_CHUNKS;
@@ -451,7 +461,8 @@ __device__ __forceinline__ void search_bookkeeping_body(const SearchArgs& a, int
     for (int k = 0; k < rows; ++k) {
       const int r = u * rows + k;
       for (int t = lane; t < a.max_new; t += 32) seq_nxt[r * a.max_new + t] = seq_cur[r * a.max_new + t];
-      for (int t = lane; t < a.t_max; t += 32) ind_nxt[r * a.t_max + t] = (t == pos) ? r : ind_cur[r * a.t_max + t];
+      for (int t = lane; t < a.t_max; t += 32)
+        ind_nxt[r * a.t_max + t] = (t == pos) ? kv_slot(a, pos, u * rows, r) : ind_cur[r * a.t_max + t];
     }
     return;
   }
@@ -525,7 +536,7 @@ __device__ __forceinline__ void search_bookkeeping_body(const SearchArgs& a, int
     for (int t = lane; t < pos; t += 32) ind_nxt[r * a.t_max + t] = ind_cur[pr * a.t_max + t];
     if (lane == 0) {
       if (gen < a.max_new) seq_nxt[r * a.max_new + gen] = tok;
-      ind_nxt[r * a.t_max + pos] = pr;  // this step's K/V were written by the parent row into its own slot
+      ind_nxt[r * a.t_max + pos] = kv_slot(a, pos, u * rows, pr);  // this step's K/V: the parent row's own slot
       a.tokens[r] = tok;
       a.cum[r] = (idx < 0) ? -INFINITY : cs[s_pick[k]] * norm;
     }
@@ -599,7 +610,7 @@ __global__ void __launch_bounds__(TK_THREADS) sample_tail_kernel(const SearchArg
     int* seq_nxt = a.seq[cur ^ 1] + static_cast<long long>(r) * a.max_new;
     const int* ind_cur = a.indir[cur] + static_cast<long long>(r) * a.t_max;
     int* ind_nxt = a.indir[cur ^ 1] + static_cast<long long>(r) * a.t_max;
-    // rows never reorder: the history and the cache indirection carry over, this step's K/V are the row's own
+    // rows never reorder: the history and the cache indirection carry over, this step's K/V are the row's own (kv_slot)
     for (int t = lane; t < gen; t += 32) seq_nxt[t] = seq_cur[t];
     for (int t = lane; t < pos; t += 32) ind_nxt[t] = ind_cur[t];
     // row log-sum-exp from the chunk partials (every lane), rule 5 as in topk_merge_body
@@ -684,7 +695,7 @@ __global__ void __launch_bounds__(TK_THREADS) sample_tail_kernel(const SearchArg
     if (lane == 0) {
       a.row_lse[r] = lse;
       if (gen < a.max_new) seq_nxt[gen] = tok;
-      ind_nxt[pos] = r;
+      ind_nxt[pos] = kv_slot(a, pos, u * n, r);
       if (finish) {
         int len = gen;
         if (tok != a.eot) {
@@ -734,28 +745,31 @@ __global__ void prefill_advance_kernel(int* tokens, const int* prompt, int promp
   if (threadIdx.x == 0) st->pos = next;
 }
 
-// shared_prefix: the prompt prefix (all but the last prompt token) is forwarded once per utterance into the cache slot of
-// its first beam by a single prefill pass; decoding then starts at the last prompt token and every beam's indirection
-// points at that slot.  MIXED: rows an utterance does not search start dead (eot, cum -inf).  SAMPLE: every row is live
-// and has no hypothesis yet (the per-row best_len / best_score).
+// fed > 0: prompt positions [0, fed) were forwarded once per utterance into the cache slot of its first beam by a single
+// prefill pass; decoding then starts at the last prompt token (fed = prompt_len: that pass also produced its logits, so
+// the first step runs no pass) and every beam's indirection points at that slot.  MIXED: rows an utterance does not
+// search start dead (eot, cum -inf).  SAMPLE: every row is live and has no hypothesis yet (the per-row best_len /
+// best_score).
 template <bool MIXED, bool SAMPLE = false>
-__global__ void search_init_kernel(const SearchArgs a, const int* prompt, int shared_prefix) {
+__global__ void search_init_kernel(const SearchArgs a, const int* prompt, int fed) {
   const int R = a.n_utt * a.beam;
   const int tid = blockIdx.x * blockDim.x + threadIdx.x, n = gridDim.x * blockDim.x;
+  const int pos0 = min(fed, a.prompt_len - 1);
   if (tid == 0) {
-    a.st->pos = shared_prefix ? a.prompt_len - 1 : 0;
+    a.st->pos = pos0;
     a.st->gen_step = 0;
     a.st->n_done = 0;
     a.st->all_done = 0;
     a.st->ticket = 0;
     *a.flip = 0;
+    if (a.prompt_fed != nullptr) *a.prompt_fed = fed;
   }
   for (int i = tid; i < R; i += n) {
     const bool dead = MIXED && i % a.beam >= a.beam_u[i / a.beam];
-    a.tokens[i] = dead ? a.eot : prompt[(i / a.beam) * a.prompt_len + (shared_prefix ? a.prompt_len - 1 : 0)];
+    a.tokens[i] = dead ? a.eot : prompt[(i / a.beam) * a.prompt_len + pos0];
     a.cum[i] = dead ? -INFINITY : 0.f;
     if (a.row_pos != nullptr) {
-      a.row_pos[i] = shared_prefix ? a.prompt_len - 1 : 0;
+      a.row_pos[i] = pos0;
       a.row_slot[i] = i;
     }
   }
@@ -772,7 +786,7 @@ __global__ void search_init_kernel(const SearchArgs a, const int* prompt, int sh
     }
   for (int i = tid; i < R * a.t_max; i += n) {
     const int r = i / a.t_max;
-    const int slot = shared_prefix ? (r / a.beam) * a.beam : r;  // else identity: every row holds its own prefix copy
+    const int slot = fed > 0 ? (r / a.beam) * a.beam : r;  // else identity: every row holds its own prefix copy
     a.indir[0][i] = slot;
     a.indir[1][i] = slot;
   }
@@ -872,13 +886,14 @@ void prefill_advance_run(int* tokens, const int* prompt, int prompt_len, int R, 
   WISB_CUDA(cudaGetLastError());
 }
 
-void search_init_run(const SearchArgs& a, const int* prompt, cudaStream_t stream, int shared_prefix) {
+void search_init_run(const SearchArgs& a, const int* prompt, cudaStream_t stream, int fed) {
+  WISB_REQUIRE(fed >= 0 && fed <= a.prompt_len, "search: more prompt positions forwarded than the prompt has");
   if (a.sample)
-    search_init_kernel<false, true><<<8, 256, 0, stream>>>(a, prompt, shared_prefix);
+    search_init_kernel<false, true><<<8, 256, 0, stream>>>(a, prompt, fed);
   else if (a.beam_u != nullptr)
-    search_init_kernel<true><<<8, 256, 0, stream>>>(a, prompt, shared_prefix);
+    search_init_kernel<true><<<8, 256, 0, stream>>>(a, prompt, fed);
   else
-    search_init_kernel<false><<<8, 256, 0, stream>>>(a, prompt, shared_prefix);
+    search_init_kernel<false><<<8, 256, 0, stream>>>(a, prompt, fed);
   WISB_CUDA(cudaGetLastError());
 }
 
