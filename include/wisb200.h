@@ -284,6 +284,31 @@ int wisb_debug_dec_embed_ln(wisb_handle* h, int R, int cap, int d, int n_vocab, 
 int wisb_debug_dec_pass(wisb_handle* h, const int32_t* prm, int n_prm, const int32_t* tokens, const int32_t* indir0,
                         const int32_t* indir1, const uint16_t* enc16, uint16_t* ckv_out, uint16_t* kcache, uint16_t* vcache,
                         float* x, float* logits);
+/* ONE batched decoder pass on caller state, with the workspaces, GEMM plans, row tables and arguments of its production
+ * caller.  prm (16) = {kind, n_utt, rows_per_utt, slot_stride, prompt_len, p0, batch_rows, t_need, chunk_max, flip,
+ * with_logits, cross_tc, ckv_sw, poison, poison_slot, poison_pos}.
+ *   kind 0  decoding step: R = n_utt * rows_per_utt (<= 8 per window) rows, row r at row_pos[r] in cache slot r, tokens[R],
+ *           indir0 / indir1 int32 [R][448] (flip picks indir1) for the positions below row_pos[r], done int32 [n_utt] or
+ *           NULL; with_logits 1; cross_tc picks the wgmma (1) or SIMT (0) cross-attention
+ *   kind 1  batched prefill: positions p0 .. p0 + rows_per_utt - 1 (<= 8) of every window of the prompt matrix tokens
+ *           [n_utt][prompt_len] as rows u * rows_per_utt + i, K/V into slot u * slot_stride; with_logits 0 / 1
+ *   kind 2  wide prefill pass (rows_per_utt <= chunk_max <= 448 positions per window) into the batched cache
+ *   kind 3  wide prefill pass into the persistent pass's cache; ckv_sw: the cross K/V are in its chunk-swizzled layout
+ * Kinds 0..2 size the batched workspaces for batch_rows rows and t_need positions (they only grow within a handle); wide
+ * passes size their own for n_utt * chunk_max rows.  ckv: fp16 [L][2][n_utt][H][1536][64] in the layout the pass reads.
+ * geom_out int64 [4] <- cache slots, positions per slot (t_cap), layer stride in elements, row capacity of the
+ * workspaces; kcache / vcache fp16 [L][slots][t_cap][d] in / out; x float32 [R][d] out; logits float32 [R][n_vocab_pad]
+ * out in columns < n_vocab (the others keep the caller's values).  kcache NULL: the geometry only, nothing allocated or
+ * launched.  plan_out (may be NULL) int32 [7][4]: BN, multicast, K splits and grid of the qkv, o, cq, co, fc1, fc2 and
+ * vocabulary GEMMs (vocabulary 0 in wide passes).
+ * poison 1: rows >= R of every activation workspace and partial slab hold NaN during the pass (restored after), row-
+ * table entries >= R point at cache cell (poison_slot, poison_pos), which the pass must not write.  Every index
+ * (tokens, positions < min(t_cap, n_text_ctx), slots, indirection entries, rows) is checked against that geometry
+ * before any workspace is sized or anything launched; a refused call returns 1 and changes nothing.  Invalidates the
+ * cached encoder output. */
+int wisb_debug_dec_batch_pass(wisb_handle* h, const int32_t* prm, int n_prm, const int32_t* tokens, const int32_t* row_pos,
+                              const int32_t* indir0, const int32_t* indir1, const int32_t* done, const uint16_t* ckv,
+                              uint16_t* kcache, uint16_t* vcache, float* x, float* logits, int64_t* geom_out, int32_t* plan_out);
 /* encoder output after the final LayerNorm, float32 [B,1500,d_model]; n_layers < 0 = all */
 int wisb_debug_encode(wisb_handle* h, const float* mel, int B, float* enc_out, int n_layers);
 /* The encoder one stage at a time, through the functions the encoder itself runs.  Sizes and indices are checked before

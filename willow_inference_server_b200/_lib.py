@@ -79,6 +79,9 @@ _SIGS = {
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "wisb_debug_dec_pass": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wisb_debug_dec_batch_pass": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p]),
     "wisb_debug_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     "wisb_debug_enc_stem": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "wisb_debug_enc_ln": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
@@ -726,6 +729,71 @@ class Handle:
         check(lib().wisb_debug_dec_pass(self._h, ptr(prm), prm.size, ptr(tokens), ptr(ind[0]), ptr(ind[1]), ptr(enc16),
                                         ptr(ckv), ptr(kcache), ptr(vcache), ptr(x), ptr(logits)))
         return ckv
+
+    BATCH_PLANS = ("qkv", "o", "cq", "co", "fc1", "fc2", "vocab")
+
+    def debug_dec_batch_geometry(self, kind: int, n_utt: int, *, batch_rows: int = 1, t_need: int = 1,
+                                 chunk_max: int = 1) -> dict:
+        """The cache geometry a batched pass of this kind would run with now (wisb_debug_dec_batch_pass with no state;
+        nothing is allocated) -> dict(slots, t_cap, layer_stride, rows_cap)."""
+        prm = np.asarray([kind, n_utt, 1, 1, 1, 0, batch_rows, t_need, chunk_max, 0, 1 if kind == 0 else 0, 1, 0, 0, 0, 0],
+                         np.int32)
+        geom = np.zeros(4, np.int64)
+        check(lib().wisb_debug_dec_batch_pass(self._h, ptr(prm), prm.size, None, None, None, None, None, None, None, None,
+                                              None, None, ptr(geom), None))
+        return dict(zip(("slots", "t_cap", "layer_stride", "rows_cap"), (int(v) for v in geom)))
+
+    def debug_dec_batch_pass(self, kind: int, tokens, ckv, kcache, vcache, *, n_utt: int, rows_per_utt: int,
+                             row_pos=None, indir0=None, indir1=None, flip: int = 0, done=None, slot_stride: int = 1,
+                             p0: int = 0, batch_rows: int = 1, t_need: int = 1, chunk_max: int = 1,
+                             with_logits: bool = False, cross_tc: int = 1, ckv_sw: int = 0, poison=None, x=None,
+                             logits=None):
+        """ONE batched decoder pass on caller state (wisb_debug_dec_batch_pass; kinds 0 step, 1 prefill, 2 / 3 wide
+        prefill into the batched / persistent cache).  tokens int [R] (step) or the prompt matrix [n_utt, prompt_len];
+        ckv float16 [L, 2, n_utt, H, 1536, 64]; kcache / vcache float16 [L, slots, t_cap, d] in / out, shaped from
+        debug_dec_batch_geometry; poison None or the (slot, position) cell row-table padding points at.  x float32
+        [>= R, d] and logits float32 [>= R, n_vocab_pad] (with logits) receive rows < R (logit columns < n_vocab); the
+        rest keeps the caller's values (default: new zero arrays of R rows).
+        -> dict(x, logits, plans, geom)."""
+        dm = self.dims()
+        d, L, H = dm["d_model"], dm["n_dec_layers"], dm["n_heads"]
+        R = n_utt * rows_per_utt
+        tokens = np.ascontiguousarray(np.asarray(tokens, np.int32))
+        if kind == 0:
+            if tokens.shape != (R,) or row_pos is None or indir0 is None or indir1 is None:
+                raise ValueError("a step needs tokens [R], row_pos [R], indir0 and indir1 [R, 448]")
+            row_pos = np.ascontiguousarray(np.asarray(row_pos, np.int32).reshape(R))
+            ind = [self._inout(np.ascontiguousarray(v, np.int32), np.int32, (R, 448), n)
+                   for v, n in ((indir0, "indir0"), (indir1, "indir1"))]
+            prompt_len = 1
+        else:
+            if tokens.ndim != 2 or tokens.shape[0] != n_utt:
+                raise ValueError("a prefill pass needs the prompt matrix [n_utt, prompt_len]")
+            prompt_len = tokens.shape[1]
+            ind = [None, None]
+        done = None if done is None else np.ascontiguousarray(np.asarray(done, np.int32).reshape(n_utt))
+        self._inout(ckv, np.float16, (L, 2, n_utt, H, 1536, 64), "ckv")
+        geom = self.debug_dec_batch_geometry(kind, n_utt, batch_rows=batch_rows, t_need=t_need, chunk_max=chunk_max)
+        shape = (L, geom["slots"], geom["t_cap"], d)
+        self._inout(kcache, np.float16, shape, "kcache")
+        self._inout(vcache, np.float16, shape, "vcache")
+        x = np.zeros((R, d), np.float32) if x is None else x
+        self._inout(x, np.float32, (max(R, x.shape[0]), d), "x")
+        if with_logits:
+            logits = np.zeros((R, dm["n_vocab_pad"]), np.float32) if logits is None else logits
+            self._inout(logits, np.float32, (max(R, logits.shape[0]), dm["n_vocab_pad"]), "logits")
+        else:
+            logits = None
+        ps, pp = poison if poison is not None else (0, 0)
+        prm = np.asarray([kind, n_utt, rows_per_utt, slot_stride, prompt_len, p0, batch_rows, t_need, chunk_max, flip,
+                          int(with_logits), cross_tc, ckv_sw, int(poison is not None), ps, pp], np.int32)
+        g = np.zeros(4, np.int64)
+        plan = np.zeros(28, np.int32)
+        check(lib().wisb_debug_dec_batch_pass(self._h, ptr(prm), prm.size, ptr(tokens), ptr(row_pos), ptr(ind[0]),
+                                              ptr(ind[1]), ptr(done), ptr(ckv), ptr(kcache), ptr(vcache), ptr(x),
+                                              ptr(logits), ptr(g), ptr(plan)))
+        plans = {k: tuple(int(v) for v in plan[4 * i: 4 * i + 4]) for i, k in enumerate(self.BATCH_PLANS)}
+        return dict(x=x, logits=logits, plans=plans, geom=geom)
 
     def debug_encode(self, mel: np.ndarray, n_layers: int = -1) -> np.ndarray:
         mel = np.ascontiguousarray(mel, np.float32)

@@ -1291,18 +1291,18 @@ void plan_batch_layers(wisb_handle* h, std::vector<BatchLayer>& layers, int Rp, 
 }
 
 // workspaces + GEMM plans of the batched pass for `rows` rows and `t_need` text positions per cache slot
+// the row capacity and positions per cache slot ensure_batch(h, rows, t_need) leaves (the workspaces only grow)
+int batch_rows_cap(const wisb_handle* h, int rows) { return std::max(round_up(rows, 128), h->bd_rows); }
+int batch_tcap(const wisb_handle* h, int t_need) { return std::max(std::min(round_up(t_need, 32), T_MAX), h->bd_tcap); }
+
 void ensure_batch(wisb_handle* h, int rows, int t_need) {
   const Dims& dm = h->dims;
   const int d = dm.d_model, L = dm.n_dec_layers;
-  int Rp = round_up(rows, 128);
-  int tc = round_up(t_need, 32);
-  if (tc > T_MAX) tc = T_MAX;
+  const int Rp = batch_rows_cap(h, rows), tc = batch_tcap(h, t_need);
   // (row tables for every row a pass can carry: a prefill pass has up to the row capacity, more than the search's rows)
-  ensure_search(h, std::max(Rp, h->bd_rows));
+  ensure_search(h, Rp);
   // (the QKV epilogues hold the row_slot / row_pos pointers of the search state: a reallocation there stales the plans)
-  if (Rp <= h->bd_rows && tc <= h->bd_tcap && h->bd_search_gen == h->search_gen) return;
-  if (Rp < h->bd_rows) Rp = h->bd_rows;
-  if (tc < h->bd_tcap) tc = h->bd_tcap;
+  if (Rp == h->bd_rows && tc == h->bd_tcap && h->bd_search_gen == h->search_gen) return;
   WISB_CUDA(cudaStreamSynchronize(h->stream));
   drop_graphs(h);
   const size_t M = static_cast<size_t>(Rp);
@@ -1378,14 +1378,30 @@ SearchArgs make_batch_search_args(wisb_handle* h, const DecodeCfg& c) {
   return sa;
 }
 
-void enqueue_batch_step(wisb_handle* h, const DecodeCfg& c) {
+// the pass of one decoding step: n_utt x beam rows at row_pos, K/V into slot row_slot, past positions through indir
+BatchArgs batch_step_args(wisb_handle* h, const DecodeCfg& c) {
   BatchArgs a = make_batch_args(h, c);
   a.R = c.n_utt * c.beam;
   a.rows_per_utt = c.beam;
   a.with_logits = 1;
   a.done = h->done.p;
+  return a;
+}
+
+void enqueue_batch_step(wisb_handle* h, const DecodeCfg& c) {
+  BatchArgs a = batch_step_args(h, c);
   h->bd_launches_step = batch_pass_run(a, h->bd_layers.data(), h->dims.n_dec_layers, h->stream) + 2;
   search_step_run(make_batch_search_args(h, c), h->stream);
+}
+
+// one batched prefill pass over the row tables prefill_rows_run wrote: chunk positions of each of the c.n_utt windows
+BatchArgs batch_prefill_args(wisb_handle* h, const DecodeCfg& c, int chunk, bool with_logits) {
+  BatchArgs a = make_batch_args(h, c);
+  a.R = c.n_utt * chunk;
+  a.rows_per_utt = chunk;
+  a.prefill = 1;
+  a.with_logits = with_logits ? 1 : 0;
+  return a;
 }
 
 // Batched prefill: positions [0, n_pos) of the token matrix in h->prompt_dev ([c.n_utt][tok_stride]) as the rows of
@@ -1404,11 +1420,7 @@ int batch_prefill(wisb_handle* h, const DecodeCfg& c, int tok_stride, int n_pos,
     const int chunk = std::min(chunk_max, n_pos - p0);
     prefill_rows_run(h->tokens.p, h->row_pos.p, h->row_slot.p, h->prompt_dev.p, tok_stride, c.n_utt, p0, chunk, slot_stride,
                      h->stream);
-    BatchArgs a = make_batch_args(h, c);
-    a.R = c.n_utt * chunk;
-    a.rows_per_utt = chunk;
-    a.prefill = 1;
-    a.with_logits = with_logits ? 1 : 0;
+    BatchArgs a = batch_prefill_args(h, c, chunk, with_logits);
     if (layer_hook) {
       hook.chunk = chunk;
       a.layer_hook = [](void* ctx, int layer, cudaStream_t) {
@@ -1425,13 +1437,15 @@ int batch_prefill(wisb_handle* h, const DecodeCfg& c, int tok_stride, int n_pos,
 
 // workspaces + GEMM plans of the wide prefill passes for `rows` rows, K/V into kc / vc (layer stride layer_cache, t_cap
 // positions per slot)
+// the row capacity ensure_prefill(h, rows, ...) leaves (the workspaces only grow)
+int prefill_rows_cap(const wisb_handle* h, int rows) { return std::max(round_up(rows, 128), h->pf_rows); }
+
 void ensure_prefill(wisb_handle* h, int rows, __half* kc, __half* vc, size_t layer_cache, int t_cap) {
   const int d = h->dims.d_model;
-  int Rp = round_up(rows, 128);
-  if (Rp <= h->pf_rows && kc == h->pf_kc && t_cap == h->pf_tcap && layer_cache == h->pf_layer_cache &&
+  const int Rp = prefill_rows_cap(h, rows);
+  if (Rp == h->pf_rows && kc == h->pf_kc && t_cap == h->pf_tcap && layer_cache == h->pf_layer_cache &&
       !h->pf_layers.empty() && h->pf_layers[0].vcache == vc)
     return;
-  if (Rp < h->pf_rows) Rp = h->pf_rows;
   WISB_CUDA(cudaStreamSynchronize(h->stream));
   const size_t M = static_cast<size_t>(Rp);
   h->px.ensure(M * d, true);
@@ -1451,6 +1465,28 @@ void ensure_prefill(wisb_handle* h, int rows, __half* kc, __half* vc, size_t lay
   h->pf_layer_cache = layer_cache;
 }
 
+// one wide prefill pass over the row tables prefill_rows_run wrote into ptok / ppos / pslot: ch positions of each of the
+// c.n_utt windows, on the wide workspaces and plans ensure_prefill made (t_cap positions per cache slot)
+BatchArgs wide_prefill_args(wisb_handle* h, const DecodeCfg& c, int ch, int t_cap) {
+  BatchArgs a = make_batch_args(h, c);
+  a.R = c.n_utt * ch;
+  a.rows_per_utt = ch;
+  a.prefill = 1;
+  a.wide = 1;
+  a.t_cap = t_cap;
+  a.tokens = h->ptok.p;
+  a.row_pos = h->ppos.p;
+  a.row_slot = h->pslot.p;
+  a.x = h->px.p;
+  a.xn = h->pxn.p;
+  a.q = h->pq.p;
+  a.ctx = h->pctx.p;
+  a.part = h->ppart.p;
+  a.part_stride = static_cast<long long>(h->pf_rows) * h->dims.d_model;
+  if (h->ckv_is_sw) a.ckv_map = &h->ckv_map_plain;
+  return a;
+}
+
 // Wide prefill: prompt positions [0, prompt_len - 1) of every utterance in h->prompt_dev as the rows of batched passes of
 // `chunk` positions per utterance, K/V into cache slot u * c.beam of kc / vc, cross-attention through
 // prefill_cross_attn_launch on h->ckv in the layout the call encoded.  Leaves what the persistent one-pass prefill leaves
@@ -1463,22 +1499,7 @@ int wide_prefill_run(wisb_handle* h, const DecodeCfg& c, int chunk, __half* kc, 
   for (int p0 = 0; p0 < n_pos; p0 += chunk, ++passes) {
     const int ch = std::min(chunk, n_pos - p0);
     prefill_rows_run(h->ptok.p, h->ppos.p, h->pslot.p, h->prompt_dev.p, c.prompt_len, c.n_utt, p0, ch, c.beam, h->stream);
-    BatchArgs a = make_batch_args(h, c);
-    a.R = c.n_utt * ch;
-    a.rows_per_utt = ch;
-    a.prefill = 1;
-    a.wide = 1;
-    a.t_cap = t_cap;
-    a.tokens = h->ptok.p;
-    a.row_pos = h->ppos.p;
-    a.row_slot = h->pslot.p;
-    a.x = h->px.p;
-    a.xn = h->pxn.p;
-    a.q = h->pq.p;
-    a.ctx = h->pctx.p;
-    a.part = h->ppart.p;
-    a.part_stride = static_cast<long long>(h->pf_rows) * h->dims.d_model;
-    if (h->ckv_is_sw) a.ckv_map = &h->ckv_map_plain;
+    BatchArgs a = wide_prefill_args(h, c, ch, t_cap);
     h->launches += 1 + batch_pass_run(a, h->pf_layers.data(), L, h->stream);
   }
   return passes;
@@ -3119,6 +3140,210 @@ int wisb_debug_dec_pass(wisb_handle* h, const int32_t* prm, int n_prm, const int
     WISB_CUDA(cudaMemcpyAsync(vcache, h->vcache.p, cache * sizeof(__half), cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaMemcpyAsync(x, h->dx.p, xs * sizeof(float), cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaMemcpyAsync(logits, h->logits.p, ls * sizeof(float), cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+int wisb_debug_dec_batch_pass(wisb_handle* h, const int32_t* prm, int n_prm, const int32_t* tokens, const int32_t* row_pos,
+                              const int32_t* indir0, const int32_t* indir1, const int32_t* done, const uint16_t* ckv,
+                              uint16_t* kcache, uint16_t* vcache, float* x, float* logits, int64_t* geom_out, int32_t* plan_out) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(h->blob != nullptr && prm != nullptr && n_prm == 16 && geom_out != nullptr, "debug_dec_batch_pass: bad arguments");
+    const Dims& dm = h->dims;
+    const int d = dm.d_model, L = dm.n_dec_layers;
+    const int kind = prm[0], n_utt = prm[1], rpu = prm[2], slot_stride = prm[3], prompt_len = prm[4], p0 = prm[5],
+              batch_rows = prm[6], t_need = prm[7], chunk_max = prm[8], flip = prm[9], with_logits = prm[10],
+              cross_tc = prm[11], ckv_sw = prm[12], poison = prm[13], poison_slot = prm[14], poison_pos = prm[15];
+    WISB_REQUIRE(kind >= 0 && kind <= 3, "debug_dec_batch_pass: kind 0 (step), 1 (prefill), 2 / 3 (wide prefill, batched / "
+                                         "persistent cache)");
+    WISB_REQUIRE(n_utt >= 1 && n_utt <= BD_CROSS_MAX_UTT,
+                 "debug_dec_batch_pass: 1.." + std::to_string(BD_CROSS_MAX_UTT) + " windows in one pass");
+    const bool wide = kind >= 2;
+    WISB_REQUIRE(rpu >= 1 && rpu <= (wide ? T_MAX : MAX_BEAM), "debug_dec_batch_pass: 1..8 rows per window, 1..448 in a wide pass");
+    const int R = n_utt * rpu;
+    WISB_REQUIRE((flip == 0 || flip == 1) && (cross_tc == 0 || cross_tc == 1) && (ckv_sw == 0 || ckv_sw == 1) &&
+                     (poison == 0 || poison == 1),
+                 "debug_dec_batch_pass: flip, cross_tc, ckv_sw and poison are 0 / 1");
+    WISB_REQUIRE(kind == 0 ? with_logits == 1 : kind == 1 ? (with_logits == 0 || with_logits == 1) : with_logits == 0,
+                 "debug_dec_batch_pass: a step has logits, a wide pass none, a prefill pass 0 / 1");
+    WISB_REQUIRE(ckv_sw == 0 || kind == 3, "debug_dec_batch_pass: only the persistent pass's cache pairs with swizzled cross K/V");
+    WISB_REQUIRE(kind == 3 || (batch_rows >= 1 && batch_rows <= 4096 && t_need >= 1 && t_need <= T_MAX),
+                 "debug_dec_batch_pass: batch_rows 1..4096, t_need 1..448");
+    WISB_REQUIRE(kind != 0 || batch_rows >= R, "debug_dec_batch_pass: a step has more rows than batch_rows");
+    WISB_REQUIRE(!wide || (chunk_max >= rpu && chunk_max <= T_MAX && static_cast<long long>(n_utt) * chunk_max <= 65536),
+                 "debug_dec_batch_pass: a wide pass needs rows_per_utt <= chunk_max <= 448, n_utt x chunk_max <= 65536");
+    WISB_REQUIRE(kind == 0 || (slot_stride >= 1 && prompt_len >= 1 && prompt_len <= T_MAX && p0 >= 0 && p0 + rpu <= prompt_len &&
+                               p0 + rpu <= dm.n_text_ctx),
+                 "debug_dec_batch_pass: prefill positions p0 .. p0 + rows_per_utt - 1 outside the prompt or n_text_ctx");
+    // the geometry the pass will have: the workspaces' growth rules, applied before anything is allocated
+    const int slots = kind == 3 ? DEC_MAX_ROWS : batch_rows_cap(h, batch_rows);
+    const int t_cap = kind == 3 ? T_MAX : batch_tcap(h, t_need);
+    const size_t layer_cache = static_cast<size_t>(slots) * t_cap * d;
+    const int cap = wide ? prefill_rows_cap(h, n_utt * chunk_max) : slots;
+    geom_out[0] = slots;
+    geom_out[1] = t_cap;
+    geom_out[2] = static_cast<int64_t>(layer_cache);
+    geom_out[3] = cap;
+    if (kcache == nullptr) return;  // geometry only: nothing allocated or launched
+    WISB_REQUIRE(tokens && ckv && vcache && x && (with_logits == 0 || logits), "debug_dec_batch_pass: NULL argument");
+    WISB_REQUIRE(R <= cap, "debug_dec_batch_pass: more rows than the workspaces hold");
+    // every index the pass forms, against those sizes: positions < t_cap and < n_text_ctx, slots < the cache's
+    const int n_pos = std::min(t_cap, dm.n_text_ctx);
+    std::vector<char> wr(static_cast<size_t>(slots) * t_cap, 0);  // cells the pass writes
+    if (kind == 0) {
+      WISB_REQUIRE(row_pos && indir0 && indir1, "debug_dec_batch_pass: a step needs row_pos, indir0 and indir1");
+      for (int r = 0; r < R; ++r) {
+        WISB_REQUIRE(tokens[r] >= 0 && tokens[r] < dm.n_vocab && row_pos[r] >= 0 && row_pos[r] < n_pos,
+                     "debug_dec_batch_pass: token / position out of range");
+        for (int t = 0; t < row_pos[r]; ++t) {
+          const size_t i = static_cast<size_t>(r) * T_MAX + t;
+          WISB_REQUIRE(indir0[i] >= 0 && indir0[i] < slots && indir1[i] >= 0 && indir1[i] < slots,
+                       "debug_dec_batch_pass: indirection entry outside the cache slots");
+        }
+        wr[static_cast<size_t>(r) * t_cap + row_pos[r]] = 1;
+      }
+    } else {
+      WISB_REQUIRE(p0 + rpu <= n_pos, "debug_dec_batch_pass: prefill position outside the cache (t_cap) or n_text_ctx");
+      WISB_REQUIRE(static_cast<long long>(n_utt - 1) * slot_stride < slots, "debug_dec_batch_pass: window slot outside the cache");
+      for (int u = 0; u < n_utt; ++u)
+        for (int p = p0; p < p0 + rpu; ++p) {
+          const int tk = tokens[static_cast<size_t>(u) * prompt_len + p];
+          WISB_REQUIRE(tk >= 0 && tk < dm.n_vocab, "debug_dec_batch_pass: token out of range");
+          wr[static_cast<size_t>(u) * slot_stride * t_cap + p] = 1;
+        }
+    }
+    if (poison)
+      WISB_REQUIRE(poison_slot >= 0 && poison_slot < slots && poison_pos >= 0 && poison_pos < n_pos &&
+                       !wr[static_cast<size_t>(poison_slot) * t_cap + poison_pos],
+                   "debug_dec_batch_pass: the poison cell must be a cache cell the pass does not write");
+    cudaStream_t s = h->stream;
+    // workspaces and plans as the production callers make them (decode_batch / align_group / wide_prefill_run)
+    ensure_search(h, n_utt);
+    if (kind <= 2) ensure_batch(h, batch_rows, t_need);
+    __half* kc = kind == 3 ? h->kcache.p : h->bkc.p;
+    __half* vc = kind == 3 ? h->vcache.p : h->bvc.p;
+    if (wide) ensure_prefill(h, n_utt * chunk_max, kc, vc, layer_cache, t_cap);
+    WISB_REQUIRE((kind == 3 || (h->bd_rows == slots && h->bd_tcap == t_cap)) && (wide ? h->pf_rows : h->bd_rows) == cap,
+                 "debug_dec_batch_pass: workspaces differ from the geometry reported");
+    std::vector<BatchLayer>& layers = wide ? h->pf_layers : h->bd_layers;
+    if (plan_out) {
+      const GemmPlan* ps[7] = {&layers[0].qkv, &layers[0].o, &layers[0].cq, &layers[0].co, &layers[0].fc1, &layers[0].fc2,
+                               &h->bd_vocab};
+      for (int i = 0; i < 7; ++i) {
+        const bool v = i < 6 || !wide;
+        plan_out[4 * i] = v ? ps[i]->BN : 0;
+        plan_out[4 * i + 1] = v ? ps[i]->mcast : 0;
+        plan_out[4 * i + 2] = v ? ps[i]->k_splits : 0;
+        plan_out[4 * i + 3] = v ? ps[i]->grid : 0;
+      }
+    }
+    // caller state: cross K/V (the layout the pass reads), caches, row tables / search state
+    ensure_encoder(h, n_utt);
+    h->enc_valid = false;  // the cross K/V below belong to no features: a later call must not reuse them
+    h->mel_cache_B = 0;
+    const size_t ckv_elems = static_cast<size_t>(L) * 2 * n_utt * T_ENC_PAD * d;
+    WISB_CUDA(cudaMemcpyAsync(h->ckv.p, ckv, ckv_elems * sizeof(__half), cudaMemcpyHostToDevice, s));
+    h->ckv_is_sw = ckv_sw;
+    const size_t cache = static_cast<size_t>(L) * layer_cache;
+    WISB_CUDA(cudaMemcpyAsync(kc, kcache, cache * sizeof(__half), cudaMemcpyHostToDevice, s));
+    WISB_CUDA(cudaMemcpyAsync(vc, vcache, cache * sizeof(__half), cudaMemcpyHostToDevice, s));
+    int* tab_tok = wide ? h->ptok.p : h->tokens.p;
+    int* tab_pos = wide ? h->ppos.p : h->row_pos.p;
+    int* tab_slot = wide ? h->pslot.p : h->row_slot.p;
+    if (poison && cap > R) {  // row-table entries >= R: one valid cell the pass does not write
+      std::vector<int> t0(cap - R, 0), tp(cap - R, poison_pos), ts(cap - R, poison_slot);
+      WISB_CUDA(cudaMemcpyAsync(tab_tok + R, t0.data(), t0.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+      WISB_CUDA(cudaMemcpyAsync(tab_pos + R, tp.data(), tp.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+      WISB_CUDA(cudaMemcpyAsync(tab_slot + R, ts.data(), ts.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+      WISB_CUDA(cudaStreamSynchronize(s));  // (host temporaries)
+    }
+    DecodeCfg c{};
+    c.u0 = 0; c.n_utt = n_utt; c.B_total = n_utt; c.max_new = 1; c.max_hyp = 1; c.lp = 1.f;
+    c.beam = kind == 0 ? rpu : slot_stride;
+    c.prompt_len = kind == 0 ? 1 : prompt_len;
+    if (kind == 0) {
+      WISB_CUDA(cudaMemcpyAsync(h->tokens.p, tokens, R * sizeof(int), cudaMemcpyHostToDevice, s));
+      WISB_CUDA(cudaMemcpyAsync(h->row_pos.p, row_pos, R * sizeof(int), cudaMemcpyHostToDevice, s));
+      std::vector<int> slot(R), dn(n_utt, 0);
+      for (int r = 0; r < R; ++r) slot[r] = r;
+      if (done) std::copy(done, done + n_utt, dn.begin());
+      WISB_CUDA(cudaMemcpyAsync(h->row_slot.p, slot.data(), R * sizeof(int), cudaMemcpyHostToDevice, s));
+      WISB_CUDA(cudaMemcpyAsync(h->done.p, dn.data(), n_utt * sizeof(int), cudaMemcpyHostToDevice, s));
+      WISB_CUDA(cudaMemcpyAsync(h->ind0.p, indir0, static_cast<size_t>(R) * T_MAX * sizeof(int), cudaMemcpyHostToDevice, s));
+      WISB_CUDA(cudaMemcpyAsync(h->ind1.p, indir1, static_cast<size_t>(R) * T_MAX * sizeof(int), cudaMemcpyHostToDevice, s));
+      WISB_CUDA(cudaMemcpyAsync(h->flip.p, &flip, sizeof(int), cudaMemcpyHostToDevice, s));
+      WISB_CUDA(cudaStreamSynchronize(s));  // (host temporaries)
+    } else {
+      WISB_CUDA(cudaMemcpyAsync(h->prompt_dev.p, tokens, static_cast<size_t>(n_utt) * prompt_len * sizeof(int),
+                                cudaMemcpyHostToDevice, s));
+      prefill_rows_run(tab_tok, tab_pos, tab_slot, h->prompt_dev.p, prompt_len, n_utt, p0, rpu, slot_stride, s);
+    }
+    // poison: rows >= R of every activation workspace and partial slab NaN (all-ones bytes) for this pass, restored after
+    float* wx = wide ? h->px.p : h->bx.p;
+    struct Region {
+      void* p;
+      size_t bytes;
+    };
+    const size_t rd = static_cast<size_t>(R) * d, cd = static_cast<size_t>(cap) * d;
+    std::vector<Region> regions;
+    if (poison) {
+      auto rows_of = [&](void* base, size_t esz, size_t width) {
+        regions.push_back({static_cast<uint8_t*>(base) + esz * width * R, esz * width * (cap - R)});
+      };
+      rows_of(wx, 4, d);
+      rows_of(wide ? static_cast<void*>(h->pxn.p) : h->bxn.p, 2, d);
+      rows_of(wide ? static_cast<void*>(h->pq.p) : h->bq.p, 4, d);
+      rows_of(wide ? static_cast<void*>(h->pctx.p) : h->bctx.p, 2, d);
+      rows_of(wide ? static_cast<void*>(h->ph.p) : h->bh.p, 2, 4 * static_cast<size_t>(d));
+      float* part = wide ? h->ppart.p : h->bpart.p;
+      for (int sl = 0; sl < 8; ++sl) regions.push_back({part + sl * cd + rd, 4 * (cd - rd)});
+    }
+    size_t saved_bytes = 0;
+    for (const Region& g : regions) saved_bytes += g.bytes;
+    DevBuf<uint8_t> saved;
+    saved.ensure(saved_bytes);
+    {
+      size_t at = 0;
+      for (const Region& g : regions) {
+        WISB_CUDA(cudaMemcpyAsync(saved.p + at, g.p, g.bytes, cudaMemcpyDeviceToDevice, s));
+        WISB_CUDA(cudaMemsetAsync(g.p, 0xFF, g.bytes, s));
+        at += g.bytes;
+      }
+    }
+    // the pass, through the argument builders of its production caller
+    const int saved_tc = h->cross_tc;
+    h->cross_tc = cross_tc;
+    try {
+      BatchArgs a;
+      if (kind == 0) {
+        bind_batch_cross_kv(h, 0, n_utt);
+        a = batch_step_args(h, c);
+      } else if (kind == 1) {
+        bind_batch_cross_kv(h, 0, n_utt);
+        a = batch_prefill_args(h, c, rpu, with_logits != 0);
+      } else {
+        for (int i = 0; i < L; ++i) bind_cross_kv(h, h->pf_layers[i], i, c.u0, c.B_total);
+        a = wide_prefill_args(h, c, rpu, t_cap);
+      }
+      batch_pass_run(a, layers.data(), L, s);
+    } catch (...) {
+      h->cross_tc = saved_tc;
+      throw;
+    }
+    h->cross_tc = saved_tc;
+    {
+      size_t at = 0;
+      for (const Region& g : regions) {
+        WISB_CUDA(cudaMemcpyAsync(g.p, saved.p + at, g.bytes, cudaMemcpyDeviceToDevice, s));
+        at += g.bytes;
+      }
+    }
+    WISB_CUDA(cudaMemcpyAsync(kcache, kc, cache * sizeof(__half), cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(vcache, vc, cache * sizeof(__half), cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaMemcpyAsync(x, wx, rd * sizeof(float), cudaMemcpyDeviceToHost, s));
+    if (with_logits)  // (columns >= n_vocab of the caller's rows stay as they were)
+      WISB_CUDA(cudaMemcpy2DAsync(logits, sizeof(float) * dm.n_vocab_pad, h->blogits.p, sizeof(float) * dm.n_vocab_pad,
+                                  sizeof(float) * dm.n_vocab, R, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaStreamSynchronize(s));
   });
 }
