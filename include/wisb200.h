@@ -187,8 +187,19 @@ int wisb_get_timing(wisb_handle* h, float* out16);
  * "wide_prefill" (default 1; 0: prompts prefill at most 8 positions per pass, one persistent pass per position when the
  * one-pass prefill does not fit), "prefill_rows" (default 1024, 8..65536: a prompt of more than 9 tokens is prefilled in
  * batched passes of min(prompt_len - 1, max(the 8-position chunk, prefill_rows / windows)) positions per window; it
- * bounds the prefill's activation workspace, about 52 d_model bytes per row) */
+ * bounds the prefill's activation workspace, about 52 d_model bytes per row),
+ * "no_speech_prob" (default 0; 1: every wisb_generate also computes each window's no-speech probability, read with
+ * wisb_get_no_speech_probs) */
 int wisb_set_option(wisb_handle* h, const char* key, int value);
+
+/* (4b) The no-speech probabilities of the handle's last wisb_generate, one per window (also when sampling), into out
+ * float32 [B].  Window b's value is softmax(l)[no_speech] of the decoder's raw logits l over the whole vocabulary at
+ * the position of the FIRST <|startoftranscript|> in its prompt (openai/whisper's sot_index), before suppression,
+ * history processors, timestamp rules and temperature; a window capped at 0 new tokens gets its value too.  With option
+ * "no_speech_prob" = 1, wisb_generate fails with code 1 for a prompt without <|startoftranscript|>, and its ids, lengths,
+ * scores and decoder passes are those of the same call without the option.  Code 1 when that call ran without the
+ * option, failed, or had another B. */
+int wisb_get_no_speech_probs(wisb_handle* h, int B, float* out);
 
 /* ---- diagnostics used by tests/ (run the product kernels on caller data) ---- */
 /* One GEMM A[M,K] . W[N,K]^T (fp16 as raw uint16) through any production epilogue, on caller data.
@@ -231,6 +242,11 @@ int wisb_debug_search_step(wisb_handle* h, const int32_t* prm, int n_prm, const 
                            const int32_t* beam_u, const int32_t* max_hyp_u, const float* length_penalty_u,
                            const uint64_t* seeds, int32_t* state_i, float* state_f, int32_t* cand_idx, float* cand_score,
                            float* row_lse);
+/* the no-speech reduction on caller data: out[u] = softmax over columns [0, n_vocab) of row rows[u] of logits float32
+ * [n_rows, ldl], at column no_speech (columns >= n_vocab are never read).  rows[u] < 0 leaves out[u] as the caller gave
+ * it.  n in [1, 65535], n_vocab <= ldl, rows[u] < n_rows. */
+int wisb_debug_no_speech_probs(wisb_handle* h, const float* logits, int n_rows, int ldl, const int32_t* rows, int n,
+                               int n_vocab, int no_speech, float* out);
 /* encoder self-attention on caller data: qkv [B*1536, 3d] fp16 -> ctx [B*1536, d] fp16, d = 64 H; impl 0 = wgmma with
  * MN-major V, 1 = wgmma with the transposed Vt layout (built from the same qkv), 2 = SIMT check */
 int wisb_debug_enc_attn(wisb_handle* h, const uint16_t* qkv16, int B, int d, int H, int impl, uint16_t* ctx16_out);

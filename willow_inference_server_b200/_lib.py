@@ -4,6 +4,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import threading
 
 import numpy as np
 
@@ -62,6 +63,9 @@ _SIGS = {
                                         C.c_void_p, C.c_void_p]),
     "wisb_get_timing": (C.c_int, [C.c_void_p, C.c_void_p]),
     "wisb_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
+    "wisb_get_no_speech_probs": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
+    "wisb_debug_no_speech_probs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                             C.c_void_p]),
     "wisb_debug_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
                                   C.c_void_p]),
@@ -145,6 +149,9 @@ class Handle:
     def __init__(self, raw, keepalive=None):
         self._h = raw
         self._keep = keepalive
+        # held around every wisb_generate: a call that asks for the no-speech probability sets a handle option around
+        # its wisb_generate, and no other call on this handle may run in between
+        self._generate_lock = threading.Lock()
 
     @classmethod
     def from_path(cls, path: str, device: int = 0):
@@ -231,8 +238,11 @@ class Handle:
         return out
 
     def generate(self, mel, prompts, beam_size=5, patience=1.0, length_penalty=1.0, max_length=448, extra_suppress=(),
-                 B=None, timestamps=False, max_initial_timestamp_index=50, repetition_penalty=1.0, no_repeat_ngram_size=0):
-        """-> (token ids per utterance, length-normalised scores).  The options are those of wisb_generate_options:
+                 B=None, timestamps=False, max_initial_timestamp_index=50, repetition_penalty=1.0, no_repeat_ngram_size=0,
+                 no_speech_out=None):
+        """-> (token ids per utterance, length-normalised scores).  no_speech_out: None, or a float32 [B] array the call
+        fills with every window's no-speech probability (wisb_get_no_speech_probs; every prompt must then contain
+        <|startoftranscript|>).  The options are those of wisb_generate_options:
         timestamps=True applies Whisper's timestamp rules to the generated tokens: the prompt may then hold any ids, timestamps
         included, before its last <|startoftranscript|> (a <|startofprev|> context), but neither <|notimestamps|> nor
         timestamp tokens from that token on (in the whole prompt when it has none); repetition_penalty != 1 or no_repeat_ngram_size > 0 switches on the history processors.
@@ -241,20 +251,22 @@ class Handle:
             mel, prompts, B, max_length, extra_suppress, 1, beam_size=beam_size, patience=patience,
             length_penalty=length_penalty, timestamps=1 if timestamps else 0,
             max_initial_timestamp_index=int(max_initial_timestamp_index), repetition_penalty=float(repetition_penalty),
-            no_repeat_ngram_size=int(no_repeat_ngram_size))
+            no_repeat_ngram_size=int(no_repeat_ngram_size), no_speech_out=no_speech_out)
         return [ids[b, : lens[b]].tolist() for b in range(len(lens))], scores.tolist()
 
     def generate_sample(self, mel, prompts, num_hypotheses, sampling_topk, sampling_temperature, seeds,
                         length_penalty=1.0, max_length=448, extra_suppress=(), B=None, timestamps=False,
-                        max_initial_timestamp_index=50, repetition_penalty=1.0, no_repeat_ngram_size=0):
+                        max_initial_timestamp_index=50, repetition_penalty=1.0, no_repeat_ngram_size=0, no_speech_out=None):
         """num_hypotheses sampled hypotheses per window (sampling_topk != 1), window b seeded by seeds[b] (uint64) ->
-        (per window the n token lists, per window the n scores), each window's sorted by score, descending."""
+        (per window the n token lists, per window the n scores), each window's sorted by score, descending.
+        no_speech_out as in generate: one value per window."""
         n = int(num_hypotheses)
         ids, lens, scores = self._generate(
             mel, prompts, B, max_length, extra_suppress, n, beam_size=1, patience=1.0, length_penalty=length_penalty,
             num_hypotheses=n, sampling_topk=int(sampling_topk), sampling_temperature=float(sampling_temperature),
             seeds=seeds, timestamps=1 if timestamps else 0, max_initial_timestamp_index=int(max_initial_timestamp_index),
-            repetition_penalty=float(repetition_penalty), no_repeat_ngram_size=int(no_repeat_ngram_size))
+            repetition_penalty=float(repetition_penalty), no_repeat_ngram_size=int(no_repeat_ngram_size),
+            no_speech_out=no_speech_out)
         seqs = [ids[i, : lens[i]].tolist() for i in range(len(lens))]
         return [seqs[b * n: (b + 1) * n] for b in range(len(lens) // n)], \
             [scores[b * n: (b + 1) * n].tolist() for b in range(len(lens) // n)]
@@ -262,11 +274,11 @@ class Handle:
     _PER_WINDOW = (("beam_size", "beam_per_window", np.int32), ("patience", "patience_per_window", np.float32),
                    ("length_penalty", "length_penalty_per_window", np.float32))
 
-    def _generate(self, mel, prompts, B, max_length, extra_suppress, n, **options):
+    def _generate(self, mel, prompts, B, max_length, extra_suppress, n, no_speech_out=None, **options):
         """The one wisb_generate call behind generate and generate_sample: checks the prompts, features, max_length (an
         int or one per window), seeds and per-window search options, sets `options` (arrays by address) over
         wisb_generate_options_init's defaults -> (ids int32 [B * n, stride], lens int32 [B * n], scores float32
-        [B * n]), n entries per window."""
+        [B * n]), n entries per window.  With no_speech_out, option no_speech_prob is on for this call alone."""
         prompts = np.ascontiguousarray(prompts, np.int32)
         if prompts.ndim != 2:
             raise ValueError("prompts must be [B, prompt_len]")
@@ -301,8 +313,22 @@ class Handle:
                        extra_suppress=extra if extra.size else None)
         for k, v in options.items():  # (the arrays stay referenced by `options` until the call returns)
             setattr(opt, k, ptr(v) if v is None or isinstance(v, np.ndarray) else v)
-        check(lib().wisb_generate(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], C.byref(opt), ptr(ids), stride,
-                                  ptr(lens), ptr(scores)))
+        if no_speech_out is not None and (not isinstance(no_speech_out, np.ndarray) or no_speech_out.dtype != np.float32
+                                          or no_speech_out.shape != (B,) or not no_speech_out.flags["C_CONTIGUOUS"]
+                                          or not no_speech_out.flags["WRITEABLE"]):
+            raise ValueError("no_speech_out must be a writeable C-contiguous float32 array with one entry per window")
+        with self._generate_lock:
+            if no_speech_out is None:
+                check(lib().wisb_generate(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], C.byref(opt), ptr(ids),
+                                          stride, ptr(lens), ptr(scores)))
+                return ids, lens, scores
+            check(lib().wisb_set_option(self._h, b"no_speech_prob", 1))
+            try:
+                check(lib().wisb_generate(self._h, ptr(mel), B, ptr(prompts), prompts.shape[1], C.byref(opt), ptr(ids),
+                                          stride, ptr(lens), ptr(scores)))
+                check(lib().wisb_get_no_speech_probs(self._h, B, ptr(no_speech_out)))
+            finally:
+                check(lib().wisb_set_option(self._h, b"no_speech_prob", 0))
         return ids, lens, scores
 
     def detect_language(self, mel, B=None):
@@ -592,6 +618,16 @@ class Handle:
             else:
                 out[k], oi = si[oi : oi + v.size].reshape(v.shape).copy(), oi + v.size
         return out, ci, cs, lse
+
+    def debug_no_speech_probs(self, logits: np.ndarray, rows, n_vocab: int, no_speech: int, out=None) -> np.ndarray:
+        """The no-speech reduction on caller data: logits float32 [n_rows, ldl], rows int [n] (< 0: out[u] kept) ->
+        out float32 [n], out[u] = softmax(logits[rows[u], :n_vocab])[no_speech]."""
+        logits = np.ascontiguousarray(logits, np.float32)
+        rows = np.ascontiguousarray(rows, np.int32)
+        out = np.zeros(rows.size, np.float32) if out is None else np.ascontiguousarray(out, np.float32).copy()
+        check(lib().wisb_debug_no_speech_probs(self._h, ptr(logits), logits.shape[0], logits.shape[1], ptr(rows), rows.size,
+                                               int(n_vocab), int(no_speech), ptr(out)))
+        return out
 
     def debug_enc_attn(self, qkv16: np.ndarray, n_heads: int, impl: int = 0) -> np.ndarray:
         """Encoder self-attention on qkv fp16 [B, 1536, 3d] -> ctx fp16 [B, 1536, d]; impl 0 = wgmma (MN-major V),

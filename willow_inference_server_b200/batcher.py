@@ -14,8 +14,9 @@ This module is the piece a WIS maintainer puts between the endpoints and the eng
     results = await batcher.generate(features, prompt, beam_size=5)      # inside the FastAPI handlers
     results = batcher.submit(features, prompt, beam_size=5).result()      # from plain threads
 
-Requests are compatible when they share the prompt and every generation option except ``max_length`` (same decoder
-configuration; the length limits travel per window).  With an engine that takes the search options per window
+Requests are compatible when they share the prompt and every generation option except ``max_length`` and
+``return_no_speech_prob`` (same decoder configuration; the length limits travel per window, and asking for the
+no-speech probability changes no result).  With an engine that takes the search options per window
 (``models.Whisper.per_window_options``) the rule is wider: prompts need only the same length and the same timestamp mode
 (whether ``<|notimestamps|>`` is in them), and ``beam_size``, ``patience`` and ``length_penalty`` travel per window too,
 so short commands at beam 1, dictation at beam 3 and requests in other languages or for translation share one call.
@@ -40,6 +41,7 @@ from __future__ import annotations
 
 import asyncio
 import collections
+import dataclasses
 import threading
 import time
 from concurrent.futures import Future
@@ -68,7 +70,8 @@ def _check_search_option(name, v):
 
 
 class _Request:
-    __slots__ = ("features", "n", "key", "prompt", "opts", "search", "max_length", "seed", "future", "t_arrival")
+    __slots__ = ("features", "n", "key", "prompt", "opts", "search", "max_length", "no_speech", "seed", "future",
+                 "t_arrival")
 
     def __init__(self, features, prompt, opts, no_timestamps=None):
         """no_timestamps: the engine's <|notimestamps|> id when it takes prompts and search options per window, else
@@ -78,6 +81,9 @@ class _Request:
         self.prompt = list(prompt)
         self.opts = dict(opts)
         self.max_length = int(self.opts.pop("max_length", 448))  # per request; merged per window by the worker
+        # a merged call asks for the no-speech probability when one of its requests does; the others get 0.0, what
+        # CTranslate2 returns when it is not asked for
+        self.no_speech = bool(self.opts.pop("return_no_speech_prob", False))
         self.search = {}
         prompt_key = tuple(self.prompt)
         # sampling: the request's seed, fixed now (its windows get seed + w); its search options stay in the key
@@ -265,6 +271,9 @@ class TranscribeBatcher:
         prompts = [r.prompt for r in live for _ in range(r.n)]
         if live[0].seed is not None:  # (a sampling batch: every request has its seed)
             opts["random_seed"] = np.concatenate([window_seeds(r.seed, r.n) for r in live])
+        asked = any(r.no_speech for r in live)
+        if asked:
+            opts["return_no_speech_prob"] = True
         out = self._model.generate(StorageView.from_array(feats), prompts, max_length=ml, **opts)
         if len(out) != n:
             raise RuntimeError(f"engine returned {len(out)} results for {n} windows")
@@ -273,5 +282,8 @@ class TranscribeBatcher:
         self.stats["max_windows_per_call"] = max(self.stats["max_windows_per_call"], n)
         pos = 0
         for r in live:
-            r.future.set_result(out[pos : pos + r.n])
+            res = out[pos : pos + r.n]
+            if asked and not r.no_speech:
+                res = [dataclasses.replace(x, no_speech_prob=0.0) for x in res]
+            r.future.set_result(res)
             pos += r.n

@@ -251,5 +251,12 @@ void dec_pass_run(const MegaArgs& a, int num_sms, cudaStream_t stream);
 // language detection head: softmax over lang ids of the logits of row u*beam (one step on <|startoftranscript|>)
 void lang_probs_run(const float* logits, long long ldl, const int* lang_ids, int n_lang, int n_utt, int row_stride,
                     float* probs /*[n_utt][n_lang]*/, cudaStream_t stream);
+// no-speech probability: out[u] = softmax over columns [0, n_vocab) of logits row rows[u], at column no_speech (raw
+// logits: no suppression, processor or temperature).  Columns n_vocab .. ldl - 1 are never read.  rows[u] < 0: the
+// window's row is not in this buffer and out[u] keeps its value.  One CTA per window, n_utt windows.
+void no_speech_run(const float* logits, long long ldl, const int* rows /*[n_utt]*/, int n_utt, int n_vocab, int no_speech,
+                   float* out /*[n_utt]*/, cudaStream_t stream);
+// dst row u = src row rows[u] of d fp16 values (rows[u] < 0: dst row u keeps its value), u < n_utt
+void row_gather_run(const __half* src, int d, const int* rows, int n_utt, __half* dst, cudaStream_t stream);
 
 }  // namespace wisb

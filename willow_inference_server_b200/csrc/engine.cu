@@ -172,6 +172,20 @@ struct wisb_handle {
   DevBuf<__half> pxn, pctx, ph;
   DevBuf<int> ptok, ppos, pslot;
   std::vector<BatchLayer> pf_layers;
+  // no-speech probability (option "no_speech_prob"): ns_prob [B] the call's values on the device, ns_host / ns_B the
+  // last wisb_generate's on the host (ns_B 0: none).  A group's reductions each read their own row table, ns_used of
+  // them staged so far in ns_pin / ns_rows.  Wide prefill: window u's final-LayerNorm row gathered into row u of ns_x
+  // (ns_cap rows, a multiple of 128), ns_vocab its vocabulary GEMM into ns_logits.
+  int no_speech = 0;
+  DevBuf<float> ns_prob, ns_logits;
+  DevBuf<int> ns_rows;
+  PinBuf<int> ns_pin;
+  int ns_used = 0;
+  DevBuf<__half> ns_x;
+  GemmPlan ns_vocab;
+  int ns_cap = 0;
+  std::vector<float> ns_host;
+  int ns_B = 0;
   DevBuf<MegaLayer> mega_layers;
   DevBuf<__half> mega_img;  // warp-MMA pass: decoder weights as per-CTA shared-memory images (mega_mma_image)
   int enc_pdl = 1;  // encoder: programmatic dependent launch along the whole kernel chain (227 launches per window)
@@ -835,6 +849,10 @@ struct DecodeCfg {
   int sample = 0, topk = 0;
   float temperature = 1.f;
   const uint64_t* seed_host = nullptr;
+  // no-speech probability requested: sot[u] (host) = the position of the first <|startoftranscript|> in utterance u's
+  // prompt, ns_out (device) [n_utt] its value; null: not requested
+  const int* sot = nullptr;
+  float* ns_out = nullptr;
 };
 
 SearchArgs make_search_args(wisb_handle* h, const DecodeCfg& c) {
@@ -1023,8 +1041,8 @@ void enqueue_decoder_forward(wisb_handle* h, const DecodeCfg& c, bool with_logit
   dec_pass_run(a, h->num_sms, h->stream);
 }
 
-void enqueue_prefill(wisb_handle* h, const DecodeCfg& c) {
-  enqueue_decoder_forward(h, c, false);
+void enqueue_prefill(wisb_handle* h, const DecodeCfg& c, bool with_logits = false) {
+  enqueue_decoder_forward(h, c, with_logits);
   prefill_advance_run(h->tokens.p, h->prompt_dev.p, c.prompt_len, c.n_utt * c.beam, c.beam, h->st.p, h->stream);
 }
 void enqueue_step(wisb_handle* h, const DecodeCfg& c) {
@@ -1172,7 +1190,58 @@ int step_loop(wisb_handle* h, int max_new, bool look_ahead, const std::function<
   return steps;
 }
 
-int wide_prefill_run(wisb_handle* h, const DecodeCfg& c, int chunk, __half* kc, __half* vc, size_t layer_cache, int t_cap);
+int wide_prefill_ns(wisb_handle* h, const DecodeCfg& c, int chunk, __half* kc, __half* vc, size_t layer_cache, int t_cap);
+
+// ------------------------------------------------------------------------------------------------- no-speech probability
+// openai/whisper's no_speech_prob: softmax of the raw logits at each window's first <|startoftranscript|> position s_u,
+// at <|nospeech|>.  Whichever pass first forwards s_u also yields that row's logits (or, for a wide prefill pass, its
+// final-LayerNorm row); the passes themselves are the ones the call runs without the request.
+
+// whether some utterance's s_u lies in [lo, hi)
+bool ns_in(const DecodeCfg& c, int lo, int hi) {
+  if (c.sot == nullptr) return false;
+  for (int u = 0; u < c.n_utt; ++u)
+    if (c.sot[u] >= lo && c.sot[u] < hi) return true;
+  return false;
+}
+
+// row tables of one group: at most one reduction per pass that forwards some s_u, the wide gather's and the first step's
+void ns_begin(wisb_handle* h, const DecodeCfg& c) {
+  h->ns_used = 0;
+  if (c.sot == nullptr) return;
+  const size_t n = static_cast<size_t>(c.n_utt) * (std::min(c.n_utt, c.prompt_len) + 2);
+  h->ns_pin.ensure(n);  // (the previous group's copies from it ended with that group's synchronise)
+  h->ns_rows.ensure(n);
+}
+
+// row(u) for every utterance, in a row table of its own (the group's copies are in flight together) -> its device
+// address, or null when no utterance has a row here
+const int* ns_table(wisb_handle* h, const DecodeCfg& c, const std::function<int(int u)>& row) {
+  if (c.sot == nullptr) return nullptr;
+  const size_t off = static_cast<size_t>(h->ns_used) * c.n_utt;
+  WISB_REQUIRE(off + c.n_utt <= h->ns_rows.n, "no-speech: more reductions than the group's row tables hold");
+  int* t = h->ns_pin.p + off;
+  bool any = false;
+  for (int u = 0; u < c.n_utt; ++u) any |= (t[u] = row(u)) >= 0;
+  if (!any) return nullptr;
+  ++h->ns_used;
+  WISB_CUDA(cudaMemcpyAsync(h->ns_rows.p + off, t, sizeof(int) * c.n_utt, cudaMemcpyHostToDevice, h->stream));
+  return h->ns_rows.p + off;
+}
+
+// c.ns_out[u] from row row(u) of logits (row(u) < 0: not in this buffer)
+void ns_reduce(wisb_handle* h, const DecodeCfg& c, const float* logits, const std::function<int(int u)>& row) {
+  const int* t = ns_table(h, c, row);
+  if (t == nullptr) return;
+  no_speech_run(logits, h->dims.n_vocab_pad, t, c.n_utt, h->dims.n_vocab, h->dims.no_speech, c.ns_out, h->stream);
+  ++h->launches;
+}
+
+// the rows of the first decoding step's pass (utterance u's first beam) for every utterance whose prompt ends at s_u
+void ns_reduce_first_step(wisb_handle* h, const DecodeCfg& c, const float* logits) {
+  const int P = c.prompt_len;
+  ns_reduce(h, c, logits, [&](int u) { return c.sot[u] == P - 1 ? u * c.beam : -1; });
+}
 
 // decode utterances [u0, u0 + n_utt) of the encoded batch with the persistent pass (<= 8 rows); writes results to the
 // host arrays
@@ -1188,32 +1257,46 @@ int decode_pass(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, cons
   // longer prompts: batched passes of up to prefill_rows rows instead of one persistent pass per position
   const bool wide = h->wide_prefill && P - 1 > MAX_BEAM;
   persistent_setup(h, c, prompts, max_new_host, fused ? P : one_pass_prefill || wide ? P - 1 : 0);
-  if (c.max_new > 0) {
+  // (capped at 0 new tokens, the prefill and the first step's pass run only for the no-speech probability: they are not
+  // decoding steps)
+  if (c.max_new > 0 || c.sot != nullptr) {
     // the persistent pass is one cooperative launch per step: no graph needed
+    int passes = 0;
     if (fused || one_pass_prefill) {
-      enqueue_decoder_forward(h, c, fused, fused ? P : P - 1);
-      ++steps;
+      const int n = fused ? P : P - 1;
+      enqueue_decoder_forward(h, c, fused || ns_in(c, 0, n), n);
+      ++passes;
       h->launches += 1;
+      ns_reduce(h, c, h->logits.p, [&](int u) { return c.sot[u] < n ? u * n + c.sot[u] : -1; });
     } else if (wide) {
       const int chunk = std::min(P - 1, std::max(1, h->prefill_rows / c.n_utt));
-      steps += wide_prefill_run(h, c, chunk, h->kcache.p, h->vcache.p, static_cast<size_t>(DEC_MAX_ROWS) * T_MAX * h->dims.d_model,
+      passes += wide_prefill_ns(h, c, chunk, h->kcache.p, h->vcache.p, static_cast<size_t>(DEC_MAX_ROWS) * T_MAX * h->dims.d_model,
                                 T_MAX);
     } else {
       for (int p = 0; p + 1 < P; ++p) {
-        enqueue_prefill(h, c);
-        ++steps;
+        enqueue_prefill(h, c, ns_in(c, p, p + 1));
+        ++passes;
         h->launches += 2;
+        ns_reduce(h, c, h->logits.p, [&](int u) { return c.sot[u] == p ? u * c.beam : -1; });
       }
     }
-    // (fused: step 0 is the search step alone, which is not a pass)
-    steps += step_loop(h, c.max_new, true, [&](int gs) {
-      if (fused && gs == 0) {
-        search_step_run(make_search_args(h, c), h->stream);
-        return 2;
-      }
-      enqueue_step(h, c);
-      return 1 + 2;  // the pass + the two kernels of the search step
-    }) - (fused ? 1 : 0);
+    if (c.max_new > 0) {
+      steps += passes;
+      // (fused: step 0 is the search step alone, which is not a pass)
+      steps += step_loop(h, c.max_new, true, [&](int gs) {
+        if (fused && gs == 0) {
+          search_step_run(make_search_args(h, c), h->stream);
+          return 2;
+        }
+        enqueue_step(h, c);
+        if (gs == 0) ns_reduce_first_step(h, c, h->logits.p);
+        return 1 + 2;  // the pass + the two kernels of the search step
+      }) - (fused ? 1 : 0);
+    } else if (!fused && ns_in(c, P - 1, P)) {
+      enqueue_decoder_forward(h, c, true);  // the first step's pass, without its search
+      ++h->launches;
+      ns_reduce_first_step(h, c, h->logits.p);
+    }
   }
   read_results(h, c, max_new_host, out_ids, out_stride, out_len, out_score);
   return steps;
@@ -1407,10 +1490,12 @@ BatchArgs batch_prefill_args(wisb_handle* h, const DecodeCfg& c, int chunk, bool
 // Batched prefill: positions [0, n_pos) of the token matrix in h->prompt_dev ([c.n_utt][tok_stride]) as the rows of
 // shared passes of at most chunk_max positions per utterance, K/V into cache slot u * slot_stride.  layer_hook(layer,
 // chunk), if given, runs after every layer's cross-query GEMM and returns its launches; after_pass(p0, chunk), if given,
-// runs after every pass.  Returns the number of passes.
+// runs after every pass.  A pass yields logits when with_logits, or when logits_if(p0, chunk) says so.  Returns the number
+// of passes.
 int batch_prefill(wisb_handle* h, const DecodeCfg& c, int tok_stride, int n_pos, int chunk_max, int slot_stride,
                   bool with_logits, const std::function<int(int layer, int chunk)>& layer_hook = nullptr,
-                  const std::function<void(int p0, int chunk)>& after_pass = nullptr) {
+                  const std::function<void(int p0, int chunk)>& after_pass = nullptr,
+                  const std::function<bool(int p0, int chunk)>& logits_if = nullptr) {
   struct Hook {
     const std::function<int(int, int)>* fn;
     int chunk;
@@ -1420,7 +1505,7 @@ int batch_prefill(wisb_handle* h, const DecodeCfg& c, int tok_stride, int n_pos,
     const int chunk = std::min(chunk_max, n_pos - p0);
     prefill_rows_run(h->tokens.p, h->row_pos.p, h->row_slot.p, h->prompt_dev.p, tok_stride, c.n_utt, p0, chunk, slot_stride,
                      h->stream);
-    BatchArgs a = batch_prefill_args(h, c, chunk, with_logits);
+    BatchArgs a = batch_prefill_args(h, c, chunk, with_logits || (logits_if && logits_if(p0, chunk)));
     if (layer_hook) {
       hook.chunk = chunk;
       a.layer_hook = [](void* ctx, int layer, cudaStream_t) {
@@ -1490,8 +1575,10 @@ BatchArgs wide_prefill_args(wisb_handle* h, const DecodeCfg& c, int ch, int t_ca
 // Wide prefill: prompt positions [0, prompt_len - 1) of every utterance in h->prompt_dev as the rows of batched passes of
 // `chunk` positions per utterance, K/V into cache slot u * c.beam of kc / vc, cross-attention through
 // prefill_cross_attn_launch on h->ckv in the layout the call encoded.  Leaves what the persistent one-pass prefill leaves
-// in the cache (the caller then starts the search with the shared-prefix indirection).  Returns the number of passes.
-int wide_prefill_run(wisb_handle* h, const DecodeCfg& c, int chunk, __half* kc, __half* vc, size_t layer_cache, int t_cap) {
+// in the cache (the caller then starts the search with the shared-prefix indirection).  after_pass(p0, ch), if given,
+// runs after every pass.  Returns the number of passes.
+int wide_prefill_run(wisb_handle* h, const DecodeCfg& c, int chunk, __half* kc, __half* vc, size_t layer_cache, int t_cap,
+                     const std::function<void(int p0, int ch)>& after_pass = nullptr) {
   const int L = h->dims.n_dec_layers, n_pos = c.prompt_len - 1;
   ensure_prefill(h, c.n_utt * chunk, kc, vc, layer_cache, t_cap);
   for (int i = 0; i < L; ++i) bind_cross_kv(h, h->pf_layers[i], i, c.u0, c.B_total);
@@ -1501,7 +1588,41 @@ int wide_prefill_run(wisb_handle* h, const DecodeCfg& c, int chunk, __half* kc, 
     prefill_rows_run(h->ptok.p, h->ppos.p, h->pslot.p, h->prompt_dev.p, c.prompt_len, c.n_utt, p0, ch, c.beam, h->stream);
     BatchArgs a = wide_prefill_args(h, c, ch, t_cap);
     h->launches += 1 + batch_pass_run(a, h->pf_layers.data(), L, h->stream);
+    if (after_pass) after_pass(p0, ch);
   }
+  return passes;
+}
+
+// the wide prefill passes over positions [0, prompt_len - 1); with the request, every s_u among them is gathered from
+// its pass's final-LayerNorm rows into ns_x, and one vocabulary GEMM over ns_x feeds the reduction (a logits buffer for
+// every wide-pass row would be n_vocab_pad floats per row: 213 MB at 1024 rows)
+int wide_prefill_ns(wisb_handle* h, const DecodeCfg& c, int chunk, __half* kc, __half* vc, size_t layer_cache, int t_cap) {
+  const int P = c.prompt_len;
+  if (!ns_in(c, 0, P - 1)) return wide_prefill_run(h, c, chunk, kc, vc, layer_cache, t_cap);
+  const Dims& dm = h->dims;
+  const int cap = round_up(c.n_utt, 128);
+  if (cap > h->ns_cap) {
+    WISB_CUDA(cudaStreamSynchronize(h->stream));
+    h->ns_x.release();
+    h->ns_x.ensure(static_cast<size_t>(cap) * dm.d_model, true);  // (rows no window fills stay finite GEMM inputs)
+    h->ns_logits.release();
+    h->ns_logits.ensure(static_cast<size_t>(cap) * dm.n_vocab_pad);
+    GemmEpi e;
+    e.mode = EPI_F32;
+    e.out = h->ns_logits.p;
+    e.ldo = dm.n_vocab_pad;
+    plan_dec_gemm(h, h->ns_vocab, h->ns_x.p, dm.d_model, h->H("dec.tok_emb"), cap, dm.n_vocab_pad, dm.d_model, e, false);
+    h->ns_cap = cap;
+  }
+  const int passes = wide_prefill_run(h, c, chunk, kc, vc, layer_cache, t_cap, [&](int p0, int ch) {
+    const int* t = ns_table(h, c, [&](int u) { return c.sot[u] >= p0 && c.sot[u] < p0 + ch ? u * ch + c.sot[u] - p0 : -1; });
+    if (t == nullptr) return;
+    row_gather_run(h->pxn.p, dm.d_model, t, c.n_utt, h->ns_x.p, h->stream);
+    ++h->launches;
+  });
+  gemm_run(h->ns_vocab, h->stream);
+  ++h->launches;
+  ns_reduce(h, c, h->ns_logits.p, [&](int u) { return c.sot[u] < P - 1 ? u : -1; });
   return passes;
 }
 
@@ -1518,7 +1639,9 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
   bind_batch_cross_kv(h, c.u0, c.B_total);
   int steps = 0;
   upload_prompts(h, prompts, max_new_host, c);
-  if (c.max_new > 0) {
+  // (capped at 0 new tokens, the prefill and the first step's pass run only for the no-speech probability: they are not
+  // decoding steps)
+  if (c.max_new > 0 || c.sot != nullptr) {
     // ---- prompt prefix: every utterance's positions [0, prompt_len - 1) as rows of shared passes (<= 8 positions and
     //      <= the row capacity per pass), K/V into the slot of the utterance's first beam
     const int P = c.prompt_len;
@@ -1527,14 +1650,29 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
     const bool fused = P <= chunk_max;
     // prompts longer than 9 tokens: wide passes of up to prefill_rows rows (> 8 positions per utterance)
     const int wide = std::min(P - 1, std::max(chunk_max, h->prefill_rows / c.n_utt));
+    // utterance u's s_u in the pass of positions [p0, p0 + chunk): its row u * chunk + s_u - p0 of blogits
+    auto ns_chunk = [&](int p0, int chunk) {
+      ns_reduce(h, c, h->blogits.p, [&](int u) { return c.sot[u] >= p0 && c.sot[u] < p0 + chunk ? u * chunk + c.sot[u] - p0 : -1; });
+    };
+    int passes;
     if (fused)
-      steps += batch_prefill(h, c, P, P, chunk_max, c.beam, true);
+      passes = batch_prefill(h, c, P, P, chunk_max, c.beam, true, nullptr, ns_chunk);
     else if (h->wide_prefill && P - 1 > MAX_BEAM && wide > chunk_max)
-      steps += wide_prefill_run(h, c, wide, h->bkc.p, h->bvc.p, static_cast<size_t>(h->bd_rows) * h->bd_tcap * h->dims.d_model,
-                                h->bd_tcap);
+      passes = wide_prefill_ns(h, c, wide, h->bkc.p, h->bvc.p, static_cast<size_t>(h->bd_rows) * h->bd_tcap * h->dims.d_model,
+                               h->bd_tcap);
     else
-      steps += batch_prefill(h, c, P, P - 1, chunk_max, c.beam, false);
+      passes = batch_prefill(h, c, P, P - 1, chunk_max, c.beam, false, nullptr, ns_chunk,
+                             [&](int p0, int chunk) { return ns_in(c, p0, p0 + chunk); });
     search_init_run(make_batch_search_args(h, c), h->prompt_dev.p, s, fused ? P : P - 1);
+    if (c.max_new == 0) {
+      if (!fused && ns_in(c, P - 1, P)) {  // the first step's pass, without its search
+        h->launches += batch_pass_run(batch_step_args(h, c), h->bd_layers.data(), h->dims.n_dec_layers, s);
+        ns_reduce_first_step(h, c, h->blogits.p);
+      }
+      read_results(h, c, max_new_host, out_ids, out_stride, out_len, out_score);
+      return steps;
+    }
+    steps += passes;
     cudaGraphExec_t g = nullptr;
     if (h->use_graphs && !h->profile) {  // (the per-kernel timing hook needs eager launches)
       GraphKey key;
@@ -1567,6 +1705,7 @@ int decode_batch(wisb_handle* h, const DecodeCfg& c, const int32_t* prompts, con
         return 2;
       }
       if (g) WISB_CUDA(cudaGraphLaunch(g, s)); else enqueue_batch_step(h, c);
+      if (gs == 0) ns_reduce_first_step(h, c, h->blogits.p);  // (outside the graph: the step graphs stay as they are)
       return h->bd_launches_step;
     }) - (fused ? 1 : 0);
   }
@@ -1887,6 +2026,7 @@ int wisb_set_option(wisb_handle* h, const char* key, int value) {
     }
     else if (k == "decoder_batch") h->decoder_batch = value;  // 2 = use the batched pass even for <= 8 rows (tests)
     else if (k == "wide_prefill") h->wide_prefill = value ? 1 : 0;  // 0: prompts prefill at most 8 positions per pass
+    else if (k == "no_speech_prob") h->no_speech = value ? 1 : 0;
     else if (k == "prefill_rows") {
       WISB_REQUIRE(value >= 8 && value <= 65536, "prefill_rows must be in [8, 65536]");
       h->prefill_rows = value;
@@ -1963,6 +2103,7 @@ int wisb_generate_options_init(wisb_generate_options* opt) {
 int wisb_generate(wisb_handle* h, const float* mel, int B, const int32_t* prompts, int prompt_len,
                   const wisb_generate_options* opt, int32_t* out_ids, int out_stride, int32_t* out_len, float* out_score) {
   return guarded(h, [&] {
+    h->ns_B = 0;  // (a failed call leaves no no-speech probabilities to read)
     const Dims& dm = h->dims;
     WISB_REQUIRE(opt != nullptr && opt->struct_size == sizeof(wisb_generate_options),
                  "options are NULL or their struct_size is not sizeof(wisb_generate_options)");
@@ -2044,6 +2185,17 @@ int wisb_generate(wisb_handle* h, const float* mel, int B, const int32_t* prompt
         }
       }
     }
+    // the no-speech probability: the position of every window's first <|startoftranscript|> (openai/whisper's sot_index)
+    std::vector<int> sot;
+    if (h->no_speech) {
+      sot.resize(B);
+      for (int b = 0; b < B; ++b) {
+        const int32_t* p = prompts + static_cast<size_t>(b) * prompt_len;
+        sot[b] = static_cast<int>(std::find(p, p + prompt_len, dm.sot) - p);
+        WISB_REQUIRE(sot[b] < prompt_len, "no_speech_prob: every prompt must contain <|startoftranscript|>");
+      }
+      h->ns_prob.ensure(B);
+    }
     auto new_tokens = [&](int ml) {  // CTranslate2: at most max_length / 2 new tokens, max_length in total
       int v = ml / 2 < ml - prompt_len ? ml / 2 : ml - prompt_len;
       return v < 0 ? 0 : v;
@@ -2120,6 +2272,11 @@ int wisb_generate(wisb_handle* h, const float* mel, int B, const int32_t* prompt
         c.max_new = 0;
         for (int u = 0; u < n; ++u) c.max_new = per_utt[g0 + u] > c.max_new ? per_utt[g0 + u] : c.max_new;
       }
+      if (!sot.empty()) {
+        c.sot = sot.data() + g0;
+        c.ns_out = h->ns_prob.p + g0;
+      }
+      ns_begin(h, c);
       const int32_t* gp = prompts + static_cast<size_t>(g0) * prompt_len;
       const int* gmx = per_utt.empty() ? nullptr : per_utt.data() + g0;
       const size_t per = sample ? o.num_hypotheses : 1;  // output entries per window
@@ -2130,9 +2287,24 @@ int wisb_generate(wisb_handle* h, const float* mel, int B, const int32_t* prompt
       WISB_CUDA(cudaEventRecord(h->ev[5], s));
       time_group(h, {2, 3, 4});  // encoder, cross K/V, decode
     }
+    if (!sot.empty()) {
+      h->ns_host.resize(B);
+      WISB_CUDA(cudaMemcpyAsync(h->ns_host.data(), h->ns_prob.p, sizeof(float) * B, cudaMemcpyDeviceToHost, s));
+      WISB_CUDA(cudaStreamSynchronize(s));
+      h->ns_B = B;
+    }
     h->timing[6] = static_cast<float>(steps);
     h->timing[7] = static_cast<float>(h->launches);
     h->prof_collect();
+  });
+}
+
+int wisb_get_no_speech_probs(wisb_handle* h, int B, float* out) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(out != nullptr, "out is NULL");
+    WISB_REQUIRE(h->ns_B > 0, "the last wisb_generate ran without option no_speech_prob, or failed");
+    WISB_REQUIRE(B == h->ns_B, "B differs from the last wisb_generate's");
+    memcpy(out, h->ns_host.data(), sizeof(float) * B);
   });
 }
 
@@ -2699,6 +2871,28 @@ int wisb_debug_align_post(wisb_handle* h, const float* weights, int A, int R, in
     if (matrix_out) WISB_CUDA(cudaMemcpyAsync(matrix_out, mat.p, cells * 4, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaMemcpyAsync(path_out, path.p, static_cast<size_t>(R + F) * 2 * 4, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaMemcpyAsync(path_len, meta.p + 2, 4, cudaMemcpyDeviceToHost, s));
+    WISB_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+int wisb_debug_no_speech_probs(wisb_handle* h, const float* logits, int n_rows, int ldl, const int32_t* rows, int n,
+                               int n_vocab, int no_speech, float* out) {
+  return guarded(h, [&] {
+    WISB_REQUIRE(logits && rows && out, "debug_no_speech_probs: NULL argument");
+    WISB_REQUIRE(n_rows >= 1 && n >= 1 && n <= 65535 && n_vocab >= 1 && ldl >= n_vocab && no_speech >= 0 && no_speech < n_vocab,
+                 "debug_no_speech_probs: bad geometry");
+    for (int u = 0; u < n; ++u) WISB_REQUIRE(rows[u] < n_rows, "debug_no_speech_probs: row index out of range");
+    cudaStream_t s = h->stream;
+    DevBuf<float> dl, dout;
+    DevBuf<int> drows;
+    dl.ensure(static_cast<size_t>(n_rows) * ldl);
+    dout.ensure(n);
+    drows.ensure(n);
+    WISB_CUDA(cudaMemcpyAsync(dl.p, logits, sizeof(float) * n_rows * static_cast<size_t>(ldl), cudaMemcpyHostToDevice, s));
+    WISB_CUDA(cudaMemcpyAsync(drows.p, rows, sizeof(int) * n, cudaMemcpyHostToDevice, s));
+    WISB_CUDA(cudaMemcpyAsync(dout.p, out, sizeof(float) * n, cudaMemcpyHostToDevice, s));
+    no_speech_run(dl.p, ldl, drows.p, n, n_vocab, no_speech, dout.p, s);
+    WISB_CUDA(cudaMemcpyAsync(out, dout.p, sizeof(float) * n, cudaMemcpyDeviceToHost, s));
     WISB_CUDA(cudaStreamSynchronize(s));
   });
 }

@@ -810,6 +810,48 @@ __global__ void lang_probs_kernel(const float* logits, long long ldl, const int*
   }
 }
 
+constexpr int NS_THREADS = 256;
+
+// sum (ADD) or max over the CTA; every thread gets the result
+template <bool ADD>
+__device__ float ns_block_reduce(float v, float* s_red) {
+  for (int o = 16; o > 0; o >>= 1) {
+    const float w = __shfl_xor_sync(0xffffffffu, v, o);
+    v = ADD ? v + w : fmaxf(v, w);
+  }
+  if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  v = s_red[0];
+  for (int i = 1; i < NS_THREADS / 32; ++i) v = ADD ? v + s_red[i] : fmaxf(v, s_red[i]);
+  __syncthreads();  // (s_red is reused by the next reduction)
+  return v;
+}
+
+// CTA u: out[u] = softmax(row)[no_speech] over columns [0, n_vocab) of logits row rows[u]; rows[u] < 0 leaves out[u]
+__global__ void __launch_bounds__(NS_THREADS) no_speech_kernel(const float* logits, long long ldl, const int* rows,
+                                                               int n_vocab, int no_speech, float* out) {
+  __shared__ float s_red[NS_THREADS / 32];
+  const int u = blockIdx.x, r = rows[u];
+  if (r < 0) return;
+  const float* row = logits + static_cast<long long>(r) * ldl;
+  float mx = -INFINITY;
+  for (int i = threadIdx.x; i < n_vocab; i += NS_THREADS) mx = fmaxf(mx, row[i]);
+  mx = ns_block_reduce<false>(mx, s_red);
+  float s = 0.f;
+  for (int i = threadIdx.x; i < n_vocab; i += NS_THREADS) s += expf(row[i] - mx);
+  s = ns_block_reduce<true>(s, s_red);
+  if (threadIdx.x == 0) out[u] = expf(row[no_speech] - mx) / s;
+}
+
+// CTA u: dst row u = src row rows[u] (d fp16 values, d % 8 == 0); rows[u] < 0 leaves dst row u
+__global__ void __launch_bounds__(128) row_gather_kernel(const __half* src, int d, const int* rows, __half* dst) {
+  const int u = blockIdx.x, r = rows[u];
+  if (r < 0) return;
+  const uint4* s = reinterpret_cast<const uint4*>(src + static_cast<long long>(r) * d);
+  uint4* t = reinterpret_cast<uint4*>(dst + static_cast<long long>(u) * d);
+  for (int i = threadIdx.x; i < d / 8; i += blockDim.x) t[i] = s[i];
+}
+
 }  // namespace
 
 void search_step_run(const SearchArgs& a, cudaStream_t stream) {
@@ -901,6 +943,19 @@ void lang_probs_run(const float* logits, long long ldl, const int* lang_ids, int
                     float* probs, cudaStream_t stream) {
   WISB_REQUIRE(n_lang <= 128, "detect_language: more than 128 language ids");
   lang_probs_kernel<<<n_utt, 128, 0, stream>>>(logits, ldl, lang_ids, n_lang, row_stride, probs);
+  WISB_CUDA(cudaGetLastError());
+}
+
+void no_speech_run(const float* logits, long long ldl, const int* rows, int n_utt, int n_vocab, int no_speech, float* out,
+                   cudaStream_t stream) {
+  WISB_REQUIRE(n_vocab >= 1 && n_vocab <= ldl && no_speech >= 0 && no_speech < n_vocab, "no-speech: bad vocabulary geometry");
+  no_speech_kernel<<<n_utt, NS_THREADS, 0, stream>>>(logits, ldl, rows, n_vocab, no_speech, out);
+  WISB_CUDA(cudaGetLastError());
+}
+
+void row_gather_run(const __half* src, int d, const int* rows, int n_utt, __half* dst, cudaStream_t stream) {
+  WISB_REQUIRE(d % 8 == 0, "row gather: d must be a multiple of 8");
+  row_gather_kernel<<<n_utt, 128, 0, stream>>>(src, d, rows, dst);
   WISB_CUDA(cudaGetLastError());
 }
 

@@ -371,7 +371,9 @@ class Whisper:
         """ctranslate2.models.Whisper.generate for the options WIS relies on (SURVEY.md section 8b defaults).  With
         beam_size=1 and sampling_topk != 1 it samples num_hypotheses hypotheses per window (``check_sampling_options``),
         returned best first; random_seed (an extension: None, an int or one int per window, ``window_seeds``) makes
-        that reproducible."""
+        that reproducible.  return_no_speech_prob=True fills each result's no_speech_prob (one per window, sampling
+        too): the probability of <|nospeech|> at the prompt's first <|startoftranscript|>, which every prompt must then
+        contain."""
         src = self._input(features)
         n = src.n
         if len(prompts) != n:
@@ -407,6 +409,13 @@ class Whisper:
             raise ValueError("max_initial_timestamp_index must be a non-negative int")
         extra = [int(t) for t in suppress_tokens if t >= 0]
         p = np.asarray(prompts, np.int32)
+        # the no-speech probability of window w is read at its prompt's first <|startoftranscript|>; the handles fill
+        # ns[s:e] for their windows (a stand-in handle that ignores no_speech_out leaves 0.0)
+        ns = np.zeros(n, np.float32) if return_no_speech_prob else None
+        if return_no_speech_prob and not (p == self._dims.get("sot", 50258)).any(axis=1).all():
+            raise ValueError("return_no_speech_prob needs <|startoftranscript|> in every prompt")
+        ns_out = lambda s, e: None if ns is None else ns[s:e]  # noqa: E731
+        no_speech = lambda w: 0.0 if ns is None else float(ns[w])  # noqa: E731
         # extension over CTranslate2: `max_length` may be one int per window (requests with different limits coalesced
         # into one call by batcher.TranscribeBatcher); a plain int is the CTranslate2 meaning
         ml = None if np.isscalar(max_length) else np.asarray(max_length, np.int32)
@@ -444,26 +453,29 @@ class Whisper:
                                                  float(sampling_temperature), seeds[s:e], float(length_penalty),
                                                  max_length if ml is None else ml[s:e], extra, B=e - s,
                                                  timestamps=timestamps,
-                                                 max_initial_timestamp_index=int(max_initial_timestamp_index), **proc)
+                                                 max_initial_timestamp_index=int(max_initial_timestamp_index),
+                                                 no_speech_out=ns_out(s, e), **proc)
                 return seqs, scores
 
             results = []
             for seqs, scores in self._dispatch(src, run_sample):
                 for hyp, sc in zip(seqs, scores):
-                    results.append(WhisperGenerationResult(hyp, list(sc) if return_scores else []))
+                    results.append(WhisperGenerationResult(hyp, list(sc) if return_scores else [],
+                                                           no_speech(len(results))))
             return results
 
         def run(h, mel, s, e):
             return h.generate(mel, p[s:e], window(search["beam_size"], s, e), window(search["patience"], s, e),
                               window(search["length_penalty"], s, e), max_length if ml is None else ml[s:e],
                               extra, B=e - s, timestamps=timestamps,
-                              max_initial_timestamp_index=int(max_initial_timestamp_index), **proc)
+                              max_initial_timestamp_index=int(max_initial_timestamp_index), no_speech_out=ns_out(s, e),
+                              **proc)
 
         outs = self._dispatch(src, run)
         results = []
         for ids, scores in outs:
             for seq, sc in zip(ids, scores):
-                results.append(WhisperGenerationResult([seq], [sc] if return_scores else []))
+                results.append(WhisperGenerationResult([seq], [sc] if return_scores else [], no_speech(len(results))))
         return results
 
     def detect_language(self, features):
